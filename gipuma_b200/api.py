@@ -110,7 +110,6 @@ def load_library():
     L.gpm_shard_comm_attach.argtypes = [vp, vp, C.c_int, C.c_int]
     L.gpm_shard_run.argtypes = [vp, fp]
     L.gpm_measure_fetch_peak.argtypes = [vp, C.POINTER(C.c_double)]
-    L.gpm_debug_packed_mismatches.argtypes = [vp, C.POINTER(C.c_uint), fp, C.c_int]
     L.gpm_batch_run.argtypes = [C.POINTER(GpmBatchDesc), C.POINTER(GpmBatchStats)]
     L.gpm_batch_last_error.restype = C.c_char_p
     L.gpm_shard_p2p_export.argtypes = [vp, C.c_int, vp, C.POINTER(vp)]
@@ -121,7 +120,7 @@ def load_library():
                  "gpm_set_rng", "gpm_set_state", "gpm_get_state", "gpm_init", "gpm_sweep", "gpm_phase",
                  "gpm_finalize", "gpm_cost_eval", "gpm_run", "gpm_get_stats", "gpm_reset_stats", "gpm_set_option",
                  "gpm_init_planes", "gpm_shard_num_stages", "gpm_shard_stage", "gpm_shard_finish_init", "gpm_shard_unique_id",
-                 "gpm_shard_comm_init", "gpm_shard_comm_attach", "gpm_shard_run", "gpm_measure_fetch_peak", "gpm_shard_p2p_export", "gpm_shard_p2p_attach", "gpm_batch_run", "gpm_debug_packed_mismatches",
+                 "gpm_shard_comm_init", "gpm_shard_comm_attach", "gpm_shard_run", "gpm_measure_fetch_peak", "gpm_shard_p2p_export", "gpm_shard_p2p_attach", "gpm_batch_run",
                  "gpm_prepare_cameras", "gpm_select_views", "gpm_write_dmb", "gpm_read_dmb", "gpm_write_result_dmb"):
         getattr(L, name).restype = C.c_int
     _lib = L
@@ -358,12 +357,6 @@ class Context:
         self._check(self.lib.gpm_get_stats(self.h, s))
         return {"launches": s[0], "hypotheses": s[1], "skipped": s[2], "pruned": s[3],
                 "pairs": s[4], "pairs_full": s[5], "collectives": s[6]}
-
-    def packed_mismatches(self, reset: bool = True):
-        n = C.c_uint(0)
-        rec = np.zeros((64, 8), np.float32)
-        self._check(self.lib.gpm_debug_packed_mismatches(self.h, C.byref(n), rec.ctypes.data_as(C.POINTER(C.c_float)), int(reset)))
-        return int(n.value), rec[: min(64, int(n.value))]
 
     def measure_fetch_peak(self) -> float:
         """Texture-unit ceiling on this GPU, in 1e9 filtered R32F fetches per second (gpm_measure_fetch_peak)."""

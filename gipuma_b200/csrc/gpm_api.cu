@@ -24,10 +24,6 @@
 
 using namespace gpm;
 
-#ifndef GPM_PREPASS_DEFAULT
-#define GPM_PREPASS_DEFAULT 0
-#endif
-
 static thread_local std::string g_err;
 
 static int fail(int code, const std::string& msg)
@@ -72,12 +68,9 @@ struct gpm_ctx {
     void* p2p_peer[8] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
     bool p2p_ipc_opened[8] = {false, false, false, false, false, false, false, false};
     unsigned p2p_seq = 0;
-    int opt_exchange = 1;
-    int opt_equal_rounds = 0;
-    int opt_prepass = GPM_PREPASS_DEFAULT;       // k_sweep's thread-per-pixel pre-pass over idle pixels (env GPM_PREPASS overrides at gpm_create)
-    int opt_fused_warps = 16;                    // warps per block of k_shard_fused: 8 -> two blocks per SM (one samples while the other waits); measured no faster
+    int opt_exchange = 1;                        // 1: peer-memory exchange when attached; 0: NCCL all-gather per stage
     int opt_async_upload = 0;                    // 1: image uploads return without a host synchronisation (caller keeps its buffers alive until the next run)
-    bool inputs_dirty = false;                   // an input changed: stored costs / memo are stale (cleared once, at the next launch)                        // 1: peer-memory exchange when attached; 0: NCCL all-gather per stage
+    bool inputs_dirty = false;                   // an input changed: stored costs / memo are stale (cleared once, at the next launch)
     unsigned* seen = nullptr;        // [H*W*ncand] identity of the plane last offered to each pixel from each of the 8 (fused kernel: 20) propagation directions
     int seen_slots = 8;
     unsigned* refseen = nullptr;     // [H*W]   identity of the plane from which the last all-rejected refinement started
@@ -89,7 +82,6 @@ struct gpm_ctx {
     int refpitch = 0, refrows = 0;   // padded reference image: refrows x refpitch texels
     CUtensorMap tmap{};              // 2-D TMA descriptor of the padded reference image for the current box size / image type
     int tmap_box = 0, tmap_color = -1;
-    int opt_tma = 1;
     float* staging = nullptr;        // W*H floats, upload scratch
     cudaArray_t srcArr = nullptr;
     cudaTextureObject_t srcTex = 0;
@@ -99,11 +91,6 @@ struct gpm_ctx {
     cudaTextureObject_t srcTex4 = 0;
     float4* refpad4 = nullptr;
     float4* staging4 = nullptr;
-    cudaArray_t gradArr = nullptr;   // layered RG32F: (Gx, Gy) central differences of every source view (packed sampling mode)
-    cudaTextureObject_t gradTex = 0;
-    float2* gradLin = nullptr;       // W*H staging for one view's gradients
-    int* d_flag = nullptr;
-    std::vector<char> view_8bit;     // per view: every pixel an integer in [0,255]
     ViewCam* d_cams = nullptr;
     std::vector<ViewCam> h_cams;
     bool cams_dirty = true;
@@ -115,7 +102,7 @@ struct gpm_ctx {
     unsigned long long* d_stats = nullptr;
     unsigned long long launches = 0;
     int opt_prune = 1, opt_dedupe = 1, opt_trust_state = 0, opt_nwarps = 0, opt_stats = 1;
-    int opt_cost_variant = -1, opt_packed = 0, opt_memo = 1, opt_quadperm = 1;
+    int opt_cost_variant = -1, opt_memo = 1, opt_quadperm = 1;
     int opt_shard_async = 0;                     // 1: gpm_shard_eval / gpm_shard_accept only enqueue on gpm_stream()
     int opt_neighbours = 8;                      // 20: the reference's fused kernel (built when SMALLKERNEL is not defined)
     int opt_site[21];                            // diagnostics: override the fused kernel's call-site variants (-1 = table)
@@ -188,17 +175,11 @@ int build_kparams(gpm_ctx* c, bool init_phase, KParams& P, bool eval_call = fals
     // faulted although cuTensorMapEncodeTiled accepts the descriptor): tile_x0 + GPM_APRON = 32 bx + 16 - halo, so the box starts (16 - halo) mod 4 texels early
     P.tile_xo = (c->color == 1) ? 0 : ((GPM_APRON - P.halo) & 3);
     // rounds of 32 consecutive samples (one per lane); the remainder forms a last, shorter round whose (view, sample) pairs
-    // are packed several views to an instruction.  (Option "equal_rounds": windows with 33..47 samples — blocksize 11 —
-    // as two equal rounds, the round-1 arrangement; 32 + 4 keeps whole 2x2 quads and measured faster, DESIGN.md §4.)
+    // share an instruction across several views
     {
         int r = 0;
-        if (P.ns > 32 && P.ns < 48 && c->opt_equal_rounds) {
-            P.round_end[r++] = (unsigned char)((P.ns + 1) / 2);
-            P.round_end[r++] = (unsigned char)P.ns;
-        } else {
-            for (int e = 32; e < P.ns && r < 15; e += 32) P.round_end[r++] = (unsigned char)e;
-            P.round_end[r++] = (unsigned char)P.ns;
-        }
+        for (int e = 32; e < P.ns && r < 15; e += 32) P.round_end[r++] = (unsigned char)e;
+        P.round_end[r++] = (unsigned char)P.ns;
         P.nrounds = r;
     }
     // lane -> sample table of each round.  The texture unit filters a warp's fetches one hardware quad (lanes 4q..4q+3) at a
@@ -206,7 +187,6 @@ int build_kparams(gpm_ctx* c, bool init_phase, KParams& P, bool eval_call = fals
     // "quadperm" the samples of a round are dealt to the lanes as 2x2 blocks (x offset i, i+2; y offset j, j+2) where the
     // round contains them, leftovers in window order.  Only WHICH lane evaluates a sample changes; the per-view FMA chain
     // still consumes the dissimilarities in the reference's order.
-    P.prepass = c->opt_prepass;
     P.quadperm = c->opt_quadperm;
     {
         int s0 = 0;
@@ -231,7 +211,6 @@ int build_kparams(gpm_ctx* c, bool init_phase, KParams& P, bool eval_call = fals
             s0 = s1;
         }
     }
-    P.refpitch = c->refpitch;
     P.tau_color = p.tau_color;  P.tau_gradient = p.tau_gradient;  P.alpha = p.alpha;  P.gamma = p.gamma;
     P.min_disp = p.min_disparity;  P.max_disp = p.max_disparity;
     P.n_best = p.n_best;  P.cost_comb = p.cost_comb;  P.good_factor = p.good_factor;
@@ -258,8 +237,6 @@ int build_kparams(gpm_ctx* c, bool init_phase, KParams& P, bool eval_call = fals
     }
     P.color = c->color == 1 ? 1 : 0;
     P.memo = c->opt_memo;
-    P.packed = c->opt_packed;
-    for (int v = 0; v < c->V; v++) if (!c->view_8bit[v]) P.packed = 0;
     P.dedupe_cand = c->opt_dedupe ? 1 : 0;
     P.rng_mode = c->rng_mode;
     P.ref = c->ref;
@@ -274,21 +251,9 @@ int build_kparams(gpm_ctx* c, bool init_phase, KParams& P, bool eval_call = fals
     if (c->opt_nwarps > 0) nw = c->opt_nwarps;
     if (nw > GPM_LB_THREADS / 32) nw = GPM_LB_THREADS / 32;
     P.nwarps = nw;
-    if (P.color) P.packed = 0;
-    if (P.packed && c->opt_packed == 1) {
-        // auto: the packed mode triples the texture bytes a warp touches per pixel (4 -> 12 B per texel and view); it only
-        // pays while the block's working set stays near the L1 (measured: +11 % at cfg 2, -17 % at cfg 3, DESIGN.md §5)
-        const size_t ws = (size_t)P.V * (box + 2) * (box + 2) * 12 * nw;
-        if (ws > 640 * 1024) P.packed = 0;
-    }
     if (block_smem_bytes(P) > (size_t)c->smem_optin)
         return fail(GPM_E_ARG, "configuration needs more shared memory per block than the device offers");
-    P.use_tma = c->opt_tma ? 1 : 0;
-    if (P.use_tma) {
-        int rc = ensure_tensor_map(c, P);
-        if (rc) return rc;
-    }
-    return GPM_OK;
+    return ensure_tensor_map(c, P);
 }
 
 // identities 1 .. W*H belong to the pixels' initial planes; fresh ones start above
@@ -315,21 +280,69 @@ int sync_cams(gpm_ctx* c)
     return GPM_OK;
 }
 
-int launch_colour(gpm_ctx* c, const KParams& P, int colour, int mask)
+// one block per 32 x 32 tile; at least ~8 waves of blocks over the SMs: gridDim.z splits each tile's pixel list into up
+// to 8 slices for small images
+dim3 tile_grid(const gpm_ctx* c)
 {
-    const size_t smem = block_smem_bytes(P);
-    dim3 grid((P.W + GPM_TILE - 1) / GPM_TILE, (P.H + GPM_TILE - 1) / GPM_TILE);
-    // at least ~8 waves of blocks over the SMs: split each tile's pixel list into up to 8 slices for small images
+    dim3 grid((c->W + GPM_TILE - 1) / GPM_TILE, (c->H + GPM_TILE - 1) / GPM_TILE);
     int split = 1;
     while (split < 8 && (long long)grid.x * grid.y * split < 8LL * c->num_sms) split *= 2;
     grid.z = split;
-    auto kern = P.ncand == 20 ? (P.color ? k_sweep<false, true, true> : k_sweep<false, false, true>)
-                              : (P.color ? k_sweep<false, true, false> : (P.packed ? k_sweep<true, false, false> : k_sweep<false, false, false>));
-    kern<<<grid, P.nwarps * 32, smem, c->stream>>>(P, c->tmap, c->d_cams, P.color ? (const float*)c->refpad4 : c->refpad, P.color ? c->srcTex4 : c->srcTex, c->gradTex, c->planes, c->cost, c->rng,
-                                                      c->prov, Memo{c->pid, c->seen, c->refseen, c->memo_mask, c->next_id}, colour, mask, c->opt_stats ? c->d_stats : nullptr);
+    return grid;
+}
+
+int launch_colour(gpm_ctx* c, const KParams& P, int colour, int mask)
+{
+    auto kern = P.ncand == 20 ? (P.color ? k_sweep<true, true> : k_sweep<false, true>)
+                              : (P.color ? k_sweep<true, false> : k_sweep<false, false>);
+    kern<<<tile_grid(c), P.nwarps * 32, block_smem_bytes(P), c->stream>>>(P, c->tmap, c->d_cams, P.color ? c->srcTex4 : c->srcTex, c->planes, c->cost, c->rng,
+        c->prov, Memo{c->pid, c->seen, c->refseen, c->memo_mask, c->next_id}, colour, mask, c->opt_stats ? c->d_stats : nullptr);
     c->launches++;
     CU(cudaGetLastError());
     return GPM_OK;
+}
+
+// cost of `planes` at every pixel into `cost` (k_cost_eval: one block per tile, no slices)
+cudaError_t launch_cost_eval(gpm_ctx* c, const KParams& P, const float4* planes, float* cost)
+{
+    dim3 grid((P.W + GPM_TILE - 1) / GPM_TILE, (P.H + GPM_TILE - 1) / GPM_TILE);
+    (P.color ? k_cost_eval<true> : k_cost_eval<false>)<<<grid, P.nwarps * 32, block_smem_bytes(P), c->stream>>>(
+        P, c->tmap, c->d_cams, P.color ? c->srcTex4 : c->srcTex, planes, cost, nullptr);
+    c->launches++;
+    return cudaGetLastError();
+}
+
+// random planes (gipuma.cu:1870-1875) and their identities; the XORWOW states are kept in GPM_RNG_STATEFUL mode
+int init_planes(gpm_ctx* c, const KParams& P)
+{
+    dim3 b(16, 16), gr((c->W + 15) / 16, (c->H + 15) / 16);
+    k_init_planes<<<gr, b, 0, c->stream>>>(P, c->seed, c->planes, c->rng_mode == GPM_RNG_STATEFUL ? c->rng : nullptr, c->pid);
+    c->launches++;
+    CU(cudaGetLastError());
+    return reset_next_id(c);
+}
+
+// source views: layered array, Linear filter, the reference's addressing (Wrap + unnormalised, main.cpp:642-648), element reads
+cudaError_t make_layered_texture(cudaArray_t arr, cudaTextureObject_t* tex)
+{
+    cudaResourceDesc res;  memset(&res, 0, sizeof(res));
+    res.resType = cudaResourceTypeArray;  res.res.array.array = arr;
+    cudaTextureDesc td;  memset(&td, 0, sizeof(td));
+    td.addressMode[0] = cudaAddressModeWrap;  td.addressMode[1] = cudaAddressModeWrap;   // main.cpp:644-645
+    td.addressMode[2] = cudaAddressModeClamp;
+    td.filterMode = cudaFilterModeLinear;  td.readMode = cudaReadModeElementType;  td.normalizedCoords = 0;
+    return cudaCreateTextureObject(tex, &res, &td, NULL);
+}
+
+void set_view_camera(gpm_ctx* c, int v, const gpm_camera* cam)
+{
+    ViewCam& vc = c->h_cams[v];
+    memcpy(vc.K, cam->K, sizeof(vc.K));
+    memcpy(vc.R, cam->R, sizeof(vc.R));
+    memcpy(vc.t, cam->t, sizeof(vc.t));
+    c->cams_dirty = true;
+    c->have_view[v] = 1;
+    c->inputs_dirty = true;
 }
 
 int upload_image(gpm_ctx* c, const float* img, size_t pitch_bytes, int on_device, float** dev_img, size_t* dev_pitch_floats)
@@ -380,10 +393,8 @@ extern "C" int gpm_create(gpm_ctx** out, int device, int width, int height, int 
     DeviceGuard g(device);
     gpm_ctx* c = new gpm_ctx;
     for (int& v : c->opt_site) v = -1;
-    if (const char* e = getenv("GPM_PREPASS")) c->opt_prepass = atoi(e) != 0;
     c->device = device;  c->W = width;  c->H = height;  c->maxV = max_views;
     c->have_view.assign(max_views, 0);
-    c->view_8bit.assign(max_views, 0);
     c->h_cams.assign(max_views, ViewCam{});
     const size_t n = (size_t)width * height;
     // the staged window of the last tile row / column reaches roundup(size, 32) + halo + GPM_APRON (+ 3 texels of TMA row padding)
@@ -403,7 +414,6 @@ extern "C" int gpm_create(gpm_ctx** out, int device, int width, int height, int 
     ok(cudaMalloc(&c->next_id, sizeof(unsigned)));
     ok(cudaMalloc(&c->memo_mask, n * sizeof(unsigned)));
     ok(cudaMalloc(&c->staging, n * sizeof(float)));
-    ok(cudaMalloc(&c->d_flag, sizeof(int)));
     ok(cudaMalloc(&c->refpad, (size_t)c->refpitch * c->refrows * sizeof(float)));
     ok(cudaMalloc(&c->d_cams, sizeof(ViewCam) * max_views));
     ok(cudaMalloc(&c->d_stats, 8 * sizeof(unsigned long long)));
@@ -418,29 +428,19 @@ extern "C" int gpm_create(gpm_ctx** out, int device, int width, int height, int 
         ok(cudaMalloc3DArray(&c->srcArr, &desc, make_cudaExtent(width, height, max_views), cudaArrayLayered));
     }
     if (err == cudaSuccess) {
-        cudaResourceDesc res;  memset(&res, 0, sizeof(res));
-        res.resType = cudaResourceTypeArray;  res.res.array.array = c->srcArr;
-        cudaTextureDesc td;  memset(&td, 0, sizeof(td));
-        td.addressMode[0] = cudaAddressModeWrap;  td.addressMode[1] = cudaAddressModeWrap;   // main.cpp:644-645
-        td.addressMode[2] = cudaAddressModeClamp;
-        td.filterMode = cudaFilterModeLinear;  td.readMode = cudaReadModeElementType;  td.normalizedCoords = 0;
-        ok(cudaCreateTextureObject(&c->srcTex, &res, &td, NULL));
+        ok(make_layered_texture(c->srcArr, &c->srcTex));
         ok(cudaDeviceGetAttribute(&c->smem_optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, device));
         ok(cudaDeviceGetAttribute(&c->num_sms, cudaDevAttrMultiProcessorCount, device));
-        ok(cudaFuncSetAttribute(k_sweep<false, false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, c->smem_optin));
-        ok(cudaFuncSetAttribute(k_sweep<true, false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, c->smem_optin));
-        ok(cudaFuncSetAttribute(k_sweep<false, true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, c->smem_optin));
-        ok(cudaFuncSetAttribute(k_sweep<false, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, c->smem_optin));
-        ok(cudaFuncSetAttribute(k_sweep<false, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, c->smem_optin));
-        ok(cudaFuncSetAttribute(k_cost_eval<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, c->smem_optin));
-        ok(cudaFuncSetAttribute(k_cost_eval<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, c->smem_optin));
-        ok(cudaFuncSetAttribute(k_cost_eval<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, c->smem_optin));
-        ok(cudaFuncSetAttribute(k_shard_stage<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, c->smem_optin));
-        ok(cudaFuncSetAttribute(k_shard_fused<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, c->smem_optin));
-        ok(cudaFuncSetAttribute(k_shard_stage<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, c->smem_optin));
-        ok(cudaFuncSetAttribute(k_shard_fused<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, c->smem_optin));
-        ok(cudaFuncSetAttribute(k_shard_stage<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, c->smem_optin));
-        ok(cudaFuncSetAttribute(k_shard_fused<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, c->smem_optin));
+        ok(cudaFuncSetAttribute(k_sweep<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, c->smem_optin));
+        ok(cudaFuncSetAttribute(k_sweep<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, c->smem_optin));
+        ok(cudaFuncSetAttribute(k_sweep<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, c->smem_optin));
+        ok(cudaFuncSetAttribute(k_sweep<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, c->smem_optin));
+        ok(cudaFuncSetAttribute(k_cost_eval<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, c->smem_optin));
+        ok(cudaFuncSetAttribute(k_cost_eval<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, c->smem_optin));
+        ok(cudaFuncSetAttribute(k_shard_stage<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, c->smem_optin));
+        ok(cudaFuncSetAttribute(k_shard_fused<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, c->smem_optin));
+        ok(cudaFuncSetAttribute(k_shard_stage<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, c->smem_optin));
+        ok(cudaFuncSetAttribute(k_shard_fused<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, c->smem_optin));
     }
     if (err != cudaSuccess) {
         std::string m = std::string("gpm_create: ") + cudaGetErrorString(err);
@@ -466,9 +466,6 @@ extern "C" void gpm_destroy(gpm_ctx* c)
     if (c->srcTex4) cudaDestroyTextureObject(c->srcTex4);
     if (c->srcArr4) cudaFreeArray(c->srcArr4);
     cudaFree(c->refpad4);  cudaFree(c->staging4);  cudaFree(c->planar);
-    if (c->gradTex) cudaDestroyTextureObject(c->gradTex);
-    if (c->gradArr) cudaFreeArray(c->gradArr);
-    cudaFree(c->gradLin);  cudaFree(c->d_flag);
     cudaFree(c->planes);  cudaFree(c->cost);  cudaFree(c->prov);  cudaFree(c->seen);  cudaFree(c->refseen);  cudaFree(c->pid);  cudaFree(c->next_id);  cudaFree(c->memo_mask);  cudaFree(c->rng);  cudaFree(c->dispbuf);  cudaFree(c->candbuf);  cudaFree(c->canddepth);  cudaFree(c->sflags);  cudaFree(c->xchg);  cudaFree(c->gath);  cudaFree(c->refpad);  cudaFree(c->staging);
     cudaFree(c->d_cams);  cudaFree(c->d_stats);
     if (c->ev0) cudaEventDestroy(c->ev0);
@@ -541,60 +538,19 @@ extern "C" int gpm_set_view(gpm_ctx* c, int v, const float* img, size_t pitch_by
     if (!c || !img || !cam) return fail(GPM_E_ARG, "gpm_set_view: null argument");
     if (v < 0 || v >= c->maxV) return fail(GPM_E_ARG, "gpm_set_view: view index out of range");
     DeviceGuard g(c->device);
-    float* d = nullptr;
-    size_t pf = 0;
     int rc = ensure_color(c, 0);
     if (rc) return rc;
+    // the image goes straight into its layer of the array: no staging copy
+    const size_t pb = pitch_bytes ? pitch_bytes : (size_t)c->W * sizeof(float);
+    if (pb % sizeof(float)) return fail(GPM_E_ARG, "pitch_bytes must be a multiple of 4");
     cudaMemcpy3DParms m;  memset(&m, 0, sizeof(m));
+    m.srcPtr = make_cudaPitchedPtr(const_cast<float*>(img), pb, c->W, c->H);
     m.dstArray = c->srcArr;
     m.dstPos = make_cudaPos(0, 0, v);
     m.extent = make_cudaExtent(c->W, c->H, 1);
-    if (!on_device && !c->opt_packed) {
-        // host image straight into its layer of the array: no staging copy
-        const size_t pb = pitch_bytes ? pitch_bytes : (size_t)c->W * sizeof(float);
-        if (pb % sizeof(float)) return fail(GPM_E_ARG, "pitch_bytes must be a multiple of 4");
-        m.srcPtr = make_cudaPitchedPtr(const_cast<float*>(img), pb, c->W, c->H);
-        m.kind = cudaMemcpyHostToDevice;
-    } else {
-        rc = upload_image(c, img, pitch_bytes, on_device, &d, &pf);      // staging buffer (the gradient planes of the packed mode read it)
-        if (rc) return rc;
-        m.srcPtr = make_cudaPitchedPtr(d, pf * sizeof(float), c->W, c->H);
-        m.kind = cudaMemcpyDeviceToDevice;
-    }
+    m.kind = on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice;
     CU(cudaMemcpy3DAsync(&m, c->stream));
-    c->view_8bit[v] = 0;
-    if (c->opt_packed) {                         // experimental packed sampling mode: central-difference planes + "8-bit valued" test
-    if (!c->gradArr) {
-        cudaChannelFormatDesc desc2 = cudaCreateChannelDesc(32, 32, 0, 0, cudaChannelFormatKindFloat);
-        CU(cudaMalloc3DArray(&c->gradArr, &desc2, make_cudaExtent(c->W, c->H, c->maxV), cudaArrayLayered));
-        cudaResourceDesc res;  memset(&res, 0, sizeof(res));
-        res.resType = cudaResourceTypeArray;  res.res.array.array = c->gradArr;
-        cudaTextureDesc td;  memset(&td, 0, sizeof(td));
-        td.addressMode[0] = cudaAddressModeWrap;  td.addressMode[1] = cudaAddressModeWrap;  td.addressMode[2] = cudaAddressModeClamp;
-        td.filterMode = cudaFilterModeLinear;  td.readMode = cudaReadModeElementType;  td.normalizedCoords = 0;
-        CU(cudaCreateTextureObject(&c->gradTex, &res, &td, NULL));
-        CU(cudaMalloc(&c->gradLin, (size_t)c->W * c->H * sizeof(float2)));
-    }
-    const int one = 1;
-    CU(cudaMemcpyAsync(c->d_flag, &one, sizeof(int), cudaMemcpyHostToDevice, c->stream));
-    dim3 b(32, 8), gr((c->W + 31) / 32, (c->H + 7) / 8);
-    k_make_gradients<<<gr, b, 0, c->stream>>>(d, pf, c->W, c->H, c->gradLin, c->d_flag);
-    CU(cudaGetLastError());
-    m.srcPtr = make_cudaPitchedPtr(c->gradLin, (size_t)c->W * sizeof(float2), c->W, c->H);
-    m.dstArray = c->gradArr;
-    CU(cudaMemcpy3DAsync(&m, c->stream));
-    int flag = 0;
-    CU(cudaMemcpyAsync(&flag, c->d_flag, sizeof(int), cudaMemcpyDeviceToHost, c->stream));
-    CU(cudaStreamSynchronize(c->stream));
-    c->view_8bit[v] = flag ? 1 : 0;
-    }
-    ViewCam& vc = c->h_cams[v];
-    memcpy(vc.K, cam->K, sizeof(vc.K));
-    memcpy(vc.R, cam->R, sizeof(vc.R));
-    memcpy(vc.t, cam->t, sizeof(vc.t));
-    c->cams_dirty = true;
-    c->have_view[v] = 1;
-    c->inputs_dirty = true;
+    set_view_camera(c, v, cam);
     if (!c->opt_async_upload) CU(cudaStreamSynchronize(c->stream));        // the caller may reuse its buffer
     return GPM_OK;
 }
@@ -609,12 +565,7 @@ static int ensure_color(gpm_ctx* c, int want)
         cudaChannelFormatDesc d1 = cudaCreateChannelDesc(32, 0, 0, 0, cudaChannelFormatKindFloat);
         CU(cudaMalloc3DArray(&c->srcArr4, &d1, make_cudaExtent(c->W, c->H, 3 * (size_t)c->maxV), cudaArrayLayered));
         CU(cudaMalloc(&c->planar, 3 * (size_t)c->W * c->H * sizeof(float)));
-        cudaResourceDesc res;  memset(&res, 0, sizeof(res));
-        res.resType = cudaResourceTypeArray;  res.res.array.array = c->srcArr4;
-        cudaTextureDesc td;  memset(&td, 0, sizeof(td));
-        td.addressMode[0] = cudaAddressModeWrap;  td.addressMode[1] = cudaAddressModeWrap;  td.addressMode[2] = cudaAddressModeClamp;
-        td.filterMode = cudaFilterModeLinear;  td.readMode = cudaReadModeElementType;  td.normalizedCoords = 0;
-        CU(cudaCreateTextureObject(&c->srcTex4, &res, &td, NULL));
+        CU(make_layered_texture(c->srcArr4, &c->srcTex4));
         CU(cudaMalloc(&c->refpad4, (size_t)c->refpitch * c->refrows * sizeof(float4)));
         CU(cudaMalloc(&c->staging4, (size_t)c->W * c->H * sizeof(float4)));
     }
@@ -675,14 +626,7 @@ extern "C" int gpm_set_view_color(gpm_ctx* c, int v, const float* rgba, size_t p
     m.extent = make_cudaExtent(c->W, c->H, 3);
     m.kind = cudaMemcpyDeviceToDevice;
     CU(cudaMemcpy3DAsync(&m, c->stream));
-    ViewCam& vc = c->h_cams[v];
-    memcpy(vc.K, cam->K, sizeof(vc.K));
-    memcpy(vc.R, cam->R, sizeof(vc.R));
-    memcpy(vc.t, cam->t, sizeof(vc.t));
-    c->cams_dirty = true;
-    c->have_view[v] = 1;
-    c->view_8bit[v] = 0;
-    c->inputs_dirty = true;
+    set_view_camera(c, v, cam);
     if (!c->opt_async_upload) CU(cudaStreamSynchronize(c->stream));
     return GPM_OK;
 }
@@ -726,16 +670,9 @@ static int do_init(gpm_ctx* c)
     if (rc) return rc;
     rc = sync_cams(c);
     if (rc) return rc;
-    dim3 b(16, 16), gr((c->W + 15) / 16, (c->H + 15) / 16);                   // gipuma.cu:1870-1875
-    k_init_planes<<<gr, b, 0, c->stream>>>(P, c->seed, c->planes, c->rng_mode == GPM_RNG_STATEFUL ? c->rng : nullptr, c->pid);
-    { int rc_ = reset_next_id(c);  if (rc_) return rc_; }
-    c->launches++;
-    CU(cudaGetLastError());
-    dim3 grid((P.W + GPM_TILE - 1) / GPM_TILE, (P.H + GPM_TILE - 1) / GPM_TILE);
-    (P.color ? k_cost_eval<false, true> : (P.packed ? k_cost_eval<true, false> : k_cost_eval<false, false>))<<<grid, P.nwarps * 32, block_smem_bytes(P), c->stream>>>(P, c->tmap, c->d_cams, P.color ? (const float*)c->refpad4 : c->refpad, P.color ? c->srcTex4 : c->srcTex, c->gradTex, c->planes,
-                                                                         c->cost, nullptr);
-    c->launches++;
-    CU(cudaGetLastError());
+    rc = init_planes(c, P);
+    if (rc) return rc;
+    CU(launch_cost_eval(c, P, c->planes, c->cost));
     CU(cudaMemsetAsync(c->prov, c->color == 1 ? 3 : 0, (size_t)c->W * c->H, c->stream));   // costs now come from the init-variant evaluation (float4: x-first + gradient folding 1)
     CU(cudaMemsetAsync(c->memo_mask, 0, (size_t)c->W * c->H * sizeof(unsigned), c->stream));
     return GPM_OK;
@@ -835,10 +772,7 @@ extern "C" int gpm_cost_eval(gpm_ctx* c, const float* planes, float* out_cost, i
         if (e1 == cudaSuccess) e1 = cudaMemcpyAsync(d_pl, planes, n * sizeof(float4), cudaMemcpyHostToDevice, c->stream);
         if (e1 != cudaSuccess) { cudaFree(d_pl);  cudaFree(d_out);  return fail(GPM_E_CUDA, std::string("gpm_cost_eval: ") + cudaGetErrorString(e1)); }
     }
-    dim3 grid((P.W + GPM_TILE - 1) / GPM_TILE, (P.H + GPM_TILE - 1) / GPM_TILE);
-    (P.color ? k_cost_eval<false, true> : (P.packed ? k_cost_eval<true, false> : k_cost_eval<false, false>))<<<grid, P.nwarps * 32, block_smem_bytes(P), c->stream>>>(P, c->tmap, c->d_cams, P.color ? (const float*)c->refpad4 : c->refpad, P.color ? c->srcTex4 : c->srcTex, c->gradTex, d_pl, d_out, nullptr);
-    c->launches++;
-    cudaError_t e = cudaGetLastError();
+    cudaError_t e = launch_cost_eval(c, P, d_pl, d_out);
     if (e == cudaSuccess && !on_device) e = cudaMemcpyAsync(out_cost, d_out, n * sizeof(float), cudaMemcpyDeviceToHost, c->stream);
     if (e == cudaSuccess) e = cudaStreamSynchronize(c->stream);
     if (!on_device) { cudaFree(d_pl);  cudaFree(d_out); }
@@ -918,14 +852,9 @@ static int shard_common(gpm_ctx* c, int stage, KParams& P)
 static int shard_launch_stage(gpm_ctx* c, const KParams& P, int colour, int stage, const float* gathered_prev, int world, float* xchg)
 {
     const int last = 1 + shard_refine_steps(c->prm);
-    dim3 grid((P.W + GPM_TILE - 1) / GPM_TILE, (P.H + GPM_TILE - 1) / GPM_TILE);
-    int split = 1;                                        // at least ~8 waves of blocks, as in launch_colour
-    while (split < 8 && (long long)grid.x * grid.y * split < 8LL * c->num_sms) split *= 2;
-    grid.z = split;
     ShardState S{c->dispbuf, c->candbuf, c->canddepth, c->sflags};
-    auto kern = P.color ? k_shard_stage<false, true> : (P.packed ? k_shard_stage<true, false> : k_shard_stage<false, false>);
-    kern<<<grid, P.nwarps * 32, block_smem_bytes(P), c->stream>>>(P, c->tmap, c->d_cams, P.color ? (const float*)c->refpad4 : c->refpad,
-        P.color ? c->srcTex4 : c->srcTex, c->gradTex, c->planes, c->cost, c->prov, S, Memo{c->pid, c->seen, c->refseen, c->memo_mask, c->next_id}, colour, stage, last,
+    (P.color ? k_shard_stage<true> : k_shard_stage<false>)<<<tile_grid(c), P.nwarps * 32, block_smem_bytes(P), c->stream>>>(P, c->tmap, c->d_cams,
+        P.color ? c->srcTex4 : c->srcTex, c->planes, c->cost, c->prov, S, Memo{c->pid, c->seen, c->refseen, c->memo_mask, c->next_id}, colour, stage, last,
         gathered_prev, world, xchg, c->opt_stats ? c->d_stats : nullptr);
     c->launches++;
     CU(cudaGetLastError());
@@ -1076,15 +1005,6 @@ static int shard_exchange(gpm_ctx* c, int stage)
 }
 
 // ---- fused peer-memory exchange: region management ------------------------------------------------------------------
-static dim3 shard_grid(gpm_ctx* c)
-{
-    dim3 grid((c->W + GPM_TILE - 1) / GPM_TILE, (c->H + GPM_TILE - 1) / GPM_TILE);
-    int split = 1;                                        // at least ~8 waves of blocks, as in launch_colour
-    while (split < 8 && (long long)grid.x * grid.y * split < 8LL * c->num_sms) split *= 2;
-    grid.z = split;
-    return grid;
-}
-
 // Allocate this rank's exchange region for a shard group of `world` ranks and return its CUDA IPC handle (64 bytes) and its
 // address (for ranks living in the same process).  Layout: [world][nblocks] arrival flags, then [2][world][slot] lists.
 extern "C" int gpm_shard_p2p_export(gpm_ctx* c, int world, void* handle64, void** local_ptr)
@@ -1095,7 +1015,7 @@ extern "C" int gpm_shard_p2p_export(gpm_ctx* c, int world, void* handle64, void*
     long long mx = 0;
     const int ns = gpm_shard_num_stages(c);
     for (int st = 0; st < ns; st++) { const long long f = gpm_shard_stage_floats(c, st);  if (f > mx) mx = f; }
-    const dim3 grid = shard_grid(c);
+    const dim3 grid = tile_grid(c);
     const int nblocks = (int)(grid.x * grid.y * grid.z);
     const size_t flag_bytes = ((size_t)world * nblocks * sizeof(unsigned) + 1023) & ~(size_t)1023;
     const size_t bytes = flag_bytes + 2ull * world * (size_t)mx * sizeof(float);
@@ -1147,7 +1067,6 @@ extern "C" int gpm_shard_p2p_attach(gpm_ctx* c, const void* handles64, void* con
 static int shard_launch_fused(gpm_ctx* c, const KParams& P, int colour, int init_phase, int exchanges)
 {
     const int last = 1 + shard_refine_steps(c->prm);
-    const dim3 grid = shard_grid(c);
     ShardState S{c->dispbuf, c->candbuf, c->canddepth, c->sflags};
     ShardP2P X;
     memset(&X, 0, sizeof(X));
@@ -1157,11 +1076,8 @@ static int shard_launch_fused(gpm_ctx* c, const KParams& P, int colour, int init
     }
     X.err = reinterpret_cast<unsigned*>(c->d_stats + 7);
     X.slot_floats = c->p2p_slot_floats;  X.me = c->shard_rank;  X.world = c->shard_world;  X.nblocks = c->p2p_nblocks;
-    auto kern = P.color ? k_shard_fused<false, true> : (P.packed ? k_shard_fused<true, false> : k_shard_fused<false, false>);
-    KParams Pf = P;                                       // half-size blocks: two per SM (128 registers x 256 threads each)
-    if (c->opt_fused_warps > 0 && c->opt_fused_warps < Pf.nwarps) Pf.nwarps = c->opt_fused_warps;
-    kern<<<grid, Pf.nwarps * 32, block_smem_bytes(Pf), c->stream>>>(Pf, c->tmap, c->d_cams, P.color ? (const float*)c->refpad4 : c->refpad,
-        P.color ? c->srcTex4 : c->srcTex, c->gradTex, c->planes, c->cost, c->prov, S, Memo{c->pid, c->seen, c->refseen, c->memo_mask, c->next_id}, colour, init_phase, last,
+    (P.color ? k_shard_fused<true> : k_shard_fused<false>)<<<tile_grid(c), P.nwarps * 32, block_smem_bytes(P), c->stream>>>(P, c->tmap, c->d_cams,
+        P.color ? c->srcTex4 : c->srcTex, c->planes, c->cost, c->prov, S, Memo{c->pid, c->seen, c->refseen, c->memo_mask, c->next_id}, colour, init_phase, last,
         X, c->p2p_seq, c->opt_stats ? c->d_stats : nullptr);
     c->launches++;
     c->p2p_seq += (unsigned)exchanges;
@@ -1190,11 +1106,7 @@ extern "C" int gpm_shard_run(gpm_ctx* c, float* sweep_ms)
     c->launches = 0;  c->collectives = 0;
     if (world > 1 && c->p2p_attached && c->opt_exchange == 1) {
         // fused flow: one launch for the initial costs, one per colour pass; the exchange happens inside the kernels
-        dim3 b(16, 16), gr((c->W + 15) / 16, (c->H + 15) / 16);
-        k_init_planes<<<gr, b, 0, c->stream>>>(P0, c->seed, c->planes, nullptr, c->pid);
-        c->launches++;
-        CU(cudaGetLastError());
-        rc = reset_next_id(c);
+        rc = init_planes(c, P0);
         if (rc) return rc;
         rc = shard_launch_fused(c, P0, 0, 1, 1);
         if (rc) return rc;
@@ -1220,11 +1132,7 @@ extern "C" int gpm_shard_run(gpm_ctx* c, float* sweep_ms)
     }
     if (world > 1 && !c->comm) return fail(GPM_E_STATE, "gpm_shard_run: neither an NCCL communicator nor peer regions are attached");
     {
-        dim3 b(16, 16), gr((c->W + 15) / 16, (c->H + 15) / 16);
-        k_init_planes<<<gr, b, 0, c->stream>>>(P0, c->seed, c->planes, nullptr, c->pid);
-        c->launches++;
-        CU(cudaGetLastError());
-        rc = reset_next_id(c);
+        rc = init_planes(c, P0);
         if (rc) return rc;
         CU(cudaMemsetAsync(c->memo_mask, 0, (size_t)c->W * c->H * sizeof(unsigned), c->stream));
         rc = shard_launch_stage(c, P0, 0, 0, nullptr, world, c->xchg);
@@ -1267,27 +1175,11 @@ extern "C" int gpm_init_planes(gpm_ctx* c)
     KParams P;
     int rc = build_kparams(c, true, P);
     if (rc) return rc;
-    dim3 b(16, 16), gr((c->W + 15) / 16, (c->H + 15) / 16);
-    k_init_planes<<<gr, b, 0, c->stream>>>(P, c->seed, c->planes, c->rng_mode == GPM_RNG_STATEFUL ? c->rng : nullptr, c->pid);
-    { int rc_ = reset_next_id(c);  if (rc_) return rc_; }
-    c->launches++;
-    CU(cudaGetLastError());
+    rc = init_planes(c, P);
+    if (rc) return rc;
     CU(cudaMemsetAsync(c->prov, GPM_PROV_UNKNOWN, (size_t)c->W * c->H, c->stream));      // every plane is new: costs and memo are stale
     CU(cudaMemsetAsync(c->memo_mask, 0, (size_t)c->W * c->H * sizeof(unsigned), c->stream));
     CU(cudaStreamSynchronize(c->stream));
-    return GPM_OK;
-}
-
-// diagnostics of the experimental packed sampling mode ("packed" = 3): number of fetches whose one-fetch gradient differed
-// from the reference's four fetches, and up to 64 records {cx, cy, view, gx packed, gx reference, gy packed, gy reference, centre}
-extern "C" int gpm_debug_packed_mismatches(gpm_ctx* c, unsigned* count, float* records512, int reset)
-{
-    if (!c || !count) return fail(GPM_E_ARG, "gpm_debug_packed_mismatches: null argument");
-    DeviceGuard g(c->device);
-    CU(cudaStreamSynchronize(c->stream));
-    CU(cudaMemcpyFromSymbol(count, g_packed_mismatch_n, sizeof(unsigned)));
-    if (records512) CU(cudaMemcpyFromSymbol(records512, g_packed_mismatch, 64 * 8 * sizeof(float)));
-    if (reset) { const unsigned z = 0;  CU(cudaMemcpyToSymbol(g_packed_mismatch_n, &z, sizeof(z))); }
     return GPM_OK;
 }
 
@@ -1360,7 +1252,6 @@ extern "C" int gpm_set_option(gpm_ctx* c, const char* name, int value)
     else if (n == "neighbours") {
         if (value != 8 && value != 20) return fail(GPM_E_ARG, "neighbours must be 8 (close + far kernels) or 20 (fused kernel)");
         DeviceGuard g(c->device);
-        if (value == 20) c->opt_packed = 0;
         const int slots = value == 20 ? 20 : 8;
         if (slots != c->seen_slots) {
             CU(cudaStreamSynchronize(c->stream));
@@ -1371,15 +1262,10 @@ extern "C" int gpm_set_option(gpm_ctx* c, const char* name, int value)
         CU(cudaMemsetAsync(c->memo_mask, 0, (size_t)c->W * c->H * sizeof(unsigned), c->stream));
         c->opt_neighbours = value;
     }
-    else if (n == "packed") { c->opt_packed = value;  if (value) for (auto& f : c->view_8bit) f = 0; }   // set BEFORE uploading views;            // 0 off (default), 1 auto, 2 force — EXPERIMENTAL, see DESIGN.md §5
     else if (n == "memo") c->opt_memo = value != 0;
     else if (n == "quadperm") c->opt_quadperm = value != 0;
-    else if (n == "tma") c->opt_tma = value != 0;
     else if (n == "exchange") c->opt_exchange = value != 0;
     else if (n == "async_upload") c->opt_async_upload = value != 0;
-    else if (n == "equal_rounds") c->opt_equal_rounds = value != 0;
-    else if (n == "prepass") c->opt_prepass = value != 0;
-    else if (n == "fused_warps") c->opt_fused_warps = value;
     else if (n == "shard_async") c->opt_shard_async = value != 0;
     else return fail(GPM_E_ARG, "gpm_set_option: unknown option '" + n + "'");
     return GPM_OK;

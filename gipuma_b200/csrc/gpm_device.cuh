@@ -87,12 +87,10 @@ struct KParams {
     int tile_stride;            // texels per row of the staged window in shared memory: tile_w rounded up to 16 (TMA box rows of 64-byte multiples)
     int tile_xo;                // texels between the start of the staged rows and the window's first column: the TMA box must start on a
                                 // 16-byte boundary of the padded image, so it starts (16 - halo) mod 4 texels early (0 for float4 texels)
-    int use_tma;                // 1: the window is staged by one cp.async.bulk.tensor (TMA) per block instead of a cooperative copy
     int nrounds;                // sample rounds; after each one an exact lower bound of the final cost is tested
     unsigned char round_end[16];// cumulative sample count at the end of each round (whole window columns)
     int ns_pad;                 // ns rounded up to a multiple of 4
     int nwarps;
-    int refpitch;               // floats per row of the padded reference image
     float tau_color, tau_gradient, alpha, gamma;
     float min_disp, max_disp;
     int n_best, cost_comb;
@@ -100,14 +98,12 @@ struct KParams {
     int prune, dedupe_self, dedupe_cand;
     int color;                  // 1: float4 (RGB) images — the reference's -color_processing path (T = float4)
     int memo;                   // 1: skip candidates / refinements already known to be rejected at this pixel (see k_sweep)
-    int packed;                 // 1: 8-bit-valued source images -> gradients come from one RG32F fetch (exact, see fetch_sample)
     int cost_variant;           // k_cost_eval: 0 = init/refine rounding, 1 = propagation rounding (see eval_plane)
     int ncand;                  // propagation candidates per pixel: 8 (close + far kernels) or 20 (fused kernel, gipuma.cu:1122-1351)
     unsigned char site[24];     // fused kernel: rounding variant (eval_plane's rt) of each inlined call site: 0..19 candidates, 20 refinement
     int cost_rt;                // k_cost_eval: full runtime variant (used when it has bits beyond cost_variant / grad_variant)
     int grad_variant;           // colour only: which of l1(gradX)/3, l1(gradY)/3 ptxas folded into the FMA (1 at initialisation)
     int rng_mode;
-    int prepass;                // 1: k_sweep lists the pixels that have work in a thread-per-pixel pre-pass (gpm_kernels.cuh)
     int quadperm;               // 1: lanes of a sampling round are permuted so that every hardware quad (lanes 4q..4q+3) samples a 2x2 block
     unsigned char perm[GPM_MAX_ROUNDS][32];   // sample (relative to the round's first) evaluated by each lane; identity without quadperm
     RefCam ref;
@@ -250,11 +246,6 @@ __device__ __forceinline__ void local_topn(const KParams& P, float c0, float c1,
 
 struct WarpStats { unsigned hyp, skip, pruned; unsigned long long pairs, pairs_full; };
 
-// diagnostics of the packed sampling mode (option "packed" = 3): fetches where the one-fetch gradient differs from the
-// reference's four fetches although the lane passed the exactness conditions — count and the first 64 cases
-__device__ unsigned g_packed_mismatch_n;
-__device__ float g_packed_mismatch[64 * 8];
-
 // ---- cost of one plane hypothesis at the warp's pixel ---------------------------------------
 // pmCostMultiview_cu (gipuma.cu:720-806) over pmCost_shared (:585-680) / pmCostComputation_shared (:223-277).
 // Returns the exact combined cost, or — if `bound` is finite and an exact lower bound of the final cost
@@ -264,9 +255,9 @@ __device__ float g_packed_mismatch[64 * 8];
 //   true : H2 + fma(H1, y, H0*x)   — the spatialPropClose/Far kernels, where nvcc hoisted the x products out of
 //          the inner (y) loop of gipuma.cu:633-634.  (Both are contractions of the same source line, gipuma.cu:213.)
 // XF = 2 takes the variant from `rt` at run time (the fused 20-neighbour kernels, whose inlined call sites differ).
-template <int XF, bool PACKED, bool COLOR>
+template <int XF, bool COLOR>
 __device__ __forceinline__ float eval_plane(const KParams& P, const float* __restrict__ sCam, const WarpScratch& ws,
-                                            cudaTextureObject_t src, cudaTextureObject_t grad, float nx, float ny, float nz, float d,
+                                            cudaTextureObject_t src, float nx, float ny, float nz, float d,
                                             float bound, unsigned lane, WarpStats& st,
                                             float* per_view0 = nullptr, float* per_view1 = nullptr, unsigned rt = 0u)
 {
@@ -323,15 +314,6 @@ __device__ __forceinline__ float eval_plane(const KParams& P, const float* __res
     // getCorrespondingPoint_cu (gipuma.cu:207-217): H (x, y, 1)^T, then / z — the division's multiply is fused with
     // the +-1 / +0.5 texel offsets in the reference binary (FFMA X, rcp(Z), {0.5, 1, -1}); then the source-view taps
     // of gipuma.cu:251-253: gx2 = tex(x+1,y) - tex(x-1,y), gy2 = tex(x,y+1) - tex(x,y-1), centre.
-    //
-    // Packed mode (P.packed, all source images 8-bit valued): bilinear filtering is linear, and for integer texels
-    // |t| <= 255 with the unit's 8-bit weights every product and sum is exactly representable in fp32, so
-    //     tex_I(x+1,y) - tex_I(x-1,y)  ==  tex_G(x,y).x   with  G.x[i,j] = I[clamp(i+1),j] - I[clamp(i-1),j]
-    // bit for bit (tools/texbench.cu checks it) — PROVIDED the three taps use
-    // the same fractional weights, i.e. the reference's rounded coordinates satisfy (x+1+0.5) - (x+0.5) == 1 exactly
-    // (tested exactly, see below), and the footprint's texel indices are inside the image
-    // (G is built from clamped *source* indices; a clamped *texel* index would differ).  Lanes that fail either test
-    // take the reference's five fetches.  Two fetches (4 + 8 bytes per texel) replace five (5 x 4 bytes).
     auto fetch_sample = [&](const float4& h0, const float4& h1, const float4& h2, float ax, float ay, int v,
                             float& gx2, float& gy2, float& t_c) {
         const float X = XFIRST ? fadd(h0.z, ffma(h0.y, ay, fmul(h0.x, ax))) : fadd(h0.z, ffma(h0.x, ax, fmul(h0.y, ay)));
@@ -342,31 +324,12 @@ __device__ __forceinline__ float eval_plane(const KParams& P, const float* __res
         const float cxp = fadd(ffma(X, r, 1.0f), 0.5f), cxm = fadd(ffma(X, r, -1.0f), 0.5f);
         const float cyp = fadd(ffma(Y, r, 1.0f), 0.5f), cym = fadd(ffma(Y, r, -1.0f), 0.5f);
         t_c = tex2DLayered<float>(src, cx, cy, v);
-        bool five = true;
-        if (PACKED) {
-            const float2 g = tex2DLayered<float2>(grad, cx, cy, v);
-            gx2 = g.x;  gy2 = g.y;
-            // The taps must be EXACTLY one texel apart.  `cxp - cx == 1.0f` is not that test: for cx in [0.5, 2) the operands sit
-            // in different binades and the rounded difference can be 1.0 although cxm is one ulp below cx - 1 — next to a
-            // weight tie ((k + 1/2) / 256) the unit then filters the taps with weights one quantum apart (root cause of the
-            // differing fetches tools/packed_probe.py found).  t - 1.0f is exact for every t >= 0.5
-            // (Sterbenz / common ulp), so comparing it with the neighbouring tap is.
-            five = !((fsub(cxp, 1.0f) == cx) & (fsub(cx, 1.0f) == cxm) & (fsub(cyp, 1.0f) == cy) & (fsub(cy, 1.0f) == cym) &
-                     (cx >= 0.5f) & (cx < (float)P.W - 0.5f) & (cy >= 0.5f) & (cy < (float)P.H - 0.5f));
-        }
-        if (five || (PACKED && P.packed == 3)) {
-            const float t_xp = tex2DLayered<float>(src, cxp, cy, v);
-            const float t_xm = tex2DLayered<float>(src, cxm, cy, v);
-            const float t_yp = tex2DLayered<float>(src, cx, cyp, v);
-            const float t_ym = tex2DLayered<float>(src, cx, cym, v);
-            const float fx = fsub(t_xp, t_xm), fy = fsub(t_yp, t_ym);
-            if (PACKED && !five && (__float_as_uint(fx) != __float_as_uint(gx2) || __float_as_uint(fy) != __float_as_uint(gy2))) {
-                const unsigned k = atomicAdd(&g_packed_mismatch_n, 1u);
-                if (k < 64u) { float* e = g_packed_mismatch + k * 8;  e[0] = cx;  e[1] = cy;  e[2] = (float)v;  e[3] = gx2;  e[4] = fx;  e[5] = gy2;  e[6] = fy;  e[7] = t_c; }
-            }
-            gx2 = fx;
-            gy2 = fy;
-        }
+        const float t_xp = tex2DLayered<float>(src, cxp, cy, v);
+        const float t_xm = tex2DLayered<float>(src, cxm, cy, v);
+        const float t_yp = tex2DLayered<float>(src, cx, cyp, v);
+        const float t_ym = tex2DLayered<float>(src, cx, cym, v);
+        gx2 = fsub(t_xp, t_xm);
+        gy2 = fsub(t_yp, t_ym);
     };
 
     // ---- colour (T = float4) variants: pmCostComputation_shared<float4>, l1_norm(float4) = (|x|+|y|+|z|) * 0.3333333f

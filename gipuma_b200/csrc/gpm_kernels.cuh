@@ -12,11 +12,6 @@ __device__ __forceinline__ unsigned long long* block_mbar(const KParams& P, floa
 {
     return reinterpret_cast<unsigned long long*>(smem_base + fixed_smem_floats(P) + (size_t)P.nwarps * warp_scratch_floats(P.ns_pad, P.V, P.color) + 2);
 }
-// list of the tile's pixels that have work to do (k_sweep's pre-pass): 512 x uint16 behind the lane table
-__device__ __forceinline__ unsigned short* block_active(const KParams& P, float* smem_base)
-{
-    return reinterpret_cast<unsigned short*>(smem_base + fixed_smem_floats(P) + (size_t)P.nwarps * warp_scratch_floats(P.ns_pad, P.V, P.color) + 4 + GPM_MAX_ROUNDS * 8);
-}
 __device__ __forceinline__ unsigned char* block_perm(const KParams& P, float* smem_base)
 {
     return reinterpret_cast<unsigned char*>(smem_base + fixed_smem_floats(P) + (size_t)P.nwarps * warp_scratch_floats(P.ns_pad, P.V, P.color) + 4);
@@ -50,35 +45,17 @@ __device__ __forceinline__ void mbar_wait(unsigned long long* bar, unsigned pari
 
 // Stage the (32+2*halo)^2 reference window of tile (bx, by) and the per-view camera table in shared memory.
 // Unlike the reference's loader (gipuma.cu:1510-1525, skipped by threads that left early — SURVEY.md §7),
-// the whole window is always defined.  With P.use_tma one elected thread issues a single 2-D TMA box copy
-// (cp.async.bulk.tensor) from the replicate-padded reference image and the block waits on its mbarrier while the other
-// threads copy the camera and lane tables; otherwise the window is a cooperative copy.  `phase` = parity of the barrier's
-// current phase (0 for the first / only tile of a block).
-__device__ __forceinline__ void stage_block(const KParams& P, const CUtensorMap* tmap, const float* __restrict__ refpad,
-                                            const ViewCam* __restrict__ cams, float* tile, float* sCam,
-                                            int tile_x0, int tile_y0, unsigned phase = 0u)
+// the whole window is always defined.  One elected thread issues a single 2-D TMA box copy (cp.async.bulk.tensor) from
+// the replicate-padded reference image and the block waits on its mbarrier while the other threads copy the camera and
+// lane tables.  `phase` = parity of the barrier's current phase (0 for the first / only tile of a block).
+__device__ __forceinline__ void stage_block(const KParams& P, const CUtensorMap* tmap, const ViewCam* __restrict__ cams,
+                                            float* tile, float* sCam, int tile_x0, int tile_y0, unsigned phase = 0u)
 {
-    const int tw = P.tile_w, ts = P.tile_stride;
     unsigned long long* bar = block_mbar(P, tile);
-    if (P.use_tma) {
-        if (threadIdx.x == 0) {
-            if (phase == 0u) mbar_init(bar, 1);
-            mbar_arrive_expect_tx(bar, (unsigned)(tile_floats(P) * sizeof(float)));
-            tma_load_2d(tile, tmap, (tile_x0 + GPM_APRON - P.tile_xo) * (P.color ? 4 : 1), tile_y0 + GPM_APRON, bar);
-        }
-    } else if (P.color) {                           // float4 texels: refpitch counts float4 elements
-        const float4* src4 = reinterpret_cast<const float4*>(refpad) + (size_t)(tile_y0 + GPM_APRON) * P.refpitch + (tile_x0 + GPM_APRON);
-        float4* tile4 = reinterpret_cast<float4*>(tile);
-        for (int e = threadIdx.x; e < tw * tw; e += blockDim.x) {
-            const int J = e / tw, I = e - J * tw;
-            tile4[J * ts + I] = src4[(size_t)J * P.refpitch + I];
-        }
-    } else {
-        const float* src = refpad + (size_t)(tile_y0 + GPM_APRON) * P.refpitch + (tile_x0 + GPM_APRON);
-        for (int e = threadIdx.x; e < tw * tw; e += blockDim.x) {
-            const int J = e / tw, I = e - J * tw;
-            tile[J * ts + P.tile_xo + I] = src[(size_t)J * P.refpitch + I];
-        }
+    if (threadIdx.x == 0) {
+        if (phase == 0u) mbar_init(bar, 1);
+        mbar_arrive_expect_tx(bar, (unsigned)(tile_floats(P) * sizeof(float)));
+        tma_load_2d(tile, tmap, (tile_x0 + GPM_APRON - P.tile_xo) * (P.color ? 4 : 1), tile_y0 + GPM_APRON, bar);
     }
     const float* c = reinterpret_cast<const float*>(cams);
     for (int e = threadIdx.x; e < P.V * GPM_VIEWCAM_FLOATS; e += blockDim.x) sCam[e] = c[e];
@@ -87,7 +64,7 @@ __device__ __forceinline__ void stage_block(const KParams& P, const CUtensorMap*
     const unsigned* gp = reinterpret_cast<const unsigned*>(&P.perm[0][0]);
     for (int e = threadIdx.x; e < GPM_MAX_ROUNDS * 8; e += blockDim.x) sp[e] = gp[e];
     __syncthreads();                                // tables visible; mbarrier initialised before anyone waits on it
-    if (P.use_tma) mbar_wait(bar, phase & 1u);
+    mbar_wait(bar, phase & 1u);
 }
 
 __device__ __forceinline__ void flush_stats(unsigned long long* stats, const WarpStats& st, unsigned lane)
@@ -101,10 +78,10 @@ __device__ __forceinline__ void flush_stats(unsigned long long* stats, const War
     }
 }
 
-// shared memory: [tile tile_stride*tile_w][cams V*21][pad to 16 B][nwarps * warp_scratch][4 ints: work counter, active count, mbarrier (8 B)][lane permutation table, GPM_MAX_ROUNDS x 32 bytes][active pixel list, 512 x uint16]
+// shared memory: [tile tile_stride*tile_w][cams V*21][pad to 16 B][nwarps * warp_scratch][4 ints: work counter, unused, mbarrier (8 B)][lane permutation table, GPM_MAX_ROUNDS x 32 bytes]
 __host__ __device__ inline size_t block_smem_bytes(const KParams& P)
 {
-    size_t fl = (size_t)fixed_smem_floats(P) + (size_t)P.nwarps * warp_scratch_floats(P.ns_pad, P.V, P.color) + 4 + GPM_MAX_ROUNDS * 8 + GPM_TILE * GPM_TILE / 4;
+    size_t fl = (size_t)fixed_smem_floats(P) + (size_t)P.nwarps * warp_scratch_floats(P.ns_pad, P.V, P.color) + 4 + GPM_MAX_ROUNDS * 8;
     return fl * sizeof(float);
 }
 
@@ -170,11 +147,10 @@ __global__ void k_init_planes(const __grid_constant__ KParams P, unsigned long l
 #define GPM_LB_THREADS 512       // max threads per block of the warp-per-pixel kernels (16 warps)
 #define GPM_LB_BLOCKS 1
 #endif
-template <bool PACKED, bool COLOR>
+template <bool COLOR>
 __global__ void __launch_bounds__(GPM_LB_THREADS, GPM_LB_BLOCKS)
-k_cost_eval(const __grid_constant__ KParams P, const __grid_constant__ CUtensorMap tmap, const ViewCam* __restrict__ cams, const float* __restrict__ refpad,
-            cudaTextureObject_t src, cudaTextureObject_t grad, const float4* __restrict__ planes, float* __restrict__ cost,
-            unsigned long long* __restrict__ stats)
+k_cost_eval(const __grid_constant__ KParams P, const __grid_constant__ CUtensorMap tmap, const ViewCam* __restrict__ cams,
+            cudaTextureObject_t src, const float4* __restrict__ planes, float* __restrict__ cost, unsigned long long* __restrict__ stats)
 {
     extern __shared__ __align__(128) float smem[];
     float* tile = smem;
@@ -182,7 +158,7 @@ k_cost_eval(const __grid_constant__ KParams P, const __grid_constant__ CUtensorM
     float* scratch = smem + fixed_smem_floats(P);
     const unsigned lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const int tile_x0 = blockIdx.x * GPM_TILE - P.halo, tile_y0 = blockIdx.y * GPM_TILE - P.halo;
-    stage_block(P, &tmap, refpad, cams, tile, sCam, tile_x0, tile_y0);
+    stage_block(P, &tmap, cams, tile, sCam, tile_x0, tile_y0);
     const WarpScratch ws = carve(scratch + (size_t)warp * warp_scratch_floats(P.ns_pad, P.V, P.color), P.ns_pad, P.V, P.color, block_perm(P, smem));
     WarpStats st = {0, 0, 0, 0, 0};
     for (int idx = warp; idx < GPM_TILE * GPM_TILE; idx += P.nwarps) {
@@ -191,9 +167,9 @@ k_cost_eval(const __grid_constant__ KParams P, const __grid_constant__ CUtensorM
         setup_window<COLOR>(P, tile + P.tile_xo, ws, px, py, tile_x0, tile_y0, lane);
         const float4 n = planes[(size_t)py * P.W + px];
         const float inf = __int_as_float(0x7f800000);
-        const float c = (P.cost_rt & 12) ? eval_plane<2, PACKED, COLOR>(P, sCam, ws, src, grad, n.x, n.y, n.z, n.w, inf, lane, st, nullptr, nullptr, (unsigned)P.cost_rt)
-                        : P.cost_variant ? eval_plane<1, PACKED, COLOR>(P, sCam, ws, src, grad, n.x, n.y, n.z, n.w, inf, lane, st)
-                                         : eval_plane<0, PACKED, COLOR>(P, sCam, ws, src, grad, n.x, n.y, n.z, n.w, inf, lane, st);
+        const float c = (P.cost_rt & 12) ? eval_plane<2, COLOR>(P, sCam, ws, src, n.x, n.y, n.z, n.w, inf, lane, st, nullptr, nullptr, (unsigned)P.cost_rt)
+                        : P.cost_variant ? eval_plane<1, COLOR>(P, sCam, ws, src, n.x, n.y, n.z, n.w, inf, lane, st)
+                                         : eval_plane<0, COLOR>(P, sCam, ws, src, n.x, n.y, n.z, n.w, inf, lane, st);
         if (lane == 0) cost[(size_t)py * P.W + px] = c;
     }
     flush_stats(stats, st, lane);
@@ -212,10 +188,10 @@ __device__ const signed char kFusedGx1[20] = { 0,  0,  0, 0, 0, 0,  0,  0,  0, 1
 __device__ const signed char kFusedGy0[20] = { 1,  3,  5, 0, 0, 0,  0,  0,  0, 0, 0, 0,  1, 0,  1,  0,  3,  3,  0, 0};
 __device__ const signed char kFusedGy1[20] = { 0,  0,  0, 1, 3, 5,  0,  0,  0, 0, 0, 0,  0, 1,  0,  1,  0,  0,  2, 2};
 
-template <bool PACKED, bool COLOR, bool FUSED>
+template <bool COLOR, bool FUSED>
 __global__ void __launch_bounds__(GPM_LB_THREADS, GPM_LB_BLOCKS)
-k_sweep(const __grid_constant__ KParams P, const __grid_constant__ CUtensorMap tmap, const ViewCam* __restrict__ cams, const float* __restrict__ refpad,
-        cudaTextureObject_t src, cudaTextureObject_t grad, float4* __restrict__ planes, float* __restrict__ cost,
+k_sweep(const __grid_constant__ KParams P, const __grid_constant__ CUtensorMap tmap, const ViewCam* __restrict__ cams,
+        cudaTextureObject_t src, float4* __restrict__ planes, float* __restrict__ cost,
         unsigned* __restrict__ rng_state, unsigned char* __restrict__ prov, Memo M, int colour, int phase_mask,
         unsigned long long* __restrict__ stats)
 {
@@ -226,8 +202,8 @@ k_sweep(const __grid_constant__ KParams P, const __grid_constant__ CUtensorMap t
     int* counter = reinterpret_cast<int*>(scratch + (size_t)P.nwarps * warp_scratch_floats(P.ns_pad, P.V, P.color));
     const unsigned lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const int tile_x0 = blockIdx.x * GPM_TILE - P.halo, tile_y0 = blockIdx.y * GPM_TILE - P.halo;
-    if (threadIdx.x == 0) { counter[0] = P.nwarps;  counter[1] = 0; }
-    stage_block(P, &tmap, refpad, cams, tile, sCam, tile_x0, tile_y0);
+    if (threadIdx.x == 0) counter[0] = P.nwarps;
+    stage_block(P, &tmap, cams, tile, sCam, tile_x0, tile_y0);
     const WarpScratch ws = carve(scratch + (size_t)warp * warp_scratch_floats(P.ns_pad, P.V, P.color), P.ns_pad, P.V, P.color, block_perm(P, smem));
     const RefCam& cam = P.ref;
     WarpStats st = {0, 0, 0, 0, 0};
@@ -239,61 +215,8 @@ k_sweep(const __grid_constant__ KParams P, const __grid_constant__ CUtensorMap t
     const int per_slice = (GPM_TILE * GPM_TILE / 2 + (int)gridDim.z - 1) / (int)gridDim.z;
     const int idx_begin = (int)blockIdx.z * per_slice;
     const int idx_end = min(GPM_TILE * GPM_TILE / 2, idx_begin + per_slice);
-
-    // Pre-pass, one THREAD per pixel: which pixels have anything to do?  A pixel whose every candidate is a memo hit (the
-    // neighbour still carries the identity it was offered before) and whose refinement is known to reject every step needs no
-    // warp at all — the warp path would read its state, skip everything and write the same state back.  In the late
-    // iterations that is most pixels; the warps then only walk the compact list of the others.  (Other exact shortcuts —
-    // history, duplicates, depth range — still run in the warp path: a pixel they would clear is merely listed.)
-    unsigned short* act = block_active(P, smem);
-    if (P.prepass) {
-        unsigned nskip = 0;
-        for (int i = idx_begin + (int)threadIdx.x; i < idx_end; i += (int)blockDim.x) {
-            const int tx = i & 31, ty = i >> 5;
-            const int px = blockIdx.x * GPM_TILE + tx;
-            const int py = blockIdx.y * GPM_TILE + 2 * ty + (((tx & 1) ^ colour) & 1);
-            if (px >= W || py >= H) continue;
-            bool idle = false;
-            unsigned ncand = 0;
-            if (P.memo) {
-                const size_t center = (size_t)py * W + px;
-                const unsigned mmask = M.mask[center];
-                bool all_hit = true;
-                for (int k = 0; k < NC; k++) {
-                    bool ok;
-                    size_t at;
-                    if (FUSED) {
-                        ok = (phase_mask & 1) && px >= kFusedGx0[k] && px <= W - 1 - kFusedGx1[k] && py >= kFusedGy0[k] && py <= H - 1 - kFusedGy1[k];
-                        at = (size_t)(py + kFusedDy[k]) * W + (px + kFusedDx[k]);
-                    } else {
-                        const int dist = k < 4 ? 1 : 5, dir = k & 3;
-                        int qx = px, qy = py;
-                        if (dir == 0)      { ok = py > dist - 1;  qy = py - dist; }
-                        else if (dir == 1) { ok = py < H - dist;  qy = py + dist; }
-                        else if (dir == 2) { ok = px > dist - 1;  qx = px - dist; }
-                        else               { ok = px < W - dist;  qx = px + dist; }
-                        ok = ok && ((phase_mask >> (k >> 2)) & 1);
-                        at = (size_t)qy * W + qx;
-                    }
-                    if (!ok) continue;
-                    ncand++;
-                    if (!((mmask >> k) & 1) || M.seen[center * NC + k] != M.pid[at]) { all_hit = false;  break; }
-                }
-                const bool refine = (phase_mask & 4) != 0;
-                const bool refine_idle = !refine || (P.rng_mode == 0 && (mmask & GPM_MEMO_REFINE) && M.refseen[center] == M.pid[center]);
-                idle = all_hit && refine_idle;
-                if (idle) nskip += ncand + (refine ? 3u : 0u);
-            }
-            if (!idle) act[atomicAdd(&counter[1], 1)] = (unsigned short)i;
-        }
-        nskip = __reduce_add_sync(GPM_FULL, nskip);
-        st.skip += nskip;                       // every lane holds the warp's sum; flush_stats takes lane 0's
-    }
-    __syncthreads();
-    const int nactive = P.prepass ? counter[1] : idx_end - idx_begin;      // without the pre-pass: every pixel of the slice, in order
-    int pos = (int)warp;
-    while (pos < nactive) {
-        const int idx = P.prepass ? (int)act[pos] : idx_begin + pos;
+    int idx = idx_begin + (int)warp;
+    while (idx < idx_end) {
         // pixel of this colour — gipuma.cu:1730-1734 / 1786-1790
         const int tx = idx & 31, ty = idx >> 5;
         const int px = blockIdx.x * GPM_TILE + tx;
@@ -370,8 +293,8 @@ k_sweep(const __grid_constant__ KParams P, const __grid_constant__ CUtensorMap t
                 const bool dup = __any_sync(GPM_FULL, same_mine);
                 if (!in_range || same_now || dup) { st.skip++; continue; }
                 if (!window_ready) { setup_window<COLOR>(P, tile + P.tile_xo, ws, px, py, tile_x0, tile_y0, lane);  window_ready = true; }
-                const float c = FUSED ? eval_plane<2, PACKED, COLOR>(P, sCam, ws, src, grad, nb.x, nb.y, nb.z, nb.w, cost_now, lane, st, nullptr, nullptr, site)
-                                      : eval_plane<(COLOR ? 0 : 1), PACKED, COLOR>(P, sCam, ws, src, grad, nb.x, nb.y, nb.z, nb.w, cost_now, lane, st);
+                const float c = FUSED ? eval_plane<2, COLOR>(P, sCam, ws, src, nb.x, nb.y, nb.z, nb.w, cost_now, lane, st, nullptr, nullptr, site)
+                                      : eval_plane<(COLOR ? 0 : 1), COLOR>(P, sCam, ws, src, nb.x, nb.y, nb.z, nb.w, cost_now, lane, st);
                 if (c < cost_now) {                                                              // :867-871
                     disp_now = disp_before;
                     norm_now = nb;
@@ -427,8 +350,8 @@ k_sweep(const __grid_constant__ KParams P, const __grid_constant__ CUtensorMap t
                     if (dot3(cand.x, cand.y, cand.z, vx, vy, vz) > 0.0f) { cand.x = -cand.x;  cand.y = -cand.y;  cand.z = -cand.z; }
                     cand.w = plane_d(cam, cand.x, cand.y, cand.z, fpx, fpy, depth_new);   // :969
                     const unsigned rsite = FUSED ? (unsigned)P.site[20] : 0u;
-                    const float c = FUSED ? eval_plane<2, PACKED, COLOR>(P, sCam, ws, src, grad, cand.x, cand.y, cand.z, cand.w, cost_now, lane, st, nullptr, nullptr, rsite)
-                                          : eval_plane<0, PACKED, COLOR>(P, sCam, ws, src, grad, cand.x, cand.y, cand.z, cand.w, cost_now, lane, st);
+                    const float c = FUSED ? eval_plane<2, COLOR>(P, sCam, ws, src, cand.x, cand.y, cand.z, cand.w, cost_now, lane, st, nullptr, nullptr, rsite)
+                                          : eval_plane<0, COLOR>(P, sCam, ws, src, cand.x, cand.y, cand.z, cand.w, cost_now, lane, st);
                     if (c < cost_now) {                                                          // :986-990 (no depth-range test)
                         prov_now = (int)rsite;
                         any_accept = true;
@@ -460,8 +383,8 @@ k_sweep(const __grid_constant__ KParams P, const __grid_constant__ CUtensorMap t
                 M.pid[center] = own_id;
             }
         }
-        if (lane == 0) pos = atomicAdd(&counter[0], 1);
-        pos = __shfl_sync(GPM_FULL, pos, 0);
+        if (lane == 0) idx = idx_begin + atomicAdd(&counter[0], 1);
+        idx = __shfl_sync(GPM_FULL, idx, 0);
     }
     flush_stats(stats, st, lane);
 }
@@ -607,10 +530,9 @@ __device__ __forceinline__ void shard_accept_pixel(const KParams& P, const float
 }
 
 // One stage of one pixel: [accept of stage-1's exchange] + evaluation of `stage` on this rank's views -> local top-n lists.
-template <bool PACKED, bool COLOR>
+template <bool COLOR>
 __device__ __forceinline__ void shard_stage_pixel(const KParams& P, const float* __restrict__ sCam, const float* __restrict__ tile,
-                                                  const WarpScratch& ws, cudaTextureObject_t src, cudaTextureObject_t grad,
-                                                  float4* __restrict__ planes, float* __restrict__ cost, unsigned char* __restrict__ prov,
+                                                  const WarpScratch& ws, cudaTextureObject_t src, float4* __restrict__ planes, float* __restrict__ cost, unsigned char* __restrict__ prov,
                                                   const ShardState& S, const Memo& M, int px, int py, int tile_x0, int tile_y0,
                                                   int stage, int last_stage, const float* __restrict__ gathered_prev, int world,
                                                   float* __restrict__ xchg, unsigned lane, WarpStats& st,
@@ -638,7 +560,7 @@ __device__ __forceinline__ void shard_stage_pixel(const KParams& P, const float*
     if (stage == 0) {                                       // initial costs (gipuma.cu:1040-1049), both colours: two half-resolution planes
         float* out = xchg + ((size_t)((px + py) & 1) * H * Wh + (size_t)py * Wh + (px >> 1)) * nb;
         setup_window<COLOR>(P, tile + P.tile_xo, ws, px, py, tile_x0, tile_y0, lane);
-        eval_plane<(COLOR ? 1 : 0), PACKED, COLOR>(P, sCam, ws, src, grad, norm_now.x, norm_now.y, norm_now.z, norm_now.w, inf, lane, st, &c0, &c1);
+        eval_plane<(COLOR ? 1 : 0), COLOR>(P, sCam, ws, src, norm_now.x, norm_now.y, norm_now.z, norm_now.w, inf, lane, st, &c0, &c1);
         local_topn(P, c0, c1, lane, out);
         publish(out, nb);
         return;
@@ -710,7 +632,7 @@ __device__ __forceinline__ void shard_stage_pixel(const KParams& P, const float*
             }
             if (skip) { st.skip++;  if ((int)lane < nb) out[k * nb + lane] = inf;  __syncwarp();  continue; }
             if (!window_ready) { setup_window<COLOR>(P, tile + P.tile_xo, ws, px, py, tile_x0, tile_y0, lane);  window_ready = true; }
-            eval_plane<(COLOR ? 0 : 1), PACKED, COLOR>(P, sCam, ws, src, grad, nbp.x, nbp.y, nbp.z, nbp.w, inf, lane, st, &c0, &c1);
+            eval_plane<(COLOR ? 0 : 1), COLOR>(P, sCam, ws, src, nbp.x, nbp.y, nbp.z, nbp.w, inf, lane, st, &c0, &c1);
             local_topn(P, c0, c1, lane, out + k * nb);
         }
         if (P.memo && mine_ok && !memo_hit) M.seen[center * 8 + lane] = mine_id;
@@ -725,7 +647,7 @@ __device__ __forceinline__ void shard_stage_pixel(const KParams& P, const float*
             const float4 cand = shard_refine_candidate(P, norm_now, disp_now, fpx, fpy, stage - 2, depth_new);
             if (lane == 0) { S.candbuf[center] = cand;  S.canddepth[center] = depth_new; }
             setup_window<COLOR>(P, tile + P.tile_xo, ws, px, py, tile_x0, tile_y0, lane);
-            eval_plane<0, PACKED, COLOR>(P, sCam, ws, src, grad, cand.x, cand.y, cand.z, cand.w, inf, lane, st, &c0, &c1);
+            eval_plane<0, COLOR>(P, sCam, ws, src, cand.x, cand.y, cand.z, cand.w, inf, lane, st, &c0, &c1);
             local_topn(P, c0, c1, lane, out);
         }
         publish(out, nb);
@@ -739,10 +661,10 @@ __device__ __forceinline__ void shard_stage_pixel(const KParams& P, const float*
 
 // One exchange stage over the whole image (NCCL flow: the all-gather runs between two launches of this kernel).
 // stage 0: both colours; 1 .. last_stage: one colour; last_stage + 1: closing accept of the colour.
-template <bool PACKED, bool COLOR>
+template <bool COLOR>
 __global__ void __launch_bounds__(GPM_LB_THREADS, GPM_LB_BLOCKS)
-k_shard_stage(const __grid_constant__ KParams P, const __grid_constant__ CUtensorMap tmap, const ViewCam* __restrict__ cams, const float* __restrict__ refpad,
-              cudaTextureObject_t src, cudaTextureObject_t grad, float4* __restrict__ planes, float* __restrict__ cost,
+k_shard_stage(const __grid_constant__ KParams P, const __grid_constant__ CUtensorMap tmap, const ViewCam* __restrict__ cams,
+              cudaTextureObject_t src, float4* __restrict__ planes, float* __restrict__ cost,
               unsigned char* __restrict__ prov, ShardState S, Memo M, int colour, int stage, int last_stage, const float* __restrict__ gathered_prev,
               int world, float* __restrict__ xchg, unsigned long long* __restrict__ stats)
 {
@@ -752,7 +674,7 @@ k_shard_stage(const __grid_constant__ KParams P, const __grid_constant__ CUtenso
     float* scratch = smem + fixed_smem_floats(P);
     const unsigned lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const int tile_x0 = blockIdx.x * GPM_TILE - P.halo, tile_y0 = blockIdx.y * GPM_TILE - P.halo;
-    if (stage <= last_stage) stage_block(P, &tmap, refpad, cams, tile, sCam, tile_x0, tile_y0);
+    if (stage <= last_stage) stage_block(P, &tmap, cams, tile, sCam, tile_x0, tile_y0);
     const WarpScratch ws = carve(scratch + (size_t)warp * warp_scratch_floats(P.ns_pad, P.V, P.color), P.ns_pad, P.V, P.color, block_perm(P, smem));
     WarpStats st = {0, 0, 0, 0, 0};
     // stage 0 visits every pixel (both colours, like gipuma_init_cu2); the others one colour
@@ -765,8 +687,8 @@ k_shard_stage(const __grid_constant__ KParams P, const __grid_constant__ CUtenso
         if (stage == 0) { px = blockIdx.x * GPM_TILE + (idx & 31);  py = blockIdx.y * GPM_TILE + (idx >> 5); }
         else { const int tx = idx & 31, ty = idx >> 5;  px = blockIdx.x * GPM_TILE + tx;  py = blockIdx.y * GPM_TILE + 2 * ty + (((tx & 1) ^ colour) & 1); }
         if (px >= P.W || py >= P.H) continue;
-        shard_stage_pixel<PACKED, COLOR>(P, sCam, tile, ws, src, grad, planes, cost, prov, S, M, px, py,
-                                         tile_x0, tile_y0, stage, last_stage, gathered_prev, world, xchg, lane, st);
+        shard_stage_pixel<COLOR>(P, sCam, tile, ws, src, planes, cost, prov, S, M, px, py,
+                                 tile_x0, tile_y0, stage, last_stage, gathered_prev, world, xchg, lane, st);
     }
     flush_stats(stats, st, lane);
 }
@@ -817,11 +739,10 @@ __device__ __forceinline__ void p2p_signal(const ShardP2P& X, unsigned bid, unsi
 // raised; before the next stage the block waits for the same block of every peer — never for another block of its own GPU,
 // so blocks need not be co-resident and the transfer of one tile overlaps the sampling of all the others.  The reference
 // window is staged once per colour instead of once per stage.  `seq0` = number of exchanges completed before this launch.
-template <bool PACKED, bool COLOR>
+template <bool COLOR>
 __global__ void __launch_bounds__(GPM_LB_THREADS, GPM_LB_BLOCKS)
 k_shard_fused(const __grid_constant__ KParams P, const __grid_constant__ CUtensorMap tmap, const ViewCam* __restrict__ cams,
-              const float* __restrict__ refpad, cudaTextureObject_t src, cudaTextureObject_t grad, float4* __restrict__ planes,
-              float* __restrict__ cost, unsigned char* __restrict__ prov, ShardState S, Memo M, int colour, int init_phase, int last_stage,
+              cudaTextureObject_t src, float4* __restrict__ planes, float* __restrict__ cost, unsigned char* __restrict__ prov, ShardState S, Memo M, int colour, int init_phase, int last_stage,
               const __grid_constant__ ShardP2P X, unsigned seq0, unsigned long long* __restrict__ stats)
 {
     extern __shared__ __align__(128) float smem[];
@@ -831,7 +752,7 @@ k_shard_fused(const __grid_constant__ KParams P, const __grid_constant__ CUtenso
     const unsigned lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const int tile_x0 = blockIdx.x * GPM_TILE - P.halo, tile_y0 = blockIdx.y * GPM_TILE - P.halo;
     const unsigned bid = (blockIdx.z * gridDim.y + blockIdx.y) * gridDim.x + blockIdx.x;
-    stage_block(P, &tmap, refpad, cams, tile, sCam, tile_x0, tile_y0);
+    stage_block(P, &tmap, cams, tile, sCam, tile_x0, tile_y0);
     const WarpScratch ws = carve(scratch + (size_t)warp * warp_scratch_floats(P.ns_pad, P.V, P.color), P.ns_pad, P.V, P.color, block_perm(P, smem));
     WarpStats st = {0, 0, 0, 0, 0};
     const int W = P.W, H = P.H, Wh = (W + 1) >> 1, nb = P.n_best;
@@ -860,8 +781,8 @@ k_shard_fused(const __grid_constant__ KParams P, const __grid_constant__ CUtenso
                 }
                 continue;
             }
-            shard_stage_pixel<PACKED, COLOR>(P, sCam, tile, ws, src, grad, planes, cost, prov, S, M, px, py,
-                                             tile_x0, tile_y0, stage, lastS, prev, X.world, outb, lane, st, slot, &X, slot_off);
+            shard_stage_pixel<COLOR>(P, sCam, tile, ws, src, planes, cost, prov, S, M, px, py,
+                                     tile_x0, tile_y0, stage, lastS, prev, X.world, outb, lane, st, slot, &X, slot_off);
         }
         if (!closing) p2p_signal(X, bid, seq);
     }
@@ -935,21 +856,6 @@ __global__ void k_split_channels(const float4* __restrict__ in, size_t pitch_ele
     const float4 p = in[(size_t)y * pitch_elems + x];
     const size_t plane = (size_t)W * H, o = (size_t)y * W + x;
     out[o] = p.x;  out[plane + o] = p.y;  out[2 * plane + o] = p.z;
-}
-
-// G[x,y] = (I[clamp(x+1),y] - I[clamp(x-1),y],  I[x,clamp(y+1)] - I[x,clamp(y-1)]) for the packed sampling mode, and a flag
-// that stays 1 only if every pixel is an integer in [0, 255] (the exactness condition of that mode).
-__global__ void k_make_gradients(const float* __restrict__ img, size_t pitch_floats, int W, int H, float2* __restrict__ out,
-                                 int* __restrict__ all_8bit)
-{
-    const int x = blockIdx.x * blockDim.x + threadIdx.x, y = blockIdx.y * blockDim.y + threadIdx.y;
-    if (x >= W || y >= H) return;
-    const float* row = img + (size_t)y * pitch_floats;
-    const float v = row[x];
-    const float gx = fsub(row[min(x + 1, W - 1)], row[max(x - 1, 0)]);
-    const float gy = fsub(img[(size_t)min(y + 1, H - 1) * pitch_floats + x], img[(size_t)max(y - 1, 0) * pitch_floats + x]);
-    out[(size_t)y * W + x] = make_float2(gx, gy);
-    if (!(v >= 0.0f && v <= 255.0f && v == rintf(v))) *all_8bit = 0;
 }
 
 __global__ void k_pad_reference4(const float4* __restrict__ img, size_t pitch_elems, int W, int H, float4* __restrict__ out, int out_pitch, int out_rows)

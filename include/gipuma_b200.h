@@ -171,11 +171,6 @@ int gpm_reset_stats(gpm_ctx* ctx);
  * bench.py's roofline.binding_unit divides the achieved fetch rate by it. */
 int gpm_measure_fetch_peak(gpm_ctx* ctx, double* gfetch_per_s);
 
-/* Diagnostics of the experimental "packed" sampling mode (option value 3 = sample both ways and compare): number of fetches
- * whose one-fetch gradient differed from the reference's four fetches and up to 64 records of 8 floats
- * {x, y, view, gx packed, gx reference, gy packed, gy reference, centre}. */
-int gpm_debug_packed_mismatches(gpm_ctx* ctx, unsigned* count, float* records512, int reset);
-
 /* Tuning / diagnostics; results are bit-identical for every setting.
  * "prune" (1): exact lower-bound early-out; "dedupe" (1): skip bit-identical candidate planes;
  * "trust_state" (0): treat a state loaded with gpm_set_state as cost-consistent; "nwarps" (0 = auto): warps per block;
@@ -185,20 +180,13 @@ int gpm_debug_packed_mismatches(gpm_ctx* ctx, unsigned* count, float* records512
  * all six sweep kernels), bit 1 = float4 gradient folding (float4 initialisation = 3); auto = the propagation kernels' form;
  * "shard_async" (0): 1 makes gpm_shard_stage / gpm_shard_finish_init return after enqueueing on gpm_stream() — run the
  * collective on that stream (or order it with events) instead of paying a host synchronisation per stage;
- * "tma" (1): stage the reference window with one cp.async.bulk.tensor (TMA) per block instead of a cooperative copy;
- * "fused_warps" (16): warps per block of the fused shard kernel (8 = two resident blocks per SM: one samples while the other
- * waits for its peers' lists — measured no faster);
  * "exchange" (1): view shard over peer memory when regions are attached, 0 = NCCL all-gather per stage;
  * "async_upload" (0): 1 lets gpm_set_reference / gpm_set_view return without a host synchronisation — the caller keeps its
  * (page-locked) image buffers unchanged until the next gpm_run / gpm_sweep returns;
- * "prepass" (0; environment GPM_PREPASS=1 at gpm_create): a thread-per-pixel pre-pass of the sweep kernel lists the pixels
- * that still have work, so that converged pixels cost no warp;
  * "quadperm" (1): deal the samples of a round to the lanes as 2x2 blocks per hardware quad (texture-unit locality);
  * "neighbours" (8): 20 selects the reference's fused sweep — the kernels it launches when built without SMALLKERNEL
  * (gipuma.cu:1122-1351, 1913-1940): 12 axial + 8 knight-move neighbours, then refinement, one launch per colour; bit-exact
- * like the default (view sharding stays 8-neighbour only).
- * EXPERIMENTAL, not covered by the bit-exactness statement: "packed" (0 = off, 1 = auto, 2 = on) samples the source-view
- * gradients with one RG32F fetch instead of four R32F fetches for 8-bit images; measured 1 differing pixel in 1.92 M at cfg 2. */
+ * like the default (view sharding stays 8-neighbour only). */
 int gpm_set_option(gpm_ctx* ctx, const char* name, int value);
 
 /* The CUDA stream all work of this context is enqueued on (as a void*), for event timing by callers. */

@@ -36,7 +36,7 @@ def test_cfg2_full_size_invariants(cfg2):
     a, ms_a, st_a = api.runcuda(sc)
     b, ms_b, st_b = api.runcuda(sc)
     assert bits_equal(a.norm4, b.norm4) == 0 and bits_equal(a.c, b.c) == 0            # deterministic
-    c, ms_c, st_c = api.runcuda(sc, options={"prune": 0, "dedupe": 0, "memo": 0, "packed": 0})
+    c, ms_c, st_c = api.runcuda(sc, options={"prune": 0, "dedupe": 0, "memo": 0})
     assert bits_equal(a.norm4, c.norm4) == 0 and bits_equal(a.c, c.c) == 0            # pruning/dedupe are exact
     assert st_c["pairs"] == st_c["pairs_full"] and st_a["pairs"] < st_c["pairs"]
     depth = a.norm4[..., 3]
@@ -84,25 +84,6 @@ def test_error_handling():
         ctx.load_scene(S.make_config(1, rows=64, cols=96))
         ctx.set_num_views(1)                              # fewer views than uploaded is fine
         ctx.run()
-
-
-def test_packed_sampling_mode_is_exact_after_the_tap_alignment_fix():
-    """Experimental option "packed" (gradients from one RG32F fetch): value 3 samples both ways and counts the lanes that
-    passed the exactness conditions and still differ from the reference's four fetches — none may remain (the old test
-    `cxp - cx == 1.0f` let taps one ulp apart through next to weight ties).  Border-heavy scene:
-    many coordinates below 2, where that happened."""
-    from gipuma_b200 import api, scene as S
-    sc = S.make_config(2, rows=96, cols=128, n_views=6, iterations=3, seed=77)
-    sc.params.box_hsize = sc.params.box_vsize = 21
-    outs = {}
-    for mode in (0, 3, 2):
-        with api.Context(sc.cols, sc.rows, sc.n_views) as ctx:
-            ctx.set_option("packed", mode)
-            ctx.load_scene(sc)
-            ctx.packed_mismatches(reset=True)
-            ctx.run()
-            outs[mode] = ctx.get_state()
-            n, _ = ctx.packed_mismatches(reset=True)
-            assert n == 0
-    for mode in (3, 2):
-        assert bits_equal(outs[mode][0], outs[0][0]) == 0 and bits_equal(outs[mode][1], outs[0][1]) == 0
+        for name in ("packed", "prepass", "equal_rounds", "fused_warps", "tma"):
+            with pytest.raises(api.GipumaError):
+                ctx.set_option(name, 0)                   # retired options fail loudly instead of being ignored

@@ -6,10 +6,9 @@ sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), ".."
 from gipuma_b200 import scene as S, api
 cfg = int(sys.argv[1]) if len(sys.argv) > 1 else 2
 sc = S.make_config(cfg)
-base, _, _ = api.runcuda(sc, options={"prune": 0, "dedupe": 0, "memo": 0, "packed": 0})
-for name, opts in [("repeat", {"prune": 0, "dedupe": 0, "memo": 0, "packed": 0}), ("prune", {"dedupe": 0, "memo": 0, "packed": 0}),
-                   ("dedupe", {"prune": 0, "memo": 0, "packed": 0}), ("memo", {"prune": 0, "dedupe": 0, "packed": 0}),
-                   ("packed", {"prune": 0, "dedupe": 0, "memo": 0, "packed": 2}), ("all", {})]:
+base, _, _ = api.runcuda(sc, options={"prune": 0, "dedupe": 0, "memo": 0})
+for name, opts in [("repeat", {"prune": 0, "dedupe": 0, "memo": 0}), ("prune", {"dedupe": 0, "memo": 0}),
+                   ("dedupe", {"prune": 0, "memo": 0}), ("memo", {"prune": 0, "dedupe": 0}), ("all", {})]:
     o, ms, st = api.runcuda(sc, options=opts)
     neq = (o.norm4.view(np.uint32) != base.norm4.view(np.uint32)).any(axis=-1) | (o.c.view(np.uint32) != base.c.view(np.uint32))
     ys, xs = np.nonzero(neq)

@@ -112,7 +112,7 @@ def main():
             ctx.set_option("trust_state", 0)
         if "full" in args.levels:
             f_n4, f_c, printed_s, wall_ms = ref.run(sc)
-            for opts in ({}, {"prune": 0, "dedupe": 0, "memo": 0, "packed": 0}):
+            for opts in ({}, {"prune": 0, "dedupe": 0, "memo": 0}):
                 ls, ms, st = api.runcuda(sc, options=opts)
                 tag = "full%s" % ("" if not opts else " (no prune/dedupe)")
                 cmp(tag + " norm4", ls.norm4, f_n4, out)
