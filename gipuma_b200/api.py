@@ -52,6 +52,27 @@ class GpmBatchStats(C.Structure):
                 ("per_job_views", C.POINTER(C.c_int)), ("per_job_device", C.POINTER(C.c_int))]
 
 
+class GpmFuseCamera(C.Structure):
+    _fields_ = [("M_inv", C.c_float * 9), ("P", C.c_float * 12), ("f", C.c_float)]
+
+
+class GpmFuseDesc(C.Structure):
+    _fields_ = [("n_views", C.c_int), ("width", C.c_int), ("height", C.c_int), ("norm4", C.c_void_p), ("images", C.c_void_p),
+                ("channels", C.c_int), ("on_device", C.c_int), ("P", C.POINTER(C.c_double)), ("cam_scale", C.c_double),
+                ("depth_min", C.c_float), ("depth_max", C.c_float), ("disp_thresh", C.c_float), ("normal_thresh", C.c_float),
+                ("num_consistent", C.c_int), ("device", C.c_int)]
+
+
+class GpmFuseResult(C.Structure):
+    _fields_ = [("count", C.c_longlong), ("capacity", C.c_longlong), ("vertices", C.c_void_p), ("source", C.c_void_p),
+                ("used", C.c_void_p), ("fuse_ms", C.c_float), ("upload_ms", C.c_float)]
+
+
+# one vertex of the fused point cloud: the packed 27-byte record of storePlyFileBinary (displayUtils.h:84-142)
+PLY_VERTEX = np.dtype([("x", "<f4"), ("y", "<f4"), ("z", "<f4"), ("nx", "<f4"), ("ny", "<f4"), ("nz", "<f4"),
+                       ("red", "u1"), ("green", "u1"), ("blue", "u1")])
+
+
 class GipumaError(RuntimeError):
     pass
 
@@ -115,13 +136,17 @@ def load_library():
     L.gpm_shard_p2p_export.argtypes = [vp, C.c_int, vp, C.POINTER(vp)]
     L.gpm_shard_p2p_attach.argtypes = [vp, vp, C.POINTER(vp), C.c_int, C.c_int]
     L.gpm_stream.restype = vp
+    L.gpm_fuse_cameras.argtypes = [C.POINTER(C.c_double), C.c_int, C.c_double, C.POINTER(GpmFuseCamera)]
+    L.gpm_fuse.argtypes = [C.POINTER(GpmFuseDesc), C.POINTER(GpmFuseResult)]
+    L.gpm_write_ply.argtypes = [C.c_char_p, vp, C.c_longlong]
     for name in ("gpm_create", "gpm_set_params", "gpm_set_reference", "gpm_set_view", "gpm_set_reference_color",
                  "gpm_set_view_color", "gpm_set_num_views",
                  "gpm_set_rng", "gpm_set_state", "gpm_get_state", "gpm_init", "gpm_sweep", "gpm_phase",
                  "gpm_finalize", "gpm_cost_eval", "gpm_run", "gpm_get_stats", "gpm_reset_stats", "gpm_set_option",
                  "gpm_init_planes", "gpm_shard_num_stages", "gpm_shard_stage", "gpm_shard_finish_init", "gpm_shard_unique_id",
                  "gpm_shard_comm_init", "gpm_shard_comm_attach", "gpm_shard_run", "gpm_measure_fetch_peak", "gpm_shard_p2p_export", "gpm_shard_p2p_attach", "gpm_batch_run",
-                 "gpm_prepare_cameras", "gpm_select_views", "gpm_write_dmb", "gpm_read_dmb", "gpm_write_result_dmb"):
+                 "gpm_prepare_cameras", "gpm_select_views", "gpm_write_dmb", "gpm_read_dmb", "gpm_write_result_dmb",
+                 "gpm_fuse_cameras", "gpm_fuse", "gpm_write_ply"):
         getattr(L, name).restype = C.c_int
     _lib = L
     return L
@@ -486,3 +511,98 @@ def write_result_dmb(depth_path: str, normal_path: str, norm4: np.ndarray):
                                              a.shape[0], a.shape[1])
     if rc != 0:
         raise GipumaError("gpm_write_result_dmb failed")
+
+
+# ---- depth-map fusion (gpm_fuse; DESIGN.md §12) ----------------------------------------------------------------------
+
+def fuse_cameras(Ps, cam_scale: float = 1.0):
+    """The fusion's per-view cameras (gpm_fuse_cameras): un-rebased world frame, K scaled by cam_scale."""
+    lib = load_library()
+    P = np.ascontiguousarray(np.stack([np.asarray(p, dtype=np.float64) for p in Ps]).reshape(-1))
+    out = (GpmFuseCamera * len(Ps))()
+    if lib.gpm_fuse_cameras(P.ctypes.data_as(C.POINTER(C.c_double)), len(Ps), float(cam_scale), out) != 0:
+        raise GipumaError("gpm_fuse_cameras: bad projection matrix or cam_scale")
+    return out
+
+
+def fuse(norm4, Ps, depth_min: float, depth_max: float, disp_thresh: float = 0.1, normal_thresh: float = 30.0,
+         num_consistent: int = 3, images=None, cam_scale: float = 1.0, device: int = 0):
+    """Fuse N views' world-frame outputs into one point cloud on the GPU (gpm_fuse).
+
+    norm4: [N, H, W, 4] float32 (world normal xyz + depth, 0 = invalid; what batch_run returns), numpy or torch (host or
+    CUDA); Ps: the N 3x4 projection matrices of those views (as passed to batch_run); images: None, [N, H, W] grey or
+    [N, H, W, 4] RGBA float in [0, 255], in the same memory as norm4.  The defaults of the thresholds are the reference's
+    DTU script's (scripts/dtu_fast.sh:23-26).  Returns (vertices: PLY_VERTEX array in (view, y, x) order, info dict with
+    count, source [count, 2] int32 (view, y*W + x), used [N, H, W] uint8 masks, fuse_ms, upload_ms)."""
+    lib = load_library()
+    shape = tuple(norm4.shape)
+    if len(shape) != 4 or shape[3] != 4 or len(Ps) != shape[0]:
+        raise ValueError("norm4 must be [N, H, W, 4] with one projection matrix per view")
+    n, H, W = shape[:3]
+    p4, dev = _ptr(norm4)
+    pi, devi, ch = None, dev, 0
+    if images is not None:
+        ishape = tuple(images.shape)
+        if ishape[:3] != (n, H, W) or len(ishape) not in (3, 4) or (len(ishape) == 4 and ishape[3] != 4):
+            raise ValueError("images must be [N, H, W] or [N, H, W, 4]")
+        pi, devi = _ptr(images)
+        ch = 1 if len(ishape) == 3 else 4
+    if devi != dev:
+        raise ValueError("norm4 and images must both be host or both be device buffers")
+    depth = norm4[..., 3]
+    lo, hi = float(np.float32(depth_min)), float(np.float32(depth_max))
+    cap = int(((depth >= lo) & (depth <= hi)).sum())                       # bounds the vertex count
+    verts = np.zeros(max(cap, 1), dtype=PLY_VERTEX)
+    src = np.zeros((max(cap, 1), 2), dtype=np.int32)
+    used = np.zeros((n, H, W), dtype=np.uint8)
+    P = np.ascontiguousarray(np.stack([np.asarray(p, dtype=np.float64) for p in Ps]).reshape(-1))
+    d = GpmFuseDesc(n, W, H, p4, pi, ch, dev, P.ctypes.data_as(C.POINTER(C.c_double)), float(cam_scale), float(depth_min),
+                    float(depth_max), float(disp_thresh), float(normal_thresh), int(num_consistent), int(device))
+    r = GpmFuseResult(0, cap, verts.ctypes.data, src.ctypes.data, used.ctypes.data, 0.0, 0.0)
+    if lib.gpm_fuse(C.byref(d), C.byref(r)) != 0:
+        raise GipumaError("gpm_fuse: %s" % lib.gpm_last_error().decode())
+    k = int(r.count)
+    return verts[:k], {"count": k, "source": src[:k], "used": used, "fuse_ms": float(r.fuse_ms), "upload_ms": float(r.upload_ms)}
+
+
+def fuse_batch_dir(out_dir: str, refs, Ps, depth_min: float, depth_max: float, disp_thresh: float = 0.1,
+                   normal_thresh: float = 30.0, num_consistent: int = 3, images=None, cam_scale: float = 1.0, device: int = 0):
+    """fuse() over what batch_run(out_dir=...) wrote: <out_dir>/<ref, 8 digits>/{disp,normals}.dmb for each of `refs`.
+    Ps and images (None or [n_images, H, W(, 4)]) are the whole sets given to batch_run, indexed by image; the fused views
+    are `refs`, in that order."""
+    maps = []
+    for ref in refs:
+        base = os.path.join(out_dir, "%08d" % int(ref))
+        dep, nrm = read_dmb(os.path.join(base, "disp.dmb")), read_dmb(os.path.join(base, "normals.dmb"))
+        if nrm.ndim != 3 or nrm.shape[2] != 3 or dep.shape != nrm.shape[:2]:
+            raise GipumaError("%s: depth and normal maps do not match" % base)
+        maps.append(np.concatenate([nrm, dep[..., None]], axis=2))
+    imgs = None if images is None else np.ascontiguousarray(np.asarray(images)[list(refs)], dtype=np.float32)
+    return fuse(np.ascontiguousarray(np.stack(maps), dtype=np.float32), [Ps[r] for r in refs], depth_min, depth_max,
+                disp_thresh, normal_thresh, num_consistent, imgs, cam_scale, device)
+
+
+def write_ply(path: str, vertices):
+    """Binary little-endian PLY with the header of storePlyFileBinary (gpm_write_ply)."""
+    v = np.ascontiguousarray(vertices, dtype=PLY_VERTEX)
+    if load_library().gpm_write_ply(path.encode(), v.ctypes.data if len(v) else None, len(v)) != 0:
+        raise GipumaError("gpm_write_ply: cannot write %s" % path)
+
+
+def read_ply(path: str) -> np.ndarray:
+    """Vertices of a PLY written by write_ply (or by the reference's storePlyFileBinary) as a PLY_VERTEX array."""
+    with open(path, "rb") as fh:
+        data = fh.read()
+    end = data.find(b"end_header\n")
+    if not data.startswith(b"ply\n") or end < 0:
+        raise GipumaError("%s: not a PLY file" % path)
+    header = data[:end].decode("ascii").splitlines()
+    props = [ln.split()[1:] for ln in header if ln.startswith("property")]
+    want = [[t, nm] for nm, t in zip(PLY_VERTEX.names, ["float"] * 6 + ["uchar"] * 3)]
+    if "format binary_little_endian 1.0" not in header or props != want:
+        raise GipumaError("%s: not the x, y, z, nx, ny, nz, red, green, blue binary layout" % path)
+    count = int(next(ln.split()[2] for ln in header if ln.startswith("element vertex")))
+    body = data[end + len(b"end_header\n"):]
+    if len(body) != count * PLY_VERTEX.itemsize:
+        raise GipumaError("%s: %d bytes of vertex data for %d vertices" % (path, len(body), count))
+    return np.frombuffer(body, dtype=PLY_VERTEX).copy()

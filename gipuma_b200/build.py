@@ -11,6 +11,7 @@ import hashlib
 import os
 import subprocess
 import sys
+import tempfile
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(HERE)
@@ -19,6 +20,10 @@ ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 # --use_fast_math: same arithmetic mode as the reference's build (CMakeLists.txt:23); the kernels pin every
 # operation with explicit .rn.ftz intrinsics on top of it (gpm_device.cuh).
 COMMON = ["-O3", "--use_fast_math", "-std=c++17", "-lineinfo", "-Xcompiler", "-fPIC", "-shared"] + ARCH
+# The fusion (gpm_fuse.cu) is compiled on its own in IEEE mode: denormals kept, no contraction, so that its decisions are
+# exactly those of the scalar restatement oracle/fusion_oracle.c (DESIGN.md §12).
+FUSE = ["-O3", "-std=c++17", "-lineinfo", "-Xcompiler", "-fPIC", "-ftz=false", "-prec-div=true", "-prec-sqrt=true",
+        "-fmad=false", "-c"] + ARCH
 
 
 def _sig(paths, extra=""):
@@ -35,14 +40,18 @@ def _run(cmd):
 
 
 def build_library(force: bool = False) -> str:
-    src = [os.path.join(HERE, "csrc", f) for f in ("gpm_api.cu", "gpm_host.cpp", "gpm_batch.cpp", "gpm_kernels.cuh", "gpm_device.cuh")]
+    src = [os.path.join(HERE, "csrc", f) for f in ("gpm_api.cu", "gpm_host.cpp", "gpm_batch.cpp", "gpm_fuse.cu", "gpm_kernels.cuh",
+                                                   "gpm_device.cuh")]
     src.append(os.path.join(ROOT, "include", "gipuma_b200.h"))
     out = os.path.join(HERE, "libgipuma_b200.so")
     stamp = out + ".sig"
-    sig = _sig(src, " ".join(COMMON))
+    sig = _sig(src, " ".join(COMMON + FUSE))
     if not force and os.path.exists(out) and os.path.exists(stamp) and open(stamp).read() == sig:
         return out
-    _run([NVCC] + COMMON + ["-o", out, src[0], src[1], src[2], "-lpthread"])
+    with tempfile.TemporaryDirectory() as tmp:
+        fuse_obj = os.path.join(tmp, "gpm_fuse.o")
+        _run([NVCC] + FUSE + ["-o", fuse_obj, src[3]])
+        _run([NVCC] + COMMON + ["-o", out, src[0], src[1], src[2], fuse_obj, "-lpthread"])
     with open(stamp, "w") as fh:
         fh.write(sig)
     return out

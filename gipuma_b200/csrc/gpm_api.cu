@@ -32,6 +32,10 @@ static int fail(int code, const std::string& msg)
     return code;
 }
 
+namespace gpm {
+int set_last_error(int code, const std::string& msg) { return fail(code, msg); }     // for the fusion (gpm_fuse.cu)
+}
+
 #define CU(call)                                                                                      \
     do {                                                                                              \
         cudaError_t e_ = (call);                                                                      \

@@ -138,6 +138,39 @@ extern "C" int gpm_prepare_cameras(const double* P, int n, double cam_scale, gpm
     return GPM_OK;
 }
 
+// The fusion's cameras: the same decomposition as above without the re-basing (transformP = false), each view with its own
+// scaled K — the camera its depth map was computed with when it was the reference view.
+extern "C" int gpm_fuse_cameras(const double* P, int n, double cam_scale, gpm_fuse_camera* out)
+{
+    if (!P || !out || n < 1 || !(cam_scale > 0)) return GPM_E_ARG;
+    for (int i = 0; i < n; i++) {
+        const double* p = P + 12 * i;
+        double sgn = 1.0;
+        M3 M = {{p[0], p[1], p[2], p[4], p[5], p[6], p[8], p[9], p[10]}};
+        if (det(M) < 0) { sgn = -1.0;  for (double& v : M.m) v = -v; }
+        if (det(M) == 0) return GPM_E_ARG;
+        M3 K, R;
+        rq3(M, K, R);
+        const double k22 = K.m[8];
+        for (double& v : K.m) v /= k22;
+        K.m[0] /= cam_scale;  K.m[4] /= cam_scale;  K.m[2] /= cam_scale;  K.m[5] /= cam_scale;
+        const V3 p4 = {{sgn * p[3], sgn * p[7], sgn * p[11]}};
+        const V3 C = mulv(inv(M), V3{{-p4.v[0], -p4.v[1], -p4.v[2]}});
+        const V3 rc = mulv(R, C);
+        const V3 t = {{-rc.v[0], -rc.v[1], -rc.v[2]}};
+        const M3 Mn = mul(K, R);
+        const V3 col = mulv(K, t);
+        gpm_fuse_camera& c = out[i];
+        store9(c.M_inv, inv(Mn));
+        for (int r = 0; r < 3; r++) {
+            for (int k = 0; k < 3; k++) c.P[4 * r + k] = (float)Mn.m[3 * r + k];
+            c.P[4 * r + 3] = (float)col.v[r];
+        }
+        c.f = (float)K.m[0];
+    }
+    return GPM_OK;
+}
+
 // Deterministic selectViews (main.cpp:430-499): cameras whose central ray makes an angle in (min_angle, max_angle) degrees
 // with the reference's; at most max_views of them, in index order (the reference shuffles with srand(time(0)) instead).
 // depth_range[0..1] receives the min/max depth estimate of main.cpp:470-474 (or is left untouched if NULL).
@@ -214,4 +247,19 @@ extern "C" int gpm_write_result_dmb(const char* depth_path, const char* normal_p
     if (depth_path) rc = gpm_write_dmb(depth_path, d.data(), rows, cols, 1);
     if (rc == GPM_OK && normal_path) rc = gpm_write_dmb(normal_path, nm.data(), rows, cols, 3);
     return rc;
+}
+
+// Point cloud in the layout storePlyFileBinary writes (displayUtils.h:84-142), with the real vertex count in the header.
+extern "C" int gpm_write_ply(const char* path, const unsigned char* vertices, long long count)
+{
+    if (!path || count < 0 || (count > 0 && !vertices)) return GPM_E_ARG;
+    FILE* f = fopen(path, "wb");
+    if (!f) return GPM_E_ARG;
+    fprintf(f, "ply\nformat binary_little_endian 1.0\nelement vertex %lld\n"
+               "property float x\nproperty float y\nproperty float z\n"
+               "property float nx\nproperty float ny\nproperty float nz\n"
+               "property uchar red\nproperty uchar green\nproperty uchar blue\nend_header\n", count);
+    const size_t n = (size_t)count * GPM_FUSE_VERTEX_BYTES;
+    const bool ok = fwrite(vertices, 1, n, f) == n;
+    return (fclose(f) == 0 && ok) ? GPM_OK : GPM_E_ARG;
 }

@@ -329,6 +329,44 @@ def _render_job(job):
     return render_view(cam, rows, cols, HeightField(**hf_args), noise_seed=noise_seed)
 
 
+def ref0_frame(Ps: Sequence[np.ndarray]):
+    """(R0, t0): a point X of the frame of the projections Ps is R0 X + t0 in the frame re-based on camera 0, where
+    prepare_cameras puts the cameras and HeightField its surface."""
+    _, R, C = decompose_projection(Ps[0])
+    return R, -R @ C
+
+
+def render_norm4(Ps: Sequence[np.ndarray], cam_scale: float, rows: int, cols: int, hf: HeightField, iters: int = 10,
+                 band: int = 256) -> np.ndarray:
+    """Ground truth of every camera in the layout of the pipeline's output (gpm_batch_run's out_norm4): [n, rows, cols, 4]
+    float32, unit surface normal in the frame of Ps, facing the camera, and depth along the camera's z axis.  The ray cast
+    of render_view does not converge on oblique rays; pixels whose ray ends more than 1e-6 z0 off the surface get depth 0
+    (invalid), so every valid depth is on the surface."""
+    cams = prepare_cameras(Ps, cam_scale)
+    R0, _ = ref0_frame(Ps)
+    out = np.empty((len(cams), rows, cols, 4), dtype=np.float32)
+    eps = 0.01 * hf.unit
+    xs = np.arange(cols, dtype=np.float64)
+    for i, cam in enumerate(cams):
+        Minv, C, p4 = cam.M_inv.astype(np.float64), cam.C.astype(np.float64), cam.P[:, 3].astype(np.float64)
+        R, t = cam.R.astype(np.float64), cam.t.astype(np.float64)
+        for y0 in range(0, rows, band):                        # the ray cast of render_view
+            gx, gy = np.meshgrid(xs, np.arange(y0, min(rows, y0 + band), dtype=np.float64))
+            d = np.stack([gx - p4[0], gy - p4[1], np.full_like(gx, 1.0 - p4[2])], axis=-1) @ Minv.T - C
+            lam = (hf.z0 - C[2]) / d[..., 2]
+            for _ in range(iters):
+                lam = (hf.height(C[0] + lam * d[..., 0], C[1] + lam * d[..., 1]) - C[2]) / d[..., 2]
+            X, Y, Z = C[0] + lam * d[..., 0], C[1] + lam * d[..., 1], C[2] + lam * d[..., 2]
+            n = np.stack([(hf.height(X + eps, Y) - hf.height(X - eps, Y)) / (2 * eps),
+                          (hf.height(X, Y + eps) - hf.height(X, Y - eps)) / (2 * eps), -np.ones_like(X)], axis=-1)
+            n /= np.linalg.norm(n, axis=-1, keepdims=True)
+            out[i, y0:y0 + len(X), :, :3] = n @ R0                    # R0^T n: back to the frame of Ps
+            dep = R[2, 0] * X + R[2, 1] * Y + R[2, 2] * Z + t[2]
+            on_surface = np.abs(Z - hf.height(X, Y)) <= 1e-6 * hf.z0
+            out[i, y0:y0 + len(X), :, 3] = np.where(on_surface & (np.abs(dep) < 1e30), dep, 0.0)
+    return out
+
+
 def render_scene(name: str, Ps: Sequence[np.ndarray], rows: int, cols: int, params: AlgorithmParameters,
                  cam_scale: float = 1.0, n_views: Optional[int] = None, z0: Optional[float] = None,
                  seed: int = 1234, only_selected: bool = True, hard: bool = False, workers: int = 0,

@@ -240,6 +240,64 @@ typedef struct gpm_batch_stats {
 int gpm_batch_run(const gpm_batch_desc* desc, gpm_batch_stats* stats);
 const char* gpm_batch_last_error(void);
 
+/* ---- depth-map fusion: the per-view world-frame outputs (norm4 of gpm_batch_run, or its .dmb files) -> one point cloud;
+ * what the reference's scripts hand to the external `fusibile` (scripts/dtu_fast.sh:56-57).  Deterministic: the same inputs
+ * give the same vertices, in the same order, on every run.  The algorithm is specified in DESIGN.md §12; in short, views are
+ * processed in ascending order as reference; a valid, unused reference pixel back-projects to X (get3Dpoint in the un-rebased
+ * world frame), X is projected into every other view j and rounded to the nearest pixel, and j is consistent when that pixel
+ * is inside the image, X is in front of camera j, the pixel's depth is in [depth_min, depth_max], the disparities
+ * f_j*0.54/z of X and of the pixel differ by less than disp_thresh and the normals are less than normal_thresh degrees apart.
+ * With at least num_consistent consistent views one vertex is emitted (mean position, normalised normal sum, mean colour)
+ * and the pixels involved are marked used; a mark only stops a pixel from being a reference in later passes.
+ * Vertices are emitted in (reference view, y, x) order. */
+#define GPM_FUSE_MAX_VIEWS   256      /* views held in one block's shared-memory camera table */
+#define GPM_FUSE_VERTEX_BYTES 27      /* float x, y, z, nx, ny, nz; uchar red, green, blue; packed, little-endian (storePlyFileBinary) */
+
+/* Per-view camera of the fusion, in the un-rebased world frame (getCameraParameters(..., transformP = false),
+ * cameraGeometryUtils.h:174-353): P = K_scaled [R | t] with K[2][2] = 1 and K's focal lengths and principal point divided
+ * by cam_scale as gpm_prepare_cameras does; M_inv = inverse of P's left 3x3; f = K_scaled[0][0]. */
+typedef struct gpm_fuse_camera {
+    float M_inv[9];
+    float P[12];                       /* row-major 3x4 */
+    float f;
+} gpm_fuse_camera;
+int gpm_fuse_cameras(const double* P, int n, double cam_scale, gpm_fuse_camera* out);
+
+typedef struct gpm_fuse_desc {
+    int n_views, width, height;        /* 2 <= n_views <= GPM_FUSE_MAX_VIEWS */
+    const float* norm4;                /* n_views * height*width * 4 floats: world normal xyz + depth (0 = invalid) per pixel */
+    const float* images;               /* NULL (black vertices) or n_views * height*width * channels floats, values in [0, 255] */
+    int channels;                      /* 1 = grey (red = green = blue), 4 = RGBA float4 (x, y, z -> red, green, blue; w unused) */
+    int on_device;                     /* norm4 and images are device pointers on `device` (1) or host memory (0) */
+    const double* P;                   /* n_views row-major 3x4 projection matrices, as passed to gpm_batch_run */
+    double cam_scale;                  /* > 0, as gpm_prepare_cameras */
+    float depth_min, depth_max;        /* 0 <= depth_min < depth_max */
+    float disp_thresh;                 /* > 0, in pixels of disparity */
+    float normal_thresh;               /* degrees, in (0, 180] */
+    int num_consistent;                /* >= 1 other views */
+    int device;                        /* CUDA device ordinal */
+} gpm_fuse_desc;
+
+/* Caller-sized result.  `count` always receives the number of fused vertices.  Up to `capacity` vertices are written to
+ * `vertices` (capacity * GPM_FUSE_VERTEX_BYTES bytes) and their sources to `source` (2 ints each: reference view,
+ * y*width + x); when count > capacity the call returns GPM_E_ARG after the whole fusion, so a caller may retry with
+ * capacity = count.  The number of pixels with depth in [depth_min, depth_max] always suffices.  `used` (NULL or
+ * n_views * height*width bytes) receives the final used masks (1 = fused into some vertex).  `fuse_ms` receives the
+ * CUDA-event time from the end of the input uploads to the last vertex download, `upload_ms` the time of the uploads of
+ * norm4 and images (0 for device inputs).  Fusion allocates its own buffers and stream and frees them before returning. */
+typedef struct gpm_fuse_result {
+    long long count;
+    long long capacity;
+    unsigned char* vertices;           /* NULL or capacity * GPM_FUSE_VERTEX_BYTES bytes */
+    int* source;                       /* NULL or capacity * 2 ints */
+    unsigned char* used;               /* NULL or n_views * height*width bytes */
+    float fuse_ms, upload_ms;
+} gpm_fuse_result;
+int gpm_fuse(const gpm_fuse_desc* desc, gpm_fuse_result* result);
+
+/* Binary little-endian PLY with the header of storePlyFileBinary (displayUtils.h:84-97) and `count` packed vertices. */
+int gpm_write_ply(const char* path, const unsigned char* vertices, long long count);
+
 const char* gpm_last_error(void);
 const char* gpm_version(void);
 
