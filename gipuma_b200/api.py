@@ -68,6 +68,16 @@ class GpmFuseResult(C.Structure):
                 ("used", C.c_void_p), ("fuse_ms", C.c_float), ("upload_ms", C.c_float)]
 
 
+class GpmNnDesc(C.Structure):
+    _fields_ = [("n_query", C.c_longlong), ("n_data", C.c_longlong), ("query", C.c_void_p), ("data", C.c_void_p),
+                ("on_device", C.c_int), ("device", C.c_int), ("max_dist", C.c_float)]
+
+
+class GpmNnResult(C.Structure):
+    _fields_ = [("dist", C.c_void_p), ("upload_ms", C.c_float), ("build_ms", C.c_float), ("query_ms", C.c_float),
+                ("cell_size", C.c_float), ("n_cells", C.c_longlong)]
+
+
 # one vertex of the fused point cloud: the packed 27-byte record of storePlyFileBinary (displayUtils.h:84-142)
 PLY_VERTEX = np.dtype([("x", "<f4"), ("y", "<f4"), ("z", "<f4"), ("nx", "<f4"), ("ny", "<f4"), ("nz", "<f4"),
                        ("red", "u1"), ("green", "u1"), ("blue", "u1")])
@@ -139,6 +149,7 @@ def load_library():
     L.gpm_fuse_cameras.argtypes = [C.POINTER(C.c_double), C.c_int, C.c_double, C.POINTER(GpmFuseCamera)]
     L.gpm_fuse.argtypes = [C.POINTER(GpmFuseDesc), C.POINTER(GpmFuseResult)]
     L.gpm_write_ply.argtypes = [C.c_char_p, vp, C.c_longlong]
+    L.gpm_nearest_dist.argtypes = [C.POINTER(GpmNnDesc), C.POINTER(GpmNnResult)]
     for name in ("gpm_create", "gpm_set_params", "gpm_set_reference", "gpm_set_view", "gpm_set_reference_color",
                  "gpm_set_view_color", "gpm_set_num_views",
                  "gpm_set_rng", "gpm_set_state", "gpm_get_state", "gpm_init", "gpm_sweep", "gpm_phase",
@@ -146,7 +157,7 @@ def load_library():
                  "gpm_init_planes", "gpm_shard_num_stages", "gpm_shard_stage", "gpm_shard_finish_init", "gpm_shard_unique_id",
                  "gpm_shard_comm_init", "gpm_shard_comm_attach", "gpm_shard_run", "gpm_measure_fetch_peak", "gpm_shard_p2p_export", "gpm_shard_p2p_attach", "gpm_batch_run",
                  "gpm_prepare_cameras", "gpm_select_views", "gpm_write_dmb", "gpm_read_dmb", "gpm_write_result_dmb",
-                 "gpm_fuse_cameras", "gpm_fuse", "gpm_write_ply"):
+                 "gpm_fuse_cameras", "gpm_fuse", "gpm_write_ply", "gpm_nearest_dist"):
         getattr(L, name).restype = C.c_int
     _lib = L
     return L
@@ -606,3 +617,108 @@ def read_ply(path: str) -> np.ndarray:
     if len(body) != count * PLY_VERTEX.itemsize:
         raise GipumaError("%s: %d bytes of vertex data for %d vertices" % (path, len(body), count))
     return np.frombuffer(body, dtype=PLY_VERTEX).copy()
+
+
+# ---- point-cloud evaluation (gpm_nearest_dist; DESIGN.md §13) ----------------------------------------------------------
+
+def _points(a, what):
+    """(N, 3) float32 points: a numpy array, a torch tensor (host or CUDA), or a structured array with x, y, z fields
+    (the vertices of fuse / read_ply).  Returns (array or tensor, is_device)."""
+    if isinstance(a, np.ndarray) and a.dtype.names is not None:
+        if not {"x", "y", "z"} <= set(a.dtype.names):
+            raise ValueError("%s: a structured array needs x, y and z fields" % what)
+        a = np.stack([a["x"], a["y"], a["z"]], axis=1).astype(np.float32)
+    if len(tuple(a.shape)) != 2 or tuple(a.shape)[1] != 3:
+        raise ValueError("%s must be an (N, 3) array of points, got shape %s" % (what, tuple(a.shape)))
+    if isinstance(a, np.ndarray):
+        if a.dtype != np.float32:
+            raise TypeError("%s must be float32 (got %s)" % (what, a.dtype))
+        return np.ascontiguousarray(a), False
+    if hasattr(a, "is_cuda"):
+        return a.contiguous(), bool(a.is_cuda)
+    raise TypeError("%s: unsupported point type %r" % (what, type(a)))
+
+
+def nearest_distance(query, data, max_dist: float):
+    """Exact distance from every query point to its nearest data point, on the GPU (gpm_nearest_dist).
+
+    query, data: (N, 3) float32 numpy arrays or torch tensors (both host or both CUDA), or structured vertex arrays as
+    fuse / read_ply return.  Per query: the fp32 sqrt of min over the data of (dx*dx + dy*dy) + dz*dz, or +inf when that
+    exceeds max_dist or the data are empty.  Returns (dist, info): dist float32 of length N, numpy for host inputs and a
+    CUDA tensor on the inputs' device otherwise; info has upload_ms, build_ms, query_ms (CUDA events), cell_size, n_cells."""
+    lib = load_library()
+    q, qdev = _points(query, "query")
+    b, bdev = _points(data, "data")
+    if qdev != bdev:
+        raise ValueError("query and data must both be host or both be CUDA buffers")
+    device = 0
+    if qdev:
+        import torch
+        if q.device != b.device:
+            raise ValueError("query and data must be on the same device")
+        device = q.device.index
+        out = torch.empty(q.shape[0], dtype=torch.float32, device=q.device)
+    else:
+        out = np.empty(q.shape[0], dtype=np.float32)
+    pq, _ = _ptr(q)
+    pb, _ = _ptr(b)
+    po, _ = _ptr(out)
+    d = GpmNnDesc(int(q.shape[0]), int(b.shape[0]), pq, pb, int(qdev), int(device), float(max_dist))
+    r = GpmNnResult(po, 0.0, 0.0, 0.0, 0.0, 0)
+    if lib.gpm_nearest_dist(C.byref(d), C.byref(r)) != 0:
+        raise GipumaError(lib.gpm_last_error().decode())
+    return out, {"upload_ms": float(r.upload_ms), "build_ms": float(r.build_ms), "query_ms": float(r.query_ms),
+                 "cell_size": float(r.cell_size), "n_cells": int(r.n_cells)}
+
+
+def _sum_in_order(x):
+    return float(np.cumsum(x)[-1]) if len(x) else 0.0
+
+
+def cloud_scores(d_rec, d_gt, max_dist: float, taus=(0.5, 1.0, 2.0)) -> dict:
+    """Accuracy, completeness and F-scores from the two directions' nearest distances (numpy, float64, sums in index order).
+
+    d_rec: distance of every reconstructed point to the ground truth; d_gt: of every ground-truth point to the
+    reconstruction (+inf beyond max_dist, as nearest_distance returns them).  As in the DTU protocol, distances >= max_dist
+    are outliers: accuracy_mean / _median are taken over d_rec < max_dist, completeness_mean / _median over d_gt < max_dist,
+    overall is their mean, and accuracy_outliers / completeness_outliers are the shares >= max_dist.  For each tau in taus:
+    precision = share of d_rec < tau, recall = share of d_gt < tau, f_score = 2 P R / (P + R), 0 when P + R = 0 (lists in
+    the order of taus).  A tau > max_dist is refused: such distances were capped.  Empty sets: means and medians over no
+    distances are NaN, shares of an empty set are 0."""
+    a = np.asarray(d_rec, dtype=np.float64).reshape(-1)
+    g = np.asarray(d_gt, dtype=np.float64).reshape(-1)
+    taus = [float(t) for t in taus]
+    if not (np.isfinite(max_dist) and max_dist > 0):
+        raise ValueError("max_dist must be finite and > 0")
+    for t in taus:
+        if not (t > 0 and t <= max_dist):
+            raise ValueError("tau %g is outside (0, max_dist = %g]: distances beyond max_dist were capped" % (t, max_dist))
+
+    def share(x, below):
+        return float(np.count_nonzero(x < below)) / len(x) if len(x) else 0.0
+
+    def mean_median(x):
+        x = x[x < max_dist]
+        return (_sum_in_order(x) / len(x), float(np.median(x))) if len(x) else (float("nan"), float("nan"))
+
+    acc, acc_med = mean_median(a)
+    comp, comp_med = mean_median(g)
+    P = [share(a, t) for t in taus]
+    R = [share(g, t) for t in taus]
+    F = [2.0 * p * r / (p + r) if p + r > 0 else 0.0 for p, r in zip(P, R)]
+    return {"accuracy_mean": acc, "accuracy_median": acc_med, "completeness_mean": comp, "completeness_median": comp_med,
+            "overall": 0.5 * (acc + comp), "accuracy_outliers": 1.0 - share(a, max_dist) if len(a) else 0.0,
+            "completeness_outliers": 1.0 - share(g, max_dist) if len(g) else 0.0,
+            "taus": taus, "precision": P, "recall": R, "f_score": F, "n_rec": len(a), "n_gt": len(g)}
+
+
+def evaluate_cloud(rec, gt, max_dist: float = 20.0, taus=(0.5, 1.0, 2.0)) -> dict:
+    """Score a reconstructed cloud against ground truth: nearest_distance in both directions on the GPU, then cloud_scores.
+    rec, gt: as nearest_distance takes them (for instance the vertices of fuse and scene.gt_points).  The result also holds
+    the two directions' timings under "accuracy_timing" and "completeness_timing"."""
+    d_rec, t_rec = nearest_distance(rec, gt, max_dist)
+    d_gt, t_gt = nearest_distance(gt, rec, max_dist)
+    host = [x.cpu().numpy() if hasattr(x, "cpu") else x for x in (d_rec, d_gt)]
+    out = cloud_scores(host[0], host[1], max_dist, taus)
+    out["accuracy_timing"], out["completeness_timing"] = t_rec, t_gt
+    return out

@@ -20,8 +20,9 @@ ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 # --use_fast_math: same arithmetic mode as the reference's build (CMakeLists.txt:23); the kernels pin every
 # operation with explicit .rn.ftz intrinsics on top of it (gpm_device.cuh).
 COMMON = ["-O3", "--use_fast_math", "-std=c++17", "-lineinfo", "-Xcompiler", "-fPIC", "-shared"] + ARCH
-# The fusion (gpm_fuse.cu) is compiled on its own in IEEE mode: denormals kept, no contraction, so that its decisions are
-# exactly those of the scalar restatement oracle/fusion_oracle.c (DESIGN.md §12).
+# The fusion (gpm_fuse.cu) and the cloud distances (gpm_cloud.cu) are compiled on their own in IEEE mode: denormals kept, no
+# contraction, so that the fusion's decisions are exactly those of the scalar restatement oracle/fusion_oracle.c (DESIGN.md
+# §12) and every distance is exactly that of the brute-force restatement oracle/pycloud.py (§13).
 FUSE = ["-O3", "-std=c++17", "-lineinfo", "-Xcompiler", "-fPIC", "-ftz=false", "-prec-div=true", "-prec-sqrt=true",
         "-fmad=false", "-c"] + ARCH
 
@@ -40,8 +41,8 @@ def _run(cmd):
 
 
 def build_library(force: bool = False) -> str:
-    src = [os.path.join(HERE, "csrc", f) for f in ("gpm_api.cu", "gpm_host.cpp", "gpm_batch.cpp", "gpm_fuse.cu", "gpm_kernels.cuh",
-                                                   "gpm_device.cuh")]
+    src = [os.path.join(HERE, "csrc", f) for f in ("gpm_api.cu", "gpm_host.cpp", "gpm_batch.cpp", "gpm_fuse.cu", "gpm_cloud.cu",
+                                                   "gpm_kernels.cuh", "gpm_device.cuh")]
     src.append(os.path.join(ROOT, "include", "gipuma_b200.h"))
     out = os.path.join(HERE, "libgipuma_b200.so")
     stamp = out + ".sig"
@@ -49,9 +50,10 @@ def build_library(force: bool = False) -> str:
     if not force and os.path.exists(out) and os.path.exists(stamp) and open(stamp).read() == sig:
         return out
     with tempfile.TemporaryDirectory() as tmp:
-        fuse_obj = os.path.join(tmp, "gpm_fuse.o")
-        _run([NVCC] + FUSE + ["-o", fuse_obj, src[3]])
-        _run([NVCC] + COMMON + ["-o", out, src[0], src[1], src[2], fuse_obj, "-lpthread"])
+        ieee_objs = [os.path.join(tmp, os.path.basename(s)[:-3] + ".o") for s in src[3:5]]
+        for s, o in zip(src[3:5], ieee_objs):
+            _run([NVCC] + FUSE + ["-o", o, s])
+        _run([NVCC] + COMMON + ["-o", out, src[0], src[1], src[2]] + ieee_objs + ["-lpthread"])
     with open(stamp, "w") as fh:
         fh.write(sig)
     return out

@@ -33,7 +33,7 @@ static int fail(int code, const std::string& msg)
 }
 
 namespace gpm {
-int set_last_error(int code, const std::string& msg) { return fail(code, msg); }     // for the fusion (gpm_fuse.cu)
+int set_last_error(int code, const std::string& msg) { return fail(code, msg); }     // for gpm_fuse.cu and gpm_cloud.cu
 }
 
 #define CU(call)                                                                                      \

@@ -367,6 +367,29 @@ def render_norm4(Ps: Sequence[np.ndarray], cam_scale: float, rows: int, cols: in
     return out
 
 
+def gt_points(Ps: Sequence[np.ndarray], cam_scale: float, rows: int, cols: int, hf: HeightField, stride: int = 1,
+              norm4: Optional[np.ndarray] = None) -> np.ndarray:
+    """Ground-truth point cloud of a height-field scene: the surface the cameras see.  Every valid pixel (depth > 0) of the
+    maps of render_norm4, taking every `stride`-th row and column, back-projected in float64 with get3Dpoint
+    (X = M_inv (d (x, y, 1) - P_col34)) through the fusion's camera of its view (DESIGN.md §12), so the points are in the
+    un-rebased world frame of gpm_fuse's vertices.  The maps were ray cast through the float32 camera fields of
+    prepare_cameras, so a point lies off the surface by up to about 3e-5 z0 (the fusion's vertices inherit the same).
+    `norm4`: those maps, if already rendered.  Returns (N, 3) float32 in (view, y, x) order.  It stands in for a dataset's
+    observation mask."""
+    if norm4 is None:
+        norm4 = render_norm4(Ps, cam_scale, rows, cols, hf)
+    ys, xs = np.mgrid[0:rows:stride, 0:cols:stride].astype(np.float64)
+    out = []
+    for P, n4 in zip(Ps, norm4):
+        K, R, C = decompose_projection(P)
+        Pv = scale_K(K / K[2, 2], cam_scale) @ np.hstack([R, (-R @ C)[:, None]])
+        d = n4[::stride, ::stride, 3].astype(np.float64)
+        ok = d > 0
+        h = np.stack([d[ok] * xs[ok], d[ok] * ys[ok], d[ok]], axis=1) - Pv[:, 3]
+        out.append(h @ np.linalg.inv(Pv[:, :3]).T)
+    return np.ascontiguousarray(np.concatenate(out), dtype=np.float32)
+
+
 def render_scene(name: str, Ps: Sequence[np.ndarray], rows: int, cols: int, params: AlgorithmParameters,
                  cam_scale: float = 1.0, n_views: Optional[int] = None, z0: Optional[float] = None,
                  seed: int = 1234, only_selected: bool = True, hard: bool = False, workers: int = 0,

@@ -298,6 +298,34 @@ int gpm_fuse(const gpm_fuse_desc* desc, gpm_fuse_result* result);
 /* Binary little-endian PLY with the header of storePlyFileBinary (displayUtils.h:84-97) and `count` packed vertices. */
 int gpm_write_ply(const char* path, const unsigned char* vertices, long long count);
 
+/* ---- point-cloud distances: the exact distance from every query point to its nearest data point, the one operation behind
+ * accuracy / completeness / F-score of a reconstructed cloud against ground truth (DESIGN.md §13).  fp32, one IEEE
+ * round-to-nearest step per operation: dx = q.x - b.x (likewise y, z), d2 = (dx*dx + dy*dy) + dz*dz, m = min over the data
+ * of d2, D = sqrt(m); dist = D if D <= max_dist, else +inf (also for an empty data set).  The search skips data only under a
+ * provably conservative bound, so every finite output equals a brute-force evaluation bit for bit; m is a minimum over a set,
+ * so the output does not depend on the order of the data, on the run, or on where the inputs live.  Refused with GPM_E_ARG
+ * before any search: null pointers, counts outside [0, 2^31 - 1], max_dist not finite and > 0, a non-finite coordinate. */
+typedef struct gpm_nn_desc {
+    long long n_query, n_data;
+    const float* query;                /* n_query * 3 floats: x y z per point */
+    const float* data;                 /* n_data * 3 floats */
+    int on_device;                     /* query, data and result->dist are device pointers on `device` (1) or host memory (0) */
+    int device;                        /* CUDA device ordinal */
+    float max_dist;                    /* finite, > 0 */
+} gpm_nn_desc;
+
+/* `dist` (n_query floats) is caller memory of the inputs' kind.  The times are CUDA events: upload_ms the host-to-device
+ * copies of query and data (0 for device inputs), build_ms the validation pass and the grid over the data, query_ms the
+ * search.  cell_size and n_cells describe the grid that was built.  The call allocates its own buffers and stream and frees
+ * them before returning. */
+typedef struct gpm_nn_result {
+    float* dist;
+    float upload_ms, build_ms, query_ms;
+    float cell_size;
+    long long n_cells;
+} gpm_nn_result;
+int gpm_nearest_dist(const gpm_nn_desc* desc, gpm_nn_result* result);
+
 const char* gpm_last_error(void);
 const char* gpm_version(void);
 
