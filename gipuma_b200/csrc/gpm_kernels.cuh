@@ -428,7 +428,10 @@ struct ShardP2P {
     int me, world, nblocks;
 };
 
-// merged cost of one slot: the n_best smallest over all ranks' lists, summed ascending, / count  (gipuma.cu:779-803)
+// merged cost of one slot: the n_best smallest over all ranks' lists, summed ascending, / count  (gipuma.cu:779-803).
+// A slot that every rank skipped (not offered, out of range, memo hit, duplicate) has only +inf entries and merges to +inf,
+// so that no accept can take it whatever the pixel's cost; an evaluated slot always has finite entries (local_topn clamps
+// every cost to MAXCOST), and MAXCOST when none of them is below MAXCOST.
 __device__ __forceinline__ float shard_merge(const float* __restrict__ g, size_t rank_stride, int world, int nb)
 {
     int pos[8] = {0, 0, 0, 0, 0, 0, 0, 0};
@@ -440,6 +443,7 @@ __device__ __forceinline__ float shard_merge(const float* __restrict__ g, size_t
         for (int r = 0; r < world; r++) {
             if (pos[r] < nb) { const float v = __ldcg(g + r * rank_stride + pos[r]); if (v < best) { best = v;  br = r; } }
         }
+        if (br < 0 && i == 0) return __int_as_float(0x7f800000);      // no rank has a finite entry: the slot was skipped
         if (br < 0 || !(best < GPM_MAXCOST)) break;        // only views with c < MAXCOST count (numValidViews)
         pos[br]++;
         sum = fadd(sum, best);

@@ -61,9 +61,10 @@ def local_topn(costs: np.ndarray, n_best: int) -> np.ndarray:
 def merge_topn(gathered: np.ndarray, n_best: int) -> np.ndarray:
     """gathered: [world, ..., n_best] ascending lists.  Returns the combined cost exactly as `shard_merge` /
     pmCostMultiview_cu (COMB_BEST_N) do: the n_best smallest valid (< MAXCOST) costs summed in ascending order in
-    float32, divided by their count; MAXCOST if none."""
+    float32, divided by their count; MAXCOST if none; +inf if no rank has a finite entry (a slot every rank skipped)."""
     g = np.moveaxis(np.asarray(gathered, dtype=np.float32), 0, -2)          # [..., world, n_best]
     flat = np.sort(g.reshape(g.shape[:-2] + (-1,)), axis=-1)[..., :n_best]
+    skipped = flat[..., 0] == np.float32(np.inf)
     valid = flat < np.float32(MAXCOST)
     total = np.zeros(flat.shape[:-1], np.float32)
     for i in range(flat.shape[-1]):                                          # ascending, float32, like the device loop
@@ -72,7 +73,7 @@ def merge_topn(gathered: np.ndarray, n_best: int) -> np.ndarray:
     with np.errstate(divide="ignore", invalid="ignore"):
         cost = np.where(cnt > 0, total / np.maximum(cnt, 1).astype(np.float32), np.float32(MAXCOST)).astype(np.float32)
     cost = np.where((cost != cost) | (cost > MAXCOST) | (cost < 0), np.float32(MAXCOST), cost)
-    return cost
+    return np.where(skipped, np.float32(np.inf), cost).astype(np.float32)
 
 
 # ----------------------------------------------------------------------------------------------------------------

@@ -10,14 +10,16 @@ from conftest import bits_equal
 pytestmark = pytest.mark.gpu
 
 
-def _sharded_run(sc, world, seed=0xC0FFEE):
-    import torch
+def open_ranks(sc, world, seed=0xC0FFEE, options=None):
+    """One context per rank of a shard group of `world` ranks, each holding its share of the source views."""
     from gipuma_b200 import multigpu as M
     from gipuma_b200 import api
     parts = M.partition_views(sc.n_views, world)
     ctxs = []
     for r in range(world):
         ctx = api.Context(sc.cols, sc.rows, len(parts[r]))
+        for k, v in (options or {}).items():
+            ctx.set_option(k, v)
         ctx.set_params(sc.params)
         ctx.set_reference(np.ascontiguousarray(sc.images[0]), sc.cameras[0])
         for v, pos in enumerate(parts[r]):
@@ -25,37 +27,84 @@ def _sharded_run(sc, world, seed=0xC0FFEE):
         ctx.set_num_views(len(parts[r]))
         ctx.set_rng(seed)
         ctxs.append(ctx)
-    n_stages = ctxs[0].shard_num_stages()
+    return ctxs
 
-    def stage(colour, st, prev):
+
+class SimulatedShard:
+    """A shard group whose ranks are contexts on this GPU; the all-gather is a torch.cat."""
+
+    def __init__(self, sc, world, seed=0xC0FFEE, options=None):
+        self.world = world
+        self.ctxs = open_ranks(sc, world, seed, options)
+        self.n_stages = self.ctxs[0].shard_num_stages()
+
+    def stage(self, colour, st, prev):
         """One exchange stage on every simulated rank: accept of the previous stage (fused) + evaluation; returns the
         rank-major concatenation of the lists, i.e. what an all-gather hands to every rank."""
-        n = ctxs[0].shard_stage_floats(st) if st < n_stages else 0
+        import torch
+        n = self.ctxs[0].shard_stage_floats(st) if st < self.n_stages else 0
         locs = []
-        for ctx in ctxs:
+        for ctx in self.ctxs:
             buf = torch.empty(n, dtype=torch.float32, device="cuda") if n else None
-            ctx.shard_stage(colour, st, prev, world, buf)
+            ctx.shard_stage(colour, st, prev, self.world, buf)
             locs.append(buf)
         torch.cuda.synchronize()
         return torch.cat(locs) if n else None
 
-    for ctx in ctxs:
-        ctx.init_planes()
-    g0 = stage(0, 0, None)
-    for ctx in ctxs:
-        ctx.shard_finish_init(g0, world)
+    def init(self):
+        """Random planes, stage 0 and its accept; returns the gathered stage-0 lists."""
+        for ctx in self.ctxs:
+            ctx.init_planes()
+        g0 = self.stage(0, 0, None)
+        for ctx in self.ctxs:
+            ctx.shard_finish_init(g0, self.world)
+        return g0
+
+    def colour(self, colour, after_stage=None):
+        """Stages 1 .. n_stages - 1 of one colour and its closing accept (stage n_stages); after_stage(st, gathered) is
+        called after each of them (gathered is None after the closing accept)."""
+        prev = None
+        for st in range(1, self.n_stages + 1):
+            prev = self.stage(colour, st, prev)
+            if after_stage is not None:
+                after_stage(st, prev)
+
+    def close(self):
+        for ctx in self.ctxs:
+            ctx.close()
+
+
+def _sharded_run(sc, world, seed=0xC0FFEE):
+    grp = SimulatedShard(sc, world, seed)
+    grp.init()
     for _ in range(sc.params.iterations):
         for colour in (0, 1):
-            prev = None
-            for st in range(1, n_stages):
-                prev = stage(colour, st, prev)
-            stage(colour, n_stages, prev)                  # closing accept of the colour
+            grp.colour(colour)
     outs = []
-    for ctx in ctxs:
+    for ctx in grp.ctxs:
         ctx.finalize()
         outs.append(ctx.get_state())
-        ctx.close()
+    grp.close()
     return outs
+
+
+def run_concurrently(ctxs, timeout=120):
+    """gpm_shard_run on every rank at once, one thread per rank (with the peer-memory exchange each rank waits for the
+    others); returns the exceptions raised."""
+    import threading
+    errs = []
+
+    def work(ctx):
+        try:
+            ctx.shard_run()
+        except Exception as e:      # noqa: BLE001
+            errs.append(e)
+    threads = [threading.Thread(target=work, args=(ctx,)) for ctx in ctxs]
+    for t in threads:
+        t.start()
+    for t in threads:
+        t.join(timeout=timeout)
+    return errs
 
 
 @pytest.mark.parametrize("cfg,rows,cols,views,world,box,nbest", [
@@ -117,39 +166,17 @@ def test_fused_peer_memory_exchange_two_ranks_on_one_gpu():
     The two gpm_shard_run calls must overlap (each waits for the other), hence the threads; the image is small enough for both
     kernels to be resident at once.  Result: bit-identical to the unsharded run on both ranks, and again on a second run
     (sequence numbers and parity buffers carry over)."""
-    import threading
-    from gipuma_b200 import api, multigpu as M, scene as S
+    from gipuma_b200 import api, scene as S
     sc = S.make_config(2, rows=64, cols=96, n_views=6, iterations=2, seed=558)
     sc.params.box_hsize = sc.params.box_vsize = 11
     single, _, _ = api.runcuda(sc, seed=0xC0FFEE)
     world = 2
-    parts = M.partition_views(sc.n_views, world)
-    ctxs = []
-    for r in range(world):
-        ctx = api.Context(sc.cols, sc.rows, len(parts[r]))
-        ctx.set_params(sc.params)
-        ctx.set_reference(np.ascontiguousarray(sc.images[0]), sc.cameras[0])
-        for v, pos in enumerate(parts[r]):
-            ctx.set_view(v, np.ascontiguousarray(sc.images[sc.subset[pos]]), sc.cameras[sc.subset[pos]])
-        ctx.set_num_views(len(parts[r]))
-        ctx.set_rng(0xC0FFEE)
-        ctxs.append(ctx)
+    ctxs = open_ranks(sc, world)
     exported = [ctx.shard_p2p_export(world) for ctx in ctxs]
     for r, ctx in enumerate(ctxs):
         ctx.shard_p2p_attach([h for h, _ in exported], r, world, local_ptrs=[p for _, p in exported])
     for _ in range(2):
-        errs = []
-
-        def work(ctx):
-            try:
-                ctx.shard_run()
-            except Exception as e:      # noqa: BLE001
-                errs.append(e)
-        threads = [threading.Thread(target=work, args=(ctx,)) for ctx in ctxs]
-        for t in threads:
-            t.start()
-        for t in threads:
-            t.join(timeout=120)
+        errs = run_concurrently(ctxs)
         assert not errs, errs
         for ctx in ctxs:
             n4, c = ctx.get_state()

@@ -38,6 +38,7 @@ def _torchrun(nproc, script_args, timeout=900):
 @pytest.mark.parametrize("world,args", [
     (2, ["--config", "4", "--rows", "96", "--cols", "128", "--views", "13", "--iters", "2"]),
     (2, ["--config", "2", "--rows", "352", "--cols", "480", "--views", "7", "--iters", "3"]),
+    (2, ["--config", "2", "--rows", "353", "--cols", "481", "--views", "7", "--iters", "2"]),     # odd width, partial tiles
 ])
 def test_view_shard_over_real_ranks_equals_single_gpu(world, args, exchange):
     """exchange = p2p: the fused kernel storing into the peer GPU's memory over NVLink (CUDA IPC); nccl: one ncclAllGather per

@@ -51,8 +51,11 @@ def test_merge_matches_reference_combination_single_process():
         costs[7] = 1500.0                                                        # a pixel with no valid view at all
         parts = M.partition_views(n_views, world)
         lists = np.stack([M.local_topn(costs[:, p], n_best) if p else np.full((200, n_best), np.inf, np.float32) for p in parts])
+        lists[:, 11] = np.inf                                                    # a slot every rank skipped: no entry at all
         merged = M.merge_topn(lists, n_best)
         want = np.array([reference_combine(row, n_best) for row in costs], dtype=np.float32)
+        want[11] = np.inf                                                        # never accepted, whatever the pixel's cost
+        assert want[7] == np.float32(M.MAXCOST)
         assert np.array_equal(merged.view(np.uint32), want.view(np.uint32))
 
 
