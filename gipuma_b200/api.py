@@ -143,8 +143,6 @@ def load_library():
     L.gpm_measure_fetch_peak.argtypes = [vp, C.POINTER(C.c_double)]
     L.gpm_batch_run.argtypes = [C.POINTER(GpmBatchDesc), C.POINTER(GpmBatchStats)]
     L.gpm_batch_last_error.restype = C.c_char_p
-    L.gpm_shard_p2p_export.argtypes = [vp, C.c_int, vp, C.POINTER(vp)]
-    L.gpm_shard_p2p_attach.argtypes = [vp, vp, C.POINTER(vp), C.c_int, C.c_int]
     L.gpm_stream.restype = vp
     L.gpm_fuse_cameras.argtypes = [C.POINTER(C.c_double), C.c_int, C.c_double, C.POINTER(GpmFuseCamera)]
     L.gpm_fuse.argtypes = [C.POINTER(GpmFuseDesc), C.POINTER(GpmFuseResult)]
@@ -155,7 +153,7 @@ def load_library():
                  "gpm_set_rng", "gpm_set_state", "gpm_get_state", "gpm_init", "gpm_sweep", "gpm_phase",
                  "gpm_finalize", "gpm_cost_eval", "gpm_run", "gpm_get_stats", "gpm_reset_stats", "gpm_set_option",
                  "gpm_init_planes", "gpm_shard_num_stages", "gpm_shard_stage", "gpm_shard_finish_init", "gpm_shard_unique_id",
-                 "gpm_shard_comm_init", "gpm_shard_comm_attach", "gpm_shard_run", "gpm_measure_fetch_peak", "gpm_shard_p2p_export", "gpm_shard_p2p_attach", "gpm_batch_run",
+                 "gpm_shard_comm_init", "gpm_shard_comm_attach", "gpm_shard_run", "gpm_measure_fetch_peak", "gpm_batch_run",
                  "gpm_prepare_cameras", "gpm_select_views", "gpm_write_dmb", "gpm_read_dmb", "gpm_write_result_dmb",
                  "gpm_fuse_cameras", "gpm_fuse", "gpm_write_ply", "gpm_nearest_dist"):
         getattr(L, name).restype = C.c_int
@@ -366,21 +364,6 @@ class Context:
         """ncclCommInitRank behind the C-ABI; `unique_id` = the 128 bytes of shard_unique_id() of the group's rank 0."""
         buf = C.create_string_buffer(unique_id, 128) if unique_id is not None else None
         self._check(self.lib.gpm_shard_comm_init(self.h, buf, rank, world))
-
-    def shard_p2p_export(self, world: int):
-        """Allocate this rank's peer-memory exchange region; returns (64-byte CUDA IPC handle, device address)."""
-        h = C.create_string_buffer(64)
-        ptr = C.c_void_p()
-        self._check(self.lib.gpm_shard_p2p_export(self.h, world, h, C.byref(ptr)))
-        return h.raw, int(ptr.value or 0)
-
-    def shard_p2p_attach(self, handles, rank: int, world: int, local_ptrs=None):
-        """handles: list of `world` 64-byte IPC handles (rank-major); local_ptrs: optional addresses of same-process ranks."""
-        blob = C.create_string_buffer(b"".join(handles), 64 * world)
-        lp = None
-        if local_ptrs is not None:
-            lp = (C.c_void_p * world)(*[C.c_void_p(p) if p else None for p in local_ptrs])
-        self._check(self.lib.gpm_shard_p2p_attach(self.h, blob, lp, rank, world))
 
     def shard_run(self) -> float:
         """runcuda() with sharded views (gpm_shard_run): returns the sweep time in ms."""

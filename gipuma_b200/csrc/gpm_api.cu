@@ -64,15 +64,6 @@ struct gpm_ctx {
     bool comm_owned = false;
     int shard_rank = 0, shard_world = 0;
     unsigned long long collectives = 0;
-    // fused peer-memory exchange (k_shard_fused): this rank's region, the peers' regions as mapped here, sequence counter
-    char* p2p_region = nullptr;
-    size_t p2p_bytes = 0, p2p_slot_floats = 0, p2p_flag_bytes = 0;
-    int p2p_world = 0, p2p_nblocks = 0;
-    bool p2p_attached = false;
-    void* p2p_peer[8] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
-    bool p2p_ipc_opened[8] = {false, false, false, false, false, false, false, false};
-    unsigned p2p_seq = 0;
-    int opt_exchange = 1;                        // 1: peer-memory exchange when attached; 0: NCCL all-gather per stage
     int opt_async_upload = 0;                    // 1: image uploads return without a host synchronisation (caller keeps its buffers alive until the next run)
     bool inputs_dirty = false;                   // an input changed: stored costs / memo are stale (cleared once, at the next launch)
     unsigned* seen = nullptr;        // [H*W*ncand] identity of the plane last offered to each pixel from each of the 8 (fused kernel: 20) propagation directions
@@ -442,9 +433,7 @@ extern "C" int gpm_create(gpm_ctx** out, int device, int width, int height, int 
         ok(cudaFuncSetAttribute(k_cost_eval<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, c->smem_optin));
         ok(cudaFuncSetAttribute(k_cost_eval<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, c->smem_optin));
         ok(cudaFuncSetAttribute(k_shard_stage<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, c->smem_optin));
-        ok(cudaFuncSetAttribute(k_shard_fused<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, c->smem_optin));
         ok(cudaFuncSetAttribute(k_shard_stage<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, c->smem_optin));
-        ok(cudaFuncSetAttribute(k_shard_fused<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, c->smem_optin));
     }
     if (err != cudaSuccess) {
         std::string m = std::string("gpm_create: ") + cudaGetErrorString(err);
@@ -463,8 +452,6 @@ extern "C" void gpm_destroy(gpm_ctx* c)
     DeviceGuard g(c->device);
     if (c->stream) cudaStreamSynchronize(c->stream);
     if (c->comm && c->comm_owned) gpm_shard_comm_destroy_(c);
-    for (int r = 0; r < 8; r++) if (c->p2p_ipc_opened[r] && c->p2p_peer[r]) cudaIpcCloseMemHandle(c->p2p_peer[r]);
-    cudaFree(c->p2p_region);
     if (c->srcTex) cudaDestroyTextureObject(c->srcTex);
     if (c->srcArr) cudaFreeArray(c->srcArr);
     if (c->srcTex4) cudaDestroyTextureObject(c->srcTex4);
@@ -1008,88 +995,6 @@ static int shard_exchange(gpm_ctx* c, int stage)
     return GPM_OK;
 }
 
-// ---- fused peer-memory exchange: region management ------------------------------------------------------------------
-// Allocate this rank's exchange region for a shard group of `world` ranks and return its CUDA IPC handle (64 bytes) and its
-// address (for ranks living in the same process).  Layout: [world][nblocks] arrival flags, then [2][world][slot] lists.
-extern "C" int gpm_shard_p2p_export(gpm_ctx* c, int world, void* handle64, void** local_ptr)
-{
-    if (!c || world < 2 || world > 8) return fail(GPM_E_ARG, "gpm_shard_p2p_export: bad arguments (2 <= world <= 8)");
-    if (!c->have_params) return fail(GPM_E_STATE, "gpm_shard_p2p_export: parameters not set");
-    DeviceGuard g(c->device);
-    long long mx = 0;
-    const int ns = gpm_shard_num_stages(c);
-    for (int st = 0; st < ns; st++) { const long long f = gpm_shard_stage_floats(c, st);  if (f > mx) mx = f; }
-    const dim3 grid = tile_grid(c);
-    const int nblocks = (int)(grid.x * grid.y * grid.z);
-    const size_t flag_bytes = ((size_t)world * nblocks * sizeof(unsigned) + 1023) & ~(size_t)1023;
-    const size_t bytes = flag_bytes + 2ull * world * (size_t)mx * sizeof(float);
-    if (!c->p2p_region || c->p2p_bytes != bytes || c->p2p_world != world) {
-        CU(cudaStreamSynchronize(c->stream));
-        for (int r = 0; r < 8; r++) { if (c->p2p_ipc_opened[r] && c->p2p_peer[r]) cudaIpcCloseMemHandle(c->p2p_peer[r]);  c->p2p_peer[r] = nullptr;  c->p2p_ipc_opened[r] = false; }
-        cudaFree(c->p2p_region);  c->p2p_region = nullptr;  c->p2p_attached = false;
-        CU(cudaMalloc(&c->p2p_region, bytes));
-        c->p2p_bytes = bytes;  c->p2p_world = world;
-    }
-    c->p2p_slot_floats = (size_t)mx;  c->p2p_flag_bytes = flag_bytes;  c->p2p_nblocks = nblocks;
-    CU(cudaMemsetAsync(c->p2p_region, 0, flag_bytes, c->stream));          // flags: nothing has arrived
-    CU(cudaStreamSynchronize(c->stream));
-    c->p2p_seq = 0;
-    if (handle64) {
-        cudaIpcMemHandle_t h;
-        CU(cudaIpcGetMemHandle(&h, c->p2p_region));
-        static_assert(sizeof(h) == 64, "cudaIpcMemHandle_t is 64 bytes");
-        memcpy(handle64, &h, 64);
-    }
-    if (local_ptr) *local_ptr = c->p2p_region;
-    return GPM_OK;
-}
-
-// Map the regions of all ranks of the group.  `handles64`: world x 64 bytes (rank-major) from gpm_shard_p2p_export of every
-// rank, opened with cudaIpcOpenMemHandle (ranks in other processes); `local_ptrs` (may be NULL): world addresses, a non-NULL
-// entry is used as is (ranks in this process).  Every rank must have exported before any rank attaches.
-extern "C" int gpm_shard_p2p_attach(gpm_ctx* c, const void* handles64, void* const* local_ptrs, int rank, int world)
-{
-    if (!c || world < 2 || world > 8 || rank < 0 || rank >= world) return fail(GPM_E_ARG, "gpm_shard_p2p_attach: bad arguments");
-    if (!c->p2p_region || c->p2p_world != world) return fail(GPM_E_STATE, "gpm_shard_p2p_attach: call gpm_shard_p2p_export(ctx, world, ...) first");
-    DeviceGuard g(c->device);
-    for (int r = 0; r < world; r++) {
-        if (c->p2p_ipc_opened[r] && c->p2p_peer[r]) cudaIpcCloseMemHandle(c->p2p_peer[r]);
-        c->p2p_peer[r] = nullptr;  c->p2p_ipc_opened[r] = false;
-        if (r == rank) { c->p2p_peer[r] = c->p2p_region;  continue; }
-        if (local_ptrs && local_ptrs[r]) { c->p2p_peer[r] = local_ptrs[r];  continue; }
-        if (!handles64) return fail(GPM_E_ARG, "gpm_shard_p2p_attach: no handle for a peer");
-        cudaIpcMemHandle_t h;
-        memcpy(&h, (const char*)handles64 + 64 * (size_t)r, 64);
-        void* ptr = nullptr;
-        CU(cudaIpcOpenMemHandle(&ptr, h, cudaIpcMemLazyEnablePeerAccess));
-        c->p2p_peer[r] = ptr;  c->p2p_ipc_opened[r] = true;
-    }
-    c->shard_rank = rank;  c->shard_world = world;  c->p2p_attached = true;
-    return GPM_OK;
-}
-
-static int shard_launch_fused(gpm_ctx* c, const KParams& P, int colour, int init_phase, int exchanges)
-{
-    const int last = 1 + shard_refine_steps(c->prm);
-    ShardState S{c->dispbuf, c->candbuf, c->canddepth, c->sflags};
-    ShardP2P X;
-    memset(&X, 0, sizeof(X));
-    for (int r = 0; r < c->shard_world; r++) {
-        X.flags[r] = reinterpret_cast<unsigned*>(c->p2p_peer[r]);
-        X.lists[r] = reinterpret_cast<float*>(reinterpret_cast<char*>(c->p2p_peer[r]) + c->p2p_flag_bytes);
-    }
-    X.err = reinterpret_cast<unsigned*>(c->d_stats + 7);
-    X.slot_floats = c->p2p_slot_floats;  X.me = c->shard_rank;  X.world = c->shard_world;  X.nblocks = c->p2p_nblocks;
-    (P.color ? k_shard_fused<true> : k_shard_fused<false>)<<<tile_grid(c), P.nwarps * 32, block_smem_bytes(P), c->stream>>>(P, c->tmap, c->d_cams,
-        P.color ? c->srcTex4 : c->srcTex, c->planes, c->cost, c->prov, S, Memo{c->pid, c->seen, c->refseen, c->memo_mask, c->next_id}, colour, init_phase, last,
-        X, c->p2p_seq, c->opt_stats ? c->d_stats : nullptr);
-    c->launches++;
-    c->p2p_seq += (unsigned)exchanges;
-    c->collectives += (unsigned long long)exchanges;
-    CU(cudaGetLastError());
-    return GPM_OK;
-}
-
 // runcuda() with the source views sharded over the ranks of the attached communicator.  Every rank calls it with the same
 // parameters, reference image and seed and ITS views; all work — kernels and collectives — is enqueued on the context's
 // stream, one host synchronisation at the end.
@@ -1108,46 +1013,18 @@ extern "C" int gpm_shard_run(gpm_ctx* c, float* sweep_ms)
     const int world = c->shard_world, last = 1 + shard_refine_steps(c->prm);
     CU(cudaMemsetAsync(c->d_stats, 0, 8 * sizeof(unsigned long long), c->stream));
     c->launches = 0;  c->collectives = 0;
-    if (world > 1 && c->p2p_attached && c->opt_exchange == 1) {
-        // fused flow: one launch for the initial costs, one per colour pass; the exchange happens inside the kernels
-        rc = init_planes(c, P0);
-        if (rc) return rc;
-        rc = shard_launch_fused(c, P0, 0, 1, 1);
-        if (rc) return rc;
-        CU(cudaMemsetAsync(c->memo_mask, 0, (size_t)c->W * c->H * sizeof(unsigned), c->stream));
-        CU(cudaEventRecord(c->ev0, c->stream));
-        for (int it = 0; it < c->prm.iterations; it++)
-            for (int colour = 0; colour < 2; colour++) {
-                rc = shard_launch_fused(c, P, colour, 0, last);
-                if (rc) return rc;
-            }
-        rc = do_finalize(c);
-        if (rc) return rc;
-        CU(cudaEventRecord(c->ev1, c->stream));
-        CU(cudaEventSynchronize(c->ev1));
-        float ms = 0.f;
-        CU(cudaEventElapsedTime(&ms, c->ev0, c->ev1));
-        if (sweep_ms) *sweep_ms = ms;
-        unsigned long long err = 0;
-        CU(cudaMemcpyAsync(&err, c->d_stats + 7, sizeof(err), cudaMemcpyDeviceToHost, c->stream));
-        CU(cudaStreamSynchronize(c->stream));
-        if (err & 0xffffffffull) return fail(GPM_E_STATE, "gpm_shard_run: a peer rank did not deliver its lists in time (peer-memory exchange)");
-        return GPM_OK;
-    }
-    if (world > 1 && !c->comm) return fail(GPM_E_STATE, "gpm_shard_run: neither an NCCL communicator nor peer regions are attached");
-    {
-        rc = init_planes(c, P0);
-        if (rc) return rc;
-        CU(cudaMemsetAsync(c->memo_mask, 0, (size_t)c->W * c->H * sizeof(unsigned), c->stream));
-        rc = shard_launch_stage(c, P0, 0, 0, nullptr, world, c->xchg);
-        if (rc) return rc;
-        rc = shard_exchange(c, 0);
-        if (rc) return rc;
-        dim3 b2(32, 8), gr2(((P0.W + 1) / 2 + 31) / 32, (P0.H + 7) / 8);
-        k_shard_accept0<<<gr2, b2, 0, c->stream>>>(P0, c->cost, c->prov, c->gath, world);
-        c->launches++;
-        CU(cudaGetLastError());
-    }
+    if (world > 1 && !c->comm) return fail(GPM_E_STATE, "gpm_shard_run: no NCCL communicator is attached");
+    rc = init_planes(c, P0);
+    if (rc) return rc;
+    CU(cudaMemsetAsync(c->memo_mask, 0, (size_t)c->W * c->H * sizeof(unsigned), c->stream));
+    rc = shard_launch_stage(c, P0, 0, 0, nullptr, world, c->xchg);
+    if (rc) return rc;
+    rc = shard_exchange(c, 0);
+    if (rc) return rc;
+    dim3 b2(32, 8), gr2(((P0.W + 1) / 2 + 31) / 32, (P0.H + 7) / 8);
+    k_shard_accept0<<<gr2, b2, 0, c->stream>>>(P0, c->cost, c->prov, c->gath, world);
+    c->launches++;
+    CU(cudaGetLastError());
     CU(cudaEventRecord(c->ev0, c->stream));
     for (int it = 0; it < c->prm.iterations; it++)
         for (int colour = 0; colour < 2; colour++) {
@@ -1192,7 +1069,7 @@ extern "C" int gpm_measure_fetch_peak(gpm_ctx* c, double* gfetch_per_s)
     if (!c || !gfetch_per_s) return fail(GPM_E_ARG, "gpm_measure_fetch_peak: null argument");
     if (c->V < 1 || c->color < 0) return fail(GPM_E_STATE, "gpm_measure_fetch_peak: no source views");
     DeviceGuard g(c->device);
-    float* sink = reinterpret_cast<float*>(c->d_stats + 7);
+    float* sink = reinterpret_cast<float*>(c->d_stats + 7);         // d_stats[7] holds no counter: it is only k_fetch_peak's sink
     const int blocks = c->num_sms * 16, threads = 256, reps = 2048;
     const cudaTextureObject_t tex = c->color == 1 ? c->srcTex4 : c->srcTex;      // colour: three R32F channel planes per view
     const int layers = c->color == 1 ? 3 * c->V : c->V;
@@ -1268,7 +1145,6 @@ extern "C" int gpm_set_option(gpm_ctx* c, const char* name, int value)
     }
     else if (n == "memo") c->opt_memo = value != 0;
     else if (n == "quadperm") c->opt_quadperm = value != 0;
-    else if (n == "exchange") c->opt_exchange = value != 0;
     else if (n == "async_upload") c->opt_async_upload = value != 0;
     else if (n == "shard_async") c->opt_shard_async = value != 0;
     else return fail(GPM_E_ARG, "gpm_set_option: unknown option '" + n + "'");

@@ -188,6 +188,30 @@ __device__ const signed char kFusedGx1[20] = { 0,  0,  0, 0, 0, 0,  0,  0,  0, 1
 __device__ const signed char kFusedGy0[20] = { 1,  3,  5, 0, 0, 0,  0,  0,  0, 0, 0, 0,  1, 0,  1,  0,  3,  3,  0, 0};
 __device__ const signed char kFusedGy1[20] = { 0,  0,  0, 1, 3, 5,  0,  0,  0, 0, 0, 0,  0, 1,  0,  1,  0,  0,  2, 2};
 
+// Pixel of checkerboard colour `colour` at index idx (0..511) of this block's tile — gipuma.cu:1730-1734 / 1786-1790.
+__device__ __forceinline__ void colour_pixel(int idx, int colour, int& px, int& py)
+{
+    const int tx = idx & 31, ty = idx >> 5;
+    px = blockIdx.x * GPM_TILE + tx;
+    py = blockIdx.y * GPM_TILE + 2 * ty + (((tx & 1) ^ colour) & 1);
+}
+
+// Candidate k of the 8-neighbour sweep: 0..3 = up, down, left, right at 1 px (gipuma.cu:1571-1582), 4..7 the same at 5 px
+// (:1450-1462).  (qx, qy) is the neighbour; the result is the reference's border guard (false: the candidate is not offered).
+// px and py are taken by reference only so that k_sweep compiles to the same instructions as with the guard written inline:
+// by value, the compiler canonicalises `py < H - dist` to `H - dist > py` before inlining.
+__device__ __forceinline__ bool close_far_neighbour(int k, const int& px, const int& py, int W, int H, int& qx, int& qy)
+{
+    const int dist = k < 4 ? 1 : 5, dir = k & 3;
+    qx = px;  qy = py;
+    bool ok;
+    if (dir == 0)      { ok = py > dist - 1;  qy = py - dist; }
+    else if (dir == 1) { ok = py < H - dist;  qy = py + dist; }
+    else if (dir == 2) { ok = px > dist - 1;  qx = px - dist; }
+    else               { ok = px < W - dist;  qx = px + dist; }
+    return ok;
+}
+
 template <bool COLOR, bool FUSED>
 __global__ void __launch_bounds__(GPM_LB_THREADS, GPM_LB_BLOCKS)
 k_sweep(const __grid_constant__ KParams P, const __grid_constant__ CUtensorMap tmap, const ViewCam* __restrict__ cams,
@@ -217,10 +241,8 @@ k_sweep(const __grid_constant__ KParams P, const __grid_constant__ CUtensorMap t
     const int idx_end = min(GPM_TILE * GPM_TILE / 2, idx_begin + per_slice);
     int idx = idx_begin + (int)warp;
     while (idx < idx_end) {
-        // pixel of this colour — gipuma.cu:1730-1734 / 1786-1790
-        const int tx = idx & 31, ty = idx >> 5;
-        const int px = blockIdx.x * GPM_TILE + tx;
-        const int py = blockIdx.y * GPM_TILE + 2 * ty + (((tx & 1) ^ colour) & 1);
+        int px, py;
+        colour_pixel(idx, colour, px, py);
         if (px < W && py < H) {
             const size_t center = (size_t)py * W + px;
             bool window_ready = false;          // the per-pixel window data is only built if something gets evaluated
@@ -244,15 +266,9 @@ k_sweep(const __grid_constant__ KParams P, const __grid_constant__ CUtensorMap t
                     mine_at = (size_t)(py + kFusedDy[lane]) * W + (px + kFusedDx[lane]);
                 }
             } else if (lane < 8) {
-                const int dist = lane < 4 ? 1 : 5;
-                const int dir = lane & 3;
                 const bool phase_on = (phase_mask >> (lane >> 2)) & 1;
-                int qx = px, qy = py;
-                bool ok;
-                if (dir == 0)      { ok = py > dist - 1;      qy = py - dist; }
-                else if (dir == 1) { ok = py < H - dist;      qy = py + dist; }
-                else if (dir == 2) { ok = px > dist - 1;      qx = px - dist; }
-                else               { ok = px < W - dist;      qx = px + dist; }
+                int qx, qy;
+                const bool ok = close_far_neighbour((int)lane, px, py, W, H, qx, qy);
                 mine_ok = ok && phase_on;
                 mine_at = (size_t)qy * W + qx;
             }
@@ -394,10 +410,10 @@ k_sweep(const __grid_constant__ KParams P, const __grid_constant__ CUtensorMap t
 // Every rank holds the full plane/cost state and a SUBSET of the source views.  Per-view costs are independent
 // (gipuma.cu:742-778); only the combination needs all views.  For COMB_BEST_N the n_best smallest costs over all views
 // are the n_best smallest of the union of every rank's n_best smallest, so each rank exports, per pixel and hypothesis
-// slot, its ascending local top-n_best; the lists of all ranks are exchanged (NCCL all-gather, or peer stores over NVLink
-// in the fused kernel below) and every rank merges them, sums in ascending order — the reference's order
-// (gipuma.cu:779-797) — and applies the accept logic redundantly.  All ranks therefore keep bit-identical state,
-// identical to a single-GPU run over all views.
+// slot, its ascending local top-n_best; the lists of all ranks are exchanged (an all-gather between two launches of
+// k_shard_stage) and every rank merges them, sums in ascending order — the reference's order (gipuma.cu:779-797) — and
+// applies the accept logic redundantly.  All ranks therefore keep bit-identical state, identical to a single-GPU run over
+// all views.
 //   stage 0        initial cost of the stored planes        (1 slot,  radius box/2, both colours)
 //   stage 1        close + far propagation candidates       (8 slots)
 //   stage 2 + s    refinement step s                         (1 slot; sequential: step s+1 depends on step s' accept)
@@ -405,7 +421,9 @@ k_sweep(const __grid_constant__ KParams P, const __grid_constant__ CUtensorMap t
 // passes plus one closing accept instead of 2 (1 + S) launches.  The exact shortcuts of k_sweep that depend only on the
 // shared state are kept — direction memo, history, duplicates (incl. the current plane), refinement memo — so every rank
 // skips the same work and the skipped slots simply carry +inf lists.
-// Exchange index of pixel (x, y): y * ceil(W/2) + x/2 (pixels of one colour have distinct x/2 within a row).
+// Exchange index of pixel (x, y): y * ceil(W/2) + x/2 (pixels of one colour have distinct x/2 within a row).  A rank's
+// lists of one stage are dense: (stage == 1 ? 8 : 1) slots of n_best floats per exchange index (stage 0: one such plane
+// per colour); the gathered lists are those of every rank, rank-major.
 // ============================================================================================================
 #define GPM_SF_SKIP_REFINE 1u     // sflags: the refinement of this colour pass is known to reject every step (memo)
 #define GPM_SF_ACCEPTED    2u     // sflags: some refinement step of this colour pass was accepted
@@ -415,17 +433,6 @@ struct ShardState {
     float4* candbuf;              // refinement candidate of the step being exchanged
     float* canddepth;
     unsigned char* sflags;
-};
-
-// Peer-memory exchange (k_shard_fused): every rank owns one exchange region = [2 parities][world source ranks][slot_floats]
-// lists + [world][nblocks] arrival flags; all regions are mapped into every rank's address space (CUDA IPC over NVLink).
-// A rank writes its lists straight into slot `me` of every peer's region and then raises flag [me][block] there.
-struct ShardP2P {
-    float* lists[8];              // list area of rank r's region as mapped here (lists[me] is local memory)
-    unsigned* flags[8];           // flag area of rank r's region
-    unsigned* err;                // local sticky error word (a peer did not arrive in time)
-    unsigned long long slot_floats;
-    int me, world, nblocks;
 };
 
 // merged cost of one slot: the n_best smallest over all ranks' lists, summed ascending, / count  (gipuma.cu:779-803).
@@ -462,7 +469,9 @@ __device__ __forceinline__ bool same_bits(const float4& a, const float4& b)
 }
 
 // refinement candidate of step `sidx` from (norm_now, disp_now) — getRndDispAndUnitVector_cu, gipuma.cu:890-927, with the
-// reference's zero-state stream (pin P2) advanced by 4 draws per earlier step
+// reference's zero-state stream (pin P2) advanced by 4 draws per earlier step.  The step restates k_sweep's refinement loop
+// body line for line, and a fix to one must go to both: k_sweep keeps its own copy because calling a shared helper there
+// changes the register allocation of its colour instantiations.
 __device__ __forceinline__ float4 shard_refine_candidate(const KParams& P, const float4& norm_now, float disp_now, float fpx, float fpy,
                                                          int sidx, float& depth_new)
 {
@@ -496,17 +505,14 @@ __device__ __forceinline__ float4 shard_refine_candidate(const KParams& P, const
 // stage 1: the 8 propagation slots in the reference's order (gipuma.cu:1571-1582, 1450-1462; accept rule :867-871);
 // stage >= 2: one refinement step (:986-990).
 __device__ __forceinline__ void shard_accept_pixel(const KParams& P, const float4* __restrict__ planes, const ShardState& S, const Memo& M,
-                                                   int px, int py, int stage, const float* __restrict__ gathered, int world, size_t rank_stride,
+                                                   int px, int py, int stage, const float* __restrict__ gathered, int world,
                                                    float4& norm_now, float& cost_now, float& disp_now, int& prov_now, unsigned& sf,
                                                    unsigned& own_id, unsigned lane)
 {
     const int W = P.W, H = P.H, Wh = (W + 1) >> 1, nb = P.n_best;
     const size_t center = (size_t)py * W + px;
-    // list layout: NCCL flow — dense per stage (8 slots per pixel in stage 1, 1 otherwise); fused flow (rank_stride != 0) — a
-    // fixed 8 slots per pixel in every stage, so that a pixel's lists only ever alias lists of the same pixel, i.e. of the
-    // same block (blocks of one launch run stages apart from each other; only same-index blocks are ordered by the flags)
-    const int slots = (stage == 1 || rank_stride) ? 8 : 1;
-    const size_t per_rank = rank_stride ? rank_stride : (size_t)H * Wh * slots * nb;
+    const int slots = stage == 1 ? 8 : 1;
+    const size_t per_rank = (size_t)H * Wh * slots * nb;
     const float* g = gathered + ((size_t)py * Wh + (px >> 1)) * slots * nb;
     const float fpx = __int2float_rn(px), fpy = __int2float_rn(py);
     if (stage == 1) {
@@ -515,8 +521,8 @@ __device__ __forceinline__ void shard_accept_pixel(const KParams& P, const float
         for (int k = 0; k < 8; k++) {
             const float c = __shfl_sync(GPM_FULL, mine, k);
             if (c < cost_now) {
-                const int dist = k < 4 ? 1 : 5, dir = k & 3;
-                const int qx = px + (dir == 2 ? -dist : dir == 3 ? dist : 0), qy = py + (dir == 0 ? -dist : dir == 1 ? dist : 0);
+                int qx, qy;
+                close_far_neighbour(k, px, py, W, H, qx, qy);       // offered, so inside the border guard
                 norm_now = planes[(size_t)qy * W + qx];                 // other colour: not written during this colour's stages
                 own_id = M.pid[(size_t)qy * W + qx];                    // a copy keeps its identity
                 disp_now = plane_depth(P.ref, norm_now.x, norm_now.y, norm_now.z, norm_now.w, fpx, fpy);
@@ -539,21 +545,8 @@ __device__ __forceinline__ void shard_stage_pixel(const KParams& P, const float*
                                                   const WarpScratch& ws, cudaTextureObject_t src, float4* __restrict__ planes, float* __restrict__ cost, unsigned char* __restrict__ prov,
                                                   const ShardState& S, const Memo& M, int px, int py, int tile_x0, int tile_y0,
                                                   int stage, int last_stage, const float* __restrict__ gathered_prev, int world,
-                                                  float* __restrict__ xchg, unsigned lane, WarpStats& st,
-                                                  size_t rank_stride = 0, const ShardP2P* X = nullptr, size_t slot_off = 0)
+                                                  float* __restrict__ xchg, unsigned lane, WarpStats& st)
 {
-    // fused exchange: copy this pixel's finished lists (count floats at `o`, just written to the local slot) into slot `me` of
-    // every peer's region — plain stores over NVLink; the block raises the arrival flags after its last pixel
-    auto publish = [&](const float* o, int count) {
-        if (!X) return;
-        __syncwarp();
-        const size_t off = slot_off + (size_t)(o - xchg);
-        for (int i = (int)lane; i < count; i += 32) {
-            const float v = o[i];
-            for (int d = 0; d < X->world; d++)
-                if (d != X->me) X->lists[d][off + i] = v;
-        }
-    };
     const RefCam& cam = P.ref;
     const int W = P.W, H = P.H, Wh = (W + 1) >> 1, nb = P.n_best;
     const size_t center = (size_t)py * W + px;
@@ -566,7 +559,6 @@ __device__ __forceinline__ void shard_stage_pixel(const KParams& P, const float*
         setup_window<COLOR>(P, tile + P.tile_xo, ws, px, py, tile_x0, tile_y0, lane);
         eval_plane<(COLOR ? 1 : 0), COLOR>(P, sCam, ws, src, norm_now.x, norm_now.y, norm_now.z, norm_now.w, inf, lane, st, &c0, &c1);
         local_topn(P, c0, c1, lane, out);
-        publish(out, nb);
         return;
     }
     float cost_now = cost[center];
@@ -577,7 +569,7 @@ __device__ __forceinline__ void shard_stage_pixel(const KParams& P, const float*
     unsigned new_mask = mmask;
     unsigned own_id = M.pid[center];
     if (stage >= 2) {
-        shard_accept_pixel(P, planes, S, M, px, py, stage - 1, gathered_prev, world, rank_stride, norm_now, cost_now, disp_now, prov_now, sf, own_id, lane);
+        shard_accept_pixel(P, planes, S, M, px, py, stage - 1, gathered_prev, world, norm_now, cost_now, disp_now, prov_now, sf, own_id, lane);
         if (stage == 2) {
             // refinement memo (see k_sweep): the S candidates are a pure function of (pixel, plane at refinement start)
             sf = 0u;
@@ -587,7 +579,7 @@ __device__ __forceinline__ void shard_stage_pixel(const KParams& P, const float*
             }
         }
     }
-    float* out = xchg + ((size_t)py * Wh + (px >> 1)) * ((stage == 1 || rank_stride) ? 8 : 1) * nb;      // see shard_accept_pixel
+    float* out = xchg + ((size_t)py * Wh + (px >> 1)) * (stage == 1 ? 8 : 1) * nb;
     if (stage > last_stage) {                               // closing pass of a colour: only the accept of the last refinement step
         if (P.memo && P.rng_mode == 0 && !(sf & (GPM_SF_SKIP_REFINE | GPM_SF_ACCEPTED))) new_mask |= GPM_MEMO_REFINE;
         if (sf & GPM_SF_ACCEPTED) {                         // the refinement created a new plane: one fresh identity
@@ -600,14 +592,8 @@ __device__ __forceinline__ void shard_stage_pixel(const KParams& P, const float*
         bool mine_ok = false;
         size_t mine_at = center;
         if (lane < 8) {
-            const int dist = lane < 4 ? 1 : 5, dir = lane & 3;
-            int qx = px, qy = py;
-            bool ok;
-            if (dir == 0)      { ok = py > dist - 1;  qy = py - dist; }
-            else if (dir == 1) { ok = py < H - dist;  qy = py + dist; }
-            else if (dir == 2) { ok = px > dist - 1;  qx = px - dist; }
-            else               { ok = px < W - dist;  qx = px + dist; }
-            mine_ok = ok;
+            int qx, qy;
+            mine_ok = close_far_neighbour((int)lane, px, py, W, H, qx, qy);
             mine_at = (size_t)qy * W + qx;
         }
         const unsigned mine_id = mine_ok ? M.pid[mine_at] : 0u;
@@ -641,7 +627,6 @@ __device__ __forceinline__ void shard_stage_pixel(const KParams& P, const float*
         }
         if (P.memo && mine_ok && !memo_hit) M.seen[center * 8 + lane] = mine_id;
         new_mask |= (cand_mask & 0xffu);
-        publish(out, 8 * nb);
     } else {
         if (sf & GPM_SF_SKIP_REFINE) {
             st.skip++;
@@ -654,7 +639,6 @@ __device__ __forceinline__ void shard_stage_pixel(const KParams& P, const float*
             eval_plane<0, COLOR>(P, sCam, ws, src, cand.x, cand.y, cand.z, cand.w, inf, lane, st, &c0, &c1);
             local_topn(P, c0, c1, lane, out);
         }
-        publish(out, nb);
     }
     if (lane == 0) {
         if (stage >= 2) { planes[center] = norm_now;  cost[center] = cost_now;  prov[center] = (unsigned char)prov_now;  M.pid[center] = own_id; }
@@ -663,7 +647,7 @@ __device__ __forceinline__ void shard_stage_pixel(const KParams& P, const float*
     }
 }
 
-// One exchange stage over the whole image (NCCL flow: the all-gather runs between two launches of this kernel).
+// One exchange stage over the whole image (the all-gather runs between two launches of this kernel).
 // stage 0: both colours; 1 .. last_stage: one colour; last_stage + 1: closing accept of the colour.
 template <bool COLOR>
 __global__ void __launch_bounds__(GPM_LB_THREADS, GPM_LB_BLOCKS)
@@ -689,106 +673,10 @@ k_shard_stage(const __grid_constant__ KParams P, const __grid_constant__ CUtenso
     for (int idx = (int)blockIdx.z * per_slice + (int)warp; idx < idx_end; idx += P.nwarps) {
         int px, py;
         if (stage == 0) { px = blockIdx.x * GPM_TILE + (idx & 31);  py = blockIdx.y * GPM_TILE + (idx >> 5); }
-        else { const int tx = idx & 31, ty = idx >> 5;  px = blockIdx.x * GPM_TILE + tx;  py = blockIdx.y * GPM_TILE + 2 * ty + (((tx & 1) ^ colour) & 1); }
+        else colour_pixel(idx, colour, px, py);
         if (px >= P.W || py >= P.H) continue;
         shard_stage_pixel<COLOR>(P, sCam, tile, ws, src, planes, cost, prov, S, M, px, py,
                                  tile_x0, tile_y0, stage, last_stage, gathered_prev, world, xchg, lane, st);
-    }
-    flush_stats(stats, st, lane);
-}
-
-// ---- fused compute + exchange over peer memory (NVLink / NVSwitch) ---------------------------------------------------
-// Polling load: relaxed, system scope (served by L2, the point of coherence for peer stores into this GPU's memory).  The
-// acquire is ONE fence after the poll succeeds: an acquiring load (or a system-scope fence) invalidates the SM's whole L1 —
-// the texture cache of every resident block — so it must not sit inside the spin loop.
-__device__ __forceinline__ unsigned ld_relaxed_sys(const unsigned* p)
-{
-    unsigned v;
-    asm volatile("ld.relaxed.sys.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
-    return v;
-}
-__device__ __forceinline__ void fence_acquire_sys() { asm volatile("fence.acq_rel.sys;" ::: "memory"); }
-__device__ __forceinline__ void st_release_sys(unsigned* p, unsigned v)
-{
-    asm volatile("st.release.sys.global.u32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
-}
-// wait until every peer has delivered its lists of exchange `seq` for this block (one spinning thread per peer)
-__device__ __forceinline__ void p2p_wait(const ShardP2P& X, unsigned bid, unsigned seq)
-{
-    if ((int)threadIdx.x < X.world && (int)threadIdx.x != X.me) {
-        const unsigned* f = X.flags[X.me] + (size_t)threadIdx.x * X.nblocks + bid;
-        const long long t0 = clock64();
-        while ((int)(ld_relaxed_sys(f) - seq) < 0) {
-            if (*(volatile unsigned*)X.err) break;
-            if (clock64() - t0 > (1LL << 33)) { atomicExch(X.err, 1u);  break; }      // ~4 s: fail loudly on the host, never hang
-            __nanosleep(200);
-        }
-        fence_acquire_sys();
-    }
-    __syncthreads();
-}
-// all lists of this block are stored: make them visible system-wide, then raise flag [me][bid] = seq at every peer
-__device__ __forceinline__ void p2p_signal(const ShardP2P& X, unsigned bid, unsigned seq)
-{
-    __syncthreads();
-    if ((int)threadIdx.x < X.world && (int)threadIdx.x != X.me) {
-        __threadfence_system();
-        st_release_sys(X.flags[threadIdx.x] + (size_t)X.me * X.nblocks + bid, seq);
-    }
-}
-
-// One whole colour pass (all 1 + S exchange stages and the closing accept) — or, with init_phase, the initial-cost stage and
-// its accept — of one tile slice per block, the exchange fused in: after every stage the block's lists are already in every
-// peer's memory (stored there pixel by pixel while the block was still sampling) and only the arrival flags remain to be
-// raised; before the next stage the block waits for the same block of every peer — never for another block of its own GPU,
-// so blocks need not be co-resident and the transfer of one tile overlaps the sampling of all the others.  The reference
-// window is staged once per colour instead of once per stage.  `seq0` = number of exchanges completed before this launch.
-template <bool COLOR>
-__global__ void __launch_bounds__(GPM_LB_THREADS, GPM_LB_BLOCKS)
-k_shard_fused(const __grid_constant__ KParams P, const __grid_constant__ CUtensorMap tmap, const ViewCam* __restrict__ cams,
-              cudaTextureObject_t src, float4* __restrict__ planes, float* __restrict__ cost, unsigned char* __restrict__ prov, ShardState S, Memo M, int colour, int init_phase, int last_stage,
-              const __grid_constant__ ShardP2P X, unsigned seq0, unsigned long long* __restrict__ stats)
-{
-    extern __shared__ __align__(128) float smem[];
-    float* tile = smem;
-    float* sCam = tile + tile_floats(P);
-    float* scratch = smem + fixed_smem_floats(P);
-    const unsigned lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    const int tile_x0 = blockIdx.x * GPM_TILE - P.halo, tile_y0 = blockIdx.y * GPM_TILE - P.halo;
-    const unsigned bid = (blockIdx.z * gridDim.y + blockIdx.y) * gridDim.x + blockIdx.x;
-    stage_block(P, &tmap, cams, tile, sCam, tile_x0, tile_y0);
-    const WarpScratch ws = carve(scratch + (size_t)warp * warp_scratch_floats(P.ns_pad, P.V, P.color), P.ns_pad, P.V, P.color, block_perm(P, smem));
-    WarpStats st = {0, 0, 0, 0, 0};
-    const int W = P.W, H = P.H, Wh = (W + 1) >> 1, nb = P.n_best;
-    const int npix = init_phase ? GPM_TILE * GPM_TILE : GPM_TILE * GPM_TILE / 2;
-    const int per_slice = (npix + (int)gridDim.z - 1) / (int)gridDim.z;
-    const int idx0 = (int)blockIdx.z * per_slice, idx_end = min(npix, idx0 + per_slice);
-    const int first = init_phase ? 0 : 1, lastS = init_phase ? 0 : last_stage;
-    const size_t slot = (size_t)X.slot_floats;
-    for (int stage = first; stage <= lastS + 1; stage++) {
-        const bool closing = stage > lastS;
-        const unsigned seq = seq0 + (unsigned)(stage - first) + 1u;          // exchange produced by `stage`
-        if (stage > first) p2p_wait(X, bid, seq - 1u);
-        const float* prev = X.lists[X.me] + (size_t)((seq - 1u) & 1u) * X.world * slot;
-        const size_t slot_off = ((size_t)(seq & 1u) * X.world + X.me) * slot;
-        float* outb = X.lists[X.me] + slot_off;
-        for (int idx = idx0 + (int)warp; idx < idx_end; idx += P.nwarps) {
-            int px, py;
-            if (init_phase) { px = blockIdx.x * GPM_TILE + (idx & 31);  py = blockIdx.y * GPM_TILE + (idx >> 5); }
-            else { const int tx = idx & 31, ty = idx >> 5;  px = blockIdx.x * GPM_TILE + tx;  py = blockIdx.y * GPM_TILE + 2 * ty + (((tx & 1) ^ colour) & 1); }
-            if (px >= W || py >= H) continue;
-            if (init_phase && closing) {                                      // merged initial cost (gipuma.cu:1040-1049 over all views)
-                if (lane == 0) {
-                    const float* g = prev + ((size_t)((px + py) & 1) * H * Wh + (size_t)py * Wh + (px >> 1)) * nb;
-                    cost[(size_t)py * W + px] = shard_merge(g, slot, X.world, nb);
-                    prov[(size_t)py * W + px] = P.color ? 3 : 0;
-                }
-                continue;
-            }
-            shard_stage_pixel<COLOR>(P, sCam, tile, ws, src, planes, cost, prov, S, M, px, py,
-                                     tile_x0, tile_y0, stage, lastS, prev, X.world, outb, lane, st, slot, &X, slot_off);
-        }
-        if (!closing) p2p_signal(X, bid, seq);
     }
     flush_stats(stats, st, lane);
 }

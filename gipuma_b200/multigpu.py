@@ -107,10 +107,12 @@ def hybrid_layout(world: int, shard: int):
 def run_hybrid(make_scene: Callable[[int], object], n_reference_views: int, rank: int, world: int, shard: int,
                device: int = 0, on_result: Optional[Callable] = None, exchange: str = "nccl") -> List[float]:
     """Reference views are dealt round-robin to world/shard groups; inside a group the source views are sharded and
-    combined with one all-gather per stage over the group's own communicator.  Returns wall seconds per reference view."""
+    combined with one all-gather per stage over the group's own communicator (`exchange` must be "nccl").  Returns wall
+    seconds per reference view."""
     import time
     import torch
     import torch.distributed as dist
+    _check_exchange(exchange)
     group_of, rank_in, members = hybrid_layout(world, shard)
     groups = [dist.new_group(ranks=m) if world > 1 else None for m in members]     # every rank creates every group
     my_group = group_of[rank]
@@ -133,15 +135,23 @@ def run_hybrid(make_scene: Callable[[int], object], n_reference_views: int, rank
 # source-view shard
 # ----------------------------------------------------------------------------------------------------------------
 
+def _check_exchange(exchange: str):
+    if exchange == "p2p":
+        raise ValueError('exchange="p2p": the fused peer-memory exchange was removed (DESIGN.md §8); use exchange="nccl"')
+    if exchange != "nccl":
+        raise ValueError(f"unknown exchange {exchange!r}: the source-view shard exchanges with NCCL only")
+
+
 class ViewShardRunner:
     """One reference view, source views sharded over `world` ranks.  All device work runs behind the C-ABI
-    (gpm_shard_run): with exchange="nccl" (default, measured fastest) one stage kernel + ncclAllGather per exchange stage;
-    with exchange="p2p" one fused kernel per colour pass that stores the lists into the peers' memory over NVLink as it samples.
-    torch.distributed is only used at set-up, to pass the NCCL unique id and the CUDA IPC handles around."""
+    (gpm_shard_run): one stage kernel + ncclAllGather per exchange stage.  `exchange` must be "nccl"; the attribute of
+    the same name is "nccl", or "none" for a single rank.  torch.distributed is only used at set-up, to pass the NCCL
+    unique id around."""
 
     def __init__(self, scene, rank: int, world: int, device: int = 0, seed: int = 0xC0FFEE, group=None, options=None,
                  exchange: str = "nccl"):
         from . import api
+        _check_exchange(exchange)
         self.scene, self.rank, self.world, self.group = scene, rank, world, group
         self.local = partition_views(scene.n_views, world)[rank]
         if not self.local:
@@ -162,15 +172,6 @@ class ViewShardRunner:
             uid = box[0]
         ctx.shard_comm_init(uid, rank, world)
         self.exchange = exchange if world > 1 else "none"
-        if world > 1 and exchange == "p2p":
-            # fused compute + exchange over peer memory: swap the CUDA IPC handles of the ranks' exchange regions
-            import torch.distributed as dist
-            handle, _ = ctx.shard_p2p_export(world)
-            handles = [None] * world
-            dist.all_gather_object(handles, handle, group=group)
-            ctx.shard_p2p_attach(handles, rank, world)
-        elif world > 1:
-            ctx.set_option("exchange", 0)
         self.collectives = 0
 
     def upload(self, scene, images=None):

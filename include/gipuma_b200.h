@@ -151,13 +151,6 @@ int gpm_shard_unique_id(void* id128);
 int gpm_shard_comm_init(gpm_ctx* ctx, const void* id128, int rank, int world);
 int gpm_shard_comm_attach(gpm_ctx* ctx, void* nccl_comm, int rank, int world);
 int gpm_shard_run(gpm_ctx* ctx, float* sweep_ms);
-/* Fused compute + exchange over peer memory (NVLink / NVSwitch), what gpm_shard_run uses once regions are attached: every rank
- * exports one exchange region (CUDA IPC handle, 64 bytes; `local_ptr` for ranks of the same process), the handles of all
- * ranks are handed to gpm_shard_p2p_attach, and from then on one kernel per colour pass stores each pixel's lists directly
- * into the peers' regions while it samples and synchronises tile by tile with arrival flags — no collective launches.
- * Option "exchange" = 0 falls back to the NCCL all-gather flow. */
-int gpm_shard_p2p_export(gpm_ctx* ctx, int world, void* handle64, void** local_ptr);
-int gpm_shard_p2p_attach(gpm_ctx* ctx, const void* handles64, void* const* local_ptrs, int rank, int world);
 
 /* Counters of the last gpm_sweep/gpm_run: [0] kernels launched, [1] hypotheses offered,
  * [2] hypotheses skipped as exact duplicates / out of depth range, [3] hypotheses cut short by the
@@ -180,7 +173,6 @@ int gpm_measure_fetch_peak(gpm_ctx* ctx, double* gfetch_per_s);
  * all six sweep kernels), bit 1 = float4 gradient folding (float4 initialisation = 3); auto = the propagation kernels' form;
  * "shard_async" (0): 1 makes gpm_shard_stage / gpm_shard_finish_init return after enqueueing on gpm_stream() — run the
  * collective on that stream (or order it with events) instead of paying a host synchronisation per stage;
- * "exchange" (1): view shard over peer memory when regions are attached, 0 = NCCL all-gather per stage;
  * "async_upload" (0): 1 lets gpm_set_reference / gpm_set_view return without a host synchronisation — the caller keeps its
  * (page-locked) image buffers unchanged until the next gpm_run / gpm_sweep returns;
  * "quadperm" (1): deal the samples of a round to the lanes as 2x2 blocks per hardware quad (texture-unit locality);

@@ -88,25 +88,6 @@ def _sharded_run(sc, world, seed=0xC0FFEE):
     return outs
 
 
-def run_concurrently(ctxs, timeout=120):
-    """gpm_shard_run on every rank at once, one thread per rank (with the peer-memory exchange each rank waits for the
-    others); returns the exceptions raised."""
-    import threading
-    errs = []
-
-    def work(ctx):
-        try:
-            ctx.shard_run()
-        except Exception as e:      # noqa: BLE001
-            errs.append(e)
-    threads = [threading.Thread(target=work, args=(ctx,)) for ctx in ctxs]
-    for t in threads:
-        t.start()
-    for t in threads:
-        t.join(timeout=timeout)
-    return errs
-
-
 @pytest.mark.parametrize("cfg,rows,cols,views,world,box,nbest", [
     (2, 64, 96, 6, 1, 15, 3),          # degenerate: one rank holds every view
     (2, 64, 96, 6, 2, 15, 3),
@@ -158,29 +139,3 @@ def test_view_shard_refuses_other_combinations():
         buf = torch.empty(ctx.shard_stage_floats(1), dtype=torch.float32, device="cuda")
         with pytest.raises(api.GipumaError):
             ctx.shard_stage(0, 1, None, 1, buf)
-
-
-def test_fused_peer_memory_exchange_two_ranks_on_one_gpu():
-    """k_shard_fused (compute + exchange over peer memory) with both ranks living in this process on the same GPU: each rank's
-    kernels store their lists straight into the other rank's exchange region and synchronise tile by tile with arrival flags.
-    The two gpm_shard_run calls must overlap (each waits for the other), hence the threads; the image is small enough for both
-    kernels to be resident at once.  Result: bit-identical to the unsharded run on both ranks, and again on a second run
-    (sequence numbers and parity buffers carry over)."""
-    from gipuma_b200 import api, scene as S
-    sc = S.make_config(2, rows=64, cols=96, n_views=6, iterations=2, seed=558)
-    sc.params.box_hsize = sc.params.box_vsize = 11
-    single, _, _ = api.runcuda(sc, seed=0xC0FFEE)
-    world = 2
-    ctxs = open_ranks(sc, world)
-    exported = [ctx.shard_p2p_export(world) for ctx in ctxs]
-    for r, ctx in enumerate(ctxs):
-        ctx.shard_p2p_attach([h for h, _ in exported], r, world, local_ptrs=[p for _, p in exported])
-    for _ in range(2):
-        errs = run_concurrently(ctxs)
-        assert not errs, errs
-        for ctx in ctxs:
-            n4, c = ctx.get_state()
-            assert bits_equal(n4, single.norm4) == 0 and bits_equal(c, single.c) == 0
-            assert ctx.stats()["collectives"] > 0
-    for ctx in ctxs:
-        ctx.close()

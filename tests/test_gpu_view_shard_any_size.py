@@ -1,6 +1,6 @@
 """The source-view shard checked exactly at ragged and odd image sizes, stage by stage.
 
-The shard runs on kernels of its own (k_shard_stage, k_shard_fused, k_shard_accept0) with their own pixel indexing:
+The shard runs on kernels of its own (k_shard_stage, k_shard_accept0) with their own pixel indexing:
 half-row lists (Wh = ceil(W / 2)), the colour parity, stage 0's two parity planes, 8 * n_best floats per pixel in stage
 1, and their own tile-slice loop and accept.  The ranks are simulated by contexts on one GPU (test_gpu_view_shard's
 SimulatedShard, all-gather = torch.cat), next to one context holding every view, all with the same seed.  After every
@@ -16,9 +16,8 @@ stage:
 - closing accept: the state equals the single context after phase(colour, 4);
 - twin groups without memo and duplicate shortcuts, and with 5 warps per block, stay bit-identical after every colour.
 The cases cover every gridDim.z split (1, 2, 4, 8 on 132 SMs), odd widths, partial tiles, n_best above the views of a
-rank, > 32 views on one rank and world sizes 1 .. 8.  The peer-memory flow (k_shard_fused) runs with all ranks on this
-GPU, adversarial states (ties, out-of-range planes, costs above MAXCOST) go through set_state, and the refusals of the
-stage entry points are checked."""
+rank, > 32 views on one rank and world sizes 1 .. 8.  Adversarial states (ties, out-of-range planes, costs above
+MAXCOST) go through set_state, and the refusals of the stage entry points are checked."""
 import time
 
 import numpy as np
@@ -26,7 +25,7 @@ import pytest
 
 from conftest import bits_equal
 from test_gpu_sweep_any_size import adversarial_state, bands, check_launch, cost_of
-from test_gpu_view_shard import SimulatedShard, open_ranks, run_concurrently
+from test_gpu_view_shard import SimulatedShard, open_ranks
 
 pytestmark = pytest.mark.gpu
 
@@ -290,39 +289,6 @@ def test_view_shard_runner_world1_equals_single_run(case):
     finally:
         run.close()
     assert bits_equal(n4, single.norm4) == 0 and bits_equal(c, single.c) == 0
-
-
-@pytest.mark.parametrize("rows,cols,views,world,colour", [
-    (45, 71, 5, 2, False),
-    (33, 47, 5, 2, True),
-    (37, 41, 40, 3, False),
-])
-def test_fused_peer_memory_exchange_at_odd_sizes(rows, cols, views, world, colour):
-    """k_shard_fused with every rank in this process on this GPU, run twice (sequence numbers and parity buffers carry over):
-    bit-identical to gpm_run on every rank.  A block of one rank waits for the same block of every other rank, so all
-    ranks' grids must be resident at once (one 16-warp block per SM)."""
-    from gipuma_b200 import api
-    sms = sm_count()
-    blocks = world * tiles(rows, cols) * grid_split(rows, cols, sms)
-    if blocks > sms:
-        pytest.skip("%d blocks of %d ranks cannot all be resident on %d SMs" % (blocks, world, sms))
-    sc = make_scene(rows, cols, views, 3, 11, colour, 2)
-    single, _, _ = api.runcuda(sc, seed=SEED)
-    ctxs = open_ranks(sc, world, SEED)
-    try:
-        exported = [ctx.shard_p2p_export(world) for ctx in ctxs]
-        for r, ctx in enumerate(ctxs):
-            ctx.shard_p2p_attach([h for h, _ in exported], r, world, local_ptrs=[p for _, p in exported])
-        for _ in range(2):
-            errs = run_concurrently(ctxs)
-            assert not errs, errs
-            for ctx in ctxs:
-                n4, c = ctx.get_state()
-                assert bits_equal(n4, single.norm4) == 0 and bits_equal(c, single.c) == 0
-                assert ctx.stats()["collectives"] > 0
-    finally:
-        for ctx in ctxs:
-            ctx.close()
 
 
 @pytest.mark.parametrize("case,world", [("53x75", 3), ("colour_45x71", 2)])

@@ -34,19 +34,18 @@ def _torchrun(nproc, script_args, timeout=900):
     return json.loads(lines[-1])
 
 
-@pytest.mark.parametrize("exchange", ["p2p", "nccl"])
+@pytest.mark.parametrize("exchange", ["nccl"])             # the only exchange; kept as a parameter so the case ids stay the same
 @pytest.mark.parametrize("world,args", [
     (2, ["--config", "4", "--rows", "96", "--cols", "128", "--views", "13", "--iters", "2"]),
     (2, ["--config", "2", "--rows", "352", "--cols", "480", "--views", "7", "--iters", "3"]),
     (2, ["--config", "2", "--rows", "353", "--cols", "481", "--views", "7", "--iters", "2"]),     # odd width, partial tiles
 ])
 def test_view_shard_over_real_ranks_equals_single_gpu(world, args, exchange):
-    """exchange = p2p: the fused kernel storing into the peer GPU's memory over NVLink (CUDA IPC); nccl: one ncclAllGather per
-    stage.  Both behind gpm_shard_run."""
+    """One ncclAllGather per exchange stage behind gpm_shard_run."""
     if _gpus() < world:
         pytest.skip("needs %d GPUs" % world)
-    out = _torchrun(world, [os.path.join("tools", "run_shard_nccl.py"), "--exchange", exchange] + args)
-    assert out["world"] == world and out["collectives"] > 0 and out["exchange"] == exchange
+    out = _torchrun(world, [os.path.join("tools", "run_shard_nccl.py")] + args)
+    assert out["world"] == world and out["collectives"] > 0 and out["exchange"] == "nccl"
     assert out["bit_identical_to_single_gpu"] is True
 
 

@@ -142,3 +142,12 @@ def test_bench_sharded_layout_covers_every_view_once():
             assert sorted(views) == list(range(nviews))
     with pytest.raises(SystemExit):
         bench.resolve(argparse.Namespace(mode="hybrid", config=0, shard=3, color=False, neighbours=8, scene="smooth"), 8)
+
+
+def test_view_shard_refuses_the_removed_peer_memory_exchange():
+    """exchange="p2p" fails before any context or process group is touched; "nccl" is the only exchange."""
+    for call in (lambda: M.ViewShardRunner(None, 0, 2, exchange="p2p"), lambda: M.run_hybrid(None, 1, 0, 2, 2, exchange="p2p")):
+        with pytest.raises(ValueError, match="peer-memory exchange was removed"):
+            call()
+    with pytest.raises(ValueError, match="NCCL only"):
+        M.ViewShardRunner(None, 0, 2, exchange="mpi")

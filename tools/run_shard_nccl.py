@@ -16,7 +16,6 @@ ap.add_argument("--views", type=int, default=None)
 ap.add_argument("--iters", type=int, default=None)
 ap.add_argument("--hybrid", type=int, default=0, help="view-shard width; world/width groups take different reference views")
 ap.add_argument("--refs", type=int, default=2)
-ap.add_argument("--exchange", default="nccl", choices=["p2p", "nccl"], help="fused peer-memory exchange or one ncclAllGather per stage")
 ap.add_argument("--repeat", type=int, default=2)
 ap.add_argument("--opt", nargs="*", default=[], help="gpm_set_option name=value pairs for the sharded contexts")
 args = ap.parse_args()
@@ -27,8 +26,7 @@ if world > 1:
 if args.hybrid:
     mk = lambda ref: S.make_config(args.config, rows=args.rows, cols=args.cols, n_views=args.views, iterations=args.iters, seed=1234 + 17 * ref)
     outs = {}
-    times = M.run_hybrid(mk, args.refs, rank, world, args.hybrid, device=local, on_result=lambda ref, n4, c: outs.__setitem__(ref, (n4, c)),
-                         exchange=args.exchange)
+    times = M.run_hybrid(mk, args.refs, rank, world, args.hybrid, device=local, on_result=lambda ref, n4, c: outs.__setitem__(ref, (n4, c)))
     ok = True
     for ref, (n4, c) in outs.items():
         single, _, _ = api.runcuda(mk(ref), device=local)
@@ -46,7 +44,7 @@ if args.hybrid:
 sc = S.make_config(args.config, rows=args.rows, cols=args.cols, n_views=args.views, iterations=args.iters,
                    workers=max(1, min(32, len(os.sched_getaffinity(0)) // max(1, world))))
 opts = {k: int(v) for k, v in (o.split("=") for o in args.opt)}
-run = M.ViewShardRunner(sc, rank, world, device=local, exchange=args.exchange, options=opts)
+run = M.ViewShardRunner(sc, rank, world, device=local, options=opts)
 run.run()                                              # warm-up (NCCL communicator, kernels)
 torch.cuda.synchronize()
 best, sweep = 1e30, 1e30
