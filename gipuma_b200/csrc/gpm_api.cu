@@ -5,9 +5,10 @@
 // Device memory layout (everything resident in HBM for the life of the context):
 //   planes   float4[H*W]   (n.xyz, d) row-major, stride W   — LineState::norm4 layout (linestate.h:10)
 //   cost     float [H*W]                                      — LineState::c
-//   refpad   float [(H+32) x pitch]  reference image, replicate-padded by 16 px, pitch multiple of 32 floats
+//   refpad   float [(H+32) x pitch]  reference image, replicate-padded by 16 px, pitch multiple of 32 texels
 //   src      cudaArray (layered, R32F, W x H x max_views) + one texture object: Linear filter, the
 //            reference's addressing (Wrap + unnormalised, main.cpp:642-648), element read mode
+//            (refpad and src are allocated by the first image upload; colour: float4 texels, 3 x max_views layers)
 //   cams     ViewCam[max_views]  (K, R, t per source view) — copied to shared memory by every block
 //   rng      uint32[H*W*6]  XORWOW state per pixel (GPM_RNG_STATEFUL only)
 // No CPU fallback exists: every entry point needs a CUDA device and reports GPM_E_CUDA otherwise.
@@ -64,8 +65,9 @@ struct gpm_ctx {
     bool comm_owned = false;
     int shard_rank = 0, shard_world = 0;
     unsigned long long collectives = 0;
-    int opt_async_upload = 0;                    // 1: image uploads return without a host synchronisation (caller keeps its buffers alive until the next run)
-    bool inputs_dirty = false;                   // an input changed: stored costs / memo are stale (cleared once, at the next launch)
+    // Setters only mark state stale; build_kparams clears it once, at the next launch (reset_state_tags)
+    bool inputs_dirty = false;       // the cost function or its inputs changed: stored costs (prov) and memo are stale
+    bool memo_dirty = false;         // only what the memo may assume changed: the memo is stale
     unsigned* seen = nullptr;        // [H*W*ncand] identity of the plane last offered to each pixel from each of the 8 (fused kernel: 20) propagation directions
     int seen_slots = 8;
     unsigned* refseen = nullptr;     // [H*W]   identity of the plane from which the last all-rejected refinement started
@@ -73,19 +75,17 @@ struct gpm_ctx {
     unsigned* next_id = nullptr;     // device counter of fresh identities
     unsigned* memo_mask = nullptr;   // [H*W] validity bits of seen (0-19) and refseen (GPM_MEMO_REFINE)
     unsigned char* prov = nullptr;   // per pixel: which rounding variant of the cost function produced cost[] (see k_sweep)
-    float* refpad = nullptr;
-    int refpitch = 0, refrows = 0;   // padded reference image: refrows x refpitch texels
-    CUtensorMap tmap{};              // 2-D TMA descriptor of the padded reference image for the current box size / image type
-    int tmap_box = 0, tmap_color = -1;
-    float* staging = nullptr;        // W*H floats, upload scratch
+    // image storage, allocated by the first upload for the context's image type (ensure_color); texel = float, colour: float4
+    float* refpad = nullptr;         // padded reference image: refrows x refpitch texels
+    int refpitch = 0, refrows = 0;
+    CUtensorMap tmap{};              // 2-D TMA descriptor of the padded reference image for the current box size
+    int tmap_box = 0;
+    float* staging = nullptr;        // W*H texels, upload scratch
+    // source views, layered R32F: one layer per view; colour: 3 channel planes per view, layer 3v + ch (an RGBA32F fetch
+    // costs several R32F ones, tools/texbench.cu)
     cudaArray_t srcArr = nullptr;
     cudaTextureObject_t srcTex = 0;
-    cudaArray_t srcArr4 = nullptr;   // colour mode: layered R32F, 3 channel planes per view (layer 3v + ch: an RGBA32F fetch costs
-                                     // several R32F ones, tools/texbench.cu) + padded float4 reference + float4 staging
-    float* planar = nullptr;         // [3][H][W] split target
-    cudaTextureObject_t srcTex4 = 0;
-    float4* refpad4 = nullptr;
-    float4* staging4 = nullptr;
+    float* planar = nullptr;         // colour only: [3][H][W] split target
     ViewCam* d_cams = nullptr;
     std::vector<ViewCam> h_cams;
     bool cams_dirty = true;
@@ -96,9 +96,8 @@ struct gpm_ctx {
     cudaEvent_t ev0 = nullptr, ev1 = nullptr;
     unsigned long long* d_stats = nullptr;
     unsigned long long launches = 0;
-    int opt_prune = 1, opt_dedupe = 1, opt_trust_state = 0, opt_nwarps = 0, opt_stats = 1;
+    int opt_prune = 1, opt_dedupe = 1, opt_trust_state = 0, opt_nwarps = 0;
     int opt_cost_variant = -1, opt_memo = 1, opt_quadperm = 1;
-    int opt_shard_async = 0;                     // 1: gpm_shard_eval / gpm_shard_accept only enqueue on gpm_stream()
     int opt_neighbours = 8;                      // 20: the reference's fused kernel (built when SMALLKERNEL is not defined)
     int opt_site[21];                            // diagnostics: override the fused kernel's call-site variants (-1 = table)
     int smem_optin = 0, num_sms = 132;
@@ -117,7 +116,7 @@ struct DeviceGuard {
 int ensure_tensor_map(gpm_ctx* c, const KParams& P)
 {
     const int box = c->prm.box_hsize;
-    if (c->tmap_box == box && c->tmap_color == P.color) return GPM_OK;
+    if (c->tmap_box == box) return GPM_OK;
     typedef CUresult (*EncodeTiled)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
                                     const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
                                     CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
@@ -130,16 +129,27 @@ int ensure_tensor_map(gpm_ctx* c, const KParams& P)
         encode = (EncodeTiled)fn;
     }
     const int comps = P.color ? 4 : 1;
-    void* base = P.color ? (void*)c->refpad4 : (void*)c->refpad;
     const cuuint64_t gdim[2] = {(cuuint64_t)c->refpitch * comps, (cuuint64_t)c->refrows};
     const cuuint64_t gstride[1] = {(cuuint64_t)c->refpitch * comps * sizeof(float)};
     const cuuint32_t bdim[2] = {(cuuint32_t)(P.tile_stride * comps), (cuuint32_t)P.tile_w};
     const cuuint32_t estr[2] = {1, 1};
     if (bdim[0] > 256 || bdim[1] > 256) return fail(GPM_E_ARG, "window too large for one TMA box");
-    const CUresult r = encode(&c->tmap, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, base, gdim, gstride, bdim, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+    const CUresult r = encode(&c->tmap, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, c->refpad, gdim, gstride, bdim, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
                               CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     if (r != CUDA_SUCCESS) return fail(GPM_E_CUDA, "cuTensorMapEncodeTiled failed: " + std::to_string((int)r));
-    c->tmap_box = box;  c->tmap_color = P.color;
+    c->tmap_box = box;
+    return GPM_OK;
+}
+
+const int PROV_KEEP = -1;
+
+// The stored state's tags: prov[] (which rounding variant produced cost[]; PROV_KEEP leaves it alone) and the memo's
+// validity bits.  Every transition that makes them stale goes through here.
+int reset_state_tags(gpm_ctx* c, int prov)
+{
+    const size_t n = (size_t)c->W * c->H;
+    if (prov != PROV_KEEP) CU(cudaMemsetAsync(c->prov, prov, n, c->stream));
+    CU(cudaMemsetAsync(c->memo_mask, 0, n * sizeof(unsigned), c->stream));
     return GPM_OK;
 }
 
@@ -150,10 +160,10 @@ int build_kparams(gpm_ctx* c, bool init_phase, KParams& P, bool eval_call = fals
     if (c->V < 1) return fail(GPM_E_STATE, "no source views (gpm_set_num_views)");
     for (int v = 0; v < c->V; v++)
         if (!c->have_view[v]) return fail(GPM_E_STATE, "source view " + std::to_string(v) + " has not been set");
-    if (c->inputs_dirty) {                 // one clearing for a whole scene upload instead of two memsets per image
-        CU(cudaMemsetAsync(c->prov, GPM_PROV_UNKNOWN, (size_t)c->W * c->H, c->stream));
-        CU(cudaMemsetAsync(c->memo_mask, 0, (size_t)c->W * c->H * sizeof(unsigned), c->stream));
-        c->inputs_dirty = false;
+    if (c->inputs_dirty || c->memo_dirty) {     // one clearing for a whole scene upload instead of two memsets per setter
+        const int rc = reset_state_tags(c, c->inputs_dirty ? GPM_PROV_UNKNOWN : PROV_KEEP);
+        if (rc) return rc;
+        c->inputs_dirty = c->memo_dirty = false;
     }
     const gpm_params& p = c->prm;
     memset(&P, 0, sizeof(P));
@@ -290,8 +300,8 @@ int launch_colour(gpm_ctx* c, const KParams& P, int colour, int mask)
 {
     auto kern = P.ncand == 20 ? (P.color ? k_sweep<true, true> : k_sweep<false, true>)
                               : (P.color ? k_sweep<true, false> : k_sweep<false, false>);
-    kern<<<tile_grid(c), P.nwarps * 32, block_smem_bytes(P), c->stream>>>(P, c->tmap, c->d_cams, P.color ? c->srcTex4 : c->srcTex, c->planes, c->cost, c->rng,
-        c->prov, Memo{c->pid, c->seen, c->refseen, c->memo_mask, c->next_id}, colour, mask, c->opt_stats ? c->d_stats : nullptr);
+    kern<<<tile_grid(c), P.nwarps * 32, block_smem_bytes(P), c->stream>>>(P, c->tmap, c->d_cams, c->srcTex, c->planes, c->cost, c->rng,
+        c->prov, Memo{c->pid, c->seen, c->refseen, c->memo_mask, c->next_id}, colour, mask, c->d_stats);
     c->launches++;
     CU(cudaGetLastError());
     return GPM_OK;
@@ -302,7 +312,7 @@ cudaError_t launch_cost_eval(gpm_ctx* c, const KParams& P, const float4* planes,
 {
     dim3 grid((P.W + GPM_TILE - 1) / GPM_TILE, (P.H + GPM_TILE - 1) / GPM_TILE);
     (P.color ? k_cost_eval<true> : k_cost_eval<false>)<<<grid, P.nwarps * 32, block_smem_bytes(P), c->stream>>>(
-        P, c->tmap, c->d_cams, P.color ? c->srcTex4 : c->srcTex, planes, cost, nullptr);
+        P, c->tmap, c->d_cams, c->srcTex, planes, cost, nullptr);
     c->launches++;
     return cudaGetLastError();
 }
@@ -340,25 +350,49 @@ void set_view_camera(gpm_ctx* c, int v, const gpm_camera* cam)
     c->inputs_dirty = true;
 }
 
-int upload_image(gpm_ctx* c, const float* img, size_t pitch_bytes, int on_device, float** dev_img, size_t* dev_pitch_floats)
+// The first image upload fixes the context's image type (0 float, 1 float4) and allocates the image storage for that type
+// only.  A failed allocation is retried by the next upload.
+int ensure_color(gpm_ctx* c, int want)
 {
-    if (pitch_bytes == 0) pitch_bytes = (size_t)c->W * sizeof(float);
-    if (pitch_bytes % sizeof(float)) return fail(GPM_E_ARG, "pitch_bytes must be a multiple of 4");
-    if (on_device) {
-        *dev_img = const_cast<float*>(img);
-        *dev_pitch_floats = pitch_bytes / sizeof(float);
-        return GPM_OK;
-    }
-    CU(cudaMemcpy2DAsync(c->staging, (size_t)c->W * sizeof(float), img, pitch_bytes, (size_t)c->W * sizeof(float), c->H,
+    if (c->color == -1) c->color = want;
+    if (c->color != want) return fail(GPM_E_STATE, "a context holds either float or float4 images, not both");
+    const size_t comps = want ? 4 : 1, n = (size_t)c->W * c->H;
+    const cudaChannelFormatDesc desc = cudaCreateChannelDesc(32, 0, 0, 0, cudaChannelFormatKindFloat);
+    if (!c->srcArr) CU(cudaMalloc3DArray(&c->srcArr, &desc, make_cudaExtent(c->W, c->H, (want ? 3 : 1) * (size_t)c->maxV), cudaArrayLayered));
+    if (!c->srcTex) CU(make_layered_texture(c->srcArr, &c->srcTex));
+    if (!c->refpad) CU(cudaMalloc(&c->refpad, (size_t)c->refpitch * c->refrows * comps * sizeof(float)));
+    if (!c->staging) CU(cudaMalloc(&c->staging, n * comps * sizeof(float)));
+    if (want && !c->planar) CU(cudaMalloc(&c->planar, 3 * n * sizeof(float)));
+    return GPM_OK;
+}
+
+// row pitch, in texels of type T, of a caller's image of W texels per row (pitch_bytes 0: rows are packed)
+template <typename T>
+int image_pitch(const gpm_ctx* c, size_t pitch_bytes, size_t* pitch_elems)
+{
+    if (pitch_bytes == 0) pitch_bytes = (size_t)c->W * sizeof(T);
+    if (pitch_bytes % sizeof(T))
+        return fail(GPM_E_ARG, sizeof(T) == sizeof(float) ? "pitch_bytes must be a multiple of 4" : "pitch_bytes must be a multiple of 16 for float4 images");
+    *pitch_elems = pitch_bytes / sizeof(T);
+    return GPM_OK;
+}
+
+// the caller's image in device memory: a device image in place, a host image copied into `staging`
+template <typename T>
+int upload_image(gpm_ctx* c, const float* img, size_t pitch_bytes, int on_device, const T** dev_img, size_t* dev_pitch_elems)
+{
+    const int rc = image_pitch<T>(c, pitch_bytes, dev_pitch_elems);
+    if (rc) return rc;
+    *dev_img = reinterpret_cast<const T*>(img);
+    if (on_device) return GPM_OK;
+    CU(cudaMemcpy2DAsync(c->staging, (size_t)c->W * sizeof(T), img, *dev_pitch_elems * sizeof(T), (size_t)c->W * sizeof(T), c->H,
                          cudaMemcpyHostToDevice, c->stream));
-    *dev_img = c->staging;
-    *dev_pitch_floats = c->W;
+    *dev_img = reinterpret_cast<const T*>(c->staging);
+    *dev_pitch_elems = c->W;
     return GPM_OK;
 }
 
 }  // namespace
-
-static int ensure_color(gpm_ctx* c, int want);
 
 static void set_ref_camera(gpm_ctx* c, const gpm_camera* cam)
 {
@@ -408,22 +442,15 @@ extern "C" int gpm_create(gpm_ctx** out, int device, int width, int height, int 
     ok(cudaMalloc(&c->pid, n * sizeof(unsigned)));
     ok(cudaMalloc(&c->next_id, sizeof(unsigned)));
     ok(cudaMalloc(&c->memo_mask, n * sizeof(unsigned)));
-    ok(cudaMalloc(&c->staging, n * sizeof(float)));
-    ok(cudaMalloc(&c->refpad, (size_t)c->refpitch * c->refrows * sizeof(float)));
     ok(cudaMalloc(&c->d_cams, sizeof(ViewCam) * max_views));
     ok(cudaMalloc(&c->d_stats, 8 * sizeof(unsigned long long)));
     if (err == cudaSuccess) {
         ok(cudaMemsetAsync(c->planes, 0, n * sizeof(float4), c->stream));      // LineState::resize zeroes (linestate.h:19-24)
         ok(cudaMemsetAsync(c->cost, 0, n * sizeof(float), c->stream));
-        ok(cudaMemsetAsync(c->prov, GPM_PROV_UNKNOWN, n, c->stream));
-        ok(cudaMemsetAsync(c->memo_mask, 0, n * sizeof(unsigned), c->stream));
         ok(cudaMemsetAsync(c->d_stats, 0, 8 * sizeof(unsigned long long), c->stream));
-        if (fill_ids(c) != GPM_OK) err = cudaErrorUnknown;
-        cudaChannelFormatDesc desc = cudaCreateChannelDesc(32, 0, 0, 0, cudaChannelFormatKindFloat);
-        ok(cudaMalloc3DArray(&c->srcArr, &desc, make_cudaExtent(width, height, max_views), cudaArrayLayered));
+        if (reset_state_tags(c, GPM_PROV_UNKNOWN) != GPM_OK || fill_ids(c) != GPM_OK) err = cudaErrorUnknown;
     }
     if (err == cudaSuccess) {
-        ok(make_layered_texture(c->srcArr, &c->srcTex));
         ok(cudaDeviceGetAttribute(&c->smem_optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, device));
         ok(cudaDeviceGetAttribute(&c->num_sms, cudaDevAttrMultiProcessorCount, device));
         ok(cudaFuncSetAttribute(k_sweep<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, c->smem_optin));
@@ -454,9 +481,7 @@ extern "C" void gpm_destroy(gpm_ctx* c)
     if (c->comm && c->comm_owned) gpm_shard_comm_destroy_(c);
     if (c->srcTex) cudaDestroyTextureObject(c->srcTex);
     if (c->srcArr) cudaFreeArray(c->srcArr);
-    if (c->srcTex4) cudaDestroyTextureObject(c->srcTex4);
-    if (c->srcArr4) cudaFreeArray(c->srcArr4);
-    cudaFree(c->refpad4);  cudaFree(c->staging4);  cudaFree(c->planar);
+    cudaFree(c->planar);
     cudaFree(c->planes);  cudaFree(c->cost);  cudaFree(c->prov);  cudaFree(c->seen);  cudaFree(c->refseen);  cudaFree(c->pid);  cudaFree(c->next_id);  cudaFree(c->memo_mask);  cudaFree(c->rng);  cudaFree(c->dispbuf);  cudaFree(c->candbuf);  cudaFree(c->canddepth);  cudaFree(c->sflags);  cudaFree(c->xchg);  cudaFree(c->gath);  cudaFree(c->refpad);  cudaFree(c->staging);
     cudaFree(c->d_cams);  cudaFree(c->d_stats);
     if (c->ev0) cudaEventDestroy(c->ev0);
@@ -476,10 +501,7 @@ extern "C" int gpm_set_params(gpm_ctx* c, const gpm_params* p)
     if (p->iterations < 0) return fail(GPM_E_ARG, "iterations must be >= 0");
     c->prm = *p;
     c->have_params = true;
-    {
-        DeviceGuard g(c->device);
-        CU(cudaMemsetAsync(c->memo_mask, 0, (size_t)c->W * c->H * sizeof(unsigned), c->stream));   // memo depends on the parameters
-    }
+    c->inputs_dirty = true;                          // the cost function depends on the parameters: stored costs / memo are stale
     return GPM_OK;
 }
 
@@ -497,7 +519,7 @@ extern "C" int gpm_set_rng(gpm_ctx* c, unsigned long long seed, int mode)
     DeviceGuard g(c->device);
     c->seed = seed;
     c->rng_mode = mode;
-    CU(cudaMemsetAsync(c->memo_mask, 0, (size_t)c->W * c->H * sizeof(unsigned), c->stream));
+    c->memo_dirty = true;                            // the refinement memo assumes the random stream it was built under
     if (mode == GPM_RNG_STATEFUL && !c->rng) {
         CU(cudaMalloc(&c->rng, (size_t)c->W * c->H * 6 * sizeof(unsigned)));
         CU(cudaMemsetAsync(c->rng, 0, (size_t)c->W * c->H * 6 * sizeof(unsigned), c->stream));
@@ -505,121 +527,84 @@ extern "C" int gpm_set_rng(gpm_ctx* c, unsigned long long seed, int mode)
     return GPM_OK;
 }
 
-extern "C" int gpm_set_reference(gpm_ctx* c, const float* img, size_t pitch_bytes, int on_device, const gpm_camera* cam)
+// Image uploads, T = float (grey) or float4 (colour: the reference's -color_processing path, main.cpp:560-605).  Each
+// returns after a stream synchronisation: the caller may reuse its buffer.
+template <typename T>
+static int set_reference(const char* fn, gpm_ctx* c, const float* img, size_t pitch_bytes, int on_device, const gpm_camera* cam)
 {
-    if (!c || !img || !cam) return fail(GPM_E_ARG, "gpm_set_reference: null argument");
+    if (!c || !img || !cam) return fail(GPM_E_ARG, std::string(fn) + ": null argument");
     DeviceGuard g(c->device);
-    float* d = nullptr;
-    size_t pf = 0;
-    int rc = ensure_color(c, 0);
+    int rc = ensure_color(c, sizeof(T) == sizeof(float4));
     if (rc) return rc;
-    rc = upload_image(c, img, pitch_bytes, on_device, &d, &pf);
+    const T* d = nullptr;
+    size_t pe = 0;
+    rc = upload_image<T>(c, img, pitch_bytes, on_device, &d, &pe);
     if (rc) return rc;
     dim3 b(32, 8), gr((c->refpitch + 31) / 32, (c->refrows + 7) / 8);
-    k_pad_reference<<<gr, b, 0, c->stream>>>(d, pf, c->W, c->H, c->refpad, c->refpitch, c->refrows);
+    k_pad_reference<T><<<gr, b, 0, c->stream>>>(d, pe, c->W, c->H, reinterpret_cast<T*>(c->refpad), c->refpitch, c->refrows);
     CU(cudaGetLastError());
     set_ref_camera(c, cam);
     c->inputs_dirty = true;
-    if (!c->opt_async_upload) CU(cudaStreamSynchronize(c->stream));     // the caller may reuse its buffer
+    CU(cudaStreamSynchronize(c->stream));
     return GPM_OK;
 }
 
-extern "C" int gpm_set_view(gpm_ctx* c, int v, const float* img, size_t pitch_bytes, int on_device, const gpm_camera* cam)
+template <typename T>
+static int set_view(const char* fn, gpm_ctx* c, int v, const float* img, size_t pitch_bytes, int on_device, const gpm_camera* cam)
 {
-    if (!c || !img || !cam) return fail(GPM_E_ARG, "gpm_set_view: null argument");
-    if (v < 0 || v >= c->maxV) return fail(GPM_E_ARG, "gpm_set_view: view index out of range");
+    if (!c || !img || !cam) return fail(GPM_E_ARG, std::string(fn) + ": null argument");
+    if (v < 0 || v >= c->maxV) return fail(GPM_E_ARG, std::string(fn) + ": view index out of range");
+    constexpr bool color = sizeof(T) == sizeof(float4);
     DeviceGuard g(c->device);
-    int rc = ensure_color(c, 0);
+    int rc = ensure_color(c, color);
     if (rc) return rc;
-    // the image goes straight into its layer of the array: no staging copy
-    const size_t pb = pitch_bytes ? pitch_bytes : (size_t)c->W * sizeof(float);
-    if (pb % sizeof(float)) return fail(GPM_E_ARG, "pitch_bytes must be a multiple of 4");
     cudaMemcpy3DParms m;  memset(&m, 0, sizeof(m));
-    m.srcPtr = make_cudaPitchedPtr(const_cast<float*>(img), pb, c->W, c->H);
     m.dstArray = c->srcArr;
-    m.dstPos = make_cudaPos(0, 0, v);
-    m.extent = make_cudaExtent(c->W, c->H, 1);
-    m.kind = on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice;
+    if (!color) {                   // the image goes straight into its layer of the array: no staging copy
+        size_t pe = 0;
+        rc = image_pitch<T>(c, pitch_bytes, &pe);
+        if (rc) return rc;
+        m.srcPtr = make_cudaPitchedPtr(const_cast<float*>(img), pe * sizeof(T), c->W, c->H);
+        m.dstPos = make_cudaPos(0, 0, v);
+        m.extent = make_cudaExtent(c->W, c->H, 1);
+        m.kind = on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice;
+    } else {                        // three channel planes, layers 3v .. 3v + 2
+        const T* d = nullptr;
+        size_t pe = 0;
+        rc = upload_image<T>(c, img, pitch_bytes, on_device, &d, &pe);
+        if (rc) return rc;
+        dim3 b(32, 8), gr((c->W + 31) / 32, (c->H + 7) / 8);
+        k_split_channels<<<gr, b, 0, c->stream>>>(reinterpret_cast<const float4*>(d), pe, c->W, c->H, c->planar);
+        CU(cudaGetLastError());
+        m.srcPtr = make_cudaPitchedPtr(c->planar, c->W * sizeof(float), c->W, c->H);
+        m.dstPos = make_cudaPos(0, 0, 3 * (size_t)v);
+        m.extent = make_cudaExtent(c->W, c->H, 3);
+        m.kind = cudaMemcpyDeviceToDevice;
+    }
     CU(cudaMemcpy3DAsync(&m, c->stream));
     set_view_camera(c, v, cam);
-    if (!c->opt_async_upload) CU(cudaStreamSynchronize(c->stream));        // the caller may reuse its buffer
+    CU(cudaStreamSynchronize(c->stream));
     return GPM_OK;
 }
 
-
-// ---- colour (float4) images: the reference's -color_processing path (T = float4, main.cpp:560-605) -------------
-static int ensure_color(gpm_ctx* c, int want)
+extern "C" int gpm_set_reference(gpm_ctx* c, const float* img, size_t pitch_bytes, int on_device, const gpm_camera* cam)
 {
-    if (c->color == -1) c->color = want;
-    if (c->color != want) return fail(GPM_E_STATE, "a context holds either float or float4 images, not both");
-    if (want == 1 && !c->srcArr4) {
-        cudaChannelFormatDesc d1 = cudaCreateChannelDesc(32, 0, 0, 0, cudaChannelFormatKindFloat);
-        CU(cudaMalloc3DArray(&c->srcArr4, &d1, make_cudaExtent(c->W, c->H, 3 * (size_t)c->maxV), cudaArrayLayered));
-        CU(cudaMalloc(&c->planar, 3 * (size_t)c->W * c->H * sizeof(float)));
-        CU(make_layered_texture(c->srcArr4, &c->srcTex4));
-        CU(cudaMalloc(&c->refpad4, (size_t)c->refpitch * c->refrows * sizeof(float4)));
-        CU(cudaMalloc(&c->staging4, (size_t)c->W * c->H * sizeof(float4)));
-    }
-    return GPM_OK;
-}
-
-static int upload_image4(gpm_ctx* c, const float* img, size_t pitch_bytes, int on_device, float4** dev_img, size_t* dev_pitch_elems)
-{
-    if (pitch_bytes == 0) pitch_bytes = (size_t)c->W * sizeof(float4);
-    if (pitch_bytes % sizeof(float4)) return fail(GPM_E_ARG, "pitch_bytes must be a multiple of 16 for float4 images");
-    if (on_device) { *dev_img = (float4*)img;  *dev_pitch_elems = pitch_bytes / sizeof(float4);  return GPM_OK; }
-    CU(cudaMemcpy2DAsync(c->staging4, (size_t)c->W * sizeof(float4), img, pitch_bytes, (size_t)c->W * sizeof(float4), c->H,
-                         cudaMemcpyHostToDevice, c->stream));
-    *dev_img = c->staging4;
-    *dev_pitch_elems = c->W;
-    return GPM_OK;
+    return set_reference<float>("gpm_set_reference", c, img, pitch_bytes, on_device, cam);
 }
 
 extern "C" int gpm_set_reference_color(gpm_ctx* c, const float* rgba, size_t pitch_bytes, int on_device, const gpm_camera* cam)
 {
-    if (!c || !rgba || !cam) return fail(GPM_E_ARG, "gpm_set_reference_color: null argument");
-    DeviceGuard g(c->device);
-    int rc = ensure_color(c, 1);
-    if (rc) return rc;
-    float4* d = nullptr;
-    size_t pe = 0;
-    rc = upload_image4(c, rgba, pitch_bytes, on_device, &d, &pe);
-    if (rc) return rc;
-    dim3 b(32, 8), gr((c->refpitch + 31) / 32, (c->refrows + 7) / 8);
-    k_pad_reference4<<<gr, b, 0, c->stream>>>(d, pe, c->W, c->H, c->refpad4, c->refpitch, c->refrows);
-    CU(cudaGetLastError());
-    set_ref_camera(c, cam);
-    c->inputs_dirty = true;
-    if (!c->opt_async_upload) CU(cudaStreamSynchronize(c->stream));
-    return GPM_OK;
+    return set_reference<float4>("gpm_set_reference_color", c, rgba, pitch_bytes, on_device, cam);
+}
+
+extern "C" int gpm_set_view(gpm_ctx* c, int v, const float* img, size_t pitch_bytes, int on_device, const gpm_camera* cam)
+{
+    return set_view<float>("gpm_set_view", c, v, img, pitch_bytes, on_device, cam);
 }
 
 extern "C" int gpm_set_view_color(gpm_ctx* c, int v, const float* rgba, size_t pitch_bytes, int on_device, const gpm_camera* cam)
 {
-    if (!c || !rgba || !cam) return fail(GPM_E_ARG, "gpm_set_view_color: null argument");
-    if (v < 0 || v >= c->maxV) return fail(GPM_E_ARG, "gpm_set_view_color: view index out of range");
-    DeviceGuard g(c->device);
-    int rc = ensure_color(c, 1);
-    if (rc) return rc;
-    float4* d = nullptr;
-    size_t pe = 0;
-    rc = upload_image4(c, rgba, pitch_bytes, on_device, &d, &pe);
-    if (rc) return rc;
-    {
-        dim3 b(32, 8), gr((c->W + 31) / 32, (c->H + 7) / 8);
-        k_split_channels<<<gr, b, 0, c->stream>>>(d, pe, c->W, c->H, c->planar);
-        CU(cudaGetLastError());
-    }
-    cudaMemcpy3DParms m;  memset(&m, 0, sizeof(m));
-    m.srcPtr = make_cudaPitchedPtr(c->planar, c->W * sizeof(float), c->W, c->H);
-    m.dstArray = c->srcArr4;
-    m.dstPos = make_cudaPos(0, 0, 3 * (size_t)v);
-    m.extent = make_cudaExtent(c->W, c->H, 3);
-    m.kind = cudaMemcpyDeviceToDevice;
-    CU(cudaMemcpy3DAsync(&m, c->stream));
-    set_view_camera(c, v, cam);
-    if (!c->opt_async_upload) CU(cudaStreamSynchronize(c->stream));
-    return GPM_OK;
+    return set_view<float4>("gpm_set_view_color", c, v, rgba, pitch_bytes, on_device, cam);
 }
 
 extern "C" int gpm_set_state(gpm_ctx* c, const float* norm4, const float* cost, int on_device)
@@ -636,8 +621,8 @@ extern "C" int gpm_set_state(gpm_ctx* c, const float* norm4, const float* cost, 
     if (cost) CU(cudaMemcpyAsync(c->cost, cost, n * sizeof(float), k, c->stream));
     // provenance of the supplied costs is unknown (GPM_PROV_UNKNOWN) unless the caller vouches that they came from an
     // initialisation / refinement evaluation of exactly these planes ("trust_state": 0)
-    CU(cudaMemsetAsync(c->prov, c->opt_trust_state ? (c->color == 1 ? 3 : 0) : GPM_PROV_UNKNOWN, n, c->stream));
-    CU(cudaMemsetAsync(c->memo_mask, 0, n * sizeof(unsigned), c->stream));
+    const int rc = reset_state_tags(c, c->opt_trust_state ? (c->color == 1 ? 3 : 0) : GPM_PROV_UNKNOWN);
+    if (rc) return rc;
     CU(cudaStreamSynchronize(c->stream));
     return GPM_OK;
 }
@@ -664,9 +649,7 @@ static int do_init(gpm_ctx* c)
     rc = init_planes(c, P);
     if (rc) return rc;
     CU(launch_cost_eval(c, P, c->planes, c->cost));
-    CU(cudaMemsetAsync(c->prov, c->color == 1 ? 3 : 0, (size_t)c->W * c->H, c->stream));   // costs now come from the init-variant evaluation (float4: x-first + gradient folding 1)
-    CU(cudaMemsetAsync(c->memo_mask, 0, (size_t)c->W * c->H * sizeof(unsigned), c->stream));
-    return GPM_OK;
+    return reset_state_tags(c, c->color == 1 ? 3 : 0);     // costs now come from the init-variant evaluation (float4: x-first + gradient folding 1)
 }
 
 static int do_sweeps(gpm_ctx* c, int iterations)
@@ -694,9 +677,7 @@ static int do_finalize(gpm_ctx* c)
     k_finalize<<<gr, b, 0, c->stream>>>(P, c->planes, c->cost);
     c->launches++;
     CU(cudaGetLastError());
-    CU(cudaMemsetAsync(c->prov, GPM_PROV_UNKNOWN, (size_t)c->W * c->H, c->stream));
-    CU(cudaMemsetAsync(c->memo_mask, 0, (size_t)c->W * c->H * sizeof(unsigned), c->stream));   // planes are world-frame outputs now
-    return GPM_OK;
+    return reset_state_tags(c, GPM_PROV_UNKNOWN);          // planes are world-frame outputs now
 }
 
 extern "C" int gpm_init(gpm_ctx* c)
@@ -845,11 +826,21 @@ static int shard_launch_stage(gpm_ctx* c, const KParams& P, int colour, int stag
     const int last = 1 + shard_refine_steps(c->prm);
     ShardState S{c->dispbuf, c->candbuf, c->canddepth, c->sflags};
     (P.color ? k_shard_stage<true> : k_shard_stage<false>)<<<tile_grid(c), P.nwarps * 32, block_smem_bytes(P), c->stream>>>(P, c->tmap, c->d_cams,
-        P.color ? c->srcTex4 : c->srcTex, c->planes, c->cost, c->prov, S, Memo{c->pid, c->seen, c->refseen, c->memo_mask, c->next_id}, colour, stage, last,
-        gathered_prev, world, xchg, c->opt_stats ? c->d_stats : nullptr);
+        c->srcTex, c->planes, c->cost, c->prov, S, Memo{c->pid, c->seen, c->refseen, c->memo_mask, c->next_id}, colour, stage, last,
+        gathered_prev, world, xchg, c->d_stats);
     c->launches++;
     CU(cudaGetLastError());
     return GPM_OK;
+}
+
+// closing accept of stage 0: the merged initial costs (the kernel sets their provenance to the initialisation variant)
+static int shard_accept0(gpm_ctx* c, const KParams& P, const float* gathered, int world)
+{
+    dim3 b(32, 8), gr(((P.W + 1) / 2 + 31) / 32, (P.H + 7) / 8);
+    k_shard_accept0<<<gr, b, 0, c->stream>>>(P, c->cost, c->prov, gathered, world);
+    c->launches++;
+    CU(cudaGetLastError());
+    return reset_state_tags(c, PROV_KEEP);
 }
 
 extern "C" int gpm_shard_stage(gpm_ctx* c, int colour, int stage, const float* gathered_prev_dev, int world, float* xchg_dev)
@@ -864,7 +855,7 @@ extern "C" int gpm_shard_stage(gpm_ctx* c, int colour, int stage, const float* g
     if (stage <= last && !xchg_dev) return fail(GPM_E_ARG, "gpm_shard_stage: no exchange buffer");
     rc = shard_launch_stage(c, P, colour, stage, gathered_prev_dev, world, xchg_dev);
     if (rc) return rc;
-    if (!c->opt_shard_async) CU(cudaStreamSynchronize(c->stream));       // the caller's collective may run on another stream
+    CU(cudaStreamSynchronize(c->stream));       // the caller's collective may run on another stream
     return GPM_OK;
 }
 
@@ -875,12 +866,9 @@ extern "C" int gpm_shard_finish_init(gpm_ctx* c, const float* gathered_dev, int 
     KParams P;
     int rc = shard_common(c, 0, P);
     if (rc) return rc;
-    dim3 b(32, 8), gr(((P.W + 1) / 2 + 31) / 32, (P.H + 7) / 8);
-    k_shard_accept0<<<gr, b, 0, c->stream>>>(P, c->cost, c->prov, gathered_dev, world);
-    c->launches++;
-    CU(cudaGetLastError());
-    CU(cudaMemsetAsync(c->memo_mask, 0, (size_t)c->W * c->H * sizeof(unsigned), c->stream));
-    if (!c->opt_shard_async) CU(cudaStreamSynchronize(c->stream));
+    rc = shard_accept0(c, P, gathered_dev, world);
+    if (rc) return rc;
+    CU(cudaStreamSynchronize(c->stream));
     return GPM_OK;
 }
 
@@ -962,8 +950,7 @@ extern "C" int gpm_shard_comm_init(gpm_ctx* c, const void* id128, int rank, int 
 {
     if (!c || world < 1 || world > 8 || rank < 0 || rank >= world) return fail(GPM_E_ARG, "gpm_shard_comm_init: bad arguments (1 <= world <= 8)");
     DeviceGuard g(c->device);
-    if (c->comm && c->comm_owned) { nccl_api()->CommDestroy(c->comm); }
-    c->comm = nullptr;  c->comm_owned = false;
+    gpm_shard_comm_destroy_(c);
     c->shard_rank = rank;  c->shard_world = world;
     if (world > 1) {
         if (!id128) return fail(GPM_E_ARG, "gpm_shard_comm_init: null unique id");
@@ -980,8 +967,8 @@ extern "C" int gpm_shard_comm_attach(gpm_ctx* c, void* nccl_comm, int rank, int 
 {
     if (!c || world < 1 || world > 8 || rank < 0 || rank >= world || (world > 1 && !nccl_comm)) return fail(GPM_E_ARG, "gpm_shard_comm_attach: bad arguments");
     if (world > 1 && !nccl_api()) return fail(GPM_E_STATE, "NCCL (libnccl.so.2) could not be loaded; set GPM_NCCL_LIB");
-    if (c->comm && c->comm_owned) nccl_api()->CommDestroy(c->comm);
-    c->comm = nccl_comm;  c->comm_owned = false;  c->shard_rank = rank;  c->shard_world = world;
+    gpm_shard_comm_destroy_(c);
+    c->comm = nccl_comm;  c->shard_rank = rank;  c->shard_world = world;
     return GPM_OK;
 }
 
@@ -1016,15 +1003,12 @@ extern "C" int gpm_shard_run(gpm_ctx* c, float* sweep_ms)
     if (world > 1 && !c->comm) return fail(GPM_E_STATE, "gpm_shard_run: no NCCL communicator is attached");
     rc = init_planes(c, P0);
     if (rc) return rc;
-    CU(cudaMemsetAsync(c->memo_mask, 0, (size_t)c->W * c->H * sizeof(unsigned), c->stream));
     rc = shard_launch_stage(c, P0, 0, 0, nullptr, world, c->xchg);
     if (rc) return rc;
     rc = shard_exchange(c, 0);
     if (rc) return rc;
-    dim3 b2(32, 8), gr2(((P0.W + 1) / 2 + 31) / 32, (P0.H + 7) / 8);
-    k_shard_accept0<<<gr2, b2, 0, c->stream>>>(P0, c->cost, c->prov, c->gath, world);
-    c->launches++;
-    CU(cudaGetLastError());
+    rc = shard_accept0(c, P0, c->gath, world);
+    if (rc) return rc;
     CU(cudaEventRecord(c->ev0, c->stream));
     for (int it = 0; it < c->prm.iterations; it++)
         for (int colour = 0; colour < 2; colour++) {
@@ -1058,8 +1042,8 @@ extern "C" int gpm_init_planes(gpm_ctx* c)
     if (rc) return rc;
     rc = init_planes(c, P);
     if (rc) return rc;
-    CU(cudaMemsetAsync(c->prov, GPM_PROV_UNKNOWN, (size_t)c->W * c->H, c->stream));      // every plane is new: costs and memo are stale
-    CU(cudaMemsetAsync(c->memo_mask, 0, (size_t)c->W * c->H * sizeof(unsigned), c->stream));
+    rc = reset_state_tags(c, GPM_PROV_UNKNOWN);                // every plane is new: costs and memo are stale
+    if (rc) return rc;
     CU(cudaStreamSynchronize(c->stream));
     return GPM_OK;
 }
@@ -1071,18 +1055,17 @@ extern "C" int gpm_measure_fetch_peak(gpm_ctx* c, double* gfetch_per_s)
     DeviceGuard g(c->device);
     float* sink = reinterpret_cast<float*>(c->d_stats + 7);         // d_stats[7] holds no counter: it is only k_fetch_peak's sink
     const int blocks = c->num_sms * 16, threads = 256, reps = 2048;
-    const cudaTextureObject_t tex = c->color == 1 ? c->srcTex4 : c->srcTex;      // colour: three R32F channel planes per view
-    const int layers = c->color == 1 ? 3 * c->V : c->V;
+    const int layers = c->color == 1 ? 3 * c->V : c->V;       // colour: three R32F channel planes per view
     // random positions inside a window of at most 512 x 512 texels of at most 4 layers: the UNIT's ceiling is wanted, so the
     // working set must stay in L2 whatever the image size (a 3200 x 2400 x 64-layer array would make this a DRAM test)
     int xmask = 1, ymask = 1;
     while (2 * xmask + 1 < c->W - 48 && xmask < 511) xmask = 2 * xmask + 1;
     while (2 * ymask + 1 < c->H - 24 && ymask < 511) ymask = 2 * ymask + 1;
-    k_fetch_peak<<<blocks, threads, 0, c->stream>>>(tex, xmask, ymask, layers, 64, sink);        // warm-up
+    k_fetch_peak<<<blocks, threads, 0, c->stream>>>(c->srcTex, xmask, ymask, layers, 64, sink);        // warm-up
     double best = 0.0;
     for (int rep = 0; rep < 3; rep++) {
         CU(cudaEventRecord(c->ev0, c->stream));
-        k_fetch_peak<<<blocks, threads, 0, c->stream>>>(tex, xmask, ymask, layers, reps, sink);
+        k_fetch_peak<<<blocks, threads, 0, c->stream>>>(c->srcTex, xmask, ymask, layers, reps, sink);
         CU(cudaEventRecord(c->ev1, c->stream));
         CU(cudaEventSynchronize(c->ev1));
         CU(cudaGetLastError());
@@ -1123,7 +1106,6 @@ extern "C" int gpm_set_option(gpm_ctx* c, const char* name, int value)
     else if (n == "dedupe") c->opt_dedupe = value != 0;
     else if (n == "trust_state") c->opt_trust_state = value != 0;
     else if (n == "nwarps") c->opt_nwarps = value;
-    else if (n == "stats") c->opt_stats = value != 0;
     else if (n == "cost_variant") c->opt_cost_variant = value < 0 ? -1 : (value & 15);
     else if (n.rfind("site", 0) == 0 && n.size() > 4 && n.size() <= 6 && std::isdigit((unsigned char)n[4])) {
         const int k = std::atoi(n.c_str() + 4);             // "site<k>": variant of call site k of the fused kernel (diagnostics)
@@ -1140,13 +1122,11 @@ extern "C" int gpm_set_option(gpm_ctx* c, const char* name, int value)
             CU(cudaMalloc(&c->seen, (size_t)c->W * c->H * slots * sizeof(unsigned)));
             c->seen_slots = slots;
         }
-        CU(cudaMemsetAsync(c->memo_mask, 0, (size_t)c->W * c->H * sizeof(unsigned), c->stream));
+        c->memo_dirty = true;
         c->opt_neighbours = value;
     }
     else if (n == "memo") c->opt_memo = value != 0;
     else if (n == "quadperm") c->opt_quadperm = value != 0;
-    else if (n == "async_upload") c->opt_async_upload = value != 0;
-    else if (n == "shard_async") c->opt_shard_async = value != 0;
     else return fail(GPM_E_ARG, "gpm_set_option: unknown option '" + n + "'");
     return GPM_OK;
 }

@@ -750,24 +750,16 @@ __global__ void k_split_channels(const float4* __restrict__ in, size_t pitch_ele
     out[o] = p.x;  out[plane + o] = p.y;  out[2 * plane + o] = p.z;
 }
 
-__global__ void k_pad_reference4(const float4* __restrict__ img, size_t pitch_elems, int W, int H, float4* __restrict__ out, int out_pitch, int out_rows)
+// replicate-pad the reference image (T = float or float4 texels) by GPM_APRON on the left / top and out to the end of the
+// allocation on the right / bottom (== the texture's clamp addressing, main.cpp:644-645): the window of the last tile row /
+// column reaches roundup(size, 32) + halo + GPM_APRON, past size + 2 * GPM_APRON whenever size % 32 is small
+template <typename T>
+__global__ void k_pad_reference(const T* __restrict__ img, size_t pitch_elems, int W, int H, T* __restrict__ out, int out_pitch, int out_rows)
 {
     const int x = blockIdx.x * blockDim.x + threadIdx.x, y = blockIdx.y * blockDim.y + threadIdx.y;
     if (x >= out_pitch || y >= out_rows) return;
     const int sx = min(max(x - GPM_APRON, 0), W - 1), sy = min(max(y - GPM_APRON, 0), H - 1);
     out[(size_t)y * out_pitch + x] = img[(size_t)sy * pitch_elems + sx];
-}
-
-// replicate-pad the reference image by GPM_APRON on the left / top and out to the end of the allocation on the right / bottom
-// (== the texture's clamp addressing, main.cpp:644-645): the window of the last tile row / column reaches
-// roundup(size, 32) + halo + GPM_APRON, past size + 2 * GPM_APRON whenever size % 32 is small
-__global__ void k_pad_reference(const float* __restrict__ img, size_t pitch_floats, int W, int H,
-                                float* __restrict__ out, int out_pitch, int out_rows)
-{
-    const int x = blockIdx.x * blockDim.x + threadIdx.x, y = blockIdx.y * blockDim.y + threadIdx.y;
-    if (x >= out_pitch || y >= out_rows) return;
-    const int sx = min(max(x - GPM_APRON, 0), W - 1), sy = min(max(y - GPM_APRON, 0), H - 1);
-    out[(size_t)y * out_pitch + x] = img[(size_t)sy * pitch_floats + sx];
 }
 
 }  // namespace gpm

@@ -167,14 +167,9 @@ int gpm_measure_fetch_peak(gpm_ctx* ctx, double* gfetch_per_s);
 /* Tuning / diagnostics; results are bit-identical for every setting.
  * "prune" (1): exact lower-bound early-out; "dedupe" (1): skip bit-identical candidate planes;
  * "trust_state" (0): treat a state loaded with gpm_set_state as cost-consistent; "nwarps" (0 = auto): warps per block;
- * "stats" (1): maintain the gpm_get_stats counters; "memo" (1): skip candidates / refinements this pixel is already
- * known to reject (exact); "cost_variant" (-1 = auto): which of the reference binary's rounding variants gpm_cost_eval
- * reproduces (DESIGN.md §2): bit 0 = x-term first (float: 1 in the propagation kernels, 0 at init / refinement; float4: 0 in
+ * "memo" (1): skip candidates / refinements this pixel is already known to reject (exact); "cost_variant" (-1 = auto):
+ * which of the reference binary's rounding variants gpm_cost_eval reproduces (DESIGN.md §2): bit 0 = x-term first (float: 1 in the propagation kernels, 0 at init / refinement; float4: 0 in
  * all six sweep kernels), bit 1 = float4 gradient folding (float4 initialisation = 3); auto = the propagation kernels' form;
- * "shard_async" (0): 1 makes gpm_shard_stage / gpm_shard_finish_init return after enqueueing on gpm_stream() — run the
- * collective on that stream (or order it with events) instead of paying a host synchronisation per stage;
- * "async_upload" (0): 1 lets gpm_set_reference / gpm_set_view return without a host synchronisation — the caller keeps its
- * (page-locked) image buffers unchanged until the next gpm_run / gpm_sweep returns;
  * "quadperm" (1): deal the samples of a round to the lanes as 2x2 blocks per hardware quad (texture-unit locality);
  * "neighbours" (8): 20 selects the reference's fused sweep — the kernels it launches when built without SMALLKERNEL
  * (gipuma.cu:1122-1351, 1913-1940): 12 axial + 8 knight-move neighbours, then refinement, one launch per colour; bit-exact

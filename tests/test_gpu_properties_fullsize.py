@@ -84,6 +84,6 @@ def test_error_handling():
         ctx.load_scene(S.make_config(1, rows=64, cols=96))
         ctx.set_num_views(1)                              # fewer views than uploaded is fine
         ctx.run()
-        for name in ("packed", "prepass", "equal_rounds", "fused_warps", "tma", "exchange"):
+        for name in ("packed", "prepass", "equal_rounds", "fused_warps", "tma", "exchange", "async_upload", "shard_async", "stats"):
             with pytest.raises(api.GipumaError):
                 ctx.set_option(name, 0)                   # retired options fail loudly instead of being ignored
