@@ -11,6 +11,7 @@ from __future__ import annotations
 
 import ctypes as C
 import os
+import time
 from typing import Optional
 
 import numpy as np
@@ -111,6 +112,8 @@ def load_library():
     L.gpm_set_reference_color.argtypes = L.gpm_set_reference.argtypes
     L.gpm_set_view_color.argtypes = L.gpm_set_view.argtypes
     L.gpm_set_num_views.argtypes = [vp, C.c_int]
+    L.gpm_set_view_depth.argtypes = [vp, C.c_int, vp, C.c_size_t, C.c_int]
+    L.gpm_set_geometric.argtypes = [vp, C.c_float, C.c_float]
     L.gpm_set_rng.argtypes = [vp, C.c_ulonglong, C.c_int]
     L.gpm_set_state.argtypes = [vp, vp, vp, C.c_int]
     L.gpm_get_state.argtypes = [vp, vp, vp, C.c_int]
@@ -149,7 +152,7 @@ def load_library():
     L.gpm_write_ply.argtypes = [C.c_char_p, vp, C.c_longlong]
     L.gpm_nearest_dist.argtypes = [C.POINTER(GpmNnDesc), C.POINTER(GpmNnResult)]
     for name in ("gpm_create", "gpm_set_params", "gpm_set_reference", "gpm_set_view", "gpm_set_reference_color",
-                 "gpm_set_view_color", "gpm_set_num_views",
+                 "gpm_set_view_color", "gpm_set_num_views", "gpm_set_view_depth", "gpm_set_geometric",
                  "gpm_set_rng", "gpm_set_state", "gpm_get_state", "gpm_init", "gpm_sweep", "gpm_phase",
                  "gpm_finalize", "gpm_cost_eval", "gpm_run", "gpm_get_stats", "gpm_reset_stats", "gpm_set_option",
                  "gpm_init_planes", "gpm_shard_num_stages", "gpm_shard_stage", "gpm_shard_finish_init", "gpm_shard_unique_id",
@@ -209,6 +212,18 @@ def _image(a):
     return a
 
 
+# Defaults of the geometric-consistency pass (DESIGN.md §14), chosen from the measurement in tools/geo_bench.py.
+GEO_WEIGHT, GEO_MAX_ERR = 0.5, 3.0
+
+
+def check_geometric(weight: float, max_err: float):
+    """The argument rules of gpm_set_geometric, checked before any call into the library."""
+    if not (np.isfinite(weight) and weight >= 0):
+        raise ValueError("weight must be finite and >= 0 (got %r)" % (weight,))
+    if not (np.isfinite(max_err) and max_err > 0):
+        raise ValueError("max_err must be finite and > 0 (got %r)" % (max_err,))
+
+
 class Context:
     """One gpm_ctx: a reference view with its source views on one GPU."""
 
@@ -254,19 +269,36 @@ class Context:
     def set_reference(self, img, cam, pitch_bytes: int = 0):
         img = _image(img)
         ptr, dev = _ptr(img)
-        g = pack_camera(cam)
+        g = cam if isinstance(cam, GpmCamera) else pack_camera(cam)
         fn = self.lib.gpm_set_reference_color if self._is_color(img) else self.lib.gpm_set_reference
         self._check(fn(self.h, ptr, pitch_bytes, dev, C.byref(g)))
 
     def set_view(self, v: int, img, cam, pitch_bytes: int = 0):
         img = _image(img)
         ptr, dev = _ptr(img)
-        g = pack_camera(cam)
+        g = cam if isinstance(cam, GpmCamera) else pack_camera(cam)
         fn = self.lib.gpm_set_view_color if self._is_color(img) else self.lib.gpm_set_view
         self._check(fn(self.h, v, ptr, pitch_bytes, dev, C.byref(g)))
 
     def set_num_views(self, n: int):
         self._check(self.lib.gpm_set_num_views(self.h, n))
+
+    def set_view_depth(self, v: int, depth, pitch_bytes: int = 0):
+        """Depth map [H, W] of source view v (numpy or torch, host or device), along that view's own optical axis as
+        finalize() writes it (0 = no depth): what the geometric-consistency term reads (DESIGN.md §14)."""
+        if not 0 <= v < self.max_views:
+            raise ValueError("view index %d outside 0..%d" % (v, self.max_views - 1))
+        if tuple(depth.shape) != (self.H, self.W):
+            raise ValueError("depth map must be [%d, %d], got %s" % (self.H, self.W, tuple(depth.shape)))
+        depth = _image(depth)
+        ptr, dev = _ptr(depth)
+        self._check(self.lib.gpm_set_view_depth(self.h, v, ptr, pitch_bytes, dev))
+
+    def set_geometric(self, weight: float, max_err: float = GEO_MAX_ERR):
+        """Geometric-consistency term of every view's cost: weight * min(reprojection error, max_err) (DESIGN.md §14);
+        weight 0 turns it off."""
+        check_geometric(weight, max_err)
+        self._check(self.lib.gpm_set_geometric(self.h, float(weight), float(max_err)))
 
     def set_rng(self, seed: int, mode: int = GPM_RNG_REFERENCE):
         self._check(self.lib.gpm_set_rng(self.h, seed, mode))
@@ -478,6 +510,97 @@ def batch_run(images, Ps, params, refs, devices=(0,), cam_scale: float = 1.0, mi
     if rc != 0:
         raise GipumaError("gpm_batch_run failed (%d): %s" % (rc, lib.gpm_batch_last_error().decode()))
     return n4, cc, {"jobs_done": st.jobs_done, "sweep_ms_total": st.sweep_ms_total, "sweep_ms": list(ms), "views": list(nv), "device": list(dv)}
+
+
+def _load_job(ctx, images, Ps, params, ref, cam_scale, min_angle, max_angle, max_views, seed):
+    """Set `ctx` up for reference view `ref` as gpm_batch_run does (cameras re-based on it, source views selected, depth
+    range and disparities as main.cpp derives them).  Returns the image indices of the selected source views."""
+    n, H, W = images.shape[:3]
+    order = [ref] + [i for i in range(n) if i != ref]
+    cams = prepare_cameras([Ps[i] for i in order], cam_scale)
+    subset, (lo, hi) = select_views(cams, W, H, min_angle, max_angle, max_views)
+    if not subset:
+        raise GipumaError("no source view passes the angle filter for reference %d" % ref)
+    p = GpmParams.from_buffer_copy(pack_params(params))
+    if p.depthMin <= 0:
+        p.depthMin = lo
+    if p.depthMax <= 0:
+        p.depthMax = hi
+    fb = np.float32(cams[0].f) * np.float32(cams[0].baseline)                  # float arithmetic, as gpm_batch.cpp
+    p.min_disparity, p.max_disparity = float(fb / np.float32(p.depthMax)), float(fb / np.float32(p.depthMin))
+    ctx._check(ctx.lib.gpm_set_params(ctx.h, C.byref(p)))
+    ctx.set_reference(images[ref], cams[0])
+    for v, k in enumerate(subset):
+        ctx.set_view(v, images[order[k]], cams[k])
+    ctx.set_num_views(len(subset))
+    ctx.set_rng(seed, GPM_RNG_REFERENCE)
+    return [order[k] for k in subset]
+
+
+def geometric_pass(images, Ps, params, refs, geo_iterations: int = 2, weight: float = GEO_WEIGHT, max_err: float = GEO_MAX_ERR,
+                   cam_scale: float = 1.0, min_angle: float = 10.0, max_angle: float = 30.0, max_views: int = 9,
+                   seed: int = 0xC0FFEE, device: int = 0):
+    """PatchMatch with a geometric-consistency second pass (DESIGN.md §14) for the reference views `refs`.
+
+    Pass 1, for every reference view and every source view one of them selects: init, params.iterations photometric sweeps,
+    finalize; the view setup is gpm_batch_run's.  Pass 2, per reference view: the selected source views' pass-1 depth maps
+    are uploaded, the geometric term is turned on (weight, max_err), the pass-1 planes get their exact costs under the new
+    cost (cost_eval), and geo_iterations sweeps and finalize follow.  So a run has params.iterations + geo_iterations
+    iterations in all.  images: [n, H, W] grey or [n, H, W, 4] colour; the other arguments as batch_run.
+    Returns (norm4 [len(refs), H, W, 4], cost [len(refs), H, W], info) with norm4 as batch_run returns it, so fuse and
+    evaluate_cloud take it unchanged; info: "pass1_views" (the views pass 1 ran), "pass1_sweep_s" and "pass2_sweep_s" (host
+    seconds of each view's sweep call, which ends in a stream synchronisation), "views" (source views per reference)."""
+    check_geometric(weight, max_err)
+    if int(geo_iterations) != geo_iterations or geo_iterations < 0:
+        raise ValueError("geo_iterations must be an integer >= 0")
+    imgs = np.ascontiguousarray(images, dtype=np.float32)
+    if imgs.ndim not in (3, 4) or (imgs.ndim == 4 and imgs.shape[3] != 4):
+        raise ValueError("images must be [n, H, W] or [n, H, W, 4]")
+    n, H, W = imgs.shape[:3]
+    if len(Ps) != n:
+        raise ValueError("one projection matrix per image is needed (%d images, %d matrices)" % (n, len(Ps)))
+    refs = [int(r) for r in refs]
+    if not refs or any(r < 0 or r >= n for r in refs):
+        raise ValueError("reference views must be image indices in 0..%d" % (n - 1))
+    if not 1 <= max_views <= 64:
+        raise ValueError("max_views must be 1..64")
+    job = dict(cam_scale=cam_scale, min_angle=min_angle, max_angle=max_angle, max_views=max_views, seed=seed)
+    n4 = np.empty((len(refs), H, W, 4), np.float32)
+    cc = np.empty((len(refs), H, W), np.float32)
+    info = {"pass1_views": [], "pass1_sweep_s": [], "pass2_sweep_s": [], "views": []}
+    with Context(W, H, max_views, device) as ctx:
+        sources, raw, depth = {}, {}, {}
+        todo = list(dict.fromkeys(refs))
+        while todo:                                        # pass 1: the reference views, then the source views they read
+            r = todo.pop(0)
+            if r in depth:
+                continue
+            sources[r] = _load_job(ctx, imgs, Ps, params, r, **job)
+            ctx.init()
+            t0 = time.perf_counter()
+            ctx.sweep(params.iterations)
+            info["pass1_sweep_s"].append(time.perf_counter() - t0)
+            if r in refs:
+                raw[r] = ctx.get_state()[0]
+            ctx.finalize()
+            depth[r] = np.ascontiguousarray(ctx.get_state()[0][..., 3])
+            info["pass1_views"].append(r)
+            if r in refs:
+                todo += [i for i in sources[r] if i not in depth]
+        for j, r in enumerate(refs):                       # pass 2
+            src = _load_job(ctx, imgs, Ps, params, r, **job)
+            for v, i in enumerate(src):
+                ctx.set_view_depth(v, depth[i])
+            ctx.set_geometric(weight, max_err)
+            ctx.set_state(raw[r], ctx.cost_eval(raw[r]))
+            t0 = time.perf_counter()
+            ctx.sweep(geo_iterations)
+            info["pass2_sweep_s"].append(time.perf_counter() - t0)
+            ctx.finalize()
+            n4[j], cc[j] = ctx.get_state()
+            ctx.set_geometric(0.0, max_err)
+            info["views"].append(src)
+    return n4, cc, info
 
 
 def write_dmb(path: str, data: np.ndarray):

@@ -17,6 +17,7 @@
 
 #include <algorithm>
 #include <cctype>
+#include <cmath>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
@@ -101,6 +102,13 @@ struct gpm_ctx {
     int opt_neighbours = 8;                      // 20: the reference's fused kernel (built when SMALLKERNEL is not defined)
     int opt_site[21];                            // diagnostics: override the fused kernel's call-site variants (-1 = table)
     int smem_optin = 0, num_sms = 132;
+    // geometric-consistency mode (DESIGN.md §14): on while geo_weight > 0 (gpm_set_geometric)
+    float geo_weight = 0.f, geo_max_err = 1.f;
+    float* geo_depth = nullptr;      // [maxV][H][W] source views' depth maps, allocated by the first gpm_set_view_depth
+    float* geo_kinv = nullptr;       // [maxV][9]    K^-1 of each source view (copied with the camera table, sync_cams)
+    std::vector<char> have_depth;
+    std::vector<float> h_kinv;
+    float ref_K[9] = {0.f};
 };
 
 namespace {
@@ -153,6 +161,16 @@ int reset_state_tags(gpm_ctx* c, int prov)
     return GPM_OK;
 }
 
+// the geometric-consistency mode's own preconditions at weight `weight` (the fused sweep and a missing depth map)
+int check_geometric(const gpm_ctx* c, float weight)
+{
+    if (weight <= 0.f) return GPM_OK;
+    if (c->opt_neighbours == 20) return fail(GPM_E_ARG, "the geometric-consistency mode supports the 8-neighbour sweep only (option neighbours = 8)");
+    for (int v = 0; v < c->V; v++)
+        if (!c->have_depth[v]) return fail(GPM_E_STATE, "geometric-consistency mode: source view " + std::to_string(v) + " has no depth map (gpm_set_view_depth)");
+    return GPM_OK;
+}
+
 int build_kparams(gpm_ctx* c, bool init_phase, KParams& P, bool eval_call = false)
 {
     if (!c->have_params) return fail(GPM_E_STATE, "gpm_set_params has not been called");
@@ -160,6 +178,7 @@ int build_kparams(gpm_ctx* c, bool init_phase, KParams& P, bool eval_call = fals
     if (c->V < 1) return fail(GPM_E_STATE, "no source views (gpm_set_num_views)");
     for (int v = 0; v < c->V; v++)
         if (!c->have_view[v]) return fail(GPM_E_STATE, "source view " + std::to_string(v) + " has not been set");
+    if (const int rc = check_geometric(c, c->geo_weight)) return rc;
     if (c->inputs_dirty || c->memo_dirty) {     // one clearing for a whole scene upload instead of two memsets per setter
         const int rc = reset_state_tags(c, c->inputs_dirty ? GPM_PROV_UNKNOWN : PROV_KEEP);
         if (rc) return rc;
@@ -222,7 +241,8 @@ int build_kparams(gpm_ctx* c, bool init_phase, KParams& P, bool eval_call = fals
     P.prune = c->opt_prune;
     // The lower bound counts a view as valid from its PARTIAL cost; a view whose final cost reaches MAXCOST (then excluded,
     // gipuma.cu:771-774) would make the bound exceed the final value.  Unreachable while ns * max dissimilarity < MAXCOST.
-    if ((float)P.ns * ((1.0f - p.alpha) * p.tau_color + p.alpha * p.tau_gradient) >= GPM_MAXCOST) P.prune = 0;
+    // The geometric term adds at most weight * max_err to a view's final cost (0 outside that mode).
+    if ((float)P.ns * ((1.0f - p.alpha) * p.tau_color + p.alpha * p.tau_gradient) + c->geo_weight * c->geo_max_err >= GPM_MAXCOST) P.prune = 0;
     P.dedupe_self = c->opt_dedupe ? 1 : 0;
     // rounding variant of k_cost_eval: at initialisation the reference's binary is y-first for float, x-first for float4;
     // gpm_cost_eval defaults to the variant of the propagation kernels (x-first for float, y-first for float4)
@@ -281,6 +301,7 @@ int sync_cams(gpm_ctx* c)
 {
     if (!c->cams_dirty) return GPM_OK;
     CU(cudaMemcpyAsync(c->d_cams, c->h_cams.data(), sizeof(ViewCam) * c->maxV, cudaMemcpyHostToDevice, c->stream));
+    if (c->geo_kinv) CU(cudaMemcpyAsync(c->geo_kinv, c->h_kinv.data(), sizeof(float) * 9 * c->maxV, cudaMemcpyHostToDevice, c->stream));
     c->cams_dirty = false;
     return GPM_OK;
 }
@@ -296,12 +317,22 @@ dim3 tile_grid(const gpm_ctx* c)
     return grid;
 }
 
+GeoParams geo_params(const gpm_ctx* c)
+{
+    GeoParams G{};
+    G.depth = c->geo_depth;  G.kinv = c->geo_kinv;
+    memcpy(G.Kref, c->ref_K, sizeof(G.Kref));
+    G.weight = c->geo_weight;  G.max_err = c->geo_max_err;
+    return G;
+}
+
 int launch_colour(gpm_ctx* c, const KParams& P, int colour, int mask)
 {
-    auto kern = P.ncand == 20 ? (P.color ? k_sweep<true, true> : k_sweep<false, true>)
+    auto kern = c->geo_weight > 0.f ? (P.color ? k_sweep<true, false, true> : k_sweep<false, false, true>)    // 8 neighbours (check_geometric)
+              : P.ncand == 20 ? (P.color ? k_sweep<true, true> : k_sweep<false, true>)
                               : (P.color ? k_sweep<true, false> : k_sweep<false, false>);
     kern<<<tile_grid(c), P.nwarps * 32, block_smem_bytes(P), c->stream>>>(P, c->tmap, c->d_cams, c->srcTex, c->planes, c->cost, c->rng,
-        c->prov, Memo{c->pid, c->seen, c->refseen, c->memo_mask, c->next_id}, colour, mask, c->d_stats);
+        c->prov, Memo{c->pid, c->seen, c->refseen, c->memo_mask, c->next_id}, colour, mask, c->d_stats, geo_params(c));
     c->launches++;
     CU(cudaGetLastError());
     return GPM_OK;
@@ -311,8 +342,9 @@ int launch_colour(gpm_ctx* c, const KParams& P, int colour, int mask)
 cudaError_t launch_cost_eval(gpm_ctx* c, const KParams& P, const float4* planes, float* cost)
 {
     dim3 grid((P.W + GPM_TILE - 1) / GPM_TILE, (P.H + GPM_TILE - 1) / GPM_TILE);
-    (P.color ? k_cost_eval<true> : k_cost_eval<false>)<<<grid, P.nwarps * 32, block_smem_bytes(P), c->stream>>>(
-        P, c->tmap, c->d_cams, c->srcTex, planes, cost, nullptr);
+    auto kern = c->geo_weight > 0.f ? (P.color ? k_cost_eval<true, true> : k_cost_eval<false, true>)
+                                    : (P.color ? k_cost_eval<true> : k_cost_eval<false>);
+    kern<<<grid, P.nwarps * 32, block_smem_bytes(P), c->stream>>>(P, c->tmap, c->d_cams, c->srcTex, planes, cost, nullptr, geo_params(c));
     c->launches++;
     return cudaGetLastError();
 }
@@ -345,6 +377,7 @@ void set_view_camera(gpm_ctx* c, int v, const gpm_camera* cam)
     memcpy(vc.K, cam->K, sizeof(vc.K));
     memcpy(vc.R, cam->R, sizeof(vc.R));
     memcpy(vc.t, cam->t, sizeof(vc.t));
+    memcpy(&c->h_kinv[9 * (size_t)v], cam->K_inv, 9 * sizeof(float));
     c->cams_dirty = true;
     c->have_view[v] = 1;
     c->inputs_dirty = true;
@@ -404,6 +437,7 @@ static void set_ref_camera(gpm_ctx* c, const gpm_camera* cam)
     memcpy(r.C, cam->C, sizeof(r.C));
     r.fx = cam->fx;  r.alpha = cam->alpha;  r.K2 = cam->K[2];  r.K5 = cam->K[5];
     r.f = cam->f;  r.f_cam = cam->f;  r.baseline = cam->baseline;
+    memcpy(c->ref_K, cam->K, sizeof(c->ref_K));
     c->have_ref = true;
 }
 
@@ -425,6 +459,8 @@ extern "C" int gpm_create(gpm_ctx** out, int device, int width, int height, int 
     c->device = device;  c->W = width;  c->H = height;  c->maxV = max_views;
     c->have_view.assign(max_views, 0);
     c->h_cams.assign(max_views, ViewCam{});
+    c->have_depth.assign(max_views, 0);
+    c->h_kinv.assign((size_t)max_views * 9, 0.f);
     const size_t n = (size_t)width * height;
     // the staged window of the last tile row / column reaches roundup(size, 32) + halo + GPM_APRON (+ 3 texels of TMA row padding)
     c->refpitch = (((width + 31) & ~31) + 2 * GPM_APRON + 4 + 31) & ~31;
@@ -459,6 +495,10 @@ extern "C" int gpm_create(gpm_ctx** out, int device, int width, int height, int 
         ok(cudaFuncSetAttribute(k_sweep<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, c->smem_optin));
         ok(cudaFuncSetAttribute(k_cost_eval<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, c->smem_optin));
         ok(cudaFuncSetAttribute(k_cost_eval<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, c->smem_optin));
+        ok(cudaFuncSetAttribute(k_sweep<false, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, c->smem_optin));
+        ok(cudaFuncSetAttribute(k_sweep<true, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, c->smem_optin));
+        ok(cudaFuncSetAttribute(k_cost_eval<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, c->smem_optin));
+        ok(cudaFuncSetAttribute(k_cost_eval<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, c->smem_optin));
         ok(cudaFuncSetAttribute(k_shard_stage<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, c->smem_optin));
         ok(cudaFuncSetAttribute(k_shard_stage<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, c->smem_optin));
     }
@@ -482,7 +522,7 @@ extern "C" void gpm_destroy(gpm_ctx* c)
     if (c->srcTex) cudaDestroyTextureObject(c->srcTex);
     if (c->srcArr) cudaFreeArray(c->srcArr);
     cudaFree(c->planar);
-    cudaFree(c->planes);  cudaFree(c->cost);  cudaFree(c->prov);  cudaFree(c->seen);  cudaFree(c->refseen);  cudaFree(c->pid);  cudaFree(c->next_id);  cudaFree(c->memo_mask);  cudaFree(c->rng);  cudaFree(c->dispbuf);  cudaFree(c->candbuf);  cudaFree(c->canddepth);  cudaFree(c->sflags);  cudaFree(c->xchg);  cudaFree(c->gath);  cudaFree(c->refpad);  cudaFree(c->staging);
+    cudaFree(c->planes);  cudaFree(c->cost);  cudaFree(c->prov);  cudaFree(c->seen);  cudaFree(c->refseen);  cudaFree(c->pid);  cudaFree(c->next_id);  cudaFree(c->memo_mask);  cudaFree(c->rng);  cudaFree(c->dispbuf);  cudaFree(c->candbuf);  cudaFree(c->canddepth);  cudaFree(c->sflags);  cudaFree(c->xchg);  cudaFree(c->gath);  cudaFree(c->refpad);  cudaFree(c->staging);  cudaFree(c->geo_depth);  cudaFree(c->geo_kinv);
     cudaFree(c->d_cams);  cudaFree(c->d_stats);
     if (c->ev0) cudaEventDestroy(c->ev0);
     if (c->ev1) cudaEventDestroy(c->ev1);
@@ -605,6 +645,44 @@ extern "C" int gpm_set_view(gpm_ctx* c, int v, const float* img, size_t pitch_by
 extern "C" int gpm_set_view_color(gpm_ctx* c, int v, const float* rgba, size_t pitch_bytes, int on_device, const gpm_camera* cam)
 {
     return set_view<float4>("gpm_set_view_color", c, v, rgba, pitch_bytes, on_device, cam);
+}
+
+extern "C" int gpm_set_view_depth(gpm_ctx* c, int v, const float* depth, size_t pitch_bytes, int on_device)
+{
+    if (!c || !depth) return fail(GPM_E_ARG, "gpm_set_view_depth: null argument");
+    if (v < 0 || v >= c->maxV) return fail(GPM_E_ARG, "gpm_set_view_depth: view index out of range");
+    size_t pe = 0;
+    int rc = image_pitch<float>(c, pitch_bytes, &pe);
+    if (rc) return rc;
+    if (pe < (size_t)c->W) return fail(GPM_E_ARG, "gpm_set_view_depth: pitch_bytes is shorter than a row");
+    DeviceGuard g(c->device);
+    const size_t n = (size_t)c->W * c->H;
+    if (!c->geo_depth) CU(cudaMalloc(&c->geo_depth, n * c->maxV * sizeof(float)));
+    if (!c->geo_kinv) {
+        CU(cudaMalloc(&c->geo_kinv, sizeof(float) * 9 * c->maxV));
+        c->cams_dirty = true;                        // sync_cams copies the K^-1 table with the cameras
+    }
+    CU(cudaMemcpy2DAsync(c->geo_depth + n * v, (size_t)c->W * sizeof(float), depth, pe * sizeof(float), (size_t)c->W * sizeof(float), c->H,
+                         on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, c->stream));
+    CU(cudaStreamSynchronize(c->stream));
+    c->have_depth[v] = 1;
+    c->inputs_dirty = true;                          // the geometric term reads it: stored costs / memo are stale
+    return GPM_OK;
+}
+
+extern "C" int gpm_set_geometric(gpm_ctx* c, float weight, float max_err)
+{
+    if (!c) return fail(GPM_E_ARG, "gpm_set_geometric: null context");
+    if (!std::isfinite(weight) || weight < 0.f) return fail(GPM_E_ARG, "gpm_set_geometric: weight must be finite and >= 0");
+    if (!std::isfinite(max_err) || max_err <= 0.f) return fail(GPM_E_ARG, "gpm_set_geometric: max_err must be finite and > 0");
+    if (weight > 0.f) {
+        if (c->shard_world > 0) return fail(GPM_E_STATE, "gpm_set_geometric: view sharding does not support the geometric-consistency mode");
+        if (const int rc = check_geometric(c, weight)) return rc;
+    }
+    if (weight != c->geo_weight || max_err != c->geo_max_err) c->inputs_dirty = true;
+    c->geo_weight = weight;
+    c->geo_max_err = max_err;
+    return GPM_OK;
 }
 
 extern "C" int gpm_set_state(gpm_ctx* c, const float* norm4, const float* cost, int on_device)
@@ -783,15 +861,23 @@ static int shard_refine_steps(const gpm_params& p)
     return n;
 }
 
+// the source-view shard has no geometric-consistency variant: refused before anything is launched
+static int shard_refuses_geometric(gpm_ctx* c)
+{
+    return c->geo_weight > 0.f ? fail(GPM_E_STATE, "view sharding does not support the geometric-consistency mode (gpm_set_geometric weight 0)") : GPM_OK;
+}
+
 extern "C" int gpm_shard_num_stages(gpm_ctx* c)
 {
     if (!c || !c->have_params) { fail(GPM_E_STATE, "gpm_shard_num_stages: parameters not set");  return -1; }
+    if (shard_refuses_geometric(c)) return -1;
     return 2 + shard_refine_steps(c->prm);
 }
 
 extern "C" long long gpm_shard_stage_floats(gpm_ctx* c, int stage)
 {
     if (!c || !c->have_params || stage < 0) { fail(GPM_E_ARG, "gpm_shard_stage_floats: bad arguments");  return -1; }
+    if (shard_refuses_geometric(c)) return -1;
     const long long half = (long long)c->H * ((c->W + 1) / 2);
     const int slots = stage == 1 ? 8 : 1;
     return (stage == 0 ? 2 : 1) * half * slots * c->prm.n_best;
@@ -799,6 +885,7 @@ extern "C" long long gpm_shard_stage_floats(gpm_ctx* c, int stage)
 
 static int shard_common(gpm_ctx* c, int stage, KParams& P)
 {
+    if (const int rc = shard_refuses_geometric(c)) return rc;
     if (c->prm.cost_comb != GPM_COMB_BEST_N) return fail(GPM_E_ARG, "view sharding supports cost_comb = best_n only");
     if (c->opt_neighbours != 8) return fail(GPM_E_ARG, "view sharding supports the 8-neighbour sweep only (option neighbours = 8)");
     if (c->prm.n_best < 1 || c->prm.n_best > 32) return fail(GPM_E_ARG, "view sharding needs 1 <= n_best <= 32");
@@ -949,6 +1036,7 @@ static int shard_alloc_exchange(gpm_ctx* c)
 extern "C" int gpm_shard_comm_init(gpm_ctx* c, const void* id128, int rank, int world)
 {
     if (!c || world < 1 || world > 8 || rank < 0 || rank >= world) return fail(GPM_E_ARG, "gpm_shard_comm_init: bad arguments (1 <= world <= 8)");
+    if (const int rc = shard_refuses_geometric(c)) return rc;
     DeviceGuard g(c->device);
     gpm_shard_comm_destroy_(c);
     c->shard_rank = rank;  c->shard_world = world;
@@ -966,6 +1054,7 @@ extern "C" int gpm_shard_comm_init(gpm_ctx* c, const void* id128, int rank, int 
 extern "C" int gpm_shard_comm_attach(gpm_ctx* c, void* nccl_comm, int rank, int world)
 {
     if (!c || world < 1 || world > 8 || rank < 0 || rank >= world || (world > 1 && !nccl_comm)) return fail(GPM_E_ARG, "gpm_shard_comm_attach: bad arguments");
+    if (const int rc = shard_refuses_geometric(c)) return rc;
     if (world > 1 && !nccl_api()) return fail(GPM_E_STATE, "NCCL (libnccl.so.2) could not be loaded; set GPM_NCCL_LIB");
     gpm_shard_comm_destroy_(c);
     c->comm = nccl_comm;  c->shard_rank = rank;  c->shard_world = world;
@@ -1114,6 +1203,7 @@ extern "C" int gpm_set_option(gpm_ctx* c, const char* name, int value)
     }
     else if (n == "neighbours") {
         if (value != 8 && value != 20) return fail(GPM_E_ARG, "neighbours must be 8 (close + far kernels) or 20 (fused kernel)");
+        if (value == 20 && c->geo_weight > 0.f) return fail(GPM_E_ARG, "the geometric-consistency mode supports the 8-neighbour sweep only");
         DeviceGuard g(c->device);
         const int slots = value == 20 ? 20 : 8;
         if (slots != c->seen_slots) {

@@ -109,6 +109,15 @@ struct KParams {
     RefCam ref;
 };
 
+// Geometric-consistency term (DESIGN.md §14): what the k_sweep / k_cost_eval variants with GEO = true read besides KParams.
+// The per-view K, R and t are those of the photometric homography (ViewCam in shared memory).
+struct GeoParams {
+    const float* depth;         // [V][H][W] each source view's depth map, along that view's own optical axis
+    const float* kinv;          // [V][9] K^-1 of each source view
+    float Kref[9];              // the reference camera's K
+    float weight, max_err;
+};
+
 enum { ST_LAUNCH = 0, ST_HYP = 1, ST_SKIP = 2, ST_PRUNED = 3, ST_PAIRS = 4, ST_PAIRS_FULL = 5 };
 
 // ---- per-warp scratch in shared memory -------------------------------------------------------
@@ -246,6 +255,57 @@ __device__ __forceinline__ void local_topn(const KParams& P, float c0, float c1,
 
 struct WarpStats { unsigned hyp, skip, pruned; unsigned long long pairs, pairs_full; };
 
+// ---- geometric-consistency cost of one source view — DESIGN.md §14 ----------------------------------------------
+// IEEE round-to-nearest multiply, add, divide and square root only (no FMA, no approximate reciprocal), each product sum
+// evaluated as (a0 b0 + a1 b1) + a2 b2, so that a numpy restatement in float32 reproduces every bit (oracle/pygeo.py).
+__device__ __forceinline__ float fdiv(float a, float b) { return __fdiv_rn(a, b); }
+__device__ __forceinline__ float sum3(const float* m, float x, float y, float z)
+{
+    return fadd(fadd(fmul(m[0], x), fmul(m[1], y)), fmul(m[2], z));
+}
+
+// g_j = weight * min(err, max_err) of view v (camera `vc`: K, R, t as ViewCam) for plane (n, d) at pixel (px, py):
+// the plane's point on the pixel's ray goes into view j, to the nearest pixel (floor(x + 0.5)), back out at that pixel's
+// depth in view j's depth map, and into the reference image; err is the distance from p.  weight * max_err where that
+// pixel is off-image, its depth is not in [depthMin, depthMax] (0 included), or a point lies behind a camera.
+__device__ __forceinline__ float geo_cost(const KParams& P, const GeoParams& G, const float* __restrict__ vc, int v,
+                                          float nx, float ny, float nz, float d, float px, float py)
+{
+    const float* K = vc;
+    const float* R = vc + 9;
+    const float* t = vc + 18;
+    const float far = fmul(G.weight, G.max_err);
+    // the point X of the plane on the ray of p (the point the homography H_j maps p through): X = z K_ref^-1 (px, py, 1)
+    const float* Ki = P.ref.K_inv;
+    const float rx = sum3(Ki, px, py, 1.0f), ry = sum3(Ki + 3, px, py, 1.0f), rz = sum3(Ki + 6, px, py, 1.0f);
+    const float z = fdiv(-d, fadd(fadd(fmul(nx, rx), fmul(ny, ry)), fmul(nz, rz)));
+    if (!(z > 0.0f)) return far;
+    const float X = fmul(z, rx), Y = fmul(z, ry), Z = fmul(z, rz);
+    // into view j: Xj = R X + t, (u, v) = K Xj, rounded to the nearest pixel
+    const float xj = fadd(sum3(R, X, Y, Z), t[0]), yj = fadd(sum3(R + 3, X, Y, Z), t[1]), zj = fadd(sum3(R + 6, X, Y, Z), t[2]);
+    if (!(zj > 0.0f)) return far;
+    const float qz = sum3(K + 6, xj, yj, zj);
+    const float u = floorf(fadd(fdiv(sum3(K, xj, yj, zj), qz), 0.5f));
+    const float w = floorf(fadd(fdiv(sum3(K + 3, xj, yj, zj), qz), 0.5f));
+    if (!(u >= 0.0f && u <= (float)(P.W - 1) && w >= 0.0f && w <= (float)(P.H - 1))) return far;
+    const float D = __ldg(G.depth + ((size_t)v * P.H + (int)w) * P.W + (int)u);
+    if (!(D > 0.0f && D >= P.ref.depthMin && D <= P.ref.depthMax)) return far;
+    // back through view j's camera: Y = D K_j^-1 (u', v', 1), X' = R^T (Y - t); then into the reference image
+    const float* Kj = G.kinv + 9 * v;
+    const float ax = fsub(fmul(D, sum3(Kj, u, w, 1.0f)), t[0]);
+    const float ay = fsub(fmul(D, sum3(Kj + 3, u, w, 1.0f)), t[1]);
+    const float az = fsub(fmul(D, sum3(Kj + 6, u, w, 1.0f)), t[2]);
+    const float bx = fadd(fadd(fmul(R[0], ax), fmul(R[3], ay)), fmul(R[6], az));
+    const float by = fadd(fadd(fmul(R[1], ax), fmul(R[4], ay)), fmul(R[7], az));
+    const float bz = fadd(fadd(fmul(R[2], ax), fmul(R[5], ay)), fmul(R[8], az));
+    if (!(bz > 0.0f)) return far;
+    const float pz = sum3(G.Kref + 6, bx, by, bz);
+    const float ex = fsub(fdiv(sum3(G.Kref, bx, by, bz), pz), px);
+    const float ey = fsub(fdiv(sum3(G.Kref + 3, bx, by, bz), pz), py);
+    const float err = __fsqrt_rn(fadd(fmul(ex, ex), fmul(ey, ey)));
+    return fmul(G.weight, err < G.max_err ? err : G.max_err);      // a NaN err counts as max_err
+}
+
 // ---- cost of one plane hypothesis at the warp's pixel ---------------------------------------
 // pmCostMultiview_cu (gipuma.cu:720-806) over pmCost_shared (:585-680) / pmCostComputation_shared (:223-277).
 // Returns the exact combined cost, or — if `bound` is finite and an exact lower bound of the final cost
@@ -255,11 +315,15 @@ struct WarpStats { unsigned hyp, skip, pruned; unsigned long long pairs, pairs_f
 //   true : H2 + fma(H1, y, H0*x)   — the spatialPropClose/Far kernels, where nvcc hoisted the x products out of
 //          the inner (y) loop of gipuma.cu:633-634.  (Both are contractions of the same source line, gipuma.cu:213.)
 // XF = 2 takes the variant from `rt` at run time (the fused 20-neighbour kernels, whose inlined call sites differ).
-template <int XF, bool COLOR>
+// GEO: every view's cost is fadd(photometric cost, geo_cost) (DESIGN.md §14); (gpx, gpy) is the pixel.  The geometric terms
+// are computed before the first round and added to the partial costs of every bound test as well: g >= 0 and a rounded
+// add is monotone, so the bound stays an exact lower bound.
+template <int XF, bool COLOR, bool GEO = false>
 __device__ __forceinline__ float eval_plane(const KParams& P, const float* __restrict__ sCam, const WarpScratch& ws,
                                             cudaTextureObject_t src, float nx, float ny, float nz, float d,
                                             float bound, unsigned lane, WarpStats& st,
-                                            float* per_view0 = nullptr, float* per_view1 = nullptr, unsigned rt = 0u)
+                                            float* per_view0 = nullptr, float* per_view1 = nullptr, unsigned rt = 0u,
+                                            const GeoParams* G = nullptr, float gpx = 0.0f, float gpy = 0.0f)
 {
     // XF = 0 / 1: compile-time variant; XF = 2: per call, rt bit 0 = x-term first, bit 1 = gradient folding variant,
     // bits 2 / 3 = the Y / Z row of H deviates from bit 0 (ptxas chose per row in one inlined site of the fused kernel)
@@ -297,6 +361,11 @@ __device__ __forceinline__ float eval_plane(const KParams& P, const float* __res
         }
     }
     __syncwarp();
+    float g0 = 0.0f, g1 = 0.0f;          // geometric terms of views lane and lane + 32
+    if constexpr (GEO) {
+        if ((int)lane < P.V) g0 = geo_cost(P, *G, sCam + lane * GPM_VIEWCAM_FLOATS, (int)lane, nx, ny, nz, d, gpx, gpy);
+        if ((int)lane + 32 < P.V) g1 = geo_cost(P, *G, sCam + (lane + 32) * GPM_VIEWCAM_FLOATS, (int)lane + 32, nx, ny, nz, d, gpx, gpy);
+    }
 
     const float one_minus_alpha = fsub(1.0f, P.alpha);
     float c0 = 0.0f, c1 = 0.0f;
@@ -477,7 +546,9 @@ __device__ __forceinline__ float eval_plane(const KParams& P, const float* __res
         if (per_view0) {                       // view-shard mode: hand back the exact per-view costs, combine elsewhere
             if (last) { *per_view0 = c0;  *per_view1 = c1;  return 0.0f; }
         } else if (last || P.prune) {
-            const float b = combine_views(P, c0, c1, lane);
+            float b;
+            if constexpr (GEO) b = combine_views(P, fadd(c0, g0), fadd(c1, g1), lane);
+            else b = combine_views(P, c0, c1, lane);
             if (last) return b;
             if (b >= bound) { st.pruned++; return b; }
         }

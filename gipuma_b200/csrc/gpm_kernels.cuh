@@ -147,10 +147,12 @@ __global__ void k_init_planes(const __grid_constant__ KParams P, unsigned long l
 #define GPM_LB_THREADS 512       // max threads per block of the warp-per-pixel kernels (16 warps)
 #define GPM_LB_BLOCKS 1
 #endif
-template <bool COLOR>
+// GEO: the cost with the geometric-consistency term (DESIGN.md §14); G is only read then.
+template <bool COLOR, bool GEO = false>
 __global__ void __launch_bounds__(GPM_LB_THREADS, GPM_LB_BLOCKS)
 k_cost_eval(const __grid_constant__ KParams P, const __grid_constant__ CUtensorMap tmap, const ViewCam* __restrict__ cams,
-            cudaTextureObject_t src, const float4* __restrict__ planes, float* __restrict__ cost, unsigned long long* __restrict__ stats)
+            cudaTextureObject_t src, const float4* __restrict__ planes, float* __restrict__ cost, unsigned long long* __restrict__ stats,
+            const __grid_constant__ GeoParams G)
 {
     extern __shared__ __align__(128) float smem[];
     float* tile = smem;
@@ -167,9 +169,11 @@ k_cost_eval(const __grid_constant__ KParams P, const __grid_constant__ CUtensorM
         setup_window<COLOR>(P, tile + P.tile_xo, ws, px, py, tile_x0, tile_y0, lane);
         const float4 n = planes[(size_t)py * P.W + px];
         const float inf = __int_as_float(0x7f800000);
-        const float c = (P.cost_rt & 12) ? eval_plane<2, COLOR>(P, sCam, ws, src, n.x, n.y, n.z, n.w, inf, lane, st, nullptr, nullptr, (unsigned)P.cost_rt)
-                        : P.cost_variant ? eval_plane<1, COLOR>(P, sCam, ws, src, n.x, n.y, n.z, n.w, inf, lane, st)
-                                         : eval_plane<0, COLOR>(P, sCam, ws, src, n.x, n.y, n.z, n.w, inf, lane, st);
+        const GeoParams* g = GEO ? &G : nullptr;
+        const float fpx = __int2float_rn(px), fpy = __int2float_rn(py);
+        const float c = (P.cost_rt & 12) ? eval_plane<2, COLOR, GEO>(P, sCam, ws, src, n.x, n.y, n.z, n.w, inf, lane, st, nullptr, nullptr, (unsigned)P.cost_rt, g, fpx, fpy)
+                        : P.cost_variant ? eval_plane<1, COLOR, GEO>(P, sCam, ws, src, n.x, n.y, n.z, n.w, inf, lane, st, nullptr, nullptr, 0u, g, fpx, fpy)
+                                         : eval_plane<0, COLOR, GEO>(P, sCam, ws, src, n.x, n.y, n.z, n.w, inf, lane, st, nullptr, nullptr, 0u, g, fpx, fpy);
         if (lane == 0) cost[(size_t)py * P.W + px] = c;
     }
     flush_stats(stats, st, lane);
@@ -212,13 +216,16 @@ __device__ __forceinline__ bool close_far_neighbour(int k, const int& px, const 
     return ok;
 }
 
-template <bool COLOR, bool FUSED>
+// GEO: the cost with the geometric-consistency term (DESIGN.md §14; 8-neighbour sweep only); G is only read then.
+template <bool COLOR, bool FUSED, bool GEO = false>
 __global__ void __launch_bounds__(GPM_LB_THREADS, GPM_LB_BLOCKS)
 k_sweep(const __grid_constant__ KParams P, const __grid_constant__ CUtensorMap tmap, const ViewCam* __restrict__ cams,
         cudaTextureObject_t src, float4* __restrict__ planes, float* __restrict__ cost,
         unsigned* __restrict__ rng_state, unsigned char* __restrict__ prov, Memo M, int colour, int phase_mask,
-        unsigned long long* __restrict__ stats)
+        unsigned long long* __restrict__ stats, const __grid_constant__ GeoParams G)
 {
+    static_assert(!(FUSED && GEO), "the geometric term is built for the 8-neighbour sweep only");
+    const GeoParams* g = GEO ? &G : nullptr;
     extern __shared__ __align__(128) float smem[];
     float* tile = smem;
     float* sCam = tile + tile_floats(P);
@@ -310,7 +317,8 @@ k_sweep(const __grid_constant__ KParams P, const __grid_constant__ CUtensorMap t
                 if (!in_range || same_now || dup) { st.skip++; continue; }
                 if (!window_ready) { setup_window<COLOR>(P, tile + P.tile_xo, ws, px, py, tile_x0, tile_y0, lane);  window_ready = true; }
                 const float c = FUSED ? eval_plane<2, COLOR>(P, sCam, ws, src, nb.x, nb.y, nb.z, nb.w, cost_now, lane, st, nullptr, nullptr, site)
-                                      : eval_plane<(COLOR ? 0 : 1), COLOR>(P, sCam, ws, src, nb.x, nb.y, nb.z, nb.w, cost_now, lane, st);
+                                      : eval_plane<(COLOR ? 0 : 1), COLOR, GEO>(P, sCam, ws, src, nb.x, nb.y, nb.z, nb.w, cost_now, lane, st,
+                                                                                nullptr, nullptr, 0u, g, fpx, fpy);
                 if (c < cost_now) {                                                              // :867-871
                     disp_now = disp_before;
                     norm_now = nb;
@@ -367,7 +375,8 @@ k_sweep(const __grid_constant__ KParams P, const __grid_constant__ CUtensorMap t
                     cand.w = plane_d(cam, cand.x, cand.y, cand.z, fpx, fpy, depth_new);   // :969
                     const unsigned rsite = FUSED ? (unsigned)P.site[20] : 0u;
                     const float c = FUSED ? eval_plane<2, COLOR>(P, sCam, ws, src, cand.x, cand.y, cand.z, cand.w, cost_now, lane, st, nullptr, nullptr, rsite)
-                                          : eval_plane<0, COLOR>(P, sCam, ws, src, cand.x, cand.y, cand.z, cand.w, cost_now, lane, st);
+                                          : eval_plane<0, COLOR, GEO>(P, sCam, ws, src, cand.x, cand.y, cand.z, cand.w, cost_now, lane, st,
+                                                                      nullptr, nullptr, 0u, g, fpx, fpy);
                     if (c < cost_now) {                                                          // :986-990 (no depth-range test)
                         prov_now = (int)rsite;
                         any_accept = true;

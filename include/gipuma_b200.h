@@ -88,6 +88,23 @@ int gpm_set_view_color(gpm_ctx* ctx, int v, const float* rgba, size_t pitch_byte
 /* Number of source views actually used (viewSelectionSubsetNumber, main.cpp:918). */
 int gpm_set_num_views(gpm_ctx* ctx, int n_views);
 
+/* ---- geometric consistency (DESIGN.md §14) ----------------------------------------------------------------------------
+ * A second PatchMatch pass may score each hypothesis against the source views' own depth maps as well: with weight > 0 the
+ * cost of view j becomes photo_j + g_j, g_j = weight * min(err, max_err), where err is the forward-backward reprojection
+ * error in pixels of the hypothesis' point through view j's depth map (weight * max_err where that depth is missing, out of
+ * [depthMin, depthMax] or the point is off-image or behind a camera).  The views are combined as before.  Every cost the
+ * context computes (gpm_init, gpm_sweep, gpm_phase, gpm_cost_eval, gpm_run) uses it while it is on.
+ * gpm_set_view_depth: view v's depth map, width x height floats (pitch_bytes between rows, 0 = packed; host or device
+ *   memory), each pixel's depth along view v's own optical axis as gpm_finalize writes it (0 = no depth).  The cameras are
+ *   those of gpm_set_view (K^-1 included) and the reference's K.  Storage is allocated by the first call.
+ * gpm_set_geometric: weight 0 (the default) turns the mode off and gives exactly the photometric cost.  Refused with
+ *   GPM_E_ARG: weight negative or not finite, max_err not finite or <= 0, option neighbours = 20 (the fused sweep has no
+ *   such variant); with GPM_E_STATE: a used view (0 .. n_views-1) without a depth map — also at the next launch, if
+ *   gpm_set_num_views adds one.  The source-view shard (every gpm_shard_* call taking a context) has no such variant and
+ *   refuses to run while the mode is on. */
+int gpm_set_view_depth(gpm_ctx* ctx, int v, const float* depth, size_t pitch_bytes, int on_device);
+int gpm_set_geometric(gpm_ctx* ctx, float weight, float max_err);
+
 /* Seed of the per-pixel curand_init(seed, y, x) at initialisation (gipuma.cu:1019; the reference uses
  * clock64()) and the refinement RNG mode. */
 int gpm_set_rng(gpm_ctx* ctx, unsigned long long seed, int mode);
