@@ -11,7 +11,6 @@ from __future__ import annotations
 
 import ctypes as C
 import os
-import time
 from typing import Optional
 
 import numpy as np
@@ -51,6 +50,16 @@ class GpmBatchDesc(C.Structure):
 class GpmBatchStats(C.Structure):
     _fields_ = [("jobs_done", C.c_int), ("sweep_ms_total", C.c_double), ("per_job_sweep_ms", C.POINTER(C.c_float)),
                 ("per_job_views", C.POINTER(C.c_int)), ("per_job_device", C.POINTER(C.c_int))]
+
+
+class GpmGeoBatchDesc(C.Structure):
+    _fields_ = [("batch", GpmBatchDesc), ("channels", C.c_int), ("geo_iterations", C.c_int), ("weight", C.c_float),
+                ("max_err", C.c_float)]
+
+
+class GpmGeoBatchStats(C.Structure):
+    _fields_ = [("batch", GpmBatchStats), ("n_pass1", C.c_int), ("pass1_views", C.POINTER(C.c_int)),
+                ("pass1_sweep_ms", C.POINTER(C.c_float)), ("ref_views", C.POINTER(C.c_int))]
 
 
 class GpmFuseCamera(C.Structure):
@@ -145,6 +154,7 @@ def load_library():
     L.gpm_shard_run.argtypes = [vp, fp]
     L.gpm_measure_fetch_peak.argtypes = [vp, C.POINTER(C.c_double)]
     L.gpm_batch_run.argtypes = [C.POINTER(GpmBatchDesc), C.POINTER(GpmBatchStats)]
+    L.gpm_geo_batch_run.argtypes = [C.POINTER(GpmGeoBatchDesc), C.POINTER(GpmGeoBatchStats)]
     L.gpm_batch_last_error.restype = C.c_char_p
     L.gpm_stream.restype = vp
     L.gpm_fuse_cameras.argtypes = [C.POINTER(C.c_double), C.c_int, C.c_double, C.POINTER(GpmFuseCamera)]
@@ -157,7 +167,7 @@ def load_library():
                  "gpm_finalize", "gpm_cost_eval", "gpm_run", "gpm_get_stats", "gpm_reset_stats", "gpm_set_option",
                  "gpm_init_planes", "gpm_shard_num_stages", "gpm_shard_stage", "gpm_shard_finish_init", "gpm_shard_unique_id",
                  "gpm_shard_comm_init", "gpm_shard_comm_attach", "gpm_shard_run", "gpm_measure_fetch_peak", "gpm_batch_run",
-                 "gpm_prepare_cameras", "gpm_select_views", "gpm_write_dmb", "gpm_read_dmb", "gpm_write_result_dmb",
+                 "gpm_geo_batch_run", "gpm_prepare_cameras", "gpm_select_views", "gpm_write_dmb", "gpm_read_dmb", "gpm_write_result_dmb",
                  "gpm_fuse_cameras", "gpm_fuse", "gpm_write_ply", "gpm_nearest_dist"):
         getattr(L, name).restype = C.c_int
     _lib = L
@@ -478,20 +488,14 @@ def select_views(cams, cols: int, rows: int, min_angle: float, max_angle: float,
     return [sub[i] for i in range(n)], (rng[0], rng[1])
 
 
-def batch_run(images, Ps, params, refs, devices=(0,), cam_scale: float = 1.0, min_angle: float = 10.0, max_angle: float = 30.0,
-              max_views: int = 9, seed: int = 0xC0FFEE, out_dir: Optional[str] = None, want_outputs: bool = True):
-    """Reference-view batch in ONE process (gpm_batch_run): `images` [n, H, W] float32 (shared, page-locked once), `Ps` n 3x4
-    projections, `refs` the reference views to process, `devices` the CUDA ordinals to use (one worker thread each).
-    Returns (norm4 [len(refs), H, W, 4] or None, cost or None, stats dict)."""
-    lib = load_library()
-    imgs = np.ascontiguousarray(images, dtype=np.float32)
-    n, H, W = imgs.shape
+def _batch_desc(imgs, Ps, params, refs, devices, cam_scale, min_angle, max_angle, max_views, seed, out_dir, n4, cc):
+    """gpm_batch_desc over contiguous float32 images [n, H, W(, 4)] and output arrays (or None).  Returns it with the arrays
+    it points into, which must outlive the call."""
+    n, H, W = imgs.shape[:3]
     ptrs = (C.c_void_p * n)(*[C.c_void_p(imgs[i].ctypes.data) for i in range(n)])
     P = np.ascontiguousarray(np.stack([np.asarray(p, dtype=np.float64) for p in Ps]).reshape(-1))
     refs_a = (C.c_int * len(refs))(*[int(r) for r in refs])
     devs = (C.c_int * len(devices))(*[int(d) for d in devices])
-    n4 = np.empty((len(refs), H, W, 4), np.float32) if want_outputs else None
-    cc = np.empty((len(refs), H, W), np.float32) if want_outputs else None
     d = GpmBatchDesc()
     d.n_images, d.width, d.height = n, W, H
     d.images, d.pitch_bytes = ptrs, 0
@@ -500,56 +504,53 @@ def batch_run(images, Ps, params, refs, devices=(0,), cam_scale: float = 1.0, mi
     d.min_angle, d.max_angle, d.max_views = float(min_angle), float(max_angle), int(max_views)
     d.ref_indices, d.n_refs, d.devices, d.n_devices, d.seed = refs_a, len(refs), devs, len(devices), seed
     d.out_dir = out_dir.encode() if out_dir else None
-    d.out_norm4 = n4.ctypes.data_as(C.POINTER(C.c_float)) if want_outputs else None
-    d.out_cost = cc.ctypes.data_as(C.POINTER(C.c_float)) if want_outputs else None
-    ms = (C.c_float * len(refs))()
-    nv = (C.c_int * len(refs))()
-    dv = (C.c_int * len(refs))()
-    st = GpmBatchStats(0, 0.0, ms, nv, dv)
+    d.out_norm4 = n4.ctypes.data_as(C.POINTER(C.c_float)) if n4 is not None else None
+    d.out_cost = cc.ctypes.data_as(C.POINTER(C.c_float)) if cc is not None else None
+    return d, (imgs, ptrs, P, refs_a, devs, n4, cc)
+
+
+def _job_stats(n_refs):
+    """gpm_batch_stats with per-job arrays for n_refs jobs."""
+    return GpmBatchStats(0, 0.0, (C.c_float * n_refs)(), (C.c_int * n_refs)(), (C.c_int * n_refs)())
+
+
+def batch_run(images, Ps, params, refs, devices=(0,), cam_scale: float = 1.0, min_angle: float = 10.0, max_angle: float = 30.0,
+              max_views: int = 9, seed: int = 0xC0FFEE, out_dir: Optional[str] = None, want_outputs: bool = True):
+    """Reference-view batch in ONE process (gpm_batch_run): `images` [n, H, W] float32 (shared, page-locked once), `Ps` n 3x4
+    projections, `refs` the reference views to process, `devices` the CUDA ordinals to use (one worker thread each).
+    Returns (norm4 [len(refs), H, W, 4] or None, cost or None, stats dict)."""
+    lib = load_library()
+    imgs = np.ascontiguousarray(images, dtype=np.float32)
+    n, H, W = imgs.shape
+    n4 = np.empty((len(refs), H, W, 4), np.float32) if want_outputs else None
+    cc = np.empty((len(refs), H, W), np.float32) if want_outputs else None
+    d, _keep = _batch_desc(imgs, Ps, params, refs, devices, cam_scale, min_angle, max_angle, max_views, seed, out_dir, n4, cc)
+    st = _job_stats(len(refs))
     rc = lib.gpm_batch_run(C.byref(d), C.byref(st))
     if rc != 0:
         raise GipumaError("gpm_batch_run failed (%d): %s" % (rc, lib.gpm_batch_last_error().decode()))
-    return n4, cc, {"jobs_done": st.jobs_done, "sweep_ms_total": st.sweep_ms_total, "sweep_ms": list(ms), "views": list(nv), "device": list(dv)}
-
-
-def _load_job(ctx, images, Ps, params, ref, cam_scale, min_angle, max_angle, max_views, seed):
-    """Set `ctx` up for reference view `ref` as gpm_batch_run does (cameras re-based on it, source views selected, depth
-    range and disparities as main.cpp derives them).  Returns the image indices of the selected source views."""
-    n, H, W = images.shape[:3]
-    order = [ref] + [i for i in range(n) if i != ref]
-    cams = prepare_cameras([Ps[i] for i in order], cam_scale)
-    subset, (lo, hi) = select_views(cams, W, H, min_angle, max_angle, max_views)
-    if not subset:
-        raise GipumaError("no source view passes the angle filter for reference %d" % ref)
-    p = GpmParams.from_buffer_copy(pack_params(params))
-    if p.depthMin <= 0:
-        p.depthMin = lo
-    if p.depthMax <= 0:
-        p.depthMax = hi
-    fb = np.float32(cams[0].f) * np.float32(cams[0].baseline)                  # float arithmetic, as gpm_batch.cpp
-    p.min_disparity, p.max_disparity = float(fb / np.float32(p.depthMax)), float(fb / np.float32(p.depthMin))
-    ctx._check(ctx.lib.gpm_set_params(ctx.h, C.byref(p)))
-    ctx.set_reference(images[ref], cams[0])
-    for v, k in enumerate(subset):
-        ctx.set_view(v, images[order[k]], cams[k])
-    ctx.set_num_views(len(subset))
-    ctx.set_rng(seed, GPM_RNG_REFERENCE)
-    return [order[k] for k in subset]
+    k = len(refs)
+    return n4, cc, {"jobs_done": st.jobs_done, "sweep_ms_total": st.sweep_ms_total, "sweep_ms": st.per_job_sweep_ms[:k],
+                    "views": st.per_job_views[:k], "device": st.per_job_device[:k]}
 
 
 def geometric_pass(images, Ps, params, refs, geo_iterations: int = 2, weight: float = GEO_WEIGHT, max_err: float = GEO_MAX_ERR,
                    cam_scale: float = 1.0, min_angle: float = 10.0, max_angle: float = 30.0, max_views: int = 9,
-                   seed: int = 0xC0FFEE, device: int = 0):
-    """PatchMatch with a geometric-consistency second pass (DESIGN.md §14) for the reference views `refs`.
+                   seed: int = 0xC0FFEE, devices=(0,), out_dir: Optional[str] = None):
+    """PatchMatch with a geometric-consistency second pass (DESIGN.md §14) for the reference views `refs`, run by the
+    native two-pass batch driver (gpm_geo_batch_run) over the worker pool of `devices` (one worker thread and context each;
+    a device may be listed more than once).
 
     Pass 1, for every reference view and every source view one of them selects: init, params.iterations photometric sweeps,
-    finalize; the view setup is gpm_batch_run's.  Pass 2, per reference view: the selected source views' pass-1 depth maps
-    are uploaded, the geometric term is turned on (weight, max_err), the pass-1 planes get their exact costs under the new
-    cost (cost_eval), and geo_iterations sweeps and finalize follow.  So a run has params.iterations + geo_iterations
-    iterations in all.  images: [n, H, W] grey or [n, H, W, 4] colour; the other arguments as batch_run.
+    finalize; the view setup is gpm_batch_run's.  Every worker finishes pass 1 before pass 2 starts.  Pass 2, per reference
+    view: the selected source views' pass-1 depth maps are uploaded, the geometric term is turned on (weight, max_err), the
+    pass-1 planes get their exact costs under the new cost (cost_eval), and geo_iterations sweeps and finalize follow.  So a
+    run has params.iterations + geo_iterations iterations in all.  images: [n, H, W] grey or [n, H, W, 4] colour; the other
+    arguments as batch_run; out_dir: None, or where <ref, 8 digits>/{disp,normals}.dmb of the pass-2 results are written.
     Returns (norm4 [len(refs), H, W, 4], cost [len(refs), H, W], info) with norm4 as batch_run returns it, so fuse and
-    evaluate_cloud take it unchanged; info: "pass1_views" (the views pass 1 ran), "pass1_sweep_s" and "pass2_sweep_s" (host
-    seconds of each view's sweep call, which ends in a stream synchronisation), "views" (source views per reference)."""
+    evaluate_cloud take it unchanged; info: "pass1_views" (the views pass 1 ran, ascending), "pass1_sweep_s" (in that order)
+    and "pass2_sweep_s" (per reference view): CUDA-event seconds of each view's sweep call on its context's stream;
+    "views" (image indices of the source views each reference view selected), "device" (the device that ran its pass 2)."""
     check_geometric(weight, max_err)
     if int(geo_iterations) != geo_iterations or geo_iterations < 0:
         raise ValueError("geo_iterations must be an integer >= 0")
@@ -564,42 +565,24 @@ def geometric_pass(images, Ps, params, refs, geo_iterations: int = 2, weight: fl
         raise ValueError("reference views must be image indices in 0..%d" % (n - 1))
     if not 1 <= max_views <= 64:
         raise ValueError("max_views must be 1..64")
-    job = dict(cam_scale=cam_scale, min_angle=min_angle, max_angle=max_angle, max_views=max_views, seed=seed)
-    n4 = np.empty((len(refs), H, W, 4), np.float32)
-    cc = np.empty((len(refs), H, W), np.float32)
-    info = {"pass1_views": [], "pass1_sweep_s": [], "pass2_sweep_s": [], "views": []}
-    with Context(W, H, max_views, device) as ctx:
-        sources, raw, depth = {}, {}, {}
-        todo = list(dict.fromkeys(refs))
-        while todo:                                        # pass 1: the reference views, then the source views they read
-            r = todo.pop(0)
-            if r in depth:
-                continue
-            sources[r] = _load_job(ctx, imgs, Ps, params, r, **job)
-            ctx.init()
-            t0 = time.perf_counter()
-            ctx.sweep(params.iterations)
-            info["pass1_sweep_s"].append(time.perf_counter() - t0)
-            if r in refs:
-                raw[r] = ctx.get_state()[0]
-            ctx.finalize()
-            depth[r] = np.ascontiguousarray(ctx.get_state()[0][..., 3])
-            info["pass1_views"].append(r)
-            if r in refs:
-                todo += [i for i in sources[r] if i not in depth]
-        for j, r in enumerate(refs):                       # pass 2
-            src = _load_job(ctx, imgs, Ps, params, r, **job)
-            for v, i in enumerate(src):
-                ctx.set_view_depth(v, depth[i])
-            ctx.set_geometric(weight, max_err)
-            ctx.set_state(raw[r], ctx.cost_eval(raw[r]))
-            t0 = time.perf_counter()
-            ctx.sweep(geo_iterations)
-            info["pass2_sweep_s"].append(time.perf_counter() - t0)
-            ctx.finalize()
-            n4[j], cc[j] = ctx.get_state()
-            ctx.set_geometric(0.0, max_err)
-            info["views"].append(src)
+    lib = load_library()
+    k = len(refs)
+    n4 = np.empty((k, H, W, 4), np.float32)
+    cc = np.empty((k, H, W), np.float32)
+    d, _keep = _batch_desc(imgs, Ps, params, refs, devices, cam_scale, min_angle, max_angle, max_views, seed, out_dir, n4, cc)
+    g = GpmGeoBatchDesc(d, 1 if imgs.ndim == 3 else 4, int(geo_iterations), float(weight), float(max_err))
+    p1_views, p1_ms = (C.c_int * n)(), (C.c_float * n)()
+    ref_views = (C.c_int * (k * int(max_views)))()
+    jobs = _job_stats(k)                                   # owns the per-job arrays st.batch points into
+    st = GpmGeoBatchStats(jobs, 0, p1_views, p1_ms, ref_views)
+    rc = lib.gpm_geo_batch_run(C.byref(g), C.byref(st))
+    if rc != 0:
+        raise GipumaError("gpm_geo_batch_run failed (%d): %s" % (rc, lib.gpm_batch_last_error().decode()))
+    m = st.n_pass1
+    views = [[v for v in ref_views[j * max_views:(j + 1) * max_views] if v >= 0] for j in range(k)]
+    info = {"pass1_views": p1_views[:m], "pass1_sweep_s": [t / 1e3 for t in p1_ms[:m]],
+            "pass2_sweep_s": [t / 1e3 for t in st.batch.per_job_sweep_ms[:k]], "views": views,
+            "device": st.batch.per_job_device[:k]}
     return n4, cc, info
 
 

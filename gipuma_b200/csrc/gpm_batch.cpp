@@ -6,12 +6,16 @@
 // cameras on it (gpm_prepare_cameras, cameraGeometryUtils.h:174-353), selects the source views (gpm_select_views,
 // main.cpp:430-499, deterministic), derives the depth / disparity range as main.cpp:480-483 and :898-906 do, runs the job
 // (gpm_run) and hands back / writes the result (disp.dmb + normals.dmb, main.cpp:1002-1003, for the external fusibile).
-// Host C++ over the C-ABI; the only CUDA calls are cudaHostRegister / cudaHostUnregister.
+// gpm_geo_batch_run runs the two-pass geometric-consistency flow (DESIGN.md §14) on the same pool and image cache.
+// Host C++ over the C-ABI; the only CUDA calls are page-locking, the geometric driver's host store and its sweep events.
 #include "../../include/gipuma_b200.h"
 
 #include <cuda_runtime.h>
 
+#include <algorithm>
 #include <atomic>
+#include <cmath>
+#include <condition_variable>
 #include <cstdio>
 #include <cstring>
 #include <mutex>
@@ -24,6 +28,118 @@ namespace {
 std::mutex g_err_mutex;
 std::string g_batch_err;
 void set_err(const std::string& m) { std::lock_guard<std::mutex> l(g_err_mutex);  if (g_batch_err.empty()) g_batch_err = m; }
+void clear_err() { std::lock_guard<std::mutex> l(g_err_mutex);  g_batch_err.clear(); }
+
+bool batch_desc_ok(const gpm_batch_desc* d)
+{
+    return d && d->images && d->P && d->n_images >= 2 && d->width >= 8 && d->height >= 8 && d->n_devices >= 1 && d->devices &&
+           d->n_refs >= 1 && d->max_views >= 1 && d->max_views <= GPM_MAX_VIEWS;
+}
+
+// One view's job as the reference's main.cpp sets it up: cameras re-based on the view (main.cpp: img_filenames[0] is the
+// reference image), the selected source views and the parameters with the depth / disparity range.  Host only.
+struct ViewSetup {
+    std::vector<double> P;
+    std::vector<gpm_camera> cams;       // cams[k]: camera of image order[k], re-based on order[0]
+    std::vector<int> order, subset;     // subset[0 .. nv-1]: positions in `order` of the selected source views
+    int nv = 0;
+    gpm_params p{};
+    int source(int v) const { return order[subset[v]]; }
+};
+
+// false: no source view passes the angle filter (or the cameras cannot be prepared)
+bool plan_view(const gpm_batch_desc* d, int ref, ViewSetup& s)
+{
+    const int n = d->n_images, W = d->width, H = d->height;
+    s.P.resize((size_t)n * 12);  s.cams.resize(n);  s.order.resize(n);  s.subset.resize(n);
+    s.order[0] = ref;
+    for (int i = 0, k = 1; i < n; i++) if (i != ref) s.order[k++] = i;
+    for (int i = 0; i < n; i++) memcpy(&s.P[(size_t)i * 12], d->P + (size_t)s.order[i] * 12, 12 * sizeof(double));
+    const int rc = gpm_prepare_cameras(s.P.data(), n, d->cam_scale > 0 ? d->cam_scale : 1.0, s.cams.data());
+    float range[2] = {0.f, 0.f};
+    s.nv = rc == GPM_OK ? gpm_select_views(s.cams.data(), n, W, H, d->min_angle, d->max_angle, d->max_views, s.subset.data(), range) : -1;
+    if (s.nv < 1) return false;
+    s.p = d->params;
+    if (s.p.depthMin <= 0) s.p.depthMin = range[0];                                   // main.cpp:480-483
+    if (s.p.depthMax <= 0) s.p.depthMax = range[1];
+    s.p.min_disparity = s.cams[0].f * s.cams[0].baseline / s.p.depthMax;             // main.cpp:905-906
+    s.p.max_disparity = s.cams[0].f * s.cams[0].baseline / s.p.depthMin;
+    return true;
+}
+
+// The per-view uploads of a job: parameters, reference and source images (grey: channels 1, RGBA: 4), view count, RNG.
+int load_view(gpm_ctx* ctx, const gpm_batch_desc* d, int channels, size_t pitch, const ViewSetup& s)
+{
+    auto set_reference = channels == 4 ? gpm_set_reference_color : gpm_set_reference;
+    auto set_view = channels == 4 ? gpm_set_view_color : gpm_set_view;
+    int rc = gpm_set_params(ctx, &s.p);
+    if (rc == GPM_OK) rc = set_reference(ctx, d->images[s.order[0]], pitch, 0, &s.cams[0]);
+    for (int v = 0; v < s.nv && rc == GPM_OK; v++) rc = set_view(ctx, v, d->images[s.source(v)], pitch, 0, &s.cams[s.subset[v]]);
+    if (rc == GPM_OK) rc = gpm_set_num_views(ctx, s.nv);
+    if (rc == GPM_OK) rc = gpm_set_rng(ctx, d->seed, GPM_RNG_REFERENCE);
+    return rc;
+}
+
+// <out_dir>/<ref as 8 digits>/disp.dmb, normals.dmb — what the per-image processes of the script leave for fusibile
+int write_result(const char* out_dir, int ref, const float* norm4, int H, int W)
+{
+    char dir[1024];
+    snprintf(dir, sizeof(dir), "%s/%08d", out_dir, ref);
+    mkdir(out_dir, 0777);  mkdir(dir, 0777);
+    const std::string dp = std::string(dir) + "/disp.dmb", np_ = std::string(dir) + "/normals.dmb";
+    return gpm_write_result_dmb(dp.c_str(), np_.c_str(), norm4, H, W);
+}
+
+// The shared image cache: every image page-locked once (cudaHostRegisterPortable: usable from every device's context) for
+// the lifetime of this object.  An image that was already pinned (or cannot be) is simply used as it is.
+class PinnedImages {
+public:
+    PinnedImages(const gpm_batch_desc* d, size_t bytes) : d_(d), registered_(d->n_images, 0)
+    {
+        for (int i = 0; i < d->n_images; i++)
+            registered_[i] = cudaHostRegister(const_cast<float*>(d->images[i]), bytes, cudaHostRegisterPortable) == cudaSuccess;
+        cudaGetLastError();
+    }
+    ~PinnedImages() { for (int i = 0; i < d_->n_images; i++) if (registered_[i]) cudaHostUnregister(const_cast<float*>(d_->images[i])); }
+    PinnedImages(const PinnedImages&) = delete;
+    PinnedImages& operator=(const PinnedImages&) = delete;
+private:
+    const gpm_batch_desc* d_;
+    std::vector<char> registered_;
+};
+
+// One worker thread and context per listed device; body(ctx, dev) runs on that thread.  A worker whose context cannot be
+// created records the error, counts as failed and still runs body with ctx = nullptr, so that it reaches any barrier in it;
+// take_jobs checks `failed` before every job, so such a body never gets to use the context.
+template <class Body>
+void run_workers(const gpm_batch_desc* d, std::atomic<int>& failed, Body body)
+{
+    auto worker = [&](int dev) {
+        gpm_ctx* ctx = nullptr;
+        if (gpm_create(&ctx, dev, d->width, d->height, d->max_views) != GPM_OK) {
+            set_err(std::string("gpm_create: ") + gpm_last_error());
+            failed++;
+            ctx = nullptr;
+        }
+        body(ctx, dev);
+        if (ctx) gpm_destroy(ctx);
+    };
+    std::vector<std::thread> pool;
+    for (int k = 0; k < d->n_devices; k++) pool.emplace_back(worker, d->devices[k]);
+    for (auto& t : pool) t.join();
+}
+
+// Jobs 0 .. n-1 from the shared counter `next` until they run out or any worker has failed; fn(job) returns false after
+// recording its error.
+template <class Fn>
+void take_jobs(std::atomic<int>& next, int n, std::atomic<int>& failed, Fn fn)
+{
+    for (;;) {
+        const int job = next.fetch_add(1);
+        if (job >= n || failed.load()) return;
+        if (!fn(job)) { failed++;  return; }
+    }
+}
 }  // namespace
 
 extern "C" const char* gpm_batch_last_error(void)
@@ -36,84 +152,240 @@ extern "C" const char* gpm_batch_last_error(void)
 
 extern "C" int gpm_batch_run(const gpm_batch_desc* d, gpm_batch_stats* stats)
 {
-    { std::lock_guard<std::mutex> l(g_err_mutex);  g_batch_err.clear(); }
-    if (!d || !d->images || !d->P || d->n_images < 2 || d->width < 8 || d->height < 8 || d->n_devices < 1 || !d->devices ||
-        d->n_refs < 1 || d->max_views < 1 || d->max_views > GPM_MAX_VIEWS) {
+    clear_err();
+    if (!batch_desc_ok(d)) {
         set_err("gpm_batch_run: bad arguments");
         return GPM_E_ARG;
     }
     const int n = d->n_images, W = d->width, H = d->height;
     const size_t pitch = d->pitch_bytes ? d->pitch_bytes : (size_t)W * sizeof(float);
     const size_t npix = (size_t)W * H;
-    // shared image cache: page-lock every image once (cudaHostRegisterPortable: usable from every device's context)
-    std::vector<char> registered(n, 0);
-    for (int i = 0; i < n; i++)
-        registered[i] = cudaHostRegister(const_cast<float*>(d->images[i]), pitch * H, cudaHostRegisterPortable) == cudaSuccess;
-    cudaGetLastError();                     // an image that was already pinned (or cannot be) is simply used as it is
+    PinnedImages pinned(d, pitch * H);
 
     std::atomic<int> next(0), failed(0);
     std::vector<double> sweep_ms(d->n_refs, 0.0);
     std::vector<int> views_used(d->n_refs, 0), device_of(d->n_refs, -1);
-    auto worker = [&](int dev) {
-        gpm_ctx* ctx = nullptr;
-        if (gpm_create(&ctx, dev, W, H, d->max_views) != GPM_OK) { set_err(std::string("gpm_create: ") + gpm_last_error());  failed++;  return; }
-        std::vector<double> P((size_t)n * 12);
-        std::vector<gpm_camera> cams(n);
-        std::vector<int> order(n), subset(n);
-        std::vector<float> n4, cost;
-        for (;;) {
-            const int job = next.fetch_add(1);
-            if (job >= d->n_refs || failed.load()) break;
+    run_workers(d, failed, [&](gpm_ctx* ctx, int dev) {
+        ViewSetup s;
+        std::vector<float> n4;
+        take_jobs(next, d->n_refs, failed, [&](int job) {
             const int ref = d->ref_indices ? d->ref_indices[job] : job;
-            if (ref < 0 || ref >= n) { set_err("gpm_batch_run: reference index out of range");  failed++;  break; }
-            // cameras with the reference first (main.cpp: img_filenames[0] is the reference image)
-            order[0] = ref;
-            for (int i = 0, k = 1; i < n; i++) if (i != ref) order[k++] = i;
-            for (int i = 0; i < n; i++) memcpy(&P[(size_t)i * 12], d->P + (size_t)order[i] * 12, 12 * sizeof(double));
-            int rc = gpm_prepare_cameras(P.data(), n, d->cam_scale > 0 ? d->cam_scale : 1.0, cams.data());
-            float range[2] = {0.f, 0.f};
-            const int nv = rc == GPM_OK ? gpm_select_views(cams.data(), n, W, H, d->min_angle, d->max_angle, d->max_views, subset.data(), range) : -1;
-            if (nv < 1) { set_err("gpm_batch_run: no source view passes the angle filter for reference " + std::to_string(ref));  failed++;  break; }
-            gpm_params p = d->params;
-            if (p.depthMin <= 0) p.depthMin = range[0];                                   // main.cpp:480-483
-            if (p.depthMax <= 0) p.depthMax = range[1];
-            p.min_disparity = cams[0].f * cams[0].baseline / p.depthMax;                 // main.cpp:905-906
-            p.max_disparity = cams[0].f * cams[0].baseline / p.depthMin;
-            rc = gpm_set_params(ctx, &p);
-            if (rc == GPM_OK) rc = gpm_set_reference(ctx, d->images[ref], pitch, 0, &cams[0]);
-            for (int v = 0; v < nv && rc == GPM_OK; v++) rc = gpm_set_view(ctx, v, d->images[order[subset[v]]], pitch, 0, &cams[subset[v]]);
-            if (rc == GPM_OK) rc = gpm_set_num_views(ctx, nv);
-            if (rc == GPM_OK) rc = gpm_set_rng(ctx, d->seed, GPM_RNG_REFERENCE);
+            if (ref < 0 || ref >= n) { set_err("gpm_batch_run: reference index out of range");  return false; }
+            if (!plan_view(d, ref, s)) { set_err("gpm_batch_run: no source view passes the angle filter for reference " + std::to_string(ref));  return false; }
+            int rc = load_view(ctx, d, 1, pitch, s);
             float ms = 0.f;
             if (rc == GPM_OK) rc = gpm_run(ctx, &ms);
-            if (rc != GPM_OK) { set_err(std::string("reference view ") + std::to_string(ref) + ": " + gpm_last_error());  failed++;  break; }
-            sweep_ms[job] = ms;  views_used[job] = nv;  device_of[job] = dev;
+            if (rc != GPM_OK) { set_err(std::string("reference view ") + std::to_string(ref) + ": " + gpm_last_error());  return false; }
+            sweep_ms[job] = ms;  views_used[job] = s.nv;  device_of[job] = dev;
             float* o4 = d->out_norm4 ? d->out_norm4 + (size_t)job * npix * 4 : nullptr;
             float* oc = d->out_cost ? d->out_cost + (size_t)job * npix : nullptr;
             if (d->out_dir && !o4) { n4.resize(npix * 4);  o4 = n4.data(); }
             if (o4 || oc) rc = gpm_get_state(ctx, o4, oc, 0);
-            if (rc == GPM_OK && d->out_dir) {
-                // <out_dir>/<ref as 8 digits>/disp.dmb, normals.dmb — what the per-image processes of the script leave for fusibile
-                char dir[1024];
-                snprintf(dir, sizeof(dir), "%s/%08d", d->out_dir, ref);
-                mkdir(d->out_dir, 0777);  mkdir(dir, 0777);
-                const std::string dp = std::string(dir) + "/disp.dmb", np_ = std::string(dir) + "/normals.dmb";
-                rc = gpm_write_result_dmb(dp.c_str(), np_.c_str(), o4, H, W);
-            }
-            if (rc != GPM_OK) { set_err("gpm_batch_run: could not store the result of reference view " + std::to_string(ref));  failed++;  break; }
-        }
-        gpm_destroy(ctx);
-    };
-    std::vector<std::thread> pool;
-    for (int k = 0; k < d->n_devices; k++) pool.emplace_back(worker, d->devices[k]);
-    for (auto& t : pool) t.join();
-    for (int i = 0; i < n; i++) if (registered[i]) cudaHostUnregister(const_cast<float*>(d->images[i]));
+            if (rc == GPM_OK && d->out_dir) rc = write_result(d->out_dir, ref, o4, H, W);
+            if (rc != GPM_OK) { set_err("gpm_batch_run: could not store the result of reference view " + std::to_string(ref));  return false; }
+            return true;
+        });
+    });
     if (stats) {
         stats->jobs_done = 0;  stats->sweep_ms_total = 0.0;
         for (int j = 0; j < d->n_refs; j++) if (device_of[j] >= 0) { stats->jobs_done++;  stats->sweep_ms_total += sweep_ms[j]; }
         if (stats->per_job_sweep_ms) for (int j = 0; j < d->n_refs; j++) stats->per_job_sweep_ms[j] = (float)sweep_ms[j];
         if (stats->per_job_views) for (int j = 0; j < d->n_refs; j++) stats->per_job_views[j] = views_used[j];
         if (stats->per_job_device) for (int j = 0; j < d->n_refs; j++) stats->per_job_device[j] = device_of[j];
+    }
+    return failed.load() ? GPM_E_STATE : GPM_OK;
+}
+
+// ---- two-pass geometric-consistency batch (DESIGN.md §14) -----------------------------------------------------------------
+namespace {
+// Page-locked host memory (portable: every device's context may copy from it) for the lifetime of this object.
+class PinnedStore {
+public:
+    explicit PinnedStore(size_t floats) { if (cudaHostAlloc(&p_, floats * sizeof(float), cudaHostAllocPortable) != cudaSuccess) p_ = nullptr; }
+    ~PinnedStore() { if (p_) cudaFreeHost(p_); }
+    PinnedStore(const PinnedStore&) = delete;
+    PinnedStore& operator=(const PinnedStore&) = delete;
+    float* get() const { return static_cast<float*>(p_); }
+private:
+    void* p_ = nullptr;
+};
+
+// Every worker of the pool waits in arrive_and_wait until all of them have arrived.
+class Barrier {
+public:
+    explicit Barrier(int n) : left_(n) {}
+    void arrive_and_wait()
+    {
+        std::unique_lock<std::mutex> l(m_);
+        if (--left_ == 0) cv_.notify_all();
+        else cv_.wait(l, [&] { return left_ == 0; });
+    }
+private:
+    std::mutex m_;
+    std::condition_variable cv_;
+    int left_;
+};
+
+// CUDA-event time of one gpm_sweep, from an event recorded on the context's stream before it to one recorded after it.
+// The events are created by the first sweep, on the calling thread's current device, which must be the context's.
+class SweepTimer {
+public:
+    SweepTimer() = default;
+    ~SweepTimer() { if (a_) cudaEventDestroy(a_);  if (b_) cudaEventDestroy(b_); }
+    SweepTimer(const SweepTimer&) = delete;
+    SweepTimer& operator=(const SweepTimer&) = delete;
+    int sweep(gpm_ctx* ctx, int iterations, float* ms)
+    {
+        cudaStream_t s = static_cast<cudaStream_t>(gpm_stream(ctx));
+        if (!a_ && cudaEventCreate(&a_) != cudaSuccess) { a_ = nullptr;  return cuda_fail(); }
+        if (!b_ && cudaEventCreate(&b_) != cudaSuccess) { b_ = nullptr;  return cuda_fail(); }
+        if (cudaEventRecord(a_, s) != cudaSuccess) return cuda_fail();
+        const int rc = gpm_sweep(ctx, iterations);
+        if (rc != GPM_OK) return rc;
+        if (cudaEventRecord(b_, s) != cudaSuccess || cudaEventSynchronize(b_) != cudaSuccess || cudaEventElapsedTime(ms, a_, b_) != cudaSuccess)
+            return cuda_fail();
+        return GPM_OK;
+    }
+    std::string error;
+private:
+    int cuda_fail() { error = std::string("sweep event: ") + cudaGetErrorString(cudaGetLastError());  return GPM_E_CUDA; }
+    cudaEvent_t a_ = nullptr, b_ = nullptr;
+};
+}  // namespace
+
+extern "C" int gpm_geo_batch_run(const gpm_geo_batch_desc* g, gpm_geo_batch_stats* stats)
+{
+    clear_err();
+    const char* bad = nullptr;
+    if (!g || !batch_desc_ok(&g->batch)) bad = "the batch descriptor is refused as gpm_batch_run refuses it";
+    else if (g->channels != 1 && g->channels != 4) bad = "channels must be 1 or 4";
+    else if (g->geo_iterations < 0) bad = "geo_iterations must be >= 0";
+    else if (!std::isfinite(g->weight) || g->weight < 0.f) bad = "weight must be finite and >= 0";
+    else if (!std::isfinite(g->max_err) || g->max_err <= 0.f) bad = "max_err must be finite and > 0";
+    if (bad) {
+        set_err(std::string("gpm_geo_batch_run: bad arguments: ") + bad);
+        return GPM_E_ARG;
+    }
+    const gpm_batch_desc* d = &g->batch;
+    const int n = d->n_images, W = d->width, H = d->height, n_refs = d->n_refs;
+    const size_t pitch = d->pitch_bytes ? d->pitch_bytes : (size_t)W * sizeof(float) * g->channels;
+    const size_t npix = (size_t)W * H;
+    auto ref_of = [&](int job) { return d->ref_indices ? d->ref_indices[job] : job; };
+    // Every reference index must be an image (without ref_indices: n_refs <= n_images); with out_dir each must be listed
+    // once, or two workers would write the same files.
+    std::vector<char> is_ref(n, 0), in_pass1(n, 0);
+    for (int j = 0; j < n_refs && !bad; j++) {
+        const int r = ref_of(j);
+        if (r < 0 || r >= n) bad = "reference index out of range";
+        else if (is_ref[r] && d->out_dir) bad = "a reference view is listed twice while out_dir is set";
+        else is_ref[r] = 1;
+    }
+    if (bad) {
+        set_err(std::string("gpm_geo_batch_run: bad arguments: ") + bad);
+        return GPM_E_ARG;
+    }
+
+    // Pass-1 set: the reference views and every view their selection picks (not recursive), planned on the host before
+    // anything runs, so that a view without source views is refused before any CUDA call.
+    std::vector<ViewSetup> setup(n);
+    for (int pass = 0; pass < 2; pass++)
+        for (int i = 0; i < n; i++) {
+            if (!(pass == 0 ? is_ref[i] : in_pass1[i] && !is_ref[i])) continue;
+            if (!plan_view(d, i, setup[i])) {
+                set_err(std::string("gpm_geo_batch_run: no source view passes the angle filter for ") +
+                        (is_ref[i] ? "reference view " : "source view ") + std::to_string(i));
+                return GPM_E_STATE;
+            }
+            in_pass1[i] = 1;
+            if (pass == 0) for (int v = 0; v < setup[i].nv; v++) in_pass1[setup[i].source(v)] = 1;
+        }
+    std::vector<int> pass1, depth_slot(n, -1), raw_slot(n, -1);
+    int n_raw = 0;
+    for (int i = 0; i < n; i++)
+        if (in_pass1[i]) {
+            depth_slot[i] = (int)pass1.size();
+            pass1.push_back(i);
+            if (is_ref[i]) raw_slot[i] = n_raw++;
+        }
+    const int n_pass1 = (int)pass1.size();
+
+    // The host store: a pass-1 depth map per pass-1 view, then the raw pass-1 planes of every reference view.
+    PinnedImages pinned(d, pitch * H);
+    PinnedStore store((size_t)n_pass1 * npix + (size_t)n_raw * npix * 4);
+    if (!store.get()) {
+        set_err(std::string("gpm_geo_batch_run: cannot allocate the page-locked host store: ") + cudaGetErrorString(cudaGetLastError()));
+        return GPM_E_CUDA;
+    }
+    float* depth_store = store.get();
+    float* raw_store = depth_store + (size_t)n_pass1 * npix;
+
+    std::atomic<int> next1(0), next2(0), failed(0);
+    std::vector<float> pass1_ms(n_pass1, 0.f), pass2_ms(n_refs, 0.f);
+    std::vector<int> device_of(n_refs, -1);
+    Barrier barrier(d->n_devices);
+    run_workers(d, failed, [&](gpm_ctx* ctx, int dev) {
+        if (ctx) cudaSetDevice(dev);                     // a worker thread of its own: the sweep events live on its device
+        SweepTimer timer;
+        std::vector<float> n4(ctx ? npix * 4 : 0), cost(ctx ? npix : 0);
+        auto fail_at = [&](const char* what, int view, int rc) {
+            set_err(std::string("gpm_geo_batch_run: ") + what + " view " + std::to_string(view) + ": " +
+                    (rc == GPM_E_CUDA && !timer.error.empty() ? timer.error : std::string(gpm_last_error())));
+            return false;
+        };
+        take_jobs(next1, n_pass1, failed, [&](int job) {          // pass 1: photometric
+            const int r = pass1[job];
+            int rc = load_view(ctx, d, g->channels, pitch, setup[r]);
+            if (rc == GPM_OK) rc = gpm_init(ctx);
+            if (rc == GPM_OK) rc = timer.sweep(ctx, d->params.iterations, &pass1_ms[job]);
+            if (rc == GPM_OK && raw_slot[r] >= 0) rc = gpm_get_state(ctx, raw_store + (size_t)raw_slot[r] * npix * 4, nullptr, 0);
+            if (rc == GPM_OK) rc = gpm_finalize(ctx);
+            if (rc == GPM_OK) rc = gpm_get_state(ctx, n4.data(), nullptr, 0);
+            if (rc != GPM_OK) return fail_at("pass 1 of", r, rc);
+            float* dep = depth_store + (size_t)depth_slot[r] * npix;
+            for (size_t k = 0; k < npix; k++) dep[k] = n4[k * 4 + 3];
+            return true;
+        });
+        barrier.arrive_and_wait();                                  // every depth map exists before any pass-2 job starts
+        take_jobs(next2, n_refs, failed, [&](int job) {            // pass 2: geometric, seeded with the pass-1 planes
+            const int r = ref_of(job);
+            const ViewSetup& s = setup[r];
+            const float* raw = raw_store + (size_t)raw_slot[r] * npix * 4;
+            int rc = load_view(ctx, d, g->channels, pitch, s);
+            for (int v = 0; v < s.nv && rc == GPM_OK; v++) rc = gpm_set_view_depth(ctx, v, depth_store + (size_t)depth_slot[s.source(v)] * npix, 0, 0);
+            if (rc == GPM_OK) rc = gpm_set_geometric(ctx, g->weight, g->max_err);
+            if (rc == GPM_OK) rc = gpm_cost_eval(ctx, raw, cost.data(), 0);
+            if (rc == GPM_OK) rc = gpm_set_state(ctx, raw, cost.data(), 0);
+            if (rc == GPM_OK) rc = timer.sweep(ctx, g->geo_iterations, &pass2_ms[job]);
+            if (rc == GPM_OK) rc = gpm_finalize(ctx);
+            float* o4 = d->out_norm4 ? d->out_norm4 + (size_t)job * npix * 4 : nullptr;
+            float* oc = d->out_cost ? d->out_cost + (size_t)job * npix : nullptr;
+            if (d->out_dir && !o4) o4 = n4.data();
+            if (rc == GPM_OK && (o4 || oc)) rc = gpm_get_state(ctx, o4, oc, 0);
+            if (rc == GPM_OK && d->out_dir && write_result(d->out_dir, r, o4, H, W) != GPM_OK) {
+                set_err("gpm_geo_batch_run: could not store the result of reference view " + std::to_string(r));
+                return false;
+            }
+            if (rc == GPM_OK) rc = gpm_set_geometric(ctx, 0.f, g->max_err);
+            if (rc != GPM_OK) return fail_at("pass 2 of reference", r, rc);
+            device_of[job] = dev;
+            return true;
+        });
+    });
+    if (stats) {
+        gpm_batch_stats* b = &stats->batch;
+        b->jobs_done = 0;  b->sweep_ms_total = 0.0;
+        for (int j = 0; j < n_refs; j++) if (device_of[j] >= 0) { b->jobs_done++;  b->sweep_ms_total += pass2_ms[j]; }
+        if (b->per_job_sweep_ms) for (int j = 0; j < n_refs; j++) b->per_job_sweep_ms[j] = pass2_ms[j];
+        if (b->per_job_views) for (int j = 0; j < n_refs; j++) b->per_job_views[j] = setup[ref_of(j)].nv;
+        if (b->per_job_device) for (int j = 0; j < n_refs; j++) b->per_job_device[j] = device_of[j];
+        stats->n_pass1 = n_pass1;
+        if (stats->pass1_views) std::copy(pass1.begin(), pass1.end(), stats->pass1_views);
+        if (stats->pass1_sweep_ms) std::copy(pass1_ms.begin(), pass1_ms.end(), stats->pass1_sweep_ms);
+        if (stats->ref_views)
+            for (int j = 0; j < n_refs; j++) {
+                const ViewSetup& s = setup[ref_of(j)];
+                for (int v = 0; v < d->max_views; v++) stats->ref_views[(size_t)j * d->max_views + v] = v < s.nv ? s.source(v) : -1;
+            }
     }
     return failed.load() ? GPM_E_STATE : GPM_OK;
 }

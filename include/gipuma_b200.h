@@ -230,7 +230,7 @@ typedef struct gpm_batch_desc {
     const int* devices;                /* CUDA device ordinals, one worker each */
     int n_devices;
     unsigned long long seed;
-    const char* out_dir;               /* NULL: no files */
+    const char* out_dir;               /* NULL: no files; else list each reference view once (a repeated one is written by two jobs, possibly at once) */
     float* out_norm4;                  /* NULL or n_refs * height*width*4 floats (world normal + depth per job) */
     float* out_cost;                   /* NULL or n_refs * height*width floats */
 } gpm_batch_desc;
@@ -243,6 +243,37 @@ typedef struct gpm_batch_stats {
 } gpm_batch_stats;
 int gpm_batch_run(const gpm_batch_desc* desc, gpm_batch_stats* stats);
 const char* gpm_batch_last_error(void);
+
+/* Two-pass geometric-consistency batch (DESIGN.md §14) on the same worker pool and shared image cache.  Pass 1, for the
+ * reference views and every view their selection picks (not recursive), on whichever worker takes the view: gpm_batch_run's
+ * per-view setup, gpm_init, gpm_sweep(params.iterations), gpm_get_state (raw planes, reference views only), gpm_finalize,
+ * gpm_get_state (depth map), kept in one page-locked host store for the call (about 4 + 16 bytes per pixel and view).  All
+ * workers finish pass 1 before any pass-2 job starts.  Pass 2, per reference view: the same setup, gpm_set_view_depth of
+ * every selected view's pass-1 depth map, gpm_set_geometric(weight, max_err), gpm_cost_eval of the raw planes and
+ * gpm_set_state of the planes with those costs, gpm_sweep(geo_iterations), gpm_finalize, gpm_get_state into out_norm4 /
+ * out_cost, the .dmb files as gpm_batch_run writes them, gpm_set_geometric(0, max_err).  Sweep times are CUDA events on
+ * gpm_stream around each gpm_sweep.
+ * Refused with GPM_E_ARG before any CUDA call: what gpm_batch_run refuses, a reference index out of range (without
+ * ref_indices: n_refs > n_images), a reference view listed twice while out_dir is set, channels other than 1 or 4,
+ * geo_iterations < 0, weight / max_err that gpm_set_geometric refuses.  GPM_E_STATE, also before any CUDA call: a pass-1
+ * view with no source view passing the angle filter (named in gpm_batch_last_error()).  A failure during the run (e.g.
+ * negative params.iterations, which gpm_set_params refuses) stops every worker with GPM_E_STATE; the contexts, the image
+ * registrations and the host store are released on every path. */
+typedef struct gpm_geo_batch_desc {
+    gpm_batch_desc batch;              /* as gpm_batch_run; batch.params.iterations = pass-1 iterations; out_norm4 / out_cost /
+                                          out_dir receive the pass-2 results */
+    int channels;                      /* 1: batch.images are float images; 4: RGBA float4 images (pitch_bytes 0 = width*16) */
+    int geo_iterations;                /* pass-2 sweeps, >= 0 */
+    float weight, max_err;             /* as gpm_set_geometric */
+} gpm_geo_batch_desc;
+typedef struct gpm_geo_batch_stats {
+    gpm_batch_stats batch;             /* per reference job: pass-2 sweep ms, views selected, device */
+    int n_pass1;                       /* views pass 1 ran */
+    int* pass1_views;                  /* NULL or n_images entries: those views, ascending */
+    float* pass1_sweep_ms;             /* NULL or n_images entries, in the order of pass1_views */
+    int* ref_views;                    /* NULL or n_refs * max_views image indices of each job's selected views, -1 after the last */
+} gpm_geo_batch_stats;
+int gpm_geo_batch_run(const gpm_geo_batch_desc* desc, gpm_geo_batch_stats* stats);
 
 /* ---- depth-map fusion: the per-view world-frame outputs (norm4 of gpm_batch_run, or its .dmb files) -> one point cloud;
  * what the reference's scripts hand to the external `fusibile` (scripts/dtu_fast.sh:56-57).  Deterministic: the same inputs
