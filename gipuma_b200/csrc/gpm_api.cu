@@ -109,6 +109,9 @@ struct gpm_ctx {
     std::vector<char> have_depth;
     std::vector<float> h_kinv;
     float ref_K[9] = {0.f};
+    // photometric cost (DESIGN.md §15): GPM_PHOTO_PM, the reference's, or GPM_PHOTO_NCC (gpm_set_photometric)
+    int photo = GPM_PHOTO_PM;
+    float ncc_min_std = 0.f;
 };
 
 namespace {
@@ -170,6 +173,11 @@ int check_geometric(const gpm_ctx* c, float weight)
         if (!c->have_depth[v]) return fail(GPM_E_STATE, "geometric-consistency mode: source view " + std::to_string(v) + " has no depth map (gpm_set_view_depth)");
     return GPM_OK;
 }
+
+bool ncc_on(const gpm_ctx* c) { return c->photo == GPM_PHOTO_NCC; }
+
+// provenance of costs from an initialisation evaluation (gpm_init, or a trusted gpm_set_state)
+int init_prov(const gpm_ctx* c) { return ncc_on(c) ? GPM_PROV_NCC : c->color == 1 ? 3 : 0; }
 
 int build_kparams(gpm_ctx* c, bool init_phase, KParams& P, bool eval_call = false)
 {
@@ -243,6 +251,7 @@ int build_kparams(gpm_ctx* c, bool init_phase, KParams& P, bool eval_call = fals
     // gipuma.cu:771-774) would make the bound exceed the final value.  Unreachable while ns * max dissimilarity < MAXCOST.
     // The geometric term adds at most weight * max_err to a view's final cost (0 outside that mode).
     if ((float)P.ns * ((1.0f - p.alpha) * p.tau_color + p.alpha * p.tau_gradient) + c->geo_weight * c->geo_max_err >= GPM_MAXCOST) P.prune = 0;
+    if (ncc_on(c)) P.prune = 0;                             // partial NCC sums bound nothing (DESIGN.md §15)
     P.dedupe_self = c->opt_dedupe ? 1 : 0;
     // rounding variant of k_cost_eval: at initialisation the reference's binary is y-first for float, x-first for float4;
     // gpm_cost_eval defaults to the variant of the propagation kernels (x-first for float, y-first for float4)
@@ -268,7 +277,7 @@ int build_kparams(gpm_ctx* c, bool init_phase, KParams& P, bool eval_call = fals
     P.ref.depthMin = p.depthMin;  P.ref.depthMax = p.depthMax;
     // warps per block: as many as fit (<= 16).  The kernels use 128 registers per thread, so one 16-warp block fills an SM
     // anyway; shared memory may therefore be spent up to the per-block opt-in limit.
-    const size_t per_warp = (size_t)warp_scratch_floats(P.ns_pad, P.V, P.color) * sizeof(float);
+    const size_t per_warp = (size_t)warp_scratch_floats(P.ns_pad, P.V, P.color, ncc_on(c)) * sizeof(float);
     const size_t fixed = ((size_t)fixed_smem_floats(P) + 4) * sizeof(float);
     int nw = GPM_LB_THREADS / 32;
     const size_t budget = (size_t)c->smem_optin > 16 * 1024 ? (size_t)c->smem_optin - 8 * 1024 : 40 * 1024;
@@ -276,7 +285,7 @@ int build_kparams(gpm_ctx* c, bool init_phase, KParams& P, bool eval_call = fals
     if (c->opt_nwarps > 0) nw = c->opt_nwarps;
     if (nw > GPM_LB_THREADS / 32) nw = GPM_LB_THREADS / 32;
     P.nwarps = nw;
-    if (block_smem_bytes(P) > (size_t)c->smem_optin)
+    if (block_smem_bytes(P, ncc_on(c)) > (size_t)c->smem_optin)
         return fail(GPM_E_ARG, "configuration needs more shared memory per block than the device offers");
     return ensure_tensor_map(c, P);
 }
@@ -323,15 +332,18 @@ GeoParams geo_params(const gpm_ctx* c)
     G.depth = c->geo_depth;  G.kinv = c->geo_kinv;
     memcpy(G.Kref, c->ref_K, sizeof(G.Kref));
     G.weight = c->geo_weight;  G.max_err = c->geo_max_err;
+    G.min_std = c->ncc_min_std;
     return G;
 }
 
 int launch_colour(gpm_ctx* c, const KParams& P, int colour, int mask)
 {
-    auto kern = c->geo_weight > 0.f ? (P.color ? k_sweep<true, false, true> : k_sweep<false, false, true>)    // 8 neighbours (check_geometric)
+    const bool ncc = ncc_on(c);          // grey images, 8 neighbours (gpm_set_photometric)
+    auto kern = ncc ? (c->geo_weight > 0.f ? k_sweep<false, false, true, true> : k_sweep<false, false, false, true>)
+              : c->geo_weight > 0.f ? (P.color ? k_sweep<true, false, true> : k_sweep<false, false, true>)    // 8 neighbours (check_geometric)
               : P.ncand == 20 ? (P.color ? k_sweep<true, true> : k_sweep<false, true>)
                               : (P.color ? k_sweep<true, false> : k_sweep<false, false>);
-    kern<<<tile_grid(c), P.nwarps * 32, block_smem_bytes(P), c->stream>>>(P, c->tmap, c->d_cams, c->srcTex, c->planes, c->cost, c->rng,
+    kern<<<tile_grid(c), P.nwarps * 32, block_smem_bytes(P, ncc), c->stream>>>(P, c->tmap, c->d_cams, c->srcTex, c->planes, c->cost, c->rng,
         c->prov, Memo{c->pid, c->seen, c->refseen, c->memo_mask, c->next_id}, colour, mask, c->d_stats, geo_params(c));
     c->launches++;
     CU(cudaGetLastError());
@@ -342,9 +354,11 @@ int launch_colour(gpm_ctx* c, const KParams& P, int colour, int mask)
 cudaError_t launch_cost_eval(gpm_ctx* c, const KParams& P, const float4* planes, float* cost)
 {
     dim3 grid((P.W + GPM_TILE - 1) / GPM_TILE, (P.H + GPM_TILE - 1) / GPM_TILE);
-    auto kern = c->geo_weight > 0.f ? (P.color ? k_cost_eval<true, true> : k_cost_eval<false, true>)
+    const bool ncc = ncc_on(c);
+    auto kern = ncc ? (c->geo_weight > 0.f ? k_cost_eval<false, true, true> : k_cost_eval<false, false, true>)
+              : c->geo_weight > 0.f ? (P.color ? k_cost_eval<true, true> : k_cost_eval<false, true>)
                                     : (P.color ? k_cost_eval<true> : k_cost_eval<false>);
-    kern<<<grid, P.nwarps * 32, block_smem_bytes(P), c->stream>>>(P, c->tmap, c->d_cams, c->srcTex, planes, cost, nullptr, geo_params(c));
+    kern<<<grid, P.nwarps * 32, block_smem_bytes(P, ncc), c->stream>>>(P, c->tmap, c->d_cams, c->srcTex, planes, cost, nullptr, geo_params(c));
     c->launches++;
     return cudaGetLastError();
 }
@@ -499,6 +513,10 @@ extern "C" int gpm_create(gpm_ctx** out, int device, int width, int height, int 
         ok(cudaFuncSetAttribute(k_sweep<true, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, c->smem_optin));
         ok(cudaFuncSetAttribute(k_cost_eval<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, c->smem_optin));
         ok(cudaFuncSetAttribute(k_cost_eval<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, c->smem_optin));
+        ok(cudaFuncSetAttribute(k_sweep<false, false, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, c->smem_optin));
+        ok(cudaFuncSetAttribute(k_sweep<false, false, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, c->smem_optin));
+        ok(cudaFuncSetAttribute(k_cost_eval<false, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, c->smem_optin));
+        ok(cudaFuncSetAttribute(k_cost_eval<false, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, c->smem_optin));
         ok(cudaFuncSetAttribute(k_shard_stage<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, c->smem_optin));
         ok(cudaFuncSetAttribute(k_shard_stage<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, c->smem_optin));
     }
@@ -567,12 +585,19 @@ extern "C" int gpm_set_rng(gpm_ctx* c, unsigned long long seed, int mode)
     return GPM_OK;
 }
 
+// the NCC cost has no colour variant: a colour upload while it is on is refused before anything changes
+static int refuse_color_under_ncc(const char* fn, const gpm_ctx* c, bool color)
+{
+    return color && ncc_on(c) ? fail(GPM_E_STATE, std::string(fn) + ": the NCC photometric cost supports grey images only (gpm_set_photometric GPM_PHOTO_PM)") : GPM_OK;
+}
+
 // Image uploads, T = float (grey) or float4 (colour: the reference's -color_processing path, main.cpp:560-605).  Each
 // returns after a stream synchronisation: the caller may reuse its buffer.
 template <typename T>
 static int set_reference(const char* fn, gpm_ctx* c, const float* img, size_t pitch_bytes, int on_device, const gpm_camera* cam)
 {
     if (!c || !img || !cam) return fail(GPM_E_ARG, std::string(fn) + ": null argument");
+    if (const int rc = refuse_color_under_ncc(fn, c, sizeof(T) == sizeof(float4))) return rc;
     DeviceGuard g(c->device);
     int rc = ensure_color(c, sizeof(T) == sizeof(float4));
     if (rc) return rc;
@@ -595,6 +620,7 @@ static int set_view(const char* fn, gpm_ctx* c, int v, const float* img, size_t 
     if (!c || !img || !cam) return fail(GPM_E_ARG, std::string(fn) + ": null argument");
     if (v < 0 || v >= c->maxV) return fail(GPM_E_ARG, std::string(fn) + ": view index out of range");
     constexpr bool color = sizeof(T) == sizeof(float4);
+    if (const int rc = refuse_color_under_ncc(fn, c, color)) return rc;
     DeviceGuard g(c->device);
     int rc = ensure_color(c, color);
     if (rc) return rc;
@@ -685,6 +711,23 @@ extern "C" int gpm_set_geometric(gpm_ctx* c, float weight, float max_err)
     return GPM_OK;
 }
 
+extern "C" int gpm_set_photometric(gpm_ctx* c, int kind, float min_std)
+{
+    if (!c) return fail(GPM_E_ARG, "gpm_set_photometric: null context");
+    if (kind != GPM_PHOTO_PM && kind != GPM_PHOTO_NCC) return fail(GPM_E_ARG, "gpm_set_photometric: kind must be GPM_PHOTO_PM or GPM_PHOTO_NCC");
+    if (kind == GPM_PHOTO_NCC) {
+        if (!std::isfinite(min_std) || min_std <= 0.f) return fail(GPM_E_ARG, "gpm_set_photometric: min_std must be finite and > 0");
+        if (c->color == 1) return fail(GPM_E_ARG, "gpm_set_photometric: the NCC cost supports grey images only; this context holds colour images");
+        if (c->opt_neighbours == 20) return fail(GPM_E_ARG, "gpm_set_photometric: the NCC cost supports the 8-neighbour sweep only (option neighbours = 8)");
+    } else {
+        min_std = 0.f;                               // not read by the PM cost
+    }
+    if (kind != c->photo || min_std != c->ncc_min_std) c->inputs_dirty = true;
+    c->photo = kind;
+    c->ncc_min_std = min_std;
+    return GPM_OK;
+}
+
 extern "C" int gpm_set_state(gpm_ctx* c, const float* norm4, const float* cost, int on_device)
 {
     if (!c) return fail(GPM_E_ARG, "gpm_set_state: null context");
@@ -699,7 +742,7 @@ extern "C" int gpm_set_state(gpm_ctx* c, const float* norm4, const float* cost, 
     if (cost) CU(cudaMemcpyAsync(c->cost, cost, n * sizeof(float), k, c->stream));
     // provenance of the supplied costs is unknown (GPM_PROV_UNKNOWN) unless the caller vouches that they came from an
     // initialisation / refinement evaluation of exactly these planes ("trust_state": 0)
-    const int rc = reset_state_tags(c, c->opt_trust_state ? (c->color == 1 ? 3 : 0) : GPM_PROV_UNKNOWN);
+    const int rc = reset_state_tags(c, c->opt_trust_state ? init_prov(c) : GPM_PROV_UNKNOWN);
     if (rc) return rc;
     CU(cudaStreamSynchronize(c->stream));
     return GPM_OK;
@@ -727,7 +770,7 @@ static int do_init(gpm_ctx* c)
     rc = init_planes(c, P);
     if (rc) return rc;
     CU(launch_cost_eval(c, P, c->planes, c->cost));
-    return reset_state_tags(c, c->color == 1 ? 3 : 0);     // costs now come from the init-variant evaluation (float4: x-first + gradient folding 1)
+    return reset_state_tags(c, init_prov(c));     // costs now come from the init-variant evaluation (float4: x-first + gradient folding 1; NCC: its own)
 }
 
 static int do_sweeps(gpm_ctx* c, int iterations)
@@ -861,23 +904,25 @@ static int shard_refine_steps(const gpm_params& p)
     return n;
 }
 
-// the source-view shard has no geometric-consistency variant: refused before anything is launched
-static int shard_refuses_geometric(gpm_ctx* c)
+// the source-view shard has no geometric-consistency and no NCC variant: refused before anything is launched
+static int shard_refuses_mode(gpm_ctx* c)
 {
-    return c->geo_weight > 0.f ? fail(GPM_E_STATE, "view sharding does not support the geometric-consistency mode (gpm_set_geometric weight 0)") : GPM_OK;
+    if (c->geo_weight > 0.f) return fail(GPM_E_STATE, "view sharding does not support the geometric-consistency mode (gpm_set_geometric weight 0)");
+    if (ncc_on(c)) return fail(GPM_E_STATE, "view sharding does not support the NCC photometric cost (gpm_set_photometric GPM_PHOTO_PM)");
+    return GPM_OK;
 }
 
 extern "C" int gpm_shard_num_stages(gpm_ctx* c)
 {
     if (!c || !c->have_params) { fail(GPM_E_STATE, "gpm_shard_num_stages: parameters not set");  return -1; }
-    if (shard_refuses_geometric(c)) return -1;
+    if (shard_refuses_mode(c)) return -1;
     return 2 + shard_refine_steps(c->prm);
 }
 
 extern "C" long long gpm_shard_stage_floats(gpm_ctx* c, int stage)
 {
     if (!c || !c->have_params || stage < 0) { fail(GPM_E_ARG, "gpm_shard_stage_floats: bad arguments");  return -1; }
-    if (shard_refuses_geometric(c)) return -1;
+    if (shard_refuses_mode(c)) return -1;
     const long long half = (long long)c->H * ((c->W + 1) / 2);
     const int slots = stage == 1 ? 8 : 1;
     return (stage == 0 ? 2 : 1) * half * slots * c->prm.n_best;
@@ -885,7 +930,7 @@ extern "C" long long gpm_shard_stage_floats(gpm_ctx* c, int stage)
 
 static int shard_common(gpm_ctx* c, int stage, KParams& P)
 {
-    if (const int rc = shard_refuses_geometric(c)) return rc;
+    if (const int rc = shard_refuses_mode(c)) return rc;
     if (c->prm.cost_comb != GPM_COMB_BEST_N) return fail(GPM_E_ARG, "view sharding supports cost_comb = best_n only");
     if (c->opt_neighbours != 8) return fail(GPM_E_ARG, "view sharding supports the 8-neighbour sweep only (option neighbours = 8)");
     if (c->prm.n_best < 1 || c->prm.n_best > 32) return fail(GPM_E_ARG, "view sharding needs 1 <= n_best <= 32");
@@ -1036,7 +1081,7 @@ static int shard_alloc_exchange(gpm_ctx* c)
 extern "C" int gpm_shard_comm_init(gpm_ctx* c, const void* id128, int rank, int world)
 {
     if (!c || world < 1 || world > 8 || rank < 0 || rank >= world) return fail(GPM_E_ARG, "gpm_shard_comm_init: bad arguments (1 <= world <= 8)");
-    if (const int rc = shard_refuses_geometric(c)) return rc;
+    if (const int rc = shard_refuses_mode(c)) return rc;
     DeviceGuard g(c->device);
     gpm_shard_comm_destroy_(c);
     c->shard_rank = rank;  c->shard_world = world;
@@ -1054,7 +1099,7 @@ extern "C" int gpm_shard_comm_init(gpm_ctx* c, const void* id128, int rank, int 
 extern "C" int gpm_shard_comm_attach(gpm_ctx* c, void* nccl_comm, int rank, int world)
 {
     if (!c || world < 1 || world > 8 || rank < 0 || rank >= world || (world > 1 && !nccl_comm)) return fail(GPM_E_ARG, "gpm_shard_comm_attach: bad arguments");
-    if (const int rc = shard_refuses_geometric(c)) return rc;
+    if (const int rc = shard_refuses_mode(c)) return rc;
     if (world > 1 && !nccl_api()) return fail(GPM_E_STATE, "NCCL (libnccl.so.2) could not be loaded; set GPM_NCCL_LIB");
     gpm_shard_comm_destroy_(c);
     c->comm = nccl_comm;  c->shard_rank = rank;  c->shard_world = world;
@@ -1204,6 +1249,7 @@ extern "C" int gpm_set_option(gpm_ctx* c, const char* name, int value)
     else if (n == "neighbours") {
         if (value != 8 && value != 20) return fail(GPM_E_ARG, "neighbours must be 8 (close + far kernels) or 20 (fused kernel)");
         if (value == 20 && c->geo_weight > 0.f) return fail(GPM_E_ARG, "the geometric-consistency mode supports the 8-neighbour sweep only");
+        if (value == 20 && ncc_on(c)) return fail(GPM_E_ARG, "the NCC photometric cost supports the 8-neighbour sweep only");
         DeviceGuard g(c->device);
         const int slots = value == 20 ? 20 : 8;
         if (slots != c->seen_slots) {

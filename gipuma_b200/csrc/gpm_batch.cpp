@@ -6,7 +6,8 @@
 // cameras on it (gpm_prepare_cameras, cameraGeometryUtils.h:174-353), selects the source views (gpm_select_views,
 // main.cpp:430-499, deterministic), derives the depth / disparity range as main.cpp:480-483 and :898-906 do, runs the job
 // (gpm_run) and hands back / writes the result (disp.dmb + normals.dmb, main.cpp:1002-1003, for the external fusibile).
-// gpm_geo_batch_run runs the two-pass geometric-consistency flow (DESIGN.md §14) on the same pool and image cache.
+// gpm_geo_batch_run runs the two-pass geometric-consistency flow (DESIGN.md §14) on the same pool and image cache.  The
+// _photo twins of both choose the photometric cost (DESIGN.md §15).
 // Host C++ over the C-ABI; the only CUDA calls are page-locking, the geometric driver's host store and its sweep events.
 #include "../../include/gipuma_b200.h"
 
@@ -67,12 +68,29 @@ bool plan_view(const gpm_batch_desc* d, int ref, ViewSetup& s)
     return true;
 }
 
-// The per-view uploads of a job: parameters, reference and source images (grey: channels 1, RGBA: 4), view count, RNG.
-int load_view(gpm_ctx* ctx, const gpm_batch_desc* d, int channels, size_t pitch, const ViewSetup& s)
+// The photometric cost of every job (gpm_set_photometric).
+struct Photo {
+    int kind;
+    float min_std;
+};
+
+// what gpm_set_photometric refuses for its arguments, and NCC on colour images; nullptr if none
+const char* photo_refusal(const Photo& ph, int channels)
+{
+    if (ph.kind != GPM_PHOTO_PM && ph.kind != GPM_PHOTO_NCC) return "kind must be GPM_PHOTO_PM or GPM_PHOTO_NCC";
+    if (ph.kind == GPM_PHOTO_NCC && !(std::isfinite(ph.min_std) && ph.min_std > 0.f)) return "min_std must be finite and > 0";
+    if (ph.kind == GPM_PHOTO_NCC && channels == 4) return "the NCC cost supports grey images only (channels 1)";
+    return nullptr;
+}
+
+// The per-view setup of a job: photometric cost, parameters, reference and source images (grey: channels 1, RGBA: 4), view
+// count, RNG.
+int load_view(gpm_ctx* ctx, const gpm_batch_desc* d, int channels, size_t pitch, const ViewSetup& s, const Photo& ph)
 {
     auto set_reference = channels == 4 ? gpm_set_reference_color : gpm_set_reference;
     auto set_view = channels == 4 ? gpm_set_view_color : gpm_set_view;
-    int rc = gpm_set_params(ctx, &s.p);
+    int rc = gpm_set_photometric(ctx, ph.kind, ph.min_std);
+    if (rc == GPM_OK) rc = gpm_set_params(ctx, &s.p);
     if (rc == GPM_OK) rc = set_reference(ctx, d->images[s.order[0]], pitch, 0, &s.cams[0]);
     for (int v = 0; v < s.nv && rc == GPM_OK; v++) rc = set_view(ctx, v, d->images[s.source(v)], pitch, 0, &s.cams[s.subset[v]]);
     if (rc == GPM_OK) rc = gpm_set_num_views(ctx, s.nv);
@@ -150,11 +168,16 @@ extern "C" const char* gpm_batch_last_error(void)
     return copy.c_str();
 }
 
-extern "C" int gpm_batch_run(const gpm_batch_desc* d, gpm_batch_stats* stats)
+// gpm_batch_run and gpm_batch_run_photo; `fn` names the entry point in error messages
+static int batch_run(const char* fn, const gpm_batch_desc* d, const Photo& ph, gpm_batch_stats* stats)
 {
     clear_err();
     if (!batch_desc_ok(d)) {
-        set_err("gpm_batch_run: bad arguments");
+        set_err(std::string(fn) + ": bad arguments");
+        return GPM_E_ARG;
+    }
+    if (const char* bad = photo_refusal(ph, 1)) {
+        set_err(std::string(fn) + ": bad arguments: " + bad);
         return GPM_E_ARG;
     }
     const int n = d->n_images, W = d->width, H = d->height;
@@ -170,9 +193,9 @@ extern "C" int gpm_batch_run(const gpm_batch_desc* d, gpm_batch_stats* stats)
         std::vector<float> n4;
         take_jobs(next, d->n_refs, failed, [&](int job) {
             const int ref = d->ref_indices ? d->ref_indices[job] : job;
-            if (ref < 0 || ref >= n) { set_err("gpm_batch_run: reference index out of range");  return false; }
-            if (!plan_view(d, ref, s)) { set_err("gpm_batch_run: no source view passes the angle filter for reference " + std::to_string(ref));  return false; }
-            int rc = load_view(ctx, d, 1, pitch, s);
+            if (ref < 0 || ref >= n) { set_err(std::string(fn) + ": reference index out of range");  return false; }
+            if (!plan_view(d, ref, s)) { set_err(std::string(fn) + ": no source view passes the angle filter for reference " + std::to_string(ref));  return false; }
+            int rc = load_view(ctx, d, 1, pitch, s, ph);
             float ms = 0.f;
             if (rc == GPM_OK) rc = gpm_run(ctx, &ms);
             if (rc != GPM_OK) { set_err(std::string("reference view ") + std::to_string(ref) + ": " + gpm_last_error());  return false; }
@@ -182,7 +205,7 @@ extern "C" int gpm_batch_run(const gpm_batch_desc* d, gpm_batch_stats* stats)
             if (d->out_dir && !o4) { n4.resize(npix * 4);  o4 = n4.data(); }
             if (o4 || oc) rc = gpm_get_state(ctx, o4, oc, 0);
             if (rc == GPM_OK && d->out_dir) rc = write_result(d->out_dir, ref, o4, H, W);
-            if (rc != GPM_OK) { set_err("gpm_batch_run: could not store the result of reference view " + std::to_string(ref));  return false; }
+            if (rc != GPM_OK) { set_err(std::string(fn) + ": could not store the result of reference view " + std::to_string(ref));  return false; }
             return true;
         });
     });
@@ -194,6 +217,16 @@ extern "C" int gpm_batch_run(const gpm_batch_desc* d, gpm_batch_stats* stats)
         if (stats->per_job_device) for (int j = 0; j < d->n_refs; j++) stats->per_job_device[j] = device_of[j];
     }
     return failed.load() ? GPM_E_STATE : GPM_OK;
+}
+
+extern "C" int gpm_batch_run(const gpm_batch_desc* d, gpm_batch_stats* stats)
+{
+    return batch_run("gpm_batch_run", d, Photo{GPM_PHOTO_PM, 0.f}, stats);
+}
+
+extern "C" int gpm_batch_run_photo(const gpm_batch_desc* d, int kind, float min_std, gpm_batch_stats* stats)
+{
+    return batch_run("gpm_batch_run_photo", d, Photo{kind, min_std}, stats);
 }
 
 // ---- two-pass geometric-consistency batch (DESIGN.md §14) -----------------------------------------------------------------
@@ -253,7 +286,8 @@ private:
 };
 }  // namespace
 
-extern "C" int gpm_geo_batch_run(const gpm_geo_batch_desc* g, gpm_geo_batch_stats* stats)
+// gpm_geo_batch_run and gpm_geo_batch_run_photo; `fn` names the entry point in error messages
+static int geo_batch_run(const char* fn, const gpm_geo_batch_desc* g, const Photo& ph, gpm_geo_batch_stats* stats)
 {
     clear_err();
     const char* bad = nullptr;
@@ -262,8 +296,9 @@ extern "C" int gpm_geo_batch_run(const gpm_geo_batch_desc* g, gpm_geo_batch_stat
     else if (g->geo_iterations < 0) bad = "geo_iterations must be >= 0";
     else if (!std::isfinite(g->weight) || g->weight < 0.f) bad = "weight must be finite and >= 0";
     else if (!std::isfinite(g->max_err) || g->max_err <= 0.f) bad = "max_err must be finite and > 0";
+    else bad = photo_refusal(ph, g->channels);
     if (bad) {
-        set_err(std::string("gpm_geo_batch_run: bad arguments: ") + bad);
+        set_err(std::string(fn) + ": bad arguments: " + bad);
         return GPM_E_ARG;
     }
     const gpm_batch_desc* d = &g->batch;
@@ -281,7 +316,7 @@ extern "C" int gpm_geo_batch_run(const gpm_geo_batch_desc* g, gpm_geo_batch_stat
         else is_ref[r] = 1;
     }
     if (bad) {
-        set_err(std::string("gpm_geo_batch_run: bad arguments: ") + bad);
+        set_err(std::string(fn) + ": bad arguments: " + bad);
         return GPM_E_ARG;
     }
 
@@ -292,7 +327,7 @@ extern "C" int gpm_geo_batch_run(const gpm_geo_batch_desc* g, gpm_geo_batch_stat
         for (int i = 0; i < n; i++) {
             if (!(pass == 0 ? is_ref[i] : in_pass1[i] && !is_ref[i])) continue;
             if (!plan_view(d, i, setup[i])) {
-                set_err(std::string("gpm_geo_batch_run: no source view passes the angle filter for ") +
+                set_err(std::string(fn) + ": no source view passes the angle filter for " +
                         (is_ref[i] ? "reference view " : "source view ") + std::to_string(i));
                 return GPM_E_STATE;
             }
@@ -313,7 +348,7 @@ extern "C" int gpm_geo_batch_run(const gpm_geo_batch_desc* g, gpm_geo_batch_stat
     PinnedImages pinned(d, pitch * H);
     PinnedStore store((size_t)n_pass1 * npix + (size_t)n_raw * npix * 4);
     if (!store.get()) {
-        set_err(std::string("gpm_geo_batch_run: cannot allocate the page-locked host store: ") + cudaGetErrorString(cudaGetLastError()));
+        set_err(std::string(fn) + ": cannot allocate the page-locked host store: " + cudaGetErrorString(cudaGetLastError()));
         return GPM_E_CUDA;
     }
     float* depth_store = store.get();
@@ -328,13 +363,13 @@ extern "C" int gpm_geo_batch_run(const gpm_geo_batch_desc* g, gpm_geo_batch_stat
         SweepTimer timer;
         std::vector<float> n4(ctx ? npix * 4 : 0), cost(ctx ? npix : 0);
         auto fail_at = [&](const char* what, int view, int rc) {
-            set_err(std::string("gpm_geo_batch_run: ") + what + " view " + std::to_string(view) + ": " +
+            set_err(std::string(fn) + ": " + what + " view " + std::to_string(view) + ": " +
                     (rc == GPM_E_CUDA && !timer.error.empty() ? timer.error : std::string(gpm_last_error())));
             return false;
         };
         take_jobs(next1, n_pass1, failed, [&](int job) {          // pass 1: photometric
             const int r = pass1[job];
-            int rc = load_view(ctx, d, g->channels, pitch, setup[r]);
+            int rc = load_view(ctx, d, g->channels, pitch, setup[r], ph);
             if (rc == GPM_OK) rc = gpm_init(ctx);
             if (rc == GPM_OK) rc = timer.sweep(ctx, d->params.iterations, &pass1_ms[job]);
             if (rc == GPM_OK && raw_slot[r] >= 0) rc = gpm_get_state(ctx, raw_store + (size_t)raw_slot[r] * npix * 4, nullptr, 0);
@@ -350,7 +385,7 @@ extern "C" int gpm_geo_batch_run(const gpm_geo_batch_desc* g, gpm_geo_batch_stat
             const int r = ref_of(job);
             const ViewSetup& s = setup[r];
             const float* raw = raw_store + (size_t)raw_slot[r] * npix * 4;
-            int rc = load_view(ctx, d, g->channels, pitch, s);
+            int rc = load_view(ctx, d, g->channels, pitch, s, ph);
             for (int v = 0; v < s.nv && rc == GPM_OK; v++) rc = gpm_set_view_depth(ctx, v, depth_store + (size_t)depth_slot[s.source(v)] * npix, 0, 0);
             if (rc == GPM_OK) rc = gpm_set_geometric(ctx, g->weight, g->max_err);
             if (rc == GPM_OK) rc = gpm_cost_eval(ctx, raw, cost.data(), 0);
@@ -362,7 +397,7 @@ extern "C" int gpm_geo_batch_run(const gpm_geo_batch_desc* g, gpm_geo_batch_stat
             if (d->out_dir && !o4) o4 = n4.data();
             if (rc == GPM_OK && (o4 || oc)) rc = gpm_get_state(ctx, o4, oc, 0);
             if (rc == GPM_OK && d->out_dir && write_result(d->out_dir, r, o4, H, W) != GPM_OK) {
-                set_err("gpm_geo_batch_run: could not store the result of reference view " + std::to_string(r));
+                set_err(std::string(fn) + ": could not store the result of reference view " + std::to_string(r));
                 return false;
             }
             if (rc == GPM_OK) rc = gpm_set_geometric(ctx, 0.f, g->max_err);
@@ -388,4 +423,14 @@ extern "C" int gpm_geo_batch_run(const gpm_geo_batch_desc* g, gpm_geo_batch_stat
             }
     }
     return failed.load() ? GPM_E_STATE : GPM_OK;
+}
+
+extern "C" int gpm_geo_batch_run(const gpm_geo_batch_desc* g, gpm_geo_batch_stats* stats)
+{
+    return geo_batch_run("gpm_geo_batch_run", g, Photo{GPM_PHOTO_PM, 0.f}, stats);
+}
+
+extern "C" int gpm_geo_batch_run_photo(const gpm_geo_batch_desc* g, int kind, float min_std, gpm_geo_batch_stats* stats)
+{
+    return geo_batch_run("gpm_geo_batch_run_photo", g, Photo{kind, min_std}, stats);
 }

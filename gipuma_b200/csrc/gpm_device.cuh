@@ -39,6 +39,7 @@ namespace gpm {
 #define GPM_FUSED_SITES_FLOAT  {1, 0, 0, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1}
 #define GPM_FUSED_SITES_FLOAT4 {0, 0, 0, 0, 0, 0, 0, 0, 0, 9, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1}
 #define GPM_PROV_UNKNOWN 0xff        // prov[]: cost of unknown rounding variant (else bit 0 = x-first, bit 1 = gradient folding)
+#define GPM_PROV_NCC 0x10            // prov[]: an NCC cost (DESIGN.md §15), which has one rounding variant at every call site
 
 // ---- exact-arithmetic primitives -------------------------------------------------------------
 // With --use_fast_math these lower to {mul,add,sub,fma}.rn.ftz.f32, which ptxas never fuses.
@@ -110,12 +111,14 @@ struct KParams {
 };
 
 // Geometric-consistency term (DESIGN.md §14): what the k_sweep / k_cost_eval variants with GEO = true read besides KParams.
-// The per-view K, R and t are those of the photometric homography (ViewCam in shared memory).
+// The per-view K, R and t are those of the photometric homography (ViewCam in shared memory).  The NCC variants read
+// min_std (DESIGN.md §15) from here too: it fills the struct's tail padding, so the other kernels' parameters stay as they were.
 struct GeoParams {
     const float* depth;         // [V][H][W] each source view's depth map, along that view's own optical axis
     const float* kinv;          // [V][9] K^-1 of each source view
     float Kref[9];              // the reference camera's K
     float weight, max_err;
+    float min_std;              // NCC: a window whose weighted standard deviation is below this, in grey levels, costs 2
 };
 
 enum { ST_LAUNCH = 0, ST_HYP = 1, ST_SKIP = 2, ST_PRUNED = 3, ST_PAIRS = 4, ST_PAIRS_FULL = 5 };
@@ -132,15 +135,17 @@ struct WarpScratch {
     float* H;       // [V][12]  homographies of the current hypothesis (rows of 3, 16-byte aligned)
     float* D;       // [V][GPM_DSTRIDE] dissimilarities of the current round
     const unsigned char* perm;   // [GPM_MAX_ROUNDS][32] lane -> sample of the round (block-wide table in shared memory)
+    float* a;       // NCC only: [ns_pad] a_s = w_s * r_s
+    float* sums;    // NCC only: [4] the window's W = sum w_s, Sr = sum a_s, Srr = sum a_s * r_s (DESIGN.md §15)
 };
 
-// multiple of 4 floats so that every warp's block stays 16-byte aligned
-__host__ __device__ inline int warp_scratch_floats(int ns_pad, int V, int color)
+// multiple of 4 floats so that every warp's block stays 16-byte aligned; ncc: the NCC variants' a_s and pixel sums
+__host__ __device__ inline int warp_scratch_floats(int ns_pad, int V, int color, bool ncc = false)
 {
-    return (6 * ns_pad + (color ? 12 * ns_pad : 0) + V * 12 + V * GPM_DSTRIDE + 3) & ~3;
+    return (6 * ns_pad + (color ? 12 * ns_pad : 0) + V * 12 + V * GPM_DSTRIDE + (ncc ? ns_pad + 4 : 0) + 3) & ~3;
 }
 
-__device__ __forceinline__ WarpScratch carve(float* base, int ns_pad, int V, int color, const unsigned char* perm)
+__device__ __forceinline__ WarpScratch carve(float* base, int ns_pad, int V, int color, const unsigned char* perm, bool ncc = false)
 {
     WarpScratch s;
     s.perm = perm;
@@ -149,6 +154,8 @@ __device__ __forceinline__ WarpScratch carve(float* base, int ns_pad, int V, int
     float* f = base + 4 * ns_pad + (color ? 12 * ns_pad : 0);
     s.left = f;                    s.w = s.left + ns_pad;
     s.H = s.w + ns_pad;            s.D = s.H + V * 12;
+    s.a = ncc ? s.D + V * GPM_DSTRIDE : nullptr;
+    s.sums = ncc ? s.a + ns_pad : nullptr;
     return s;
 }
 
@@ -306,6 +313,21 @@ __device__ __forceinline__ float geo_cost(const KParams& P, const GeoParams& G, 
     return fmul(G.weight, err < G.max_err ? err : G.max_err);      // a NaN err counts as max_err
 }
 
+// ---- NCC cost of one source view from the window sums — DESIGN.md §15 ---------------------------------------------
+// Same arithmetic rules as geo_cost (oracle/pyncc.py restates it).  Wsum, Sr, Srr: the pixel's sums (setup_window);
+// St, Stt, Srt: the view's sums for the hypothesis; min_var = min_std * min_std.
+__device__ __forceinline__ float ncc_cost(float Wsum, float Sr, float Srr, float St, float Stt, float Srt, float min_var)
+{
+    const float mr = fdiv(Sr, Wsum), mt = fdiv(St, Wsum);
+    const float vr = fsub(fdiv(Srr, Wsum), fmul(mr, mr));
+    const float vt = fsub(fdiv(Stt, Wsum), fmul(mt, mt));
+    const float c = fsub(fdiv(Srt, Wsum), fmul(mr, mt));
+    if (!(Wsum > 0.0f) || !(vr >= min_var) || !(vt >= min_var)) return 2.0f;     // flat window, or one-pass cancellation
+    const float x = fsub(1.0f, fdiv(c, __fsqrt_rn(fmul(vr, vt))));
+    if (x != x) return 2.0f;
+    return x < 0.0f ? 0.0f : (x > 2.0f ? 2.0f : x);
+}
+
 // ---- cost of one plane hypothesis at the warp's pixel ---------------------------------------
 // pmCostMultiview_cu (gipuma.cu:720-806) over pmCost_shared (:585-680) / pmCostComputation_shared (:223-277).
 // Returns the exact combined cost, or — if `bound` is finite and an exact lower bound of the final cost
@@ -318,7 +340,9 @@ __device__ __forceinline__ float geo_cost(const KParams& P, const GeoParams& G, 
 // GEO: every view's cost is fadd(photometric cost, geo_cost) (DESIGN.md §14); (gpx, gpy) is the pixel.  The geometric terms
 // are computed before the first round and added to the partial costs of every bound test as well: g >= 0 and a rounded
 // add is monotone, so the bound stays an exact lower bound.
-template <int XF, bool COLOR, bool GEO = false>
+// NCC: the photometric cost of every view is the NCC cost (DESIGN.md §15, grey images only; G->min_std).  XF and `rt` are
+// ignored: every call site uses one rounding variant.  No bound is tested (partial sums bound nothing); `bound` is ignored.
+template <int XF, bool COLOR, bool GEO = false, bool NCC = false>
 __device__ __forceinline__ float eval_plane(const KParams& P, const float* __restrict__ sCam, const WarpScratch& ws,
                                             cudaTextureObject_t src, float nx, float ny, float nz, float d,
                                             float bound, unsigned lane, WarpStats& st,
@@ -365,6 +389,80 @@ __device__ __forceinline__ float eval_plane(const KParams& P, const float* __res
     if constexpr (GEO) {
         if ((int)lane < P.V) g0 = geo_cost(P, *G, sCam + lane * GPM_VIEWCAM_FLOATS, (int)lane, nx, ny, nz, d, gpx, gpy);
         if ((int)lane + 32 < P.V) g1 = geo_cost(P, *G, sCam + (lane + 32) * GPM_VIEWCAM_FLOATS, (int)lane + 32, nx, ny, nz, d, gpx, gpy);
+    }
+    if constexpr (NCC) {
+        static_assert(!COLOR, "the NCC cost is built for grey images only");
+        st.hyp++;
+        st.pairs_full += (unsigned long long)P.V * P.ns;
+        // t_s of view v at sample s: one fetch at the PM cost's centre tap, the x-term first in every row of H
+        auto fetch_centre = [&](int v, int s) {
+            const float4* H4 = reinterpret_cast<const float4*>(ws.H + v * 12);
+            const float4 h0 = H4[0], h1 = H4[1], h2 = H4[2];
+            const float4 a = ws.A[s];
+            const float X = fadd(h0.z, ffma(h0.y, a.y, fmul(h0.x, a.x)));
+            const float Y = fadd(h1.y, ffma(h1.x, a.y, fmul(h0.w, a.x)));
+            const float Z = fadd(h2.x, ffma(h1.w, a.y, fmul(h1.z, a.x)));
+            const float r = frcp(Z);
+            return tex2DLayered<float>(src, ffma(X, r, 0.5f), ffma(Y, r, 0.5f), v);
+        };
+        // lane handles pair q = (view v, sample k of the round) of N consecutive groups of 32 pairs, all fetches in flight
+        // before D[v][k] = t is written.  In a round of 32 samples lane = sample, and a step covers N views.  Two views per
+        // step measured fastest (DESIGN.md §15: 4 and 8 hold more fetches in flight but cost registers and were slower).
+        auto ncc_steps = [&](auto nconst, int q0, int s0, int len, int npairs, unsigned M, const unsigned char* prow) {
+            constexpr int N = decltype(nconst)::value;
+            float t[N];
+            int dst[N];
+#pragma unroll
+            for (int u = 0; u < N; u++) {
+                const int q = q0 + u * 32 + (int)lane;
+                const int qc = min(q, npairs - 1);
+                const int v = (int)(((unsigned)qc * M) >> 20);                       // qc / len
+                const int k = prow[qc - v * len];
+                t[u] = fetch_centre(v, s0 + k);
+                dst[u] = (q < npairs) ? v * GPM_DSTRIDE + k : -1;
+            }
+#pragma unroll
+            for (int u = 0; u < N; u++)
+                if (dst[u] >= 0) ws.D[dst[u]] = t[u];
+        };
+        // the three sums of views lane and lane + 32, sequential in sample order
+        float St0 = 0.0f, Stt0 = 0.0f, Srt0 = 0.0f, St1 = 0.0f, Stt1 = 0.0f, Srt1 = 0.0f;
+        int s0 = 0;
+        for (int r = 0; r < P.nrounds; r++) {
+            const int s1 = P.round_end[r];
+            const int len = s1 - s0;
+            const int npairs = P.V * len;
+            const unsigned M = (1u << 20) / (unsigned)len + 1u;
+            const unsigned char* prow = ws.perm + r * 32;
+            int q0 = 0;
+            for (; q0 + 32 < npairs; q0 += 64) ncc_steps(std::integral_constant<int, 2>(), q0, s0, len, npairs, M, prow);
+            if (q0 < npairs) ncc_steps(std::integral_constant<int, 1>(), q0, s0, len, npairs, M, prow);
+            st.pairs += npairs;
+            __syncwarp();
+            const float* w = ws.w + s0;
+            const float* a = ws.a + s0;
+            const float* D0 = ws.D + lane * GPM_DSTRIDE;
+            if ((int)lane < P.V)
+                for (int k = 0; k < len; k++) {
+                    const float t = D0[k], wt = fmul(w[k], t);
+                    St0 = fadd(St0, wt);  Stt0 = fadd(Stt0, fmul(wt, t));  Srt0 = fadd(Srt0, fmul(a[k], t));
+                }
+            if ((int)lane + 32 < P.V) {
+                const float* D1 = D0 + 32 * GPM_DSTRIDE;
+                for (int k = 0; k < len; k++) {
+                    const float t = D1[k], wt = fmul(w[k], t);
+                    St1 = fadd(St1, wt);  Stt1 = fadd(Stt1, fmul(wt, t));  Srt1 = fadd(Srt1, fmul(a[k], t));
+                }
+            }
+            __syncwarp();
+            s0 = s1;
+        }
+        const float Wsum = ws.sums[0], Sr = ws.sums[1], Srr = ws.sums[2];
+        const float min_var = fmul(G->min_std, G->min_std);
+        const float c0 = ncc_cost(Wsum, Sr, Srr, St0, Stt0, Srt0, min_var);
+        const float c1 = ncc_cost(Wsum, Sr, Srr, St1, Stt1, Srt1, min_var);
+        if constexpr (GEO) return combine_views(P, fadd(c0, g0), fadd(c1, g1), lane);
+        else return combine_views(P, c0, c1, lane);
     }
 
     const float one_minus_alpha = fsub(1.0f, P.alpha);
@@ -558,7 +656,8 @@ __device__ __forceinline__ float eval_plane(const KParams& P, const float* __res
 }
 
 // ---- per-pixel, hypothesis-independent window data ------------------------------------------
-template <bool COLOR>
+// NCC: also a_s = w_s * r_s and the pixel's sums W, Sr, Srr (DESIGN.md §15), added from +0 in sample order.
+template <bool COLOR, bool NCC = false>
 __device__ __forceinline__ void setup_window(const KParams& P, const float* __restrict__ tile, const WarpScratch& ws,
                                              int px, int py, int tile_x0, int tile_y0, unsigned lane)
 {
@@ -597,8 +696,20 @@ __device__ __forceinline__ void setup_window(const KParams& P, const float* __re
         ws.left[s] = left;
         // expf(-|left - center| / gamma) under --use_fast_math: (|.| * -rcp(gamma)) * log2(e) -> ex2
         ws.w[s] = fex2(fmul(fmul(fabsf(fsub(left, center)), nrg), 1.4426950216293334961f));
+        if constexpr (NCC) ws.a[s] = fmul(ws.w[s], left);
     }
     __syncwarp();
+    if constexpr (NCC) {
+        if (lane == 0) {
+            float Wsum = 0.0f, Sr = 0.0f, Srr = 0.0f;
+            for (int s = 0; s < P.ns; s++) {
+                const float a = ws.a[s];
+                Wsum = fadd(Wsum, ws.w[s]);  Sr = fadd(Sr, a);  Srr = fadd(Srr, fmul(a, ws.left[s]));
+            }
+            ws.sums[0] = Wsum;  ws.sums[1] = Sr;  ws.sums[2] = Srr;
+        }
+        __syncwarp();
+    }
 }
 
 }  // namespace gpm

@@ -8,13 +8,14 @@ namespace gpm {
 
 __host__ __device__ inline int tile_floats(const KParams& P) { return P.tile_stride * P.tile_w * (P.color ? 4 : 1); }
 __host__ __device__ inline int fixed_smem_floats(const KParams& P) { return (tile_floats(P) + P.V * GPM_VIEWCAM_FLOATS + 3) & ~3; }
-__device__ __forceinline__ unsigned long long* block_mbar(const KParams& P, float* smem_base)
+// ncc: the NCC kernels' larger per-warp scratch (warp_scratch_floats)
+__device__ __forceinline__ unsigned long long* block_mbar(const KParams& P, float* smem_base, bool ncc = false)
 {
-    return reinterpret_cast<unsigned long long*>(smem_base + fixed_smem_floats(P) + (size_t)P.nwarps * warp_scratch_floats(P.ns_pad, P.V, P.color) + 2);
+    return reinterpret_cast<unsigned long long*>(smem_base + fixed_smem_floats(P) + (size_t)P.nwarps * warp_scratch_floats(P.ns_pad, P.V, P.color, ncc) + 2);
 }
-__device__ __forceinline__ unsigned char* block_perm(const KParams& P, float* smem_base)
+__device__ __forceinline__ unsigned char* block_perm(const KParams& P, float* smem_base, bool ncc = false)
 {
-    return reinterpret_cast<unsigned char*>(smem_base + fixed_smem_floats(P) + (size_t)P.nwarps * warp_scratch_floats(P.ns_pad, P.V, P.color) + 4);
+    return reinterpret_cast<unsigned char*>(smem_base + fixed_smem_floats(P) + (size_t)P.nwarps * warp_scratch_floats(P.ns_pad, P.V, P.color, ncc) + 4);
 }
 
 // ---- TMA (cp.async.bulk.tensor) + mbarrier primitives -------------------------------------------------------------
@@ -49,9 +50,9 @@ __device__ __forceinline__ void mbar_wait(unsigned long long* bar, unsigned pari
 // the replicate-padded reference image and the block waits on its mbarrier while the other threads copy the camera and
 // lane tables.  `phase` = parity of the barrier's current phase (0 for the first / only tile of a block).
 __device__ __forceinline__ void stage_block(const KParams& P, const CUtensorMap* tmap, const ViewCam* __restrict__ cams,
-                                            float* tile, float* sCam, int tile_x0, int tile_y0, unsigned phase = 0u)
+                                            float* tile, float* sCam, int tile_x0, int tile_y0, unsigned phase = 0u, bool ncc = false)
 {
-    unsigned long long* bar = block_mbar(P, tile);
+    unsigned long long* bar = block_mbar(P, tile, ncc);
     if (threadIdx.x == 0) {
         if (phase == 0u) mbar_init(bar, 1);
         mbar_arrive_expect_tx(bar, (unsigned)(tile_floats(P) * sizeof(float)));
@@ -60,7 +61,7 @@ __device__ __forceinline__ void stage_block(const KParams& P, const CUtensorMap*
     const float* c = reinterpret_cast<const float*>(cams);
     for (int e = threadIdx.x; e < P.V * GPM_VIEWCAM_FLOATS; e += blockDim.x) sCam[e] = c[e];
     // lane -> sample table of the sampling rounds (KParams::perm), word by word
-    unsigned* sp = reinterpret_cast<unsigned*>(block_perm(P, tile));
+    unsigned* sp = reinterpret_cast<unsigned*>(block_perm(P, tile, ncc));
     const unsigned* gp = reinterpret_cast<const unsigned*>(&P.perm[0][0]);
     for (int e = threadIdx.x; e < GPM_MAX_ROUNDS * 8; e += blockDim.x) sp[e] = gp[e];
     __syncthreads();                                // tables visible; mbarrier initialised before anyone waits on it
@@ -79,9 +80,9 @@ __device__ __forceinline__ void flush_stats(unsigned long long* stats, const War
 }
 
 // shared memory: [tile tile_stride*tile_w][cams V*21][pad to 16 B][nwarps * warp_scratch][4 ints: work counter, unused, mbarrier (8 B)][lane permutation table, GPM_MAX_ROUNDS x 32 bytes]
-__host__ __device__ inline size_t block_smem_bytes(const KParams& P)
+__host__ __device__ inline size_t block_smem_bytes(const KParams& P, bool ncc = false)
 {
-    size_t fl = (size_t)fixed_smem_floats(P) + (size_t)P.nwarps * warp_scratch_floats(P.ns_pad, P.V, P.color) + 4 + GPM_MAX_ROUNDS * 8;
+    size_t fl = (size_t)fixed_smem_floats(P) + (size_t)P.nwarps * warp_scratch_floats(P.ns_pad, P.V, P.color, ncc) + 4 + GPM_MAX_ROUNDS * 8;
     return fl * sizeof(float);
 }
 
@@ -147,8 +148,9 @@ __global__ void k_init_planes(const __grid_constant__ KParams P, unsigned long l
 #define GPM_LB_THREADS 512       // max threads per block of the warp-per-pixel kernels (16 warps)
 #define GPM_LB_BLOCKS 1
 #endif
-// GEO: the cost with the geometric-consistency term (DESIGN.md §14); G is only read then.
-template <bool COLOR, bool GEO = false>
+// GEO: the cost with the geometric-consistency term (DESIGN.md §14); NCC: the NCC photometric cost (§15, grey only).
+// G is only read in those variants.
+template <bool COLOR, bool GEO = false, bool NCC = false>
 __global__ void __launch_bounds__(GPM_LB_THREADS, GPM_LB_BLOCKS)
 k_cost_eval(const __grid_constant__ KParams P, const __grid_constant__ CUtensorMap tmap, const ViewCam* __restrict__ cams,
             cudaTextureObject_t src, const float4* __restrict__ planes, float* __restrict__ cost, unsigned long long* __restrict__ stats,
@@ -160,20 +162,23 @@ k_cost_eval(const __grid_constant__ KParams P, const __grid_constant__ CUtensorM
     float* scratch = smem + fixed_smem_floats(P);
     const unsigned lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const int tile_x0 = blockIdx.x * GPM_TILE - P.halo, tile_y0 = blockIdx.y * GPM_TILE - P.halo;
-    stage_block(P, &tmap, cams, tile, sCam, tile_x0, tile_y0);
-    const WarpScratch ws = carve(scratch + (size_t)warp * warp_scratch_floats(P.ns_pad, P.V, P.color), P.ns_pad, P.V, P.color, block_perm(P, smem));
+    stage_block(P, &tmap, cams, tile, sCam, tile_x0, tile_y0, 0u, NCC);
+    const WarpScratch ws = carve(scratch + (size_t)warp * warp_scratch_floats(P.ns_pad, P.V, P.color, NCC), P.ns_pad, P.V, P.color,
+                                 block_perm(P, smem, NCC), NCC);
     WarpStats st = {0, 0, 0, 0, 0};
     for (int idx = warp; idx < GPM_TILE * GPM_TILE; idx += P.nwarps) {
         const int px = blockIdx.x * GPM_TILE + (idx & 31), py = blockIdx.y * GPM_TILE + (idx >> 5);
         if (px >= P.W || py >= P.H) continue;
-        setup_window<COLOR>(P, tile + P.tile_xo, ws, px, py, tile_x0, tile_y0, lane);
+        setup_window<COLOR, NCC>(P, tile + P.tile_xo, ws, px, py, tile_x0, tile_y0, lane);
         const float4 n = planes[(size_t)py * P.W + px];
         const float inf = __int_as_float(0x7f800000);
-        const GeoParams* g = GEO ? &G : nullptr;
+        const GeoParams* g = (GEO || NCC) ? &G : nullptr;
         const float fpx = __int2float_rn(px), fpy = __int2float_rn(py);
-        const float c = (P.cost_rt & 12) ? eval_plane<2, COLOR, GEO>(P, sCam, ws, src, n.x, n.y, n.z, n.w, inf, lane, st, nullptr, nullptr, (unsigned)P.cost_rt, g, fpx, fpy)
-                        : P.cost_variant ? eval_plane<1, COLOR, GEO>(P, sCam, ws, src, n.x, n.y, n.z, n.w, inf, lane, st, nullptr, nullptr, 0u, g, fpx, fpy)
-                                         : eval_plane<0, COLOR, GEO>(P, sCam, ws, src, n.x, n.y, n.z, n.w, inf, lane, st, nullptr, nullptr, 0u, g, fpx, fpy);
+        float c;
+        if constexpr (NCC) c = eval_plane<1, COLOR, GEO, true>(P, sCam, ws, src, n.x, n.y, n.z, n.w, inf, lane, st, nullptr, nullptr, 0u, g, fpx, fpy);
+        else c = (P.cost_rt & 12) ? eval_plane<2, COLOR, GEO>(P, sCam, ws, src, n.x, n.y, n.z, n.w, inf, lane, st, nullptr, nullptr, (unsigned)P.cost_rt, g, fpx, fpy)
+                 : P.cost_variant ? eval_plane<1, COLOR, GEO>(P, sCam, ws, src, n.x, n.y, n.z, n.w, inf, lane, st, nullptr, nullptr, 0u, g, fpx, fpy)
+                                  : eval_plane<0, COLOR, GEO>(P, sCam, ws, src, n.x, n.y, n.z, n.w, inf, lane, st, nullptr, nullptr, 0u, g, fpx, fpy);
         if (lane == 0) cost[(size_t)py * P.W + px] = c;
     }
     flush_stats(stats, st, lane);
@@ -216,8 +221,9 @@ __device__ __forceinline__ bool close_far_neighbour(int k, const int& px, const 
     return ok;
 }
 
-// GEO: the cost with the geometric-consistency term (DESIGN.md §14; 8-neighbour sweep only); G is only read then.
-template <bool COLOR, bool FUSED, bool GEO = false>
+// GEO: the cost with the geometric-consistency term (DESIGN.md §14; 8-neighbour sweep only); NCC: the NCC photometric cost
+// (§15; 8-neighbour sweep, grey images only).  G is only read in those variants.
+template <bool COLOR, bool FUSED, bool GEO = false, bool NCC = false>
 __global__ void __launch_bounds__(GPM_LB_THREADS, GPM_LB_BLOCKS)
 k_sweep(const __grid_constant__ KParams P, const __grid_constant__ CUtensorMap tmap, const ViewCam* __restrict__ cams,
         cudaTextureObject_t src, float4* __restrict__ planes, float* __restrict__ cost,
@@ -225,17 +231,19 @@ k_sweep(const __grid_constant__ KParams P, const __grid_constant__ CUtensorMap t
         unsigned long long* __restrict__ stats, const __grid_constant__ GeoParams G)
 {
     static_assert(!(FUSED && GEO), "the geometric term is built for the 8-neighbour sweep only");
-    const GeoParams* g = GEO ? &G : nullptr;
+    static_assert(!(NCC && (FUSED || COLOR)), "the NCC cost is built for the 8-neighbour sweep on grey images only");
+    const GeoParams* g = (GEO || NCC) ? &G : nullptr;
     extern __shared__ __align__(128) float smem[];
     float* tile = smem;
     float* sCam = tile + tile_floats(P);
     float* scratch = smem + fixed_smem_floats(P);
-    int* counter = reinterpret_cast<int*>(scratch + (size_t)P.nwarps * warp_scratch_floats(P.ns_pad, P.V, P.color));
+    int* counter = reinterpret_cast<int*>(scratch + (size_t)P.nwarps * warp_scratch_floats(P.ns_pad, P.V, P.color, NCC));
     const unsigned lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const int tile_x0 = blockIdx.x * GPM_TILE - P.halo, tile_y0 = blockIdx.y * GPM_TILE - P.halo;
     if (threadIdx.x == 0) counter[0] = P.nwarps;
-    stage_block(P, &tmap, cams, tile, sCam, tile_x0, tile_y0);
-    const WarpScratch ws = carve(scratch + (size_t)warp * warp_scratch_floats(P.ns_pad, P.V, P.color), P.ns_pad, P.V, P.color, block_perm(P, smem));
+    stage_block(P, &tmap, cams, tile, sCam, tile_x0, tile_y0, 0u, NCC);
+    const WarpScratch ws = carve(scratch + (size_t)warp * warp_scratch_floats(P.ns_pad, P.V, P.color, NCC), P.ns_pad, P.V, P.color,
+                                 block_perm(P, smem, NCC), NCC);
     const RefCam& cam = P.ref;
     WarpStats st = {0, 0, 0, 0, 0};
     const int W = P.W, H = P.H;
@@ -287,7 +295,8 @@ k_sweep(const __grid_constant__ KParams P, const __grid_constant__ CUtensorMap t
             // without evaluation, in every later iteration.  Exact, not a heuristic.
             // the cost function of the fused kernel differs between its inlined call sites (P.site): the duplicate / memo
             // shortcuts below only pair candidates of sites with the same rounding variant
-            const unsigned my_site = FUSED ? (unsigned)P.site[lane < NC ? lane : 0] : (COLOR ? 0u : 1u);
+            // (NCC costs have a provenance code of their own, GPM_PROV_NCC)
+            const unsigned my_site = NCC ? GPM_PROV_NCC : FUSED ? (unsigned)P.site[lane < NC ? lane : 0] : (COLOR ? 0u : 1u);
             unsigned mmask = P.memo ? M.mask[center] : 0u;
             const bool old_ok = P.memo && lane < NC && ((mmask >> lane) & 1);
             const unsigned old_id = old_ok ? M.seen[center * NC + lane] : 0u;
@@ -298,7 +307,7 @@ k_sweep(const __grid_constant__ KParams P, const __grid_constant__ CUtensorMap t
                 if (!((cand_mask >> k) & 1)) continue;
                 // rounding variant of this call site: x-first for float images, y-first for float4 (DESIGN.md §2); the fused
                 // kernel's inlined sites are looked up (bit 0 = x-first, bit 1 = gradient folding)
-                const unsigned site = FUSED ? (unsigned)P.site[k] : (COLOR ? 0u : 1u);
+                const unsigned site = NCC ? GPM_PROV_NCC : FUSED ? (unsigned)P.site[k] : (COLOR ? 0u : 1u);
                 float4 nb;
                 nb.x = __shfl_sync(GPM_FULL, mine.x, k);  nb.y = __shfl_sync(GPM_FULL, mine.y, k);
                 nb.z = __shfl_sync(GPM_FULL, mine.z, k);  nb.w = __shfl_sync(GPM_FULL, mine.w, k);
@@ -315,9 +324,9 @@ k_sweep(const __grid_constant__ KParams P, const __grid_constant__ CUtensorMap t
                 const bool same_mine = P.dedupe_cand && mine_ok && (int)lane < k && my_site == site && cand_id == mine_id;
                 const bool dup = __any_sync(GPM_FULL, same_mine);
                 if (!in_range || same_now || dup) { st.skip++; continue; }
-                if (!window_ready) { setup_window<COLOR>(P, tile + P.tile_xo, ws, px, py, tile_x0, tile_y0, lane);  window_ready = true; }
+                if (!window_ready) { setup_window<COLOR, NCC>(P, tile + P.tile_xo, ws, px, py, tile_x0, tile_y0, lane);  window_ready = true; }
                 const float c = FUSED ? eval_plane<2, COLOR>(P, sCam, ws, src, nb.x, nb.y, nb.z, nb.w, cost_now, lane, st, nullptr, nullptr, site)
-                                      : eval_plane<(COLOR ? 0 : 1), COLOR, GEO>(P, sCam, ws, src, nb.x, nb.y, nb.z, nb.w, cost_now, lane, st,
+                                      : eval_plane<(COLOR ? 0 : 1), COLOR, GEO, NCC>(P, sCam, ws, src, nb.x, nb.y, nb.z, nb.w, cost_now, lane, st,
                                                                                 nullptr, nullptr, 0u, g, fpx, fpy);
                 if (c < cost_now) {                                                              // :867-871
                     disp_now = disp_before;
@@ -343,7 +352,7 @@ k_sweep(const __grid_constant__ KParams P, const __grid_constant__ CUtensorMap t
                 }
             }
             if (refine) {
-                if (!window_ready) { setup_window<COLOR>(P, tile + P.tile_xo, ws, px, py, tile_x0, tile_y0, lane);  window_ready = true; }
+                if (!window_ready) { setup_window<COLOR, NCC>(P, tile + P.tile_xo, ws, px, py, tile_x0, tile_y0, lane);  window_ready = true; }
                 const unsigned id_start = own_id;
                 bool any_accept = false;
                 // planeRefinement_cu, gipuma.cu:928-994 with getRndDispAndUnitVector_cu, :890-927
@@ -373,9 +382,9 @@ k_sweep(const __grid_constant__ KParams P, const __grid_constant__ CUtensorMap t
                     cand.x = fmul(ax, rs);  cand.y = fmul(ay, rs);  cand.z = fmul(az, rs);
                     if (dot3(cand.x, cand.y, cand.z, vx, vy, vz) > 0.0f) { cand.x = -cand.x;  cand.y = -cand.y;  cand.z = -cand.z; }
                     cand.w = plane_d(cam, cand.x, cand.y, cand.z, fpx, fpy, depth_new);   // :969
-                    const unsigned rsite = FUSED ? (unsigned)P.site[20] : 0u;
+                    const unsigned rsite = NCC ? GPM_PROV_NCC : FUSED ? (unsigned)P.site[20] : 0u;
                     const float c = FUSED ? eval_plane<2, COLOR>(P, sCam, ws, src, cand.x, cand.y, cand.z, cand.w, cost_now, lane, st, nullptr, nullptr, rsite)
-                                          : eval_plane<0, COLOR, GEO>(P, sCam, ws, src, cand.x, cand.y, cand.z, cand.w, cost_now, lane, st,
+                                          : eval_plane<0, COLOR, GEO, NCC>(P, sCam, ws, src, cand.x, cand.y, cand.z, cand.w, cost_now, lane, st,
                                                                       nullptr, nullptr, 0u, g, fpx, fpy);
                     if (c < cost_now) {                                                          // :986-990 (no depth-range test)
                         prov_now = (int)rsite;

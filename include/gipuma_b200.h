@@ -105,6 +105,18 @@ int gpm_set_num_views(gpm_ctx* ctx, int n_views);
 int gpm_set_view_depth(gpm_ctx* ctx, int v, const float* depth, size_t pitch_bytes, int on_device);
 int gpm_set_geometric(gpm_ctx* ctx, float weight, float max_err);
 
+/* ---- photometric cost (DESIGN.md §15) ---------------------------------------------------------------------------------
+ * GPM_PHOTO_PM (the default) is the reference's adaptive-support-weight cost.  GPM_PHOTO_NCC replaces each view's cost by
+ * 1 - the support-weighted normalised cross-correlation of the window (clamped to [0, 2]), which a gain and an offset of the
+ * source image leave unchanged; a window whose weighted standard deviation, in the reference or the source view, is below
+ * min_std grey levels costs 2.  Grey images and the 8-neighbour sweep only.  With the geometric mode on, view j's cost is
+ * ncc_j + g_j.  The lower-bound early-out (option "prune") has no effect on NCC costs.  min_std is ignored for PM.
+ * Refused with GPM_E_ARG: an unknown kind; NCC with min_std not finite or <= 0, on a context holding colour images, or with
+ * option neighbours = 20 (and neighbours = 20 while NCC is on).  With GPM_E_STATE: a colour image upload while NCC is on, and
+ * every gpm_shard_* call taking a context.  A refused call changes nothing. */
+enum { GPM_PHOTO_PM = 0, GPM_PHOTO_NCC = 1 };
+int gpm_set_photometric(gpm_ctx* ctx, int kind, float min_std);
+
 /* Seed of the per-pixel curand_init(seed, y, x) at initialisation (gipuma.cu:1019; the reference uses
  * clock64()) and the refinement RNG mode. */
 int gpm_set_rng(gpm_ctx* ctx, unsigned long long seed, int mode);
@@ -274,6 +286,13 @@ typedef struct gpm_geo_batch_stats {
     int* ref_views;                    /* NULL or n_refs * max_views image indices of each job's selected views, -1 after the last */
 } gpm_geo_batch_stats;
 int gpm_geo_batch_run(const gpm_geo_batch_desc* desc, gpm_geo_batch_stats* stats);
+
+/* The batch drivers with a choice of photometric cost: every job's context gets gpm_set_photometric(kind, min_std) in the
+ * per-view setup (both passes of the geometric driver).  gpm_batch_run and gpm_geo_batch_run are these with GPM_PHOTO_PM.
+ * Refused with GPM_E_ARG before any CUDA call, besides what those refuse: what gpm_set_photometric refuses for its
+ * arguments, and channels = 4 with GPM_PHOTO_NCC. */
+int gpm_batch_run_photo(const gpm_batch_desc* desc, int kind, float min_std, gpm_batch_stats* stats);
+int gpm_geo_batch_run_photo(const gpm_geo_batch_desc* desc, int kind, float min_std, gpm_geo_batch_stats* stats);
 
 /* ---- depth-map fusion: the per-view world-frame outputs (norm4 of gpm_batch_run, or its .dmb files) -> one point cloud;
  * what the reference's scripts hand to the external `fusibile` (scripts/dtu_fast.sh:56-57).  Deterministic: the same inputs
