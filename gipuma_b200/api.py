@@ -62,6 +62,10 @@ class GpmGeoBatchStats(C.Structure):
                 ("pass1_sweep_ms", C.POINTER(C.c_float)), ("ref_views", C.POINTER(C.c_int))]
 
 
+class GpmJobOpts(C.Structure):
+    _fields_ = [("photometric", C.c_int), ("ncc_min_std", C.c_float), ("propagation", C.c_int)]
+
+
 class GpmFuseCamera(C.Structure):
     _fields_ = [("M_inv", C.c_float * 9), ("P", C.c_float * 12), ("f", C.c_float)]
 
@@ -124,6 +128,7 @@ def load_library():
     L.gpm_set_view_depth.argtypes = [vp, C.c_int, vp, C.c_size_t, C.c_int]
     L.gpm_set_geometric.argtypes = [vp, C.c_float, C.c_float]
     L.gpm_set_photometric.argtypes = [vp, C.c_int, C.c_float]
+    L.gpm_set_propagation.argtypes = [vp, C.c_int]
     L.gpm_set_rng.argtypes = [vp, C.c_ulonglong, C.c_int]
     L.gpm_set_state.argtypes = [vp, vp, vp, C.c_int]
     L.gpm_get_state.argtypes = [vp, vp, vp, C.c_int]
@@ -158,6 +163,8 @@ def load_library():
     L.gpm_geo_batch_run.argtypes = [C.POINTER(GpmGeoBatchDesc), C.POINTER(GpmGeoBatchStats)]
     L.gpm_batch_run_photo.argtypes = [C.POINTER(GpmBatchDesc), C.c_int, C.c_float, C.POINTER(GpmBatchStats)]
     L.gpm_geo_batch_run_photo.argtypes = [C.POINTER(GpmGeoBatchDesc), C.c_int, C.c_float, C.POINTER(GpmGeoBatchStats)]
+    L.gpm_batch_run_opts.argtypes = [C.POINTER(GpmBatchDesc), C.POINTER(GpmJobOpts), C.POINTER(GpmBatchStats)]
+    L.gpm_geo_batch_run_opts.argtypes = [C.POINTER(GpmGeoBatchDesc), C.POINTER(GpmJobOpts), C.POINTER(GpmGeoBatchStats)]
     L.gpm_batch_last_error.restype = C.c_char_p
     L.gpm_stream.restype = vp
     L.gpm_fuse_cameras.argtypes = [C.POINTER(C.c_double), C.c_int, C.c_double, C.POINTER(GpmFuseCamera)]
@@ -166,11 +173,12 @@ def load_library():
     L.gpm_nearest_dist.argtypes = [C.POINTER(GpmNnDesc), C.POINTER(GpmNnResult)]
     for name in ("gpm_create", "gpm_set_params", "gpm_set_reference", "gpm_set_view", "gpm_set_reference_color",
                  "gpm_set_view_color", "gpm_set_num_views", "gpm_set_view_depth", "gpm_set_geometric", "gpm_set_photometric",
-                 "gpm_set_rng", "gpm_set_state", "gpm_get_state", "gpm_init", "gpm_sweep", "gpm_phase",
+                 "gpm_set_propagation", "gpm_set_rng", "gpm_set_state", "gpm_get_state", "gpm_init", "gpm_sweep", "gpm_phase",
                  "gpm_finalize", "gpm_cost_eval", "gpm_run", "gpm_get_stats", "gpm_reset_stats", "gpm_set_option",
                  "gpm_init_planes", "gpm_shard_num_stages", "gpm_shard_stage", "gpm_shard_finish_init", "gpm_shard_unique_id",
                  "gpm_shard_comm_init", "gpm_shard_comm_attach", "gpm_shard_run", "gpm_measure_fetch_peak", "gpm_batch_run",
-                 "gpm_geo_batch_run", "gpm_batch_run_photo", "gpm_geo_batch_run_photo", "gpm_prepare_cameras", "gpm_select_views", "gpm_write_dmb", "gpm_read_dmb", "gpm_write_result_dmb",
+                 "gpm_geo_batch_run", "gpm_batch_run_photo", "gpm_geo_batch_run_photo", "gpm_batch_run_opts", "gpm_geo_batch_run_opts",
+                 "gpm_prepare_cameras", "gpm_select_views", "gpm_write_dmb", "gpm_read_dmb", "gpm_write_result_dmb",
                  "gpm_fuse_cameras", "gpm_fuse", "gpm_write_ply", "gpm_nearest_dist"):
         getattr(L, name).restype = C.c_int
     _lib = L
@@ -250,6 +258,25 @@ def check_photometric(kind: str, min_std: float) -> int:
     if kind == "ncc" and not (np.isfinite(min_std) and min_std > 0):
         raise ValueError("min_std must be finite and > 0 (got %r)" % (min_std,))
     return PHOTOMETRIC[kind]
+
+
+# Propagation (DESIGN.md §16): "fixed", the reference's 8 neighbours (the default), and "adaptive", ACMH's adaptive
+# checkerboard sampling.
+PROPAGATION = {"fixed": 0, "adaptive": 1}
+
+
+def check_propagation(kind: str) -> int:
+    """The argument rule of gpm_set_propagation, checked before any call into the library; returns the C-ABI's kind."""
+    if kind not in PROPAGATION:
+        raise ValueError("propagation must be one of %s (got %r)" % (sorted(PROPAGATION), kind))
+    return PROPAGATION[kind]
+
+
+def job_opts(photometric: str = "pm", ncc_min_std: float = NCC_MIN_STD, propagation: str = "fixed") -> GpmJobOpts:
+    """gpm_job_opts of the batch drivers, every argument checked before any call into the library."""
+    kind = check_photometric(photometric, ncc_min_std)
+    prop = check_propagation(propagation)
+    return GpmJobOpts(kind, float(ncc_min_std) if photometric == "ncc" else 0.0, prop)
 
 
 class Context:
@@ -334,6 +361,12 @@ class Context:
         a window whose weighted standard deviation is below it costs 2; ignored for "pm"."""
         k = check_photometric(kind, min_std)
         self._check(self.lib.gpm_set_photometric(self.h, k, float(min_std) if kind == "ncc" else 0.0))
+
+    def set_propagation(self, kind: str = "fixed"):
+        """Which plane each pixel is offered from each of its 8 directions (DESIGN.md §16): "fixed", the reference's
+        neighbours at 1 and 5 px (the default), or "adaptive", the cheapest pixel of a larger region per direction (ACMH's
+        adaptive checkerboard sampling).  8-neighbour sweep only; may be switched at any point of a run."""
+        self._check(self.lib.gpm_set_propagation(self.h, check_propagation(kind)))
 
     def set_rng(self, seed: int, mode: int = GPM_RNG_REFERENCE):
         self._check(self.lib.gpm_set_rng(self.h, seed, mode))
@@ -541,12 +574,13 @@ def _job_stats(n_refs):
 
 def batch_run(images, Ps, params, refs, devices=(0,), cam_scale: float = 1.0, min_angle: float = 10.0, max_angle: float = 30.0,
               max_views: int = 9, seed: int = 0xC0FFEE, out_dir: Optional[str] = None, want_outputs: bool = True,
-              photometric: str = "pm", ncc_min_std: float = NCC_MIN_STD):
-    """Reference-view batch in ONE process (gpm_batch_run_photo): `images` [n, H, W] float32 (shared, page-locked once), `Ps`
+              photometric: str = "pm", ncc_min_std: float = NCC_MIN_STD, propagation: str = "fixed"):
+    """Reference-view batch in ONE process (gpm_batch_run_opts): `images` [n, H, W] float32 (shared, page-locked once), `Ps`
     n 3x4 projections, `refs` the reference views to process, `devices` the CUDA ordinals to use (one worker thread each),
-    `photometric` the cost, "pm" or "ncc" with min_std `ncc_min_std` (Context.set_photometric).
+    `photometric` the cost, "pm" or "ncc" with min_std `ncc_min_std` (Context.set_photometric), `propagation` "fixed" or
+    "adaptive" (Context.set_propagation).
     Returns (norm4 [len(refs), H, W, 4] or None, cost or None, stats dict)."""
-    kind = check_photometric(photometric, ncc_min_std)
+    opts = job_opts(photometric, ncc_min_std, propagation)
     lib = load_library()
     imgs = np.ascontiguousarray(images, dtype=np.float32)
     n, H, W = imgs.shape
@@ -554,7 +588,7 @@ def batch_run(images, Ps, params, refs, devices=(0,), cam_scale: float = 1.0, mi
     cc = np.empty((len(refs), H, W), np.float32) if want_outputs else None
     d, _keep = _batch_desc(imgs, Ps, params, refs, devices, cam_scale, min_angle, max_angle, max_views, seed, out_dir, n4, cc)
     st = _job_stats(len(refs))
-    rc = lib.gpm_batch_run_photo(C.byref(d), kind, float(ncc_min_std) if photometric == "ncc" else 0.0, C.byref(st))
+    rc = lib.gpm_batch_run_opts(C.byref(d), C.byref(opts), C.byref(st))
     if rc != 0:
         raise GipumaError("gpm_batch_run failed (%d): %s" % (rc, lib.gpm_batch_last_error().decode()))
     k = len(refs)
@@ -565,7 +599,7 @@ def batch_run(images, Ps, params, refs, devices=(0,), cam_scale: float = 1.0, mi
 def geometric_pass(images, Ps, params, refs, geo_iterations: int = 2, weight: float = GEO_WEIGHT, max_err: float = GEO_MAX_ERR,
                    cam_scale: float = 1.0, min_angle: float = 10.0, max_angle: float = 30.0, max_views: int = 9,
                    seed: int = 0xC0FFEE, devices=(0,), out_dir: Optional[str] = None, photometric: str = "pm",
-                   ncc_min_std: float = NCC_MIN_STD):
+                   ncc_min_std: float = NCC_MIN_STD, propagation: str = "fixed"):
     """PatchMatch with a geometric-consistency second pass (DESIGN.md §14) for the reference views `refs`, run by the
     native two-pass batch driver (gpm_geo_batch_run) over the worker pool of `devices` (one worker thread and context each;
     a device may be listed more than once).
@@ -576,13 +610,14 @@ def geometric_pass(images, Ps, params, refs, geo_iterations: int = 2, weight: fl
     pass-1 planes get their exact costs under the new cost (cost_eval), and geo_iterations sweeps and finalize follow.  So a
     run has params.iterations + geo_iterations iterations in all.  images: [n, H, W] grey or [n, H, W, 4] colour; the other
     arguments as batch_run; out_dir: None, or where <ref, 8 digits>/{disp,normals}.dmb of the pass-2 results are written;
-    photometric / ncc_min_std: the photometric cost of both passes, as batch_run ("ncc": grey images only).
+    photometric / ncc_min_std: the photometric cost of both passes, as batch_run ("ncc": grey images only); propagation:
+    the propagation mode of both passes, as batch_run.
     Returns (norm4 [len(refs), H, W, 4], cost [len(refs), H, W], info) with norm4 as batch_run returns it, so fuse and
     evaluate_cloud take it unchanged; info: "pass1_views" (the views pass 1 ran, ascending), "pass1_sweep_s" (in that order)
     and "pass2_sweep_s" (per reference view): CUDA-event seconds of each view's sweep call on its context's stream;
     "views" (image indices of the source views each reference view selected), "device" (the device that ran its pass 2)."""
     check_geometric(weight, max_err)
-    kind = check_photometric(photometric, ncc_min_std)
+    opts = job_opts(photometric, ncc_min_std, propagation)
     if int(geo_iterations) != geo_iterations or geo_iterations < 0:
         raise ValueError("geo_iterations must be an integer >= 0")
     imgs = np.ascontiguousarray(images, dtype=np.float32)
@@ -608,7 +643,7 @@ def geometric_pass(images, Ps, params, refs, geo_iterations: int = 2, weight: fl
     ref_views = (C.c_int * (k * int(max_views)))()
     jobs = _job_stats(k)                                   # owns the per-job arrays st.batch points into
     st = GpmGeoBatchStats(jobs, 0, p1_views, p1_ms, ref_views)
-    rc = lib.gpm_geo_batch_run_photo(C.byref(g), kind, float(ncc_min_std) if photometric == "ncc" else 0.0, C.byref(st))
+    rc = lib.gpm_geo_batch_run_opts(C.byref(g), C.byref(opts), C.byref(st))
     if rc != 0:
         raise GipumaError("gpm_geo_batch_run failed (%d): %s" % (rc, lib.gpm_batch_last_error().decode()))
     m = st.n_pass1

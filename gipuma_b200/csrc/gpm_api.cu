@@ -112,6 +112,8 @@ struct gpm_ctx {
     // photometric cost (DESIGN.md §15): GPM_PHOTO_PM, the reference's, or GPM_PHOTO_NCC (gpm_set_photometric)
     int photo = GPM_PHOTO_PM;
     float ncc_min_std = 0.f;
+    // propagation (DESIGN.md §16): GPM_PROP_FIXED, the reference's neighbours, or GPM_PROP_ADAPTIVE (gpm_set_propagation)
+    int propagation = GPM_PROP_FIXED;
 };
 
 namespace {
@@ -339,8 +341,13 @@ GeoParams geo_params(const gpm_ctx* c)
 int launch_colour(gpm_ctx* c, const KParams& P, int colour, int mask)
 {
     const bool ncc = ncc_on(c);          // grey images, 8 neighbours (gpm_set_photometric)
-    auto kern = ncc ? (c->geo_weight > 0.f ? k_sweep<false, false, true, true> : k_sweep<false, false, false, true>)
-              : c->geo_weight > 0.f ? (P.color ? k_sweep<true, false, true> : k_sweep<false, false, true>)    // 8 neighbours (check_geometric)
+    const bool geo = c->geo_weight > 0.f;
+    auto kern = c->propagation == GPM_PROP_ADAPTIVE                                                  // 8 neighbours (gpm_set_propagation)
+              ? (ncc ? (geo ? k_sweep<false, false, true, true, true> : k_sweep<false, false, false, true, true>)
+                 : geo ? (P.color ? k_sweep<true, false, true, false, true> : k_sweep<false, false, true, false, true>)
+                       : (P.color ? k_sweep<true, false, false, false, true> : k_sweep<false, false, false, false, true>))
+              : ncc ? (geo ? k_sweep<false, false, true, true> : k_sweep<false, false, false, true>)
+              : geo ? (P.color ? k_sweep<true, false, true> : k_sweep<false, false, true>)    // 8 neighbours (check_geometric)
               : P.ncand == 20 ? (P.color ? k_sweep<true, true> : k_sweep<false, true>)
                               : (P.color ? k_sweep<true, false> : k_sweep<false, false>);
     kern<<<tile_grid(c), P.nwarps * 32, block_smem_bytes(P, ncc), c->stream>>>(P, c->tmap, c->d_cams, c->srcTex, c->planes, c->cost, c->rng,
@@ -519,6 +526,14 @@ extern "C" int gpm_create(gpm_ctx** out, int device, int width, int height, int 
         ok(cudaFuncSetAttribute(k_cost_eval<false, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, c->smem_optin));
         ok(cudaFuncSetAttribute(k_shard_stage<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, c->smem_optin));
         ok(cudaFuncSetAttribute(k_shard_stage<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, c->smem_optin));
+        ok(cudaFuncSetAttribute(k_sweep<false, false, false, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, c->smem_optin));
+        ok(cudaFuncSetAttribute(k_sweep<true, false, false, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, c->smem_optin));
+        ok(cudaFuncSetAttribute(k_sweep<false, false, true, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, c->smem_optin));
+        ok(cudaFuncSetAttribute(k_sweep<true, false, true, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, c->smem_optin));
+        ok(cudaFuncSetAttribute(k_sweep<false, false, false, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, c->smem_optin));
+        ok(cudaFuncSetAttribute(k_sweep<false, false, true, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, c->smem_optin));
+        ok(cudaFuncSetAttribute(k_shard_stage<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, c->smem_optin));
+        ok(cudaFuncSetAttribute(k_shard_stage<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, c->smem_optin));
     }
     if (err != cudaSuccess) {
         std::string m = std::string("gpm_create: ") + cudaGetErrorString(err);
@@ -725,6 +740,18 @@ extern "C" int gpm_set_photometric(gpm_ctx* c, int kind, float min_std)
     if (kind != c->photo || min_std != c->ncc_min_std) c->inputs_dirty = true;
     c->photo = kind;
     c->ncc_min_std = min_std;
+    return GPM_OK;
+}
+
+// Only which plane is offered from each direction changes; the accept rule and cost(p, plane) do not, so stored costs, their
+// provenance and the memo stay valid across a switch.
+extern "C" int gpm_set_propagation(gpm_ctx* c, int kind)
+{
+    if (!c) return fail(GPM_E_ARG, "gpm_set_propagation: null context");
+    if (kind != GPM_PROP_FIXED && kind != GPM_PROP_ADAPTIVE) return fail(GPM_E_ARG, "gpm_set_propagation: kind must be GPM_PROP_FIXED or GPM_PROP_ADAPTIVE");
+    if (kind == GPM_PROP_ADAPTIVE && c->opt_neighbours == 20)
+        return fail(GPM_E_ARG, "gpm_set_propagation: adaptive sampling supports the 8-neighbour sweep only (option neighbours = 8)");
+    c->propagation = kind;
     return GPM_OK;
 }
 
@@ -957,7 +984,9 @@ static int shard_launch_stage(gpm_ctx* c, const KParams& P, int colour, int stag
 {
     const int last = 1 + shard_refine_steps(c->prm);
     ShardState S{c->dispbuf, c->candbuf, c->canddepth, c->sflags};
-    (P.color ? k_shard_stage<true> : k_shard_stage<false>)<<<tile_grid(c), P.nwarps * 32, block_smem_bytes(P), c->stream>>>(P, c->tmap, c->d_cams,
+    auto kern = c->propagation == GPM_PROP_ADAPTIVE ? (P.color ? k_shard_stage<true, true> : k_shard_stage<false, true>)
+                                                    : (P.color ? k_shard_stage<true> : k_shard_stage<false>);
+    kern<<<tile_grid(c), P.nwarps * 32, block_smem_bytes(P), c->stream>>>(P, c->tmap, c->d_cams,
         c->srcTex, c->planes, c->cost, c->prov, S, Memo{c->pid, c->seen, c->refseen, c->memo_mask, c->next_id}, colour, stage, last,
         gathered_prev, world, xchg, c->d_stats);
     c->launches++;
@@ -1250,6 +1279,7 @@ extern "C" int gpm_set_option(gpm_ctx* c, const char* name, int value)
         if (value != 8 && value != 20) return fail(GPM_E_ARG, "neighbours must be 8 (close + far kernels) or 20 (fused kernel)");
         if (value == 20 && c->geo_weight > 0.f) return fail(GPM_E_ARG, "the geometric-consistency mode supports the 8-neighbour sweep only");
         if (value == 20 && ncc_on(c)) return fail(GPM_E_ARG, "the NCC photometric cost supports the 8-neighbour sweep only");
+        if (value == 20 && c->propagation == GPM_PROP_ADAPTIVE) return fail(GPM_E_ARG, "adaptive checkerboard sampling supports the 8-neighbour sweep only");
         DeviceGuard g(c->device);
         const int slots = value == 20 ? 20 : 8;
         if (slots != c->seen_slots) {

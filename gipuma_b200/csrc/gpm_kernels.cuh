@@ -221,9 +221,44 @@ __device__ __forceinline__ bool close_far_neighbour(int k, const int& px, const 
     return ok;
 }
 
+// Candidate k of the adaptive checkerboard sampling (ACMH, Xu & Tao 2019; DESIGN.md §16): the pixel with the lowest stored
+// cost of region k, NaN counting as +inf and a tie going to the earliest offset of the region's scan order.  Regions 0..3
+// (near up, down, left, right) are V shapes of 7 offsets: the 1 px neighbour, then (a, ±(a - 1)) for a = 2, 3, 4 along the
+// direction; regions 4..7 (far) are the 11 axial offsets 3, 5, ..., 23 px.  Every offset has odd |dy| + |dx|, so region
+// pixels are of the other checkerboard colour, whose planes and costs a launch never writes.  false: no offset lies in the
+// image (the candidate is not offered); (qx, qy) is then (px, py).
+__device__ __forceinline__ bool acs_neighbour(int k, int px, int py, int W, int H, const float* cost, int& qx, int& qy)
+{
+    const int dir = k & 3, n = k < 4 ? 7 : 11, sgn = (dir == 0 || dir == 2) ? -1 : 1;
+    qx = px;  qy = py;
+    float best = 0.0f;
+    bool found = false;
+    for (int j = 0; j < n; j++) {
+        const int i = (j + 1) >> 1;
+        const int a = k < 4 ? 1 + i : 3 + 2 * j;                   // distance along the direction
+        const int b = k < 4 ? ((j & 1) ? -i : i) : 0;              // offset across it
+        const int x = px + (dir < 2 ? b : sgn * a), y = py + (dir < 2 ? sgn * a : b);
+        if (x < 0 || x >= W || y < 0 || y >= H) continue;
+        float c = cost[(size_t)y * W + x];
+        if (c != c) c = __int_as_float(0x7f800000);
+        if (!found || c < best) { best = c;  qx = x;  qy = y;  found = true; }
+    }
+    return found;
+}
+
+// The sweep's and the shard's neighbour choice: the fixed neighbour of direction k (with the reference's border guard) or,
+// ADAPTIVE, the cheapest pixel of region k by the costs the launch started from.
+template <bool ADAPTIVE>
+__device__ __forceinline__ bool sweep_neighbour(int k, const int& px, const int& py, int W, int H, const float* cost, int& qx, int& qy)
+{
+    if constexpr (ADAPTIVE) return acs_neighbour(k, px, py, W, H, cost, qx, qy);
+    else return close_far_neighbour(k, px, py, W, H, qx, qy);
+}
+
 // GEO: the cost with the geometric-consistency term (DESIGN.md §14; 8-neighbour sweep only); NCC: the NCC photometric cost
-// (§15; 8-neighbour sweep, grey images only).  G is only read in those variants.
-template <bool COLOR, bool FUSED, bool GEO = false, bool NCC = false>
+// (§15; 8-neighbour sweep, grey images only).  G is only read in those variants.  ADAPTIVE: adaptive checkerboard sampling
+// (§16; 8-neighbour sweep), candidate k is acs_neighbour's choice instead of the fixed neighbour.
+template <bool COLOR, bool FUSED, bool GEO = false, bool NCC = false, bool ADAPTIVE = false>
 __global__ void __launch_bounds__(GPM_LB_THREADS, GPM_LB_BLOCKS)
 k_sweep(const __grid_constant__ KParams P, const __grid_constant__ CUtensorMap tmap, const ViewCam* __restrict__ cams,
         cudaTextureObject_t src, float4* __restrict__ planes, float* __restrict__ cost,
@@ -232,6 +267,7 @@ k_sweep(const __grid_constant__ KParams P, const __grid_constant__ CUtensorMap t
 {
     static_assert(!(FUSED && GEO), "the geometric term is built for the 8-neighbour sweep only");
     static_assert(!(NCC && (FUSED || COLOR)), "the NCC cost is built for the 8-neighbour sweep on grey images only");
+    static_assert(!(FUSED && ADAPTIVE), "adaptive checkerboard sampling is built for the 8-neighbour sweep only");
     const GeoParams* g = (GEO || NCC) ? &G : nullptr;
     extern __shared__ __align__(128) float smem[];
     float* tile = smem;
@@ -283,7 +319,7 @@ k_sweep(const __grid_constant__ KParams P, const __grid_constant__ CUtensorMap t
             } else if (lane < 8) {
                 const bool phase_on = (phase_mask >> (lane >> 2)) & 1;
                 int qx, qy;
-                const bool ok = close_far_neighbour((int)lane, px, py, W, H, qx, qy);
+                const bool ok = sweep_neighbour<ADAPTIVE>((int)lane, px, py, W, H, cost, qx, qy);
                 mine_ok = ok && phase_on;
                 mine_at = (size_t)qy * W + qx;
             }
@@ -521,8 +557,11 @@ __device__ __forceinline__ float4 shard_refine_candidate(const KParams& P, const
 
 // Accept of stage `stage` at pixel (px, py) from the exchanged lists (one warp; every lane returns the same state).
 // stage 1: the 8 propagation slots in the reference's order (gipuma.cu:1571-1582, 1450-1462; accept rule :867-871);
-// stage >= 2: one refinement step (:986-990).
-__device__ __forceinline__ void shard_accept_pixel(const KParams& P, const float4* __restrict__ planes, const ShardState& S, const Memo& M,
+// stage >= 2: one refinement step (:986-990).  ADAPTIVE: slot k is acs_neighbour's choice, re-derived from the costs of the
+// other colour, which no stage of this colour writes, so it is the pixel stage 1 evaluated.
+template <bool ADAPTIVE>
+__device__ __forceinline__ void shard_accept_pixel(const KParams& P, const float4* __restrict__ planes, const float* __restrict__ cost,
+                                                   const ShardState& S, const Memo& M,
                                                    int px, int py, int stage, const float* __restrict__ gathered, int world,
                                                    float4& norm_now, float& cost_now, float& disp_now, int& prov_now, unsigned& sf,
                                                    unsigned& own_id, unsigned lane)
@@ -540,7 +579,7 @@ __device__ __forceinline__ void shard_accept_pixel(const KParams& P, const float
             const float c = __shfl_sync(GPM_FULL, mine, k);
             if (c < cost_now) {
                 int qx, qy;
-                close_far_neighbour(k, px, py, W, H, qx, qy);       // offered, so inside the border guard
+                sweep_neighbour<ADAPTIVE>(k, px, py, W, H, cost, qx, qy);   // offered, so inside the border guard / region
                 norm_now = planes[(size_t)qy * W + qx];                 // other colour: not written during this colour's stages
                 own_id = M.pid[(size_t)qy * W + qx];                    // a copy keeps its identity
                 disp_now = plane_depth(P.ref, norm_now.x, norm_now.y, norm_now.z, norm_now.w, fpx, fpy);
@@ -558,7 +597,7 @@ __device__ __forceinline__ void shard_accept_pixel(const KParams& P, const float
 }
 
 // One stage of one pixel: [accept of stage-1's exchange] + evaluation of `stage` on this rank's views -> local top-n lists.
-template <bool COLOR>
+template <bool COLOR, bool ADAPTIVE>
 __device__ __forceinline__ void shard_stage_pixel(const KParams& P, const float* __restrict__ sCam, const float* __restrict__ tile,
                                                   const WarpScratch& ws, cudaTextureObject_t src, float4* __restrict__ planes, float* __restrict__ cost, unsigned char* __restrict__ prov,
                                                   const ShardState& S, const Memo& M, int px, int py, int tile_x0, int tile_y0,
@@ -587,7 +626,7 @@ __device__ __forceinline__ void shard_stage_pixel(const KParams& P, const float*
     unsigned new_mask = mmask;
     unsigned own_id = M.pid[center];
     if (stage >= 2) {
-        shard_accept_pixel(P, planes, S, M, px, py, stage - 1, gathered_prev, world, norm_now, cost_now, disp_now, prov_now, sf, own_id, lane);
+        shard_accept_pixel<ADAPTIVE>(P, planes, cost, S, M, px, py, stage - 1, gathered_prev, world, norm_now, cost_now, disp_now, prov_now, sf, own_id, lane);
         if (stage == 2) {
             // refinement memo (see k_sweep): the S candidates are a pure function of (pixel, plane at refinement start)
             sf = 0u;
@@ -611,7 +650,7 @@ __device__ __forceinline__ void shard_stage_pixel(const KParams& P, const float*
         size_t mine_at = center;
         if (lane < 8) {
             int qx, qy;
-            mine_ok = close_far_neighbour((int)lane, px, py, W, H, qx, qy);
+            mine_ok = sweep_neighbour<ADAPTIVE>((int)lane, px, py, W, H, cost, qx, qy);
             mine_at = (size_t)qy * W + qx;
         }
         const unsigned mine_id = mine_ok ? M.pid[mine_at] : 0u;
@@ -667,7 +706,8 @@ __device__ __forceinline__ void shard_stage_pixel(const KParams& P, const float*
 
 // One exchange stage over the whole image (the all-gather runs between two launches of this kernel).
 // stage 0: both colours; 1 .. last_stage: one colour; last_stage + 1: closing accept of the colour.
-template <bool COLOR>
+// ADAPTIVE: adaptive checkerboard sampling (DESIGN.md §16); the exchange format is the same.
+template <bool COLOR, bool ADAPTIVE = false>
 __global__ void __launch_bounds__(GPM_LB_THREADS, GPM_LB_BLOCKS)
 k_shard_stage(const __grid_constant__ KParams P, const __grid_constant__ CUtensorMap tmap, const ViewCam* __restrict__ cams,
               cudaTextureObject_t src, float4* __restrict__ planes, float* __restrict__ cost,
@@ -693,7 +733,7 @@ k_shard_stage(const __grid_constant__ KParams P, const __grid_constant__ CUtenso
         if (stage == 0) { px = blockIdx.x * GPM_TILE + (idx & 31);  py = blockIdx.y * GPM_TILE + (idx >> 5); }
         else colour_pixel(idx, colour, px, py);
         if (px >= P.W || py >= P.H) continue;
-        shard_stage_pixel<COLOR>(P, sCam, tile, ws, src, planes, cost, prov, S, M, px, py,
+        shard_stage_pixel<COLOR, ADAPTIVE>(P, sCam, tile, ws, src, planes, cost, prov, S, M, px, py,
                                  tile_x0, tile_y0, stage, last_stage, gathered_prev, world, xchg, lane, st);
     }
     flush_stats(stats, st, lane);

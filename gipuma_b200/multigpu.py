@@ -105,21 +105,25 @@ def hybrid_layout(world: int, shard: int):
 
 
 def run_hybrid(make_scene: Callable[[int], object], n_reference_views: int, rank: int, world: int, shard: int,
-               device: int = 0, on_result: Optional[Callable] = None, exchange: str = "nccl") -> List[float]:
+               device: int = 0, on_result: Optional[Callable] = None, exchange: str = "nccl",
+               propagation: str = "fixed") -> List[float]:
     """Reference views are dealt round-robin to world/shard groups; inside a group the source views are sharded and
-    combined with one all-gather per stage over the group's own communicator (`exchange` must be "nccl").  Returns wall
-    seconds per reference view."""
+    combined with one all-gather per stage over the group's own communicator (`exchange` must be "nccl").  `propagation`
+    as ViewShardRunner.  Returns wall seconds per reference view."""
     import time
     import torch
     import torch.distributed as dist
+    from . import api
     _check_exchange(exchange)
+    api.check_propagation(propagation)
     group_of, rank_in, members = hybrid_layout(world, shard)
     groups = [dist.new_group(ranks=m) if world > 1 else None for m in members]     # every rank creates every group
     my_group = group_of[rank]
     times = []
     for ref in assign_reference_views(n_reference_views, my_group, len(members)):
         sc = make_scene(ref)
-        runner = ViewShardRunner(sc, rank_in[rank], shard, device=device, group=groups[my_group], exchange=exchange)
+        runner = ViewShardRunner(sc, rank_in[rank], shard, device=device, group=groups[my_group], exchange=exchange,
+                                  propagation=propagation)
         torch.cuda.synchronize(device)
         t0 = time.perf_counter()
         n4, c = runner.run()
@@ -146,12 +150,14 @@ class ViewShardRunner:
     """One reference view, source views sharded over `world` ranks.  All device work runs behind the C-ABI
     (gpm_shard_run): one stage kernel + ncclAllGather per exchange stage.  `exchange` must be "nccl"; the attribute of
     the same name is "nccl", or "none" for a single rank.  torch.distributed is only used at set-up, to pass the NCCL
-    unique id around."""
+    unique id around.  `propagation` ("fixed" or "adaptive", api.Context.set_propagation) is set on every rank's context;
+    all ranks must pass the same."""
 
     def __init__(self, scene, rank: int, world: int, device: int = 0, seed: int = 0xC0FFEE, group=None, options=None,
-                 exchange: str = "nccl"):
+                 exchange: str = "nccl", propagation: str = "fixed"):
         from . import api
         _check_exchange(exchange)
+        api.check_propagation(propagation)
         self.scene, self.rank, self.world, self.group = scene, rank, world, group
         self.local = partition_views(scene.n_views, world)[rank]
         if not self.local:
@@ -160,6 +166,7 @@ class ViewShardRunner:
         ctx = self.ctx
         for k, v in (options or {}).items():
             ctx.set_option(k, v)
+        ctx.set_propagation(propagation)
         ctx.set_params(scene.params)
         self.upload(scene)
         ctx.set_rng(seed)

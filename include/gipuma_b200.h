@@ -117,6 +117,19 @@ int gpm_set_geometric(gpm_ctx* ctx, float weight, float max_err);
 enum { GPM_PHOTO_PM = 0, GPM_PHOTO_NCC = 1 };
 int gpm_set_photometric(gpm_ctx* ctx, int kind, float min_std);
 
+/* ---- propagation (DESIGN.md §16) ----------------------------------------------------------------------------------------
+ * GPM_PROP_FIXED (the default) offers each pixel the reference's 8 neighbours: the other-colour pixels at 1 px (close) and
+ * 5 px (far) up, down, left and right.  GPM_PROP_ADAPTIVE is the adaptive checkerboard sampling of ACMH (Xu & Tao, CVPR
+ * 2019): candidate k is instead the pixel with the lowest stored cost, at the start of the launch, in region k: four
+ * V-shaped regions of 7 pixels reaching 4 px (close) and four axial strips of 11 pixels at 3, 5, .., 23 px (far).  NaN
+ * costs count as +inf and a tie goes to the earliest pixel of the region's scan order.  The accept rule, the refinement and
+ * every cost are unchanged, so the mode may be switched at any point of a run and works with every cost mode, grey or
+ * colour, and with the source-view shard (gpm_shard_*).
+ * Refused with GPM_E_ARG: an unknown kind; ADAPTIVE with option neighbours = 20 (and neighbours = 20 while ADAPTIVE is
+ * on).  A refused call changes nothing. */
+enum { GPM_PROP_FIXED = 0, GPM_PROP_ADAPTIVE = 1 };
+int gpm_set_propagation(gpm_ctx* ctx, int kind);
+
 /* Seed of the per-pixel curand_init(seed, y, x) at initialisation (gipuma.cu:1019; the reference uses
  * clock64()) and the refinement RNG mode. */
 int gpm_set_rng(gpm_ctx* ctx, unsigned long long seed, int mode);
@@ -293,6 +306,18 @@ int gpm_geo_batch_run(const gpm_geo_batch_desc* desc, gpm_geo_batch_stats* stats
  * arguments, and channels = 4 with GPM_PHOTO_NCC. */
 int gpm_batch_run_photo(const gpm_batch_desc* desc, int kind, float min_std, gpm_batch_stats* stats);
 int gpm_geo_batch_run_photo(const gpm_geo_batch_desc* desc, int kind, float min_std, gpm_geo_batch_stats* stats);
+
+/* The batch drivers with per-job options: every job's context gets gpm_set_photometric(photometric, ncc_min_std) and
+ * gpm_set_propagation(propagation) in the per-view setup (both passes of the geometric driver).  The _photo twins are these
+ * with GPM_PROP_FIXED.  Refused with GPM_E_ARG before any CUDA call, besides what those refuse: what the two setters refuse
+ * for their arguments, channels = 4 with GPM_PHOTO_NCC, and a NULL `opts`. */
+typedef struct gpm_job_opts {
+    int photometric;                   /* GPM_PHOTO_PM or GPM_PHOTO_NCC */
+    float ncc_min_std;                 /* as gpm_set_photometric (ignored for PM) */
+    int propagation;                   /* GPM_PROP_FIXED or GPM_PROP_ADAPTIVE */
+} gpm_job_opts;
+int gpm_batch_run_opts(const gpm_batch_desc* desc, const gpm_job_opts* opts, gpm_batch_stats* stats);
+int gpm_geo_batch_run_opts(const gpm_geo_batch_desc* desc, const gpm_job_opts* opts, gpm_geo_batch_stats* stats);
 
 /* ---- depth-map fusion: the per-view world-frame outputs (norm4 of gpm_batch_run, or its .dmb files) -> one point cloud;
  * what the reference's scripts hand to the external `fusibile` (scripts/dtu_fast.sh:56-57).  Deterministic: the same inputs

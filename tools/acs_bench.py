@@ -1,0 +1,170 @@
+"""Fused-cloud quality, convergence and sweep speed of adaptive checkerboard sampling (DESIGN.md §16) against the reference's
+fixed neighbours; prints one JSON line.
+
+    python tools/acs_bench.py [--rows 600] [--cols 800] [--cams 16] [--iterations 6] [--geo-iterations 2]
+                              [--converge 2,3,4,6] [--scenes smooth,hard,lit] [--costs pm,ncc] [--speed-iterations 4]
+                              [--dtu-preset]
+
+Quality: tools/ncc_bench.py's workload (the first `--cams` DTU cameras at `--cols` x `--rows`, every second camera a reference
+view, box 11, n_best 3, depth 300..800, views at 5..45 degrees, at most 6 per reference; the same fusion and evaluate_cloud
+set-up; scenes smooth, hard and lit).  Per scene, cost (PM, NCC at api.NCC_MIN_STD) and propagation (fixed, adaptive):
+photometric only (batch_run, `--iterations`), with the geometric pass (geometric_pass, `--iterations` - `--geo-iterations`
+photometric then `--geo-iterations` geometric iterations), and the photometric F-scores after each of `--converge`
+iterations.  Each run reports F-score at 0.25, 0.5 and 1 unit, mean accuracy and completeness (units), vertices and the batch
+driver's summed sweep ms per iteration (CUDA events on gpm_stream).
+Speed: sweep ms per iteration from CUDA events on gpm_stream around gpm_sweep(`--speed-iterations`) after gpm_init and a
+one-iteration warm-up, fixed against adaptive, PM and NCC, at 1600 x 1200 and 800 x 600 (10 views, box 15), with
+gpm_get_stats' hypotheses offered, skipped and (view, sample) pairs evaluated of the timed sweep.
+--dtu-preset adds a DTU-size batch: 49 cameras at 1600 x 1200, every camera a reference view, PM, one worker, fixed against
+adaptive, total sweep seconds.  Needs a CUDA device; there is no CPU path.
+"""
+import argparse
+import json
+import os
+import subprocess
+import sys
+import time
+
+import numpy as np
+
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+
+MODES = ("fixed", "adaptive")
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--rows", type=int, default=600)
+    ap.add_argument("--cols", type=int, default=800)
+    ap.add_argument("--cams", type=int, default=16)
+    ap.add_argument("--iterations", type=int, default=6)
+    ap.add_argument("--geo-iterations", type=int, default=2)
+    ap.add_argument("--converge", default="2,3,4,6")
+    ap.add_argument("--scenes", default="smooth,hard,lit")
+    ap.add_argument("--costs", default="pm,ncc")
+    ap.add_argument("--speed-iterations", type=int, default=4)
+    ap.add_argument("--dtu-preset", action="store_true")
+    a = ap.parse_args()
+    import torch
+    if not torch.cuda.is_available():
+        sys.exit("acs_bench: needs a CUDA device")
+    from gipuma_b200 import api, scene as S
+    gpu = {"name": torch.cuda.get_device_name(0)}
+    try:
+        gpu["power_limit_w"] = subprocess.run(["nvidia-smi", "--query-gpu=power.limit", "--format=csv,noheader,nounits"],
+                                              capture_output=True, text=True, timeout=30).stdout.split()
+    except Exception as e:      # noqa: BLE001
+        gpu["power_limit_w"] = "unknown (%s)" % e
+
+    def log(msg):
+        print("acs_bench: %s" % msg, file=sys.stderr, flush=True)
+
+    out = {"gpu": gpu, "workload": "%d DTU cameras at %dx%d, %d iterations (geometric: last %d)" %
+           (a.cams, a.cols, a.rows, a.iterations, a.geo_iterations)}
+    converge = [int(x) for x in a.converge.split(",") if x]
+    costs = {"pm": {}, "ncc": dict(photometric="ncc", ncc_min_std=api.NCC_MIN_STD)}
+    costs = {k: costs[k] for k in a.costs.split(",") if k}
+
+    def params(iterations):
+        p = S.AlgorithmParameters(box_hsize=11, box_vsize=11, iterations=iterations, n_best=3, cost_comb=S.COMB_BEST_N, gamma=10.0)
+        p.depthMin, p.depthMax = 300.0, 800.0
+        return p
+
+    def render(Ps, scale, rows, cols, hard):
+        cams = S.prepare_cameras(Ps, scale)
+        hf = S.HeightField(z0=550.0, unit=550.0 / cams[0].fx, seed=77, hard=hard)
+        images = np.stack([S.render_view(c, rows, cols, hf, noise_seed=(1000 + i) if hf.hard else None)[0]
+                           for i, c in enumerate(cams)]).astype(np.float32)
+        return hf, images
+
+    Ps = [S.load_dtu_projections()[i] for i in range(a.cams)]
+    scale = 1600.0 / a.cols
+    refs = list(range(0, a.cams, 2))
+    fPs = [Ps[r] for r in refs]
+    kw = dict(cam_scale=scale, min_angle=5.0, max_angle=45.0, max_views=6, seed=4242)
+    fuse_kw = dict(depth_min=300.0, depth_max=800.0, disp_thresh=0.1, normal_thresh=30.0, num_consistent=2)
+    for scene in [x for x in a.scenes.split(",") if x]:                    # --scenes "": speed only
+        log("%s: rendering" % scene)
+        hf, images = render(Ps, scale, a.rows, a.cols, scene == "hard")
+        res = {}
+        if scene == "lit":
+            rng = np.random.default_rng(2024)
+            lit = np.stack([rng.uniform(0.6, 1.4) * im + rng.uniform(-40, 40) for im in images])
+            res["clipped_share"] = round(float(((lit < 0) | (lit > 255)).mean()), 4)
+            images = np.clip(lit, 0, 255).astype(np.float32)
+        gt = S.gt_points(fPs, scale, a.rows, a.cols, hf, stride=2)
+        unit = hf.unit
+
+        def score(n4):
+            v, _ = api.fuse(n4, fPs, cam_scale=scale, **fuse_kw)
+            s = api.evaluate_cloud(v, gt, max_dist=10 * unit, taus=(0.25 * unit, 0.5 * unit, unit))
+            return {"vertices": len(v), "accuracy_mean_units": round(s["accuracy_mean"] / unit, 4),
+                    "completeness_mean_units": round(s["completeness_mean"] / unit, 4), "f_score": [round(f, 4) for f in s["f_score"]]}
+
+        for cost, photo in costs.items():
+            for mode in MODES:
+                r = {}
+                for it in sorted(set(converge + [a.iterations])):
+                    n4, _, st = api.batch_run(images, Ps, params(it), refs, propagation=mode, **kw, **photo)
+                    sc = score(n4)
+                    if it == a.iterations:
+                        r["photometric"] = dict(sc, sweep_ms_per_iteration=round(st["sweep_ms_total"] / it, 2))
+                    if it in converge:
+                        r.setdefault("f_score_1unit_after_iterations", {})[it] = sc["f_score"][2]
+                n4, _, info = api.geometric_pass(images, Ps, params(a.iterations - a.geo_iterations), refs,
+                                                 geo_iterations=a.geo_iterations, propagation=mode, **kw, **photo)
+                r["with_geometric"] = dict(score(n4), pass2_sweep_ms_per_iteration=round(
+                    1e3 * sum(info["pass2_sweep_s"]) / max(1, a.geo_iterations), 2))
+                res["%s %s" % (cost, mode)] = r
+                log("%s %s %s: %s" % (scene, cost, mode, r))
+        out[scene] = res
+
+    speed = {}
+    for rows, cols in ((1200, 1600), (600, 800)):
+        sc = S.make_config(2, rows=rows, cols=cols, n_views=10, iterations=1, seed=7)
+        sc.params.box_hsize = sc.params.box_vsize = 15
+        row = {}
+        for cost in costs:
+            for mode in MODES:
+                with api.Context(cols, rows, len(sc.subset)) as ctx:
+                    ctx.load_scene(sc)
+                    if cost == "ncc":
+                        ctx.set_photometric("ncc", api.NCC_MIN_STD)
+                    ctx.set_propagation(mode)
+                    ctx.init()
+                    ctx.sweep(1)
+                    stream = torch.cuda.ExternalStream(ctx.stream)
+                    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+                    ctx.reset_stats()
+                    e0.record(stream)
+                    ctx.sweep(a.speed_iterations)
+                    e1.record(stream)
+                    e1.synchronize()
+                    st = ctx.stats()
+                    row["%s %s" % (cost, mode)] = {"ms_per_iteration": round(e0.elapsed_time(e1) / a.speed_iterations, 3),
+                                                   "offered": st["hypotheses"], "skipped": st["skipped"], "pairs": st["pairs"]}
+            row["%s adaptive_over_fixed" % cost] = round(row["%s adaptive" % cost]["ms_per_iteration"] /
+                                                         row["%s fixed" % cost]["ms_per_iteration"], 3)
+        speed["%dx%d, 10 views, box 15" % (cols, rows)] = row
+        log("speed %dx%d: %s" % (cols, rows, row))
+    out["speed"] = speed
+
+    if a.dtu_preset:
+        n = 49
+        allP = S.load_dtu_projections()[:n]
+        log("DTU preset: rendering %d views at 1600x1200" % n)
+        hf, images = render(allP, 1.0, 1200, 1600, False)
+        dtu = {}
+        for mode in MODES:
+            t0 = time.perf_counter()
+            _, _, st = api.batch_run(images, allP, params(a.iterations), list(range(n)), cam_scale=1.0, min_angle=5.0,
+                                     max_angle=45.0, max_views=6, seed=4242, want_outputs=False, propagation=mode)
+            dtu[mode] = {"sweep_s_total": round(st["sweep_ms_total"] / 1e3, 3), "wall_s": round(time.perf_counter() - t0, 2)}
+        dtu["adaptive_over_fixed"] = round(dtu["adaptive"]["sweep_s_total"] / dtu["fixed"]["sweep_s_total"], 3)
+        out["dtu_preset"] = dict(dtu, workload="%d views at 1600x1200, PM, %d iterations, one worker" % (n, a.iterations))
+        log("DTU preset: %s" % dtu)
+    print(json.dumps(out))
+
+
+if __name__ == "__main__":
+    main()

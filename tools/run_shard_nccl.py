@@ -18,6 +18,7 @@ ap.add_argument("--hybrid", type=int, default=0, help="view-shard width; world/w
 ap.add_argument("--refs", type=int, default=2)
 ap.add_argument("--repeat", type=int, default=2)
 ap.add_argument("--opt", nargs="*", default=[], help="gpm_set_option name=value pairs for the sharded contexts")
+ap.add_argument("--propagation", default="fixed", choices=["fixed", "adaptive"], help="propagation mode of every context (view-shard mode)")
 args = ap.parse_args()
 rank, world, local = int(os.environ.get("RANK", 0)), int(os.environ.get("WORLD_SIZE", 1)), int(os.environ.get("LOCAL_RANK", 0))
 torch.cuda.set_device(local)
@@ -44,7 +45,7 @@ if args.hybrid:
 sc = S.make_config(args.config, rows=args.rows, cols=args.cols, n_views=args.views, iterations=args.iters,
                    workers=max(1, min(32, len(os.sched_getaffinity(0)) // max(1, world))))
 opts = {k: int(v) for k, v in (o.split("=") for o in args.opt)}
-run = M.ViewShardRunner(sc, rank, world, device=local, options=opts)
+run = M.ViewShardRunner(sc, rank, world, device=local, options=opts, propagation=args.propagation)
 run.run()                                              # warm-up (NCCL communicator, kernels)
 torch.cuda.synchronize()
 best, sweep = 1e30, 1e30
@@ -66,11 +67,12 @@ out = None
 if rank == 0:
     with api.Context(sc.cols, sc.rows, sc.n_views, device=local) as one:
         one.load_scene(sc)
+        one.set_propagation(args.propagation)
         one.run()
         ms = one.run()
         s4, s1 = one.get_state()
     same = np.array_equal(n4.view(np.uint32), s4.view(np.uint32)) and np.array_equal(c.view(np.uint32), s1.view(np.uint32))
-    out = {"mode": "view_shard", "exchange": run.exchange, "opts": opts, "config": sc.name, "rows": sc.rows, "cols": sc.cols, "views": sc.n_views, "world": world,
+    out = {"mode": "view_shard", "exchange": run.exchange, "opts": opts, "propagation": args.propagation, "config": sc.name, "rows": sc.rows, "cols": sc.cols, "views": sc.n_views, "world": world,
            "wall_s_incl_init": float(t), "sweep_ms_max_over_ranks": sweep, "single_over_sharded_sweep": ms / sweep, "mpixel_iters_per_s": sc.rows * sc.cols * sc.params.iterations / 1e6 / float(t),
            "single_gpu_sweep_ms": ms, "bit_identical_to_single_gpu": bool(same), "collectives": run.collectives}
 if world > 1:
