@@ -66,6 +66,11 @@ class GpmJobOpts(C.Structure):
     _fields_ = [("photometric", C.c_int), ("ncc_min_std", C.c_float), ("propagation", C.c_int)]
 
 
+class GpmViewSel(C.Structure):
+    _fields_ = [("kind", C.c_int), ("tau_init", C.c_float), ("alpha", C.c_float), ("tau_bad", C.c_float),
+                ("n_good", C.c_int), ("n_bad", C.c_int), ("beta", C.c_float), ("w_keep", C.c_float)]
+
+
 class GpmFuseCamera(C.Structure):
     _fields_ = [("M_inv", C.c_float * 9), ("P", C.c_float * 12), ("f", C.c_float)]
 
@@ -129,6 +134,8 @@ def load_library():
     L.gpm_set_geometric.argtypes = [vp, C.c_float, C.c_float]
     L.gpm_set_photometric.argtypes = [vp, C.c_int, C.c_float]
     L.gpm_set_propagation.argtypes = [vp, C.c_int]
+    L.gpm_set_view_selection.argtypes = [vp, C.POINTER(GpmViewSel)]
+    L.gpm_get_view_masks.argtypes = [vp, vp]
     L.gpm_set_rng.argtypes = [vp, C.c_ulonglong, C.c_int]
     L.gpm_set_state.argtypes = [vp, vp, vp, C.c_int]
     L.gpm_get_state.argtypes = [vp, vp, vp, C.c_int]
@@ -165,6 +172,9 @@ def load_library():
     L.gpm_geo_batch_run_photo.argtypes = [C.POINTER(GpmGeoBatchDesc), C.c_int, C.c_float, C.POINTER(GpmGeoBatchStats)]
     L.gpm_batch_run_opts.argtypes = [C.POINTER(GpmBatchDesc), C.POINTER(GpmJobOpts), C.POINTER(GpmBatchStats)]
     L.gpm_geo_batch_run_opts.argtypes = [C.POINTER(GpmGeoBatchDesc), C.POINTER(GpmJobOpts), C.POINTER(GpmGeoBatchStats)]
+    L.gpm_batch_run_vsel.argtypes = [C.POINTER(GpmBatchDesc), C.POINTER(GpmJobOpts), C.POINTER(GpmViewSel), C.POINTER(GpmBatchStats)]
+    L.gpm_geo_batch_run_vsel.argtypes = [C.POINTER(GpmGeoBatchDesc), C.POINTER(GpmJobOpts), C.POINTER(GpmViewSel),
+                                         C.POINTER(GpmGeoBatchStats)]
     L.gpm_batch_last_error.restype = C.c_char_p
     L.gpm_stream.restype = vp
     L.gpm_fuse_cameras.argtypes = [C.POINTER(C.c_double), C.c_int, C.c_double, C.POINTER(GpmFuseCamera)]
@@ -173,11 +183,12 @@ def load_library():
     L.gpm_nearest_dist.argtypes = [C.POINTER(GpmNnDesc), C.POINTER(GpmNnResult)]
     for name in ("gpm_create", "gpm_set_params", "gpm_set_reference", "gpm_set_view", "gpm_set_reference_color",
                  "gpm_set_view_color", "gpm_set_num_views", "gpm_set_view_depth", "gpm_set_geometric", "gpm_set_photometric",
-                 "gpm_set_propagation", "gpm_set_rng", "gpm_set_state", "gpm_get_state", "gpm_init", "gpm_sweep", "gpm_phase",
+                 "gpm_set_propagation", "gpm_set_view_selection", "gpm_get_view_masks", "gpm_set_rng", "gpm_set_state", "gpm_get_state", "gpm_init", "gpm_sweep", "gpm_phase",
                  "gpm_finalize", "gpm_cost_eval", "gpm_run", "gpm_get_stats", "gpm_reset_stats", "gpm_set_option",
                  "gpm_init_planes", "gpm_shard_num_stages", "gpm_shard_stage", "gpm_shard_finish_init", "gpm_shard_unique_id",
                  "gpm_shard_comm_init", "gpm_shard_comm_attach", "gpm_shard_run", "gpm_measure_fetch_peak", "gpm_batch_run",
                  "gpm_geo_batch_run", "gpm_batch_run_photo", "gpm_geo_batch_run_photo", "gpm_batch_run_opts", "gpm_geo_batch_run_opts",
+                 "gpm_batch_run_vsel", "gpm_geo_batch_run_vsel",
                  "gpm_prepare_cameras", "gpm_select_views", "gpm_write_dmb", "gpm_read_dmb", "gpm_write_result_dmb",
                  "gpm_fuse_cameras", "gpm_fuse", "gpm_write_ply", "gpm_nearest_dist"):
         getattr(L, name).restype = C.c_int
@@ -270,6 +281,44 @@ def check_propagation(kind: str) -> int:
     if kind not in PROPAGATION:
         raise ValueError("propagation must be one of %s (got %r)" % (sorted(PROPAGATION), kind))
     return PROPAGATION[kind]
+
+
+# View selection (DESIGN.md §17): "off", each hypothesis scored by the combination rule of the parameters (the default), and
+# "joint", ACMH's multi-hypothesis joint view selection, for the NCC cost on grey images.  JVS_DEFAULTS are ACMH's parameters.
+VIEW_SELECTION = {"off": 0, "joint": 1}
+JVS_DEFAULTS = {"tau_init": 0.8, "alpha": 90.0, "tau_bad": 1.2, "n_good": 3, "n_bad": 3, "beta": 0.3, "w_keep": 0.2}
+
+
+def view_sel(kind: str = "off", **params) -> GpmViewSel:
+    """gpm_view_sel of `kind` with JVS_DEFAULTS overridden by `params`, every argument checked before any call into the
+    library by the rules of gpm_set_view_selection."""
+    if kind not in VIEW_SELECTION:
+        raise ValueError("view selection must be one of %s (got %r)" % (sorted(VIEW_SELECTION), kind))
+    unknown = sorted(set(params) - set(JVS_DEFAULTS))
+    if unknown:
+        raise ValueError("unknown view-selection parameters %s (known: %s)" % (unknown, sorted(JVS_DEFAULTS)))
+    p = dict(JVS_DEFAULTS, **params)
+    if kind == "joint":
+        for k in ("tau_init", "alpha", "tau_bad", "beta"):
+            if not (isinstance(p[k], (int, float, np.floating, np.integer)) and np.isfinite(p[k]) and p[k] > 0):
+                raise ValueError("%s must be finite and > 0 (got %r)" % (k, p[k]))
+        if not (isinstance(p["w_keep"], (int, float, np.floating, np.integer)) and np.isfinite(p["w_keep"]) and p["w_keep"] >= 0):
+            raise ValueError("w_keep must be finite and >= 0 (got %r)" % (p["w_keep"],))
+        for k, hi in (("n_good", 8), ("n_bad", 9)):
+            if int(p[k]) != p[k] or not 1 <= p[k] <= hi:
+                raise ValueError("%s must be an integer in 1..%d (got %r)" % (k, hi, p[k]))
+    return GpmViewSel(VIEW_SELECTION[kind], float(p["tau_init"]), float(p["alpha"]), float(p["tau_bad"]), int(p["n_good"]),
+                      int(p["n_bad"]), float(p["beta"]), float(p["w_keep"]))
+
+
+def check_view_selection(kind: str, photometric: str, channels: int = 1, **params) -> GpmViewSel:
+    """view_sel plus what the batch drivers refuse for the combination: "joint" needs the NCC cost and grey images."""
+    v = view_sel(kind, **params)
+    if kind == "joint" and photometric != "ncc":
+        raise ValueError("view_selection='joint' is built for the NCC cost (photometric='ncc')")
+    if kind == "joint" and channels == 4:
+        raise ValueError("view_selection='joint' supports grey images only")
+    return v
 
 
 def job_opts(photometric: str = "pm", ncc_min_std: float = NCC_MIN_STD, propagation: str = "fixed") -> GpmJobOpts:
@@ -367,6 +416,20 @@ class Context:
         neighbours at 1 and 5 px (the default), or "adaptive", the cheapest pixel of a larger region per direction (ACMH's
         adaptive checkerboard sampling).  8-neighbour sweep only; may be switched at any point of a run."""
         self._check(self.lib.gpm_set_propagation(self.h, check_propagation(kind)))
+
+    def set_view_selection(self, kind: str = "off", **params):
+        """Which source views score a pixel's hypotheses (DESIGN.md §17): "off", each hypothesis its own by the parameters'
+        combination rule (the default), or "joint", ACMH's multi-hypothesis joint view selection, whose parameters
+        (JVS_DEFAULTS) may be overridden by keyword.  "joint" needs the NCC cost (set_photometric("ncc")), grey images and
+        the 8-neighbour sweep."""
+        v = view_sel(kind, **params)
+        self._check(self.lib.gpm_set_view_selection(self.h, C.byref(v)))
+
+    def view_masks(self) -> np.ndarray:
+        """[H, W] uint64: bit j set where the last joint-view-selection launch selected view j."""
+        m = np.empty((self.H, self.W), dtype=np.uint64)
+        self._check(self.lib.gpm_get_view_masks(self.h, C.c_void_p(m.ctypes.data)))
+        return m
 
     def set_rng(self, seed: int, mode: int = GPM_RNG_REFERENCE):
         self._check(self.lib.gpm_set_rng(self.h, seed, mode))
@@ -574,13 +637,16 @@ def _job_stats(n_refs):
 
 def batch_run(images, Ps, params, refs, devices=(0,), cam_scale: float = 1.0, min_angle: float = 10.0, max_angle: float = 30.0,
               max_views: int = 9, seed: int = 0xC0FFEE, out_dir: Optional[str] = None, want_outputs: bool = True,
-              photometric: str = "pm", ncc_min_std: float = NCC_MIN_STD, propagation: str = "fixed"):
-    """Reference-view batch in ONE process (gpm_batch_run_opts): `images` [n, H, W] float32 (shared, page-locked once), `Ps`
+              photometric: str = "pm", ncc_min_std: float = NCC_MIN_STD, propagation: str = "fixed",
+              view_selection: str = "off", jvs_params: Optional[dict] = None):
+    """Reference-view batch in ONE process (gpm_batch_run_vsel): `images` [n, H, W] float32 (shared, page-locked once), `Ps`
     n 3x4 projections, `refs` the reference views to process, `devices` the CUDA ordinals to use (one worker thread each),
     `photometric` the cost, "pm" or "ncc" with min_std `ncc_min_std` (Context.set_photometric), `propagation` "fixed" or
-    "adaptive" (Context.set_propagation).
+    "adaptive" (Context.set_propagation), `view_selection` "off" or "joint" with `jvs_params` overriding JVS_DEFAULTS
+    (Context.set_view_selection; "joint" needs photometric="ncc").
     Returns (norm4 [len(refs), H, W, 4] or None, cost or None, stats dict)."""
     opts = job_opts(photometric, ncc_min_std, propagation)
+    vsel = check_view_selection(view_selection, photometric, 1, **(jvs_params or {}))
     lib = load_library()
     imgs = np.ascontiguousarray(images, dtype=np.float32)
     n, H, W = imgs.shape
@@ -588,7 +654,7 @@ def batch_run(images, Ps, params, refs, devices=(0,), cam_scale: float = 1.0, mi
     cc = np.empty((len(refs), H, W), np.float32) if want_outputs else None
     d, _keep = _batch_desc(imgs, Ps, params, refs, devices, cam_scale, min_angle, max_angle, max_views, seed, out_dir, n4, cc)
     st = _job_stats(len(refs))
-    rc = lib.gpm_batch_run_opts(C.byref(d), C.byref(opts), C.byref(st))
+    rc = lib.gpm_batch_run_vsel(C.byref(d), C.byref(opts), C.byref(vsel), C.byref(st))
     if rc != 0:
         raise GipumaError("gpm_batch_run failed (%d): %s" % (rc, lib.gpm_batch_last_error().decode()))
     k = len(refs)
@@ -599,7 +665,8 @@ def batch_run(images, Ps, params, refs, devices=(0,), cam_scale: float = 1.0, mi
 def geometric_pass(images, Ps, params, refs, geo_iterations: int = 2, weight: float = GEO_WEIGHT, max_err: float = GEO_MAX_ERR,
                    cam_scale: float = 1.0, min_angle: float = 10.0, max_angle: float = 30.0, max_views: int = 9,
                    seed: int = 0xC0FFEE, devices=(0,), out_dir: Optional[str] = None, photometric: str = "pm",
-                   ncc_min_std: float = NCC_MIN_STD, propagation: str = "fixed"):
+                   ncc_min_std: float = NCC_MIN_STD, propagation: str = "fixed", view_selection: str = "off",
+                   jvs_params: Optional[dict] = None):
     """PatchMatch with a geometric-consistency second pass (DESIGN.md §14) for the reference views `refs`, run by the
     native two-pass batch driver (gpm_geo_batch_run) over the worker pool of `devices` (one worker thread and context each;
     a device may be listed more than once).
@@ -611,7 +678,8 @@ def geometric_pass(images, Ps, params, refs, geo_iterations: int = 2, weight: fl
     run has params.iterations + geo_iterations iterations in all.  images: [n, H, W] grey or [n, H, W, 4] colour; the other
     arguments as batch_run; out_dir: None, or where <ref, 8 digits>/{disp,normals}.dmb of the pass-2 results are written;
     photometric / ncc_min_std: the photometric cost of both passes, as batch_run ("ncc": grey images only); propagation:
-    the propagation mode of both passes, as batch_run.
+    the propagation mode of both passes, as batch_run; view_selection / jvs_params: the view selection of both passes, as
+    batch_run (pass 2 starts over at t = 0).
     Returns (norm4 [len(refs), H, W, 4], cost [len(refs), H, W], info) with norm4 as batch_run returns it, so fuse and
     evaluate_cloud take it unchanged; info: "pass1_views" (the views pass 1 ran, ascending), "pass1_sweep_s" (in that order)
     and "pass2_sweep_s" (per reference view): CUDA-event seconds of each view's sweep call on its context's stream;
@@ -623,6 +691,7 @@ def geometric_pass(images, Ps, params, refs, geo_iterations: int = 2, weight: fl
     imgs = np.ascontiguousarray(images, dtype=np.float32)
     if imgs.ndim not in (3, 4) or (imgs.ndim == 4 and imgs.shape[3] != 4):
         raise ValueError("images must be [n, H, W] or [n, H, W, 4]")
+    vsel = check_view_selection(view_selection, photometric, 4 if imgs.ndim == 4 else 1, **(jvs_params or {}))
     if photometric == "ncc" and imgs.ndim == 4:
         raise ValueError("the NCC photometric cost supports grey images only")
     n, H, W = imgs.shape[:3]
@@ -643,7 +712,7 @@ def geometric_pass(images, Ps, params, refs, geo_iterations: int = 2, weight: fl
     ref_views = (C.c_int * (k * int(max_views)))()
     jobs = _job_stats(k)                                   # owns the per-job arrays st.batch points into
     st = GpmGeoBatchStats(jobs, 0, p1_views, p1_ms, ref_views)
-    rc = lib.gpm_geo_batch_run_opts(C.byref(g), C.byref(opts), C.byref(st))
+    rc = lib.gpm_geo_batch_run_vsel(C.byref(g), C.byref(opts), C.byref(vsel), C.byref(st))
     if rc != 0:
         raise GipumaError("gpm_geo_batch_run failed (%d): %s" % (rc, lib.gpm_batch_last_error().decode()))
     m = st.n_pass1

@@ -114,6 +114,10 @@ struct gpm_ctx {
     float ncc_min_std = 0.f;
     // propagation (DESIGN.md §16): GPM_PROP_FIXED, the reference's neighbours, or GPM_PROP_ADAPTIVE (gpm_set_propagation)
     int propagation = GPM_PROP_FIXED;
+    // view selection (DESIGN.md §17): GPM_VSEL_OFF or GPM_VSEL_JOINT with its parameters (gpm_set_view_selection)
+    gpm_view_sel vsel{GPM_VSEL_OFF, 0.f, 0.f, 0.f, 0, 0, 0.f, 0.f};
+    unsigned long long* vsel_mask = nullptr;   // [H*W] selected-views masks, allocated by the first switch to JOINT
+    int vsel_t = 0;                            // iterations of gpm_sweep since gpm_init / gpm_set_state
 };
 
 namespace {
@@ -177,6 +181,16 @@ int check_geometric(const gpm_ctx* c, float weight)
 }
 
 bool ncc_on(const gpm_ctx* c) { return c->photo == GPM_PHOTO_NCC; }
+bool jvs_on(const gpm_ctx* c) { return c->vsel.kind == GPM_VSEL_JOINT; }
+// per-warp floats of the JVS kernel variant the context launches (0 without view selection)
+int jvs_extra(const gpm_ctx* c) { return jvs_on(c) ? jvs_floats(c->V, c->geo_weight > 0.f) : 0; }
+
+// selected-views masks back to "none selected" (gpm_init, gpm_set_state, a switch to JOINT)
+int clear_vsel_masks(gpm_ctx* c)
+{
+    if (c->vsel_mask) CU(cudaMemsetAsync(c->vsel_mask, 0, (size_t)c->W * c->H * sizeof(unsigned long long), c->stream));
+    return GPM_OK;
+}
 
 // provenance of costs from an initialisation evaluation (gpm_init, or a trusted gpm_set_state)
 int init_prov(const gpm_ctx* c) { return ncc_on(c) ? GPM_PROV_NCC : c->color == 1 ? 3 : 0; }
@@ -279,7 +293,7 @@ int build_kparams(gpm_ctx* c, bool init_phase, KParams& P, bool eval_call = fals
     P.ref.depthMin = p.depthMin;  P.ref.depthMax = p.depthMax;
     // warps per block: as many as fit (<= 16).  The kernels use 128 registers per thread, so one 16-warp block fills an SM
     // anyway; shared memory may therefore be spent up to the per-block opt-in limit.
-    const size_t per_warp = (size_t)warp_scratch_floats(P.ns_pad, P.V, P.color, ncc_on(c)) * sizeof(float);
+    const size_t per_warp = (size_t)warp_scratch_floats(P.ns_pad, P.V, P.color, ncc_on(c), jvs_extra(c)) * sizeof(float);
     const size_t fixed = ((size_t)fixed_smem_floats(P) + 4) * sizeof(float);
     int nw = GPM_LB_THREADS / 32;
     const size_t budget = (size_t)c->smem_optin > 16 * 1024 ? (size_t)c->smem_optin - 8 * 1024 : 40 * 1024;
@@ -287,7 +301,7 @@ int build_kparams(gpm_ctx* c, bool init_phase, KParams& P, bool eval_call = fals
     if (c->opt_nwarps > 0) nw = c->opt_nwarps;
     if (nw > GPM_LB_THREADS / 32) nw = GPM_LB_THREADS / 32;
     P.nwarps = nw;
-    if (block_smem_bytes(P, ncc_on(c)) > (size_t)c->smem_optin)
+    if (block_smem_bytes(P, ncc_on(c), jvs_extra(c)) > (size_t)c->smem_optin)
         return fail(GPM_E_ARG, "configuration needs more shared memory per block than the device offers");
     return ensure_tensor_map(c, P);
 }
@@ -338,11 +352,29 @@ GeoParams geo_params(const gpm_ctx* c)
     return G;
 }
 
+// JVS launches' parameters at the context's iteration count t (DESIGN.md §17); thresholds in double, rounded once
+JvsParams jvs_params(const gpm_ctx* c)
+{
+    JvsParams J{};
+    if (!jvs_on(c)) return J;
+    const gpm_view_sel& v = c->vsel;
+    const double t = (double)c->vsel_t, beta = (double)v.beta;
+    J.mask = c->vsel_mask;
+    J.tau_t = (float)((double)v.tau_init * std::exp(-t * t / (double)v.alpha));
+    J.kb = (float)(-1.4426950408889634 / (2.0 * beta * beta));
+    J.tau_bad = v.tau_bad;  J.w_keep = v.w_keep;  J.n_good = v.n_good;  J.n_bad = v.n_bad;
+    return J;
+}
+
 int launch_colour(gpm_ctx* c, const KParams& P, int colour, int mask)
 {
     const bool ncc = ncc_on(c);          // grey images, 8 neighbours (gpm_set_photometric)
     const bool geo = c->geo_weight > 0.f;
-    auto kern = c->propagation == GPM_PROP_ADAPTIVE                                                  // 8 neighbours (gpm_set_propagation)
+    const bool adaptive = c->propagation == GPM_PROP_ADAPTIVE;
+    auto kern = jvs_on(c)                                                                           // NCC only (gpm_set_view_selection)
+              ? (adaptive ? (geo ? k_sweep<false, false, true, true, true, true> : k_sweep<false, false, false, true, true, true>)
+                          : (geo ? k_sweep<false, false, true, true, false, true> : k_sweep<false, false, false, true, false, true>))
+              : c->propagation == GPM_PROP_ADAPTIVE                                                  // 8 neighbours (gpm_set_propagation)
               ? (ncc ? (geo ? k_sweep<false, false, true, true, true> : k_sweep<false, false, false, true, true>)
                  : geo ? (P.color ? k_sweep<true, false, true, false, true> : k_sweep<false, false, true, false, true>)
                        : (P.color ? k_sweep<true, false, false, false, true> : k_sweep<false, false, false, false, true>))
@@ -350,8 +382,9 @@ int launch_colour(gpm_ctx* c, const KParams& P, int colour, int mask)
               : geo ? (P.color ? k_sweep<true, false, true> : k_sweep<false, false, true>)    // 8 neighbours (check_geometric)
               : P.ncand == 20 ? (P.color ? k_sweep<true, true> : k_sweep<false, true>)
                               : (P.color ? k_sweep<true, false> : k_sweep<false, false>);
-    kern<<<tile_grid(c), P.nwarps * 32, block_smem_bytes(P, ncc), c->stream>>>(P, c->tmap, c->d_cams, c->srcTex, c->planes, c->cost, c->rng,
-        c->prov, Memo{c->pid, c->seen, c->refseen, c->memo_mask, c->next_id}, colour, mask, c->d_stats, geo_params(c));
+    kern<<<tile_grid(c), P.nwarps * 32, block_smem_bytes(P, ncc, jvs_extra(c)), c->stream>>>(P, c->tmap, c->d_cams, c->srcTex, c->planes,
+        c->cost, c->rng, c->prov, Memo{c->pid, c->seen, c->refseen, c->memo_mask, c->next_id}, colour, mask, c->d_stats, geo_params(c),
+        jvs_params(c));
     c->launches++;
     CU(cudaGetLastError());
     return GPM_OK;
@@ -534,6 +567,10 @@ extern "C" int gpm_create(gpm_ctx** out, int device, int width, int height, int 
         ok(cudaFuncSetAttribute(k_sweep<false, false, true, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, c->smem_optin));
         ok(cudaFuncSetAttribute(k_shard_stage<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, c->smem_optin));
         ok(cudaFuncSetAttribute(k_shard_stage<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, c->smem_optin));
+        ok(cudaFuncSetAttribute(k_sweep<false, false, false, true, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, c->smem_optin));
+        ok(cudaFuncSetAttribute(k_sweep<false, false, true, true, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, c->smem_optin));
+        ok(cudaFuncSetAttribute(k_sweep<false, false, false, true, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, c->smem_optin));
+        ok(cudaFuncSetAttribute(k_sweep<false, false, true, true, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, c->smem_optin));
     }
     if (err != cudaSuccess) {
         std::string m = std::string("gpm_create: ") + cudaGetErrorString(err);
@@ -555,7 +592,7 @@ extern "C" void gpm_destroy(gpm_ctx* c)
     if (c->srcTex) cudaDestroyTextureObject(c->srcTex);
     if (c->srcArr) cudaFreeArray(c->srcArr);
     cudaFree(c->planar);
-    cudaFree(c->planes);  cudaFree(c->cost);  cudaFree(c->prov);  cudaFree(c->seen);  cudaFree(c->refseen);  cudaFree(c->pid);  cudaFree(c->next_id);  cudaFree(c->memo_mask);  cudaFree(c->rng);  cudaFree(c->dispbuf);  cudaFree(c->candbuf);  cudaFree(c->canddepth);  cudaFree(c->sflags);  cudaFree(c->xchg);  cudaFree(c->gath);  cudaFree(c->refpad);  cudaFree(c->staging);  cudaFree(c->geo_depth);  cudaFree(c->geo_kinv);
+    cudaFree(c->planes);  cudaFree(c->cost);  cudaFree(c->prov);  cudaFree(c->seen);  cudaFree(c->refseen);  cudaFree(c->pid);  cudaFree(c->next_id);  cudaFree(c->memo_mask);  cudaFree(c->rng);  cudaFree(c->dispbuf);  cudaFree(c->candbuf);  cudaFree(c->canddepth);  cudaFree(c->sflags);  cudaFree(c->xchg);  cudaFree(c->gath);  cudaFree(c->refpad);  cudaFree(c->staging);  cudaFree(c->geo_depth);  cudaFree(c->geo_kinv);  cudaFree(c->vsel_mask);
     cudaFree(c->d_cams);  cudaFree(c->d_stats);
     if (c->ev0) cudaEventDestroy(c->ev0);
     if (c->ev1) cudaEventDestroy(c->ev1);
@@ -600,9 +637,11 @@ extern "C" int gpm_set_rng(gpm_ctx* c, unsigned long long seed, int mode)
     return GPM_OK;
 }
 
-// the NCC cost has no colour variant: a colour upload while it is on is refused before anything changes
+// the NCC cost and joint view selection have no colour variant: a colour upload while either is on is refused before
+// anything changes
 static int refuse_color_under_ncc(const char* fn, const gpm_ctx* c, bool color)
 {
+    if (color && jvs_on(c)) return fail(GPM_E_ARG, std::string(fn) + ": joint view selection supports grey images only (gpm_set_view_selection GPM_VSEL_OFF)");
     return color && ncc_on(c) ? fail(GPM_E_STATE, std::string(fn) + ": the NCC photometric cost supports grey images only (gpm_set_photometric GPM_PHOTO_PM)") : GPM_OK;
 }
 
@@ -735,6 +774,7 @@ extern "C" int gpm_set_photometric(gpm_ctx* c, int kind, float min_std)
         if (c->color == 1) return fail(GPM_E_ARG, "gpm_set_photometric: the NCC cost supports grey images only; this context holds colour images");
         if (c->opt_neighbours == 20) return fail(GPM_E_ARG, "gpm_set_photometric: the NCC cost supports the 8-neighbour sweep only (option neighbours = 8)");
     } else {
+        if (jvs_on(c)) return fail(GPM_E_ARG, "gpm_set_photometric: joint view selection is built for the NCC cost (gpm_set_view_selection GPM_VSEL_OFF first)");
         min_std = 0.f;                               // not read by the PM cost
     }
     if (kind != c->photo || min_std != c->ncc_min_std) c->inputs_dirty = true;
@@ -755,6 +795,55 @@ extern "C" int gpm_set_propagation(gpm_ctx* c, int kind)
     return GPM_OK;
 }
 
+namespace gpm {
+// what gpm_set_view_selection refuses for its arguments alone (the batch drivers check the same before any CUDA call)
+const char* view_sel_refusal(const gpm_view_sel* v)
+{
+    if (!v) return "vsel is NULL";
+    if (v->kind != GPM_VSEL_OFF && v->kind != GPM_VSEL_JOINT) return "kind must be GPM_VSEL_OFF or GPM_VSEL_JOINT";
+    if (v->kind == GPM_VSEL_OFF) return nullptr;
+    auto positive = [](float x) { return std::isfinite(x) && x > 0.f; };
+    if (!positive(v->tau_init) || !positive(v->alpha) || !positive(v->tau_bad) || !positive(v->beta))
+        return "tau_init, alpha, tau_bad and beta must be finite and > 0";
+    if (!std::isfinite(v->w_keep) || v->w_keep < 0.f) return "w_keep must be finite and >= 0";
+    if (v->n_good < 1 || v->n_good > 8) return "n_good must be 1..8";
+    if (v->n_bad < 1 || v->n_bad > 9) return "n_bad must be 1..9";
+    return nullptr;
+}
+}  // namespace gpm
+
+// A switch either way changes what the stored costs mean (weighted or combined): they and the memo are marked stale.
+extern "C" int gpm_set_view_selection(gpm_ctx* c, const gpm_view_sel* vsel)
+{
+    if (!c) return fail(GPM_E_ARG, "gpm_set_view_selection: null context");
+    if (const char* bad = view_sel_refusal(vsel)) return fail(GPM_E_ARG, std::string("gpm_set_view_selection: ") + bad);
+    if (vsel->kind == GPM_VSEL_JOINT) {
+        if (!ncc_on(c)) return fail(GPM_E_ARG, "gpm_set_view_selection: joint view selection is built for the NCC cost (gpm_set_photometric GPM_PHOTO_NCC)");
+        if (c->color == 1) return fail(GPM_E_ARG, "gpm_set_view_selection: joint view selection supports grey images only; this context holds colour images");
+        if (c->opt_neighbours == 20) return fail(GPM_E_ARG, "gpm_set_view_selection: joint view selection supports the 8-neighbour sweep only (option neighbours = 8)");
+        if (!jvs_on(c)) {
+            DeviceGuard g(c->device);
+            if (!c->vsel_mask) CU(cudaMalloc(&c->vsel_mask, (size_t)c->W * c->H * sizeof(unsigned long long)));
+            const int rc = clear_vsel_masks(c);
+            if (rc) return rc;
+        }
+    }
+    if (vsel->kind != c->vsel.kind) c->inputs_dirty = true;
+    c->vsel = *vsel;
+    return GPM_OK;
+}
+
+extern "C" int gpm_get_view_masks(gpm_ctx* c, unsigned long long* masks)
+{
+    if (!c || !masks) return fail(GPM_E_ARG, "gpm_get_view_masks: null argument");
+    DeviceGuard g(c->device);
+    const size_t n = (size_t)c->W * c->H;
+    if (!c->vsel_mask) { memset(masks, 0, n * sizeof(unsigned long long));  return GPM_OK; }
+    CU(cudaMemcpyAsync(masks, c->vsel_mask, n * sizeof(unsigned long long), cudaMemcpyDeviceToHost, c->stream));
+    CU(cudaStreamSynchronize(c->stream));
+    return GPM_OK;
+}
+
 extern "C" int gpm_set_state(gpm_ctx* c, const float* norm4, const float* cost, int on_device)
 {
     if (!c) return fail(GPM_E_ARG, "gpm_set_state: null context");
@@ -769,8 +858,11 @@ extern "C" int gpm_set_state(gpm_ctx* c, const float* norm4, const float* cost, 
     if (cost) CU(cudaMemcpyAsync(c->cost, cost, n * sizeof(float), k, c->stream));
     // provenance of the supplied costs is unknown (GPM_PROV_UNKNOWN) unless the caller vouches that they came from an
     // initialisation / refinement evaluation of exactly these planes ("trust_state": 0)
-    const int rc = reset_state_tags(c, c->opt_trust_state ? init_prov(c) : GPM_PROV_UNKNOWN);
+    int rc = reset_state_tags(c, c->opt_trust_state ? init_prov(c) : GPM_PROV_UNKNOWN);
     if (rc) return rc;
+    rc = clear_vsel_masks(c);                        // a new start state: no view selected, t = 0
+    if (rc) return rc;
+    c->vsel_t = 0;
     CU(cudaStreamSynchronize(c->stream));
     return GPM_OK;
 }
@@ -797,6 +889,9 @@ static int do_init(gpm_ctx* c)
     rc = init_planes(c, P);
     if (rc) return rc;
     CU(launch_cost_eval(c, P, c->planes, c->cost));
+    rc = clear_vsel_masks(c);                      // view selection starts over: no view selected, t = 0
+    if (rc) return rc;
+    c->vsel_t = 0;
     return reset_state_tags(c, init_prov(c));     // costs now come from the init-variant evaluation (float4: x-first + gradient folding 1; NCC: its own)
 }
 
@@ -812,6 +907,7 @@ static int do_sweeps(gpm_ctx* c, int iterations)
         if (rc) return rc;
         rc = launch_colour(c, P, 1, 7);
         if (rc) return rc;
+        c->vsel_t++;                                                           // view selection's iteration count (§17)
     }
     return GPM_OK;
 }
@@ -931,9 +1027,10 @@ static int shard_refine_steps(const gpm_params& p)
     return n;
 }
 
-// the source-view shard has no geometric-consistency and no NCC variant: refused before anything is launched
+// the source-view shard has no geometric-consistency, NCC or view-selection variant: refused before anything is launched
 static int shard_refuses_mode(gpm_ctx* c)
 {
+    if (jvs_on(c)) return fail(GPM_E_STATE, "view sharding does not support joint view selection: the exchange carries top-n lists, not per-view costs (gpm_set_view_selection GPM_VSEL_OFF)");
     if (c->geo_weight > 0.f) return fail(GPM_E_STATE, "view sharding does not support the geometric-consistency mode (gpm_set_geometric weight 0)");
     if (ncc_on(c)) return fail(GPM_E_STATE, "view sharding does not support the NCC photometric cost (gpm_set_photometric GPM_PHOTO_PM)");
     return GPM_OK;
@@ -1280,6 +1377,7 @@ extern "C" int gpm_set_option(gpm_ctx* c, const char* name, int value)
         if (value == 20 && c->geo_weight > 0.f) return fail(GPM_E_ARG, "the geometric-consistency mode supports the 8-neighbour sweep only");
         if (value == 20 && ncc_on(c)) return fail(GPM_E_ARG, "the NCC photometric cost supports the 8-neighbour sweep only");
         if (value == 20 && c->propagation == GPM_PROP_ADAPTIVE) return fail(GPM_E_ARG, "adaptive checkerboard sampling supports the 8-neighbour sweep only");
+        if (value == 20 && jvs_on(c)) return fail(GPM_E_ARG, "joint view selection supports the 8-neighbour sweep only");
         DeviceGuard g(c->device);
         const int slots = value == 20 ? 20 : 8;
         if (slots != c->seen_slots) {

@@ -8,7 +8,7 @@
 // (gpm_run) and hands back / writes the result (disp.dmb + normals.dmb, main.cpp:1002-1003, for the external fusibile).
 // gpm_geo_batch_run runs the two-pass geometric-consistency flow (DESIGN.md §14) on the same pool and image cache.  The
 // _photo twins of both choose the photometric cost (DESIGN.md §15), the _opts ones every per-job option (gpm_job_opts):
-// the photometric cost and the propagation mode (§16).
+// the photometric cost and the propagation mode (§16), and the _vsel ones the view selection besides (§17).
 // Host C++ over the C-ABI; the only CUDA calls are page-locking, the geometric driver's host store and its sweep events.
 #include "../../include/gipuma_b200.h"
 
@@ -25,6 +25,10 @@
 #include <thread>
 #include <vector>
 #include <sys/stat.h>
+
+namespace gpm {
+const char* view_sel_refusal(const gpm_view_sel* v);     // gpm_api.cu
+}
 
 namespace {
 std::mutex g_err_mutex;
@@ -72,25 +76,33 @@ bool plan_view(const gpm_batch_desc* d, int ref, ViewSetup& s)
 // the options of the _photo twins
 gpm_job_opts photo_opts(int kind, float min_std) { return gpm_job_opts{kind, min_std, GPM_PROP_FIXED}; }
 
-// what gpm_set_photometric and gpm_set_propagation refuse for their arguments, and NCC on colour images; nullptr if none
-const char* opts_refusal(const gpm_job_opts* o, int channels)
+const gpm_view_sel kVselOff{GPM_VSEL_OFF, 0.f, 0.f, 0.f, 0, 0, 0.f, 0.f};
+
+// what gpm_set_photometric, gpm_set_propagation and gpm_set_view_selection refuse for their arguments, NCC on colour images
+// and joint view selection with the PM cost or colour images; nullptr if none
+const char* opts_refusal(const gpm_job_opts* o, const gpm_view_sel* v, int channels)
 {
     if (!o) return "opts is NULL";
     if (o->photometric != GPM_PHOTO_PM && o->photometric != GPM_PHOTO_NCC) return "kind must be GPM_PHOTO_PM or GPM_PHOTO_NCC";
     if (o->photometric == GPM_PHOTO_NCC && !(std::isfinite(o->ncc_min_std) && o->ncc_min_std > 0.f)) return "min_std must be finite and > 0";
     if (o->photometric == GPM_PHOTO_NCC && channels == 4) return "the NCC cost supports grey images only (channels 1)";
     if (o->propagation != GPM_PROP_FIXED && o->propagation != GPM_PROP_ADAPTIVE) return "propagation must be GPM_PROP_FIXED or GPM_PROP_ADAPTIVE";
+    if (const char* bad = gpm::view_sel_refusal(v)) return bad;
+    if (v->kind == GPM_VSEL_JOINT && o->photometric != GPM_PHOTO_NCC) return "joint view selection is built for the NCC cost (GPM_PHOTO_NCC)";
+    if (v->kind == GPM_VSEL_JOINT && channels == 4) return "joint view selection supports grey images only (channels 1)";
     return nullptr;
 }
 
-// The per-view setup of a job: photometric cost, propagation, parameters, reference and source images (grey: channels 1,
-// RGBA: 4), view count, RNG.
-int load_view(gpm_ctx* ctx, const gpm_batch_desc* d, int channels, size_t pitch, const ViewSetup& s, const gpm_job_opts& o)
+// The per-view setup of a job: photometric cost, propagation, view selection, parameters, reference and source images
+// (grey: channels 1, RGBA: 4), view count, RNG.
+int load_view(gpm_ctx* ctx, const gpm_batch_desc* d, int channels, size_t pitch, const ViewSetup& s, const gpm_job_opts& o,
+              const gpm_view_sel& v)
 {
     auto set_reference = channels == 4 ? gpm_set_reference_color : gpm_set_reference;
     auto set_view = channels == 4 ? gpm_set_view_color : gpm_set_view;
     int rc = gpm_set_photometric(ctx, o.photometric, o.ncc_min_std);
     if (rc == GPM_OK) rc = gpm_set_propagation(ctx, o.propagation);
+    if (rc == GPM_OK) rc = gpm_set_view_selection(ctx, &v);
     if (rc == GPM_OK) rc = gpm_set_params(ctx, &s.p);
     if (rc == GPM_OK) rc = set_reference(ctx, d->images[s.order[0]], pitch, 0, &s.cams[0]);
     for (int v = 0; v < s.nv && rc == GPM_OK; v++) rc = set_view(ctx, v, d->images[s.source(v)], pitch, 0, &s.cams[s.subset[v]]);
@@ -169,15 +181,15 @@ extern "C" const char* gpm_batch_last_error(void)
     return copy.c_str();
 }
 
-// gpm_batch_run and its _photo / _opts twins; `fn` names the entry point in error messages
-static int batch_run(const char* fn, const gpm_batch_desc* d, const gpm_job_opts* opts, gpm_batch_stats* stats)
+// gpm_batch_run and its _photo / _opts / _vsel twins; `fn` names the entry point in error messages
+static int batch_run(const char* fn, const gpm_batch_desc* d, const gpm_job_opts* opts, const gpm_view_sel* vsel, gpm_batch_stats* stats)
 {
     clear_err();
     if (!batch_desc_ok(d)) {
         set_err(std::string(fn) + ": bad arguments");
         return GPM_E_ARG;
     }
-    if (const char* bad = opts_refusal(opts, 1)) {
+    if (const char* bad = opts_refusal(opts, vsel, 1)) {
         set_err(std::string(fn) + ": bad arguments: " + bad);
         return GPM_E_ARG;
     }
@@ -196,7 +208,7 @@ static int batch_run(const char* fn, const gpm_batch_desc* d, const gpm_job_opts
             const int ref = d->ref_indices ? d->ref_indices[job] : job;
             if (ref < 0 || ref >= n) { set_err(std::string(fn) + ": reference index out of range");  return false; }
             if (!plan_view(d, ref, s)) { set_err(std::string(fn) + ": no source view passes the angle filter for reference " + std::to_string(ref));  return false; }
-            int rc = load_view(ctx, d, 1, pitch, s, *opts);
+            int rc = load_view(ctx, d, 1, pitch, s, *opts, *vsel);
             float ms = 0.f;
             if (rc == GPM_OK) rc = gpm_run(ctx, &ms);
             if (rc != GPM_OK) { set_err(std::string("reference view ") + std::to_string(ref) + ": " + gpm_last_error());  return false; }
@@ -223,18 +235,23 @@ static int batch_run(const char* fn, const gpm_batch_desc* d, const gpm_job_opts
 extern "C" int gpm_batch_run(const gpm_batch_desc* d, gpm_batch_stats* stats)
 {
     const gpm_job_opts o = photo_opts(GPM_PHOTO_PM, 0.f);
-    return batch_run("gpm_batch_run", d, &o, stats);
+    return batch_run("gpm_batch_run", d, &o, &kVselOff, stats);
 }
 
 extern "C" int gpm_batch_run_photo(const gpm_batch_desc* d, int kind, float min_std, gpm_batch_stats* stats)
 {
     const gpm_job_opts o = photo_opts(kind, min_std);
-    return batch_run("gpm_batch_run_photo", d, &o, stats);
+    return batch_run("gpm_batch_run_photo", d, &o, &kVselOff, stats);
 }
 
 extern "C" int gpm_batch_run_opts(const gpm_batch_desc* d, const gpm_job_opts* opts, gpm_batch_stats* stats)
 {
-    return batch_run("gpm_batch_run_opts", d, opts, stats);
+    return batch_run("gpm_batch_run_opts", d, opts, &kVselOff, stats);
+}
+
+extern "C" int gpm_batch_run_vsel(const gpm_batch_desc* d, const gpm_job_opts* opts, const gpm_view_sel* vsel, gpm_batch_stats* stats)
+{
+    return batch_run("gpm_batch_run_vsel", d, opts, vsel ? vsel : &kVselOff, stats);
 }
 
 // ---- two-pass geometric-consistency batch (DESIGN.md §14) -----------------------------------------------------------------
@@ -294,8 +311,9 @@ private:
 };
 }  // namespace
 
-// gpm_geo_batch_run and its _photo / _opts twins; `fn` names the entry point in error messages
-static int geo_batch_run(const char* fn, const gpm_geo_batch_desc* g, const gpm_job_opts* opts, gpm_geo_batch_stats* stats)
+// gpm_geo_batch_run and its _photo / _opts / _vsel twins; `fn` names the entry point in error messages
+static int geo_batch_run(const char* fn, const gpm_geo_batch_desc* g, const gpm_job_opts* opts, const gpm_view_sel* vsel,
+                         gpm_geo_batch_stats* stats)
 {
     clear_err();
     const char* bad = nullptr;
@@ -304,7 +322,7 @@ static int geo_batch_run(const char* fn, const gpm_geo_batch_desc* g, const gpm_
     else if (g->geo_iterations < 0) bad = "geo_iterations must be >= 0";
     else if (!std::isfinite(g->weight) || g->weight < 0.f) bad = "weight must be finite and >= 0";
     else if (!std::isfinite(g->max_err) || g->max_err <= 0.f) bad = "max_err must be finite and > 0";
-    else bad = opts_refusal(opts, g->channels);
+    else bad = opts_refusal(opts, vsel, g->channels);
     if (bad) {
         set_err(std::string(fn) + ": bad arguments: " + bad);
         return GPM_E_ARG;
@@ -377,7 +395,7 @@ static int geo_batch_run(const char* fn, const gpm_geo_batch_desc* g, const gpm_
         };
         take_jobs(next1, n_pass1, failed, [&](int job) {          // pass 1: photometric
             const int r = pass1[job];
-            int rc = load_view(ctx, d, g->channels, pitch, setup[r], *opts);
+            int rc = load_view(ctx, d, g->channels, pitch, setup[r], *opts, *vsel);
             if (rc == GPM_OK) rc = gpm_init(ctx);
             if (rc == GPM_OK) rc = timer.sweep(ctx, d->params.iterations, &pass1_ms[job]);
             if (rc == GPM_OK && raw_slot[r] >= 0) rc = gpm_get_state(ctx, raw_store + (size_t)raw_slot[r] * npix * 4, nullptr, 0);
@@ -393,7 +411,7 @@ static int geo_batch_run(const char* fn, const gpm_geo_batch_desc* g, const gpm_
             const int r = ref_of(job);
             const ViewSetup& s = setup[r];
             const float* raw = raw_store + (size_t)raw_slot[r] * npix * 4;
-            int rc = load_view(ctx, d, g->channels, pitch, s, *opts);
+            int rc = load_view(ctx, d, g->channels, pitch, s, *opts, *vsel);
             for (int v = 0; v < s.nv && rc == GPM_OK; v++) rc = gpm_set_view_depth(ctx, v, depth_store + (size_t)depth_slot[s.source(v)] * npix, 0, 0);
             if (rc == GPM_OK) rc = gpm_set_geometric(ctx, g->weight, g->max_err);
             if (rc == GPM_OK) rc = gpm_cost_eval(ctx, raw, cost.data(), 0);
@@ -436,16 +454,22 @@ static int geo_batch_run(const char* fn, const gpm_geo_batch_desc* g, const gpm_
 extern "C" int gpm_geo_batch_run(const gpm_geo_batch_desc* g, gpm_geo_batch_stats* stats)
 {
     const gpm_job_opts o = photo_opts(GPM_PHOTO_PM, 0.f);
-    return geo_batch_run("gpm_geo_batch_run", g, &o, stats);
+    return geo_batch_run("gpm_geo_batch_run", g, &o, &kVselOff, stats);
 }
 
 extern "C" int gpm_geo_batch_run_photo(const gpm_geo_batch_desc* g, int kind, float min_std, gpm_geo_batch_stats* stats)
 {
     const gpm_job_opts o = photo_opts(kind, min_std);
-    return geo_batch_run("gpm_geo_batch_run_photo", g, &o, stats);
+    return geo_batch_run("gpm_geo_batch_run_photo", g, &o, &kVselOff, stats);
 }
 
 extern "C" int gpm_geo_batch_run_opts(const gpm_geo_batch_desc* g, const gpm_job_opts* opts, gpm_geo_batch_stats* stats)
 {
-    return geo_batch_run("gpm_geo_batch_run_opts", g, opts, stats);
+    return geo_batch_run("gpm_geo_batch_run_opts", g, opts, &kVselOff, stats);
+}
+
+extern "C" int gpm_geo_batch_run_vsel(const gpm_geo_batch_desc* g, const gpm_job_opts* opts, const gpm_view_sel* vsel,
+                                      gpm_geo_batch_stats* stats)
+{
+    return geo_batch_run("gpm_geo_batch_run_vsel", g, opts, vsel ? vsel : &kVselOff, stats);
 }

@@ -40,6 +40,7 @@ namespace gpm {
 #define GPM_FUSED_SITES_FLOAT4 {0, 0, 0, 0, 0, 0, 0, 0, 0, 9, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1}
 #define GPM_PROV_UNKNOWN 0xff        // prov[]: cost of unknown rounding variant (else bit 0 = x-first, bit 1 = gradient folding)
 #define GPM_PROV_NCC 0x10            // prov[]: an NCC cost (DESIGN.md §15), which has one rounding variant at every call site
+#define GPM_PROV_JVS 0x20            // prov[]: a cost weighted by joint view selection (DESIGN.md §17): not a pure function of the plane
 
 // ---- exact-arithmetic primitives -------------------------------------------------------------
 // With --use_fast_math these lower to {mul,add,sub,fma}.rn.ftz.f32, which ptxas never fuses.
@@ -139,10 +140,11 @@ struct WarpScratch {
     float* sums;    // NCC only: [4] the window's W = sum w_s, Sr = sum a_s, Srr = sum a_s * r_s (DESIGN.md §15)
 };
 
-// multiple of 4 floats so that every warp's block stays 16-byte aligned; ncc: the NCC variants' a_s and pixel sums
-__host__ __device__ inline int warp_scratch_floats(int ns_pad, int V, int color, bool ncc = false)
+// multiple of 4 floats so that every warp's block stays 16-byte aligned; ncc: the NCC variants' a_s and pixel sums;
+// extra: floats a kernel variant keeps per warp after the common block (joint view selection's cost rows, jvs_floats)
+__host__ __device__ inline int warp_scratch_floats(int ns_pad, int V, int color, bool ncc = false, int extra = 0)
 {
-    return (6 * ns_pad + (color ? 12 * ns_pad : 0) + V * 12 + V * GPM_DSTRIDE + (ncc ? ns_pad + 4 : 0) + 3) & ~3;
+    return ((6 * ns_pad + (color ? 12 * ns_pad : 0) + V * 12 + V * GPM_DSTRIDE + (ncc ? ns_pad + 4 : 0) + 3) & ~3) + ((extra + 3) & ~3);
 }
 
 __device__ __forceinline__ WarpScratch carve(float* base, int ns_pad, int V, int color, const unsigned char* perm, bool ncc = false)
@@ -342,13 +344,16 @@ __device__ __forceinline__ float ncc_cost(float Wsum, float Sr, float Srr, float
 // add is monotone, so the bound stays an exact lower bound.
 // NCC: the photometric cost of every view is the NCC cost (DESIGN.md §15, grey images only; G->min_std).  XF and `rt` are
 // ignored: every call site uses one rounding variant.  No bound is tested (partial sums bound nothing); `bound` is ignored.
-template <int XF, bool COLOR, bool GEO = false, bool NCC = false>
+// ROWS (NCC only; joint view selection, DESIGN.md §17): nothing is combined; view v's NCC cost goes to per_view0[v] and,
+// with GEO, its geometric term to per_view1[v] (written by lanes v and v + 32), and the result is 0.
+template <int XF, bool COLOR, bool GEO = false, bool NCC = false, bool ROWS = false>
 __device__ __forceinline__ float eval_plane(const KParams& P, const float* __restrict__ sCam, const WarpScratch& ws,
                                             cudaTextureObject_t src, float nx, float ny, float nz, float d,
                                             float bound, unsigned lane, WarpStats& st,
                                             float* per_view0 = nullptr, float* per_view1 = nullptr, unsigned rt = 0u,
                                             const GeoParams* G = nullptr, float gpx = 0.0f, float gpy = 0.0f)
 {
+    static_assert(!ROWS || NCC, "per-view cost rows are built for the NCC cost only");
     // XF = 0 / 1: compile-time variant; XF = 2: per call, rt bit 0 = x-term first, bit 1 = gradient folding variant,
     // bits 2 / 3 = the Y / Z row of H deviates from bit 0 (ptxas chose per row in one inlined site of the fused kernel)
     const bool XFIRST = XF == 2 ? (rt & 1u) != 0u : XF == 1;
@@ -461,6 +466,11 @@ __device__ __forceinline__ float eval_plane(const KParams& P, const float* __res
         const float min_var = fmul(G->min_std, G->min_std);
         const float c0 = ncc_cost(Wsum, Sr, Srr, St0, Stt0, Srt0, min_var);
         const float c1 = ncc_cost(Wsum, Sr, Srr, St1, Stt1, Srt1, min_var);
+        if constexpr (ROWS) {
+            if ((int)lane < P.V) { per_view0[lane] = c0;  if (GEO) per_view1[lane] = g0; }
+            if ((int)lane + 32 < P.V) { per_view0[lane + 32] = c1;  if (GEO) per_view1[lane + 32] = g1; }
+            return 0.0f;
+        }
         if constexpr (GEO) return combine_views(P, fadd(c0, g0), fadd(c1, g1), lane);
         else return combine_views(P, c0, c1, lane);
     }

@@ -8,14 +8,14 @@ namespace gpm {
 
 __host__ __device__ inline int tile_floats(const KParams& P) { return P.tile_stride * P.tile_w * (P.color ? 4 : 1); }
 __host__ __device__ inline int fixed_smem_floats(const KParams& P) { return (tile_floats(P) + P.V * GPM_VIEWCAM_FLOATS + 3) & ~3; }
-// ncc: the NCC kernels' larger per-warp scratch (warp_scratch_floats)
-__device__ __forceinline__ unsigned long long* block_mbar(const KParams& P, float* smem_base, bool ncc = false)
+// ncc, extra: the NCC kernels' larger per-warp scratch and a variant's extra floats per warp (warp_scratch_floats)
+__device__ __forceinline__ unsigned long long* block_mbar(const KParams& P, float* smem_base, bool ncc = false, int extra = 0)
 {
-    return reinterpret_cast<unsigned long long*>(smem_base + fixed_smem_floats(P) + (size_t)P.nwarps * warp_scratch_floats(P.ns_pad, P.V, P.color, ncc) + 2);
+    return reinterpret_cast<unsigned long long*>(smem_base + fixed_smem_floats(P) + (size_t)P.nwarps * warp_scratch_floats(P.ns_pad, P.V, P.color, ncc, extra) + 2);
 }
-__device__ __forceinline__ unsigned char* block_perm(const KParams& P, float* smem_base, bool ncc = false)
+__device__ __forceinline__ unsigned char* block_perm(const KParams& P, float* smem_base, bool ncc = false, int extra = 0)
 {
-    return reinterpret_cast<unsigned char*>(smem_base + fixed_smem_floats(P) + (size_t)P.nwarps * warp_scratch_floats(P.ns_pad, P.V, P.color, ncc) + 4);
+    return reinterpret_cast<unsigned char*>(smem_base + fixed_smem_floats(P) + (size_t)P.nwarps * warp_scratch_floats(P.ns_pad, P.V, P.color, ncc, extra) + 4);
 }
 
 // ---- TMA (cp.async.bulk.tensor) + mbarrier primitives -------------------------------------------------------------
@@ -50,9 +50,10 @@ __device__ __forceinline__ void mbar_wait(unsigned long long* bar, unsigned pari
 // the replicate-padded reference image and the block waits on its mbarrier while the other threads copy the camera and
 // lane tables.  `phase` = parity of the barrier's current phase (0 for the first / only tile of a block).
 __device__ __forceinline__ void stage_block(const KParams& P, const CUtensorMap* tmap, const ViewCam* __restrict__ cams,
-                                            float* tile, float* sCam, int tile_x0, int tile_y0, unsigned phase = 0u, bool ncc = false)
+                                            float* tile, float* sCam, int tile_x0, int tile_y0, unsigned phase = 0u, bool ncc = false,
+                                            int extra = 0)
 {
-    unsigned long long* bar = block_mbar(P, tile, ncc);
+    unsigned long long* bar = block_mbar(P, tile, ncc, extra);
     if (threadIdx.x == 0) {
         if (phase == 0u) mbar_init(bar, 1);
         mbar_arrive_expect_tx(bar, (unsigned)(tile_floats(P) * sizeof(float)));
@@ -61,7 +62,7 @@ __device__ __forceinline__ void stage_block(const KParams& P, const CUtensorMap*
     const float* c = reinterpret_cast<const float*>(cams);
     for (int e = threadIdx.x; e < P.V * GPM_VIEWCAM_FLOATS; e += blockDim.x) sCam[e] = c[e];
     // lane -> sample table of the sampling rounds (KParams::perm), word by word
-    unsigned* sp = reinterpret_cast<unsigned*>(block_perm(P, tile, ncc));
+    unsigned* sp = reinterpret_cast<unsigned*>(block_perm(P, tile, ncc, extra));
     const unsigned* gp = reinterpret_cast<const unsigned*>(&P.perm[0][0]);
     for (int e = threadIdx.x; e < GPM_MAX_ROUNDS * 8; e += blockDim.x) sp[e] = gp[e];
     __syncthreads();                                // tables visible; mbarrier initialised before anyone waits on it
@@ -80,11 +81,26 @@ __device__ __forceinline__ void flush_stats(unsigned long long* stats, const War
 }
 
 // shared memory: [tile tile_stride*tile_w][cams V*21][pad to 16 B][nwarps * warp_scratch][4 ints: work counter, unused, mbarrier (8 B)][lane permutation table, GPM_MAX_ROUNDS x 32 bytes]
-__host__ __device__ inline size_t block_smem_bytes(const KParams& P, bool ncc = false)
+__host__ __device__ inline size_t block_smem_bytes(const KParams& P, bool ncc = false, int extra = 0)
 {
-    size_t fl = (size_t)fixed_smem_floats(P) + (size_t)P.nwarps * warp_scratch_floats(P.ns_pad, P.V, P.color, ncc) + 4 + GPM_MAX_ROUNDS * 8;
+    size_t fl = (size_t)fixed_smem_floats(P) + (size_t)P.nwarps * warp_scratch_floats(P.ns_pad, P.V, P.color, ncc, extra) + 4 + GPM_MAX_ROUNDS * 8;
     return fl * sizeof(float);
 }
+
+// ---- joint view selection (ACMH's multi-hypothesis view selection, DESIGN.md §17) ------------------------------------
+// What the JVS variants of k_sweep read besides KParams: the per-pixel selected-views masks and the launch's thresholds.
+// A kernel parameter of its own, so that KParams and GeoParams keep their layout in every other kernel.
+struct JvsParams {
+    unsigned long long* mask;   // [H*W] bit j: view j was selected at this pixel by the last JVS launch
+    float tau_t;                // good threshold of this launch: tau_init * exp(-t^2 / alpha), computed on the host
+    float kb;                   // -log2(e) / (2 beta^2): conf(m) = ex2(m * m * kb)
+    float tau_bad, w_keep;
+    int n_good, n_bad;
+};
+
+// per-warp floats of the JVS variants after the common scratch: 9 rows of V photometric costs (8 candidates, then the
+// current plane or the refinement candidate), as many geometric terms with GEO, and the V view weights
+__host__ __device__ inline int jvs_floats(int V, bool geo) { return (geo ? 18 : 9) * V + V; }
 
 // ---- exact memo of rejected work: plane identities ------------------------------------------------------------
 // Every plane carries a 32-bit identity: pid[p] = p + 1 at initialisation, a fresh number (atomic counter) whenever a
@@ -255,17 +271,196 @@ __device__ __forceinline__ bool sweep_neighbour(int k, const int& px, const int&
     else return close_far_neighbour(k, px, py, W, H, qx, qy);
 }
 
+// One pixel of a joint-view-selection launch (ACMH, Xu & Tao 2019; DESIGN.md §17): NCC cost, grey images, 8-neighbour
+// sweep.  The steps as §17 numbers them: (1) the per-view cost rows of the current plane and of every offered candidate
+// whose depth is in range (E), a candidate whose identity equals the current plane's or an earlier candidate's reusing
+// that row; (2, 3) lane j reduces view j's column over E into good_j, bad_j and s_j and forms the weight w_j; (4) every
+// hypothesis is scored sum_j w_j c_j / sum_j w_j, both sums sequential from +0 (lane 0), or by combine_views where
+// sum_j w_j = 0; (5) the fold starts at the current plane's re-scored cost.  Weighted costs are not a pure function of the
+// plane, so neither memo nor the duplicate-of-current skip is used, and the stored cost is tagged GPM_PROV_JVS.  The
+// refinement restates k_sweep's loop body line for line (see shard_refine_candidate).
+template <bool GEO, bool ADAPTIVE>
+__device__ __forceinline__ void jvs_pixel(const KParams& P, const JvsParams& J, const GeoParams* g, const float* __restrict__ sCam,
+                                          const float* __restrict__ tile, const WarpScratch& ws, float* __restrict__ jv,
+                                          cudaTextureObject_t src, float4* __restrict__ planes, float* __restrict__ cost,
+                                          unsigned* __restrict__ rng_state, unsigned char* __restrict__ prov, const Memo& M,
+                                          int px, int py, int tile_x0, int tile_y0, int phase_mask, unsigned lane, WarpStats& st)
+{
+    const RefCam& cam = P.ref;
+    const int W = P.W, H = P.H, V = P.V;
+    const size_t center = (size_t)py * W + px;
+    const float fpx = __int2float_rn(px), fpy = __int2float_rn(py);
+    const float inf = __int_as_float(0x7f800000);
+    float* Mr = jv;                                  // [9][V] photometric costs: rows 0..7 candidates, 8 current / refinement
+    float* Gr = jv + 9 * V;                          // GEO: [9][V] geometric terms
+    float* wv = jv + (GEO ? 18 : 9) * V;             // [V] view weights
+    float4 norm_now = planes[center];
+    unsigned own_id = M.pid[center];
+    const unsigned long long remembered = J.mask[center];
+
+    // candidate k in lane k, its depth at p and the range test (gipuma.cu:829-830)
+    float4 mine = make_float4(0.f, 0.f, 0.f, 0.f);
+    bool mine_ok = false, in_range = false;
+    float mine_disp = 0.0f;
+    size_t mine_at = center;
+    if (lane < 8) {
+        const bool phase_on = (phase_mask >> (lane >> 2)) & 1;
+        int qx, qy;
+        const bool ok = sweep_neighbour<ADAPTIVE>((int)lane, px, py, W, H, cost, qx, qy);
+        mine_ok = ok && phase_on;
+        mine_at = (size_t)qy * W + qx;
+    }
+    const unsigned mine_id = mine_ok ? M.pid[mine_at] : 0u;
+    if (mine_ok) {
+        mine = planes[mine_at];
+        mine_disp = plane_depth(cam, mine.x, mine.y, mine.z, mine.w, fpx, fpy);
+        in_range = mine_disp >= cam.depthMin && mine_disp <= cam.depthMax;
+    }
+    const unsigned offered = __ballot_sync(GPM_FULL, mine_ok), E = __ballot_sync(GPM_FULL, in_range);
+    st.skip += __popc(offered & ~E);
+
+    setup_window<false, true>(P, tile + P.tile_xo, ws, px, py, tile_x0, tile_y0, lane);
+    auto eval_row = [&](float nx, float ny, float nz, float nd, int r) {
+        eval_plane<1, false, GEO, true, true>(P, sCam, ws, src, nx, ny, nz, nd, inf, lane, st, Mr + r * V, Gr + r * V, 0u, g, fpx, fpy);
+    };
+    // (1) rows: 4 bits per candidate k name the row that holds its costs
+    eval_row(norm_now.x, norm_now.y, norm_now.z, norm_now.w, 8);
+    unsigned rows = 0u;
+    for (int k = 0; k < 8; k++) {
+        if (!((E >> k) & 1)) continue;
+        const unsigned cand_id = __shfl_sync(GPM_FULL, mine_id, k);
+        const unsigned earlier = __ballot_sync(GPM_FULL, (int)lane < k && in_range && mine_id == cand_id);
+        int r = k;
+        if (P.dedupe_self && cand_id == own_id) r = 8;
+        else if (P.dedupe_cand && earlier) r = (int)((rows >> (4 * (__ffs(earlier) - 1))) & 15u);
+        const float nx = __shfl_sync(GPM_FULL, mine.x, k), ny = __shfl_sync(GPM_FULL, mine.y, k);
+        const float nz = __shfl_sync(GPM_FULL, mine.z, k), nd = __shfl_sync(GPM_FULL, mine.w, k);
+        if (r == k) eval_row(nx, ny, nz, nd, k);
+        else st.skip++;
+        rows |= (unsigned)r << (4 * k);
+    }
+    __syncwarp();
+    // (2, 3) view statistics over E and the weights; the new selected-views mask is {j : w_j > 0}
+    auto weight = [&](int j) {
+        int good = 0, bad = 0;
+        float s = 0.0f;
+        for (int k = 0; k < 8; k++) {
+            if (!((E >> k) & 1)) continue;
+            const float m = Mr[(int)((rows >> (4 * k)) & 15u) * V + j];
+            if (m < J.tau_t) { good++;  s = fadd(s, fex2(fmul(fmul(m, m), J.kb))); }
+            if (m > J.tau_bad) bad++;
+        }
+        if (good >= J.n_good && bad < J.n_bad) return fdiv(s, __int2float_rn(good));
+        if (((remembered >> j) & 1ull) && bad < J.n_bad) return J.w_keep;
+        return 0.0f;
+    };
+    float w0 = 0.0f, w1 = 0.0f;
+    if ((int)lane < V) { w0 = weight((int)lane);  wv[lane] = w0; }
+    if ((int)lane + 32 < V) { w1 = weight((int)lane + 32);  wv[lane + 32] = w1; }
+    const unsigned long long selected = (unsigned long long)__ballot_sync(GPM_FULL, w0 > 0.0f) |
+                                        ((unsigned long long)__ballot_sync(GPM_FULL, w1 > 0.0f) << 32);
+    __syncwarp();
+    float wsum = 0.0f;
+    if (lane == 0) for (int j = 0; j < V; j++) wsum = fadd(wsum, wv[j]);
+    wsum = __shfl_sync(GPM_FULL, wsum, 0);
+    // (4) the cost of the hypothesis in row r
+    auto score = [&](int r) {
+        const float* m = Mr + r * V;
+        const float* gr = Gr + r * V;
+        if (wsum == 0.0f) {                          // no reliable view: today's NCC cost
+            float c0 = 0.0f, c1 = 0.0f;
+            if ((int)lane < V) c0 = GEO ? fadd(m[lane], gr[lane]) : m[lane];
+            if ((int)lane + 32 < V) c1 = GEO ? fadd(m[lane + 32], gr[lane + 32]) : m[lane + 32];
+            return combine_views(P, c0, c1, lane);
+        }
+        float num = 0.0f;
+        if (lane == 0) for (int j = 0; j < V; j++) num = fadd(num, fmul(wv[j], GEO ? fadd(m[j], gr[j]) : m[j]));
+        return __shfl_sync(GPM_FULL, fdiv(num, wsum), 0);
+    };
+    // (5) the fold: strict <, candidates in k order (gipuma.cu:867-871)
+    float cost_now = score(8);
+    float disp_now = plane_depth(cam, norm_now.x, norm_now.y, norm_now.z, norm_now.w, fpx, fpy);
+    for (int k = 0; k < 8; k++) {
+        if (!((E >> k) & 1)) continue;
+        const float c = score((int)((rows >> (4 * k)) & 15u));
+        float4 nb;
+        nb.x = __shfl_sync(GPM_FULL, mine.x, k);  nb.y = __shfl_sync(GPM_FULL, mine.y, k);
+        nb.z = __shfl_sync(GPM_FULL, mine.z, k);  nb.w = __shfl_sync(GPM_FULL, mine.w, k);
+        const float d = __shfl_sync(GPM_FULL, mine_disp, k);
+        const unsigned id = __shfl_sync(GPM_FULL, mine_id, k);
+        if (c < cost_now) { norm_now = nb;  cost_now = c;  disp_now = d;  own_id = id; }      // a copy keeps its identity
+    }
+    if (phase_mask & 4) {                            // planeRefinement_cu, gipuma.cu:928-994, scored with the same weights
+        bool any_accept = false;
+        Xorwow r = {0u, 0u, 0u, 0u, 0u, 0u};
+        if (P.rng_mode == 1) {
+            const unsigned* in = rng_state + center * 6;
+            r.v0 = in[0];  r.v1 = in[1];  r.v2 = in[2];  r.v3 = in[3];  r.v4 = in[4];  r.d = in[5];
+        }
+        float vx, vy, vz;
+        view_vector(cam, fpx, fpy, vx, vy, vz);
+        const float fb = fmul(cam.baseline, cam.f);
+        float deltaN = 1.0f;
+        for (float deltaZ = fmul(P.max_disp, 0.5f); deltaZ >= 0.01f; deltaZ = fmul(deltaZ, 0.1f)) {
+            const float rdisp = frcp(disp_now);
+            const float hi = fmin_(ffma(rdisp, -fb, P.max_disp), deltaZ);
+            const float lo = fmin_(ffma(rdisp, fb, P.min_disp), deltaZ);
+            const float dz = ffma(xorwow_uniform(r), fadd(lo, hi), -lo);
+            float dnew = ffma(rdisp, fb, dz);
+            dnew = fmin_(P.max_disp, fmax_(P.min_disp, dnew));
+            const float depth_new = fmul(frcp(dnew), fb);
+            const float twoN = fadd(deltaN, deltaN);
+            const float ax = fadd(norm_now.x, ffma(xorwow_uniform(r), twoN, -deltaN));
+            const float ay = fadd(norm_now.y, ffma(twoN, xorwow_uniform(r), -deltaN));
+            const float az = fadd(norm_now.z, ffma(twoN, xorwow_uniform(r), -deltaN));
+            const float rs = frsq(ffma(az, az, ffma(ax, ax, fmul(ay, ay))));
+            float4 cand;
+            cand.x = fmul(ax, rs);  cand.y = fmul(ay, rs);  cand.z = fmul(az, rs);
+            if (dot3(cand.x, cand.y, cand.z, vx, vy, vz) > 0.0f) { cand.x = -cand.x;  cand.y = -cand.y;  cand.z = -cand.z; }
+            cand.w = plane_d(cam, cand.x, cand.y, cand.z, fpx, fpy, depth_new);
+            eval_row(cand.x, cand.y, cand.z, cand.w, 8);
+            __syncwarp();
+            const float c = score(8);
+            if (c < cost_now) {                                                          // no depth-range test (:986-990)
+                any_accept = true;
+                cost_now = c;
+                disp_now = depth_new;
+                norm_now = cand;
+            }
+            deltaN = fmul(deltaN, 0.25f);
+        }
+        if (P.rng_mode == 1 && lane == 0) {
+            unsigned* o = rng_state + center * 6;
+            o[0] = r.v0;  o[1] = r.v1;  o[2] = r.v2;  o[3] = r.v3;  o[4] = r.v4;  o[5] = r.d;
+        }
+        if (any_accept) {                                 // a new plane: one fresh identity
+            unsigned fresh = 0u;
+            if (lane == 0) fresh = atomicAdd(M.next_id, 1u);
+            own_id = __shfl_sync(GPM_FULL, fresh, 0);
+        }
+    }
+    if (lane == 0) {
+        cost[center] = cost_now;
+        planes[center] = norm_now;
+        prov[center] = (unsigned char)GPM_PROV_JVS;
+        M.pid[center] = own_id;
+        J.mask[center] = selected;
+    }
+}
+
 // GEO: the cost with the geometric-consistency term (DESIGN.md §14; 8-neighbour sweep only); NCC: the NCC photometric cost
 // (§15; 8-neighbour sweep, grey images only).  G is only read in those variants.  ADAPTIVE: adaptive checkerboard sampling
-// (§16; 8-neighbour sweep), candidate k is acs_neighbour's choice instead of the fixed neighbour.
-template <bool COLOR, bool FUSED, bool GEO = false, bool NCC = false, bool ADAPTIVE = false>
+// (§16; 8-neighbour sweep), candidate k is acs_neighbour's choice instead of the fixed neighbour.  JVS: joint view
+// selection (§17; NCC only), every pixel goes through jvs_pixel; J is only read in those variants.
+template <bool COLOR, bool FUSED, bool GEO = false, bool NCC = false, bool ADAPTIVE = false, bool JVS = false>
 __global__ void __launch_bounds__(GPM_LB_THREADS, GPM_LB_BLOCKS)
 k_sweep(const __grid_constant__ KParams P, const __grid_constant__ CUtensorMap tmap, const ViewCam* __restrict__ cams,
         cudaTextureObject_t src, float4* __restrict__ planes, float* __restrict__ cost,
         unsigned* __restrict__ rng_state, unsigned char* __restrict__ prov, Memo M, int colour, int phase_mask,
-        unsigned long long* __restrict__ stats, const __grid_constant__ GeoParams G)
+        unsigned long long* __restrict__ stats, const __grid_constant__ GeoParams G, const JvsParams J)
 {
     static_assert(!(FUSED && GEO), "the geometric term is built for the 8-neighbour sweep only");
+    static_assert(!JVS || NCC, "joint view selection is built for the NCC cost (8-neighbour sweep, grey images) only");
     static_assert(!(NCC && (FUSED || COLOR)), "the NCC cost is built for the 8-neighbour sweep on grey images only");
     static_assert(!(FUSED && ADAPTIVE), "adaptive checkerboard sampling is built for the 8-neighbour sweep only");
     const GeoParams* g = (GEO || NCC) ? &G : nullptr;
@@ -273,13 +468,14 @@ k_sweep(const __grid_constant__ KParams P, const __grid_constant__ CUtensorMap t
     float* tile = smem;
     float* sCam = tile + tile_floats(P);
     float* scratch = smem + fixed_smem_floats(P);
-    int* counter = reinterpret_cast<int*>(scratch + (size_t)P.nwarps * warp_scratch_floats(P.ns_pad, P.V, P.color, NCC));
+    const int extra = JVS ? jvs_floats(P.V, GEO) : 0;
+    int* counter = reinterpret_cast<int*>(scratch + (size_t)P.nwarps * warp_scratch_floats(P.ns_pad, P.V, P.color, NCC, extra));
     const unsigned lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const int tile_x0 = blockIdx.x * GPM_TILE - P.halo, tile_y0 = blockIdx.y * GPM_TILE - P.halo;
     if (threadIdx.x == 0) counter[0] = P.nwarps;
-    stage_block(P, &tmap, cams, tile, sCam, tile_x0, tile_y0, 0u, NCC);
-    const WarpScratch ws = carve(scratch + (size_t)warp * warp_scratch_floats(P.ns_pad, P.V, P.color, NCC), P.ns_pad, P.V, P.color,
-                                 block_perm(P, smem, NCC), NCC);
+    stage_block(P, &tmap, cams, tile, sCam, tile_x0, tile_y0, 0u, NCC, extra);
+    float* warp_base = scratch + (size_t)warp * warp_scratch_floats(P.ns_pad, P.V, P.color, NCC, extra);
+    const WarpScratch ws = carve(warp_base, P.ns_pad, P.V, P.color, block_perm(P, smem, NCC, extra), NCC);
     const RefCam& cam = P.ref;
     WarpStats st = {0, 0, 0, 0, 0};
     const int W = P.W, H = P.H;
@@ -294,7 +490,11 @@ k_sweep(const __grid_constant__ KParams P, const __grid_constant__ CUtensorMap t
     while (idx < idx_end) {
         int px, py;
         colour_pixel(idx, colour, px, py);
-        if (px < W && py < H) {
+        if constexpr (JVS) {
+            if (px < W && py < H)
+                jvs_pixel<GEO, ADAPTIVE>(P, J, g, sCam, tile, ws, warp_base + warp_scratch_floats(P.ns_pad, P.V, P.color, NCC), src, planes,
+                                         cost, rng_state, prov, M, px, py, tile_x0, tile_y0, phase_mask, lane, st);
+        } else if (px < W && py < H) {
             const size_t center = (size_t)py * W + px;
             bool window_ready = false;          // the per-pixel window data is only built if something gets evaluated
             const float fpx = __int2float_rn(px), fpy = __int2float_rn(py);

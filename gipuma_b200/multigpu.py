@@ -106,16 +106,17 @@ def hybrid_layout(world: int, shard: int):
 
 def run_hybrid(make_scene: Callable[[int], object], n_reference_views: int, rank: int, world: int, shard: int,
                device: int = 0, on_result: Optional[Callable] = None, exchange: str = "nccl",
-               propagation: str = "fixed") -> List[float]:
+               propagation: str = "fixed", view_selection: str = "off") -> List[float]:
     """Reference views are dealt round-robin to world/shard groups; inside a group the source views are sharded and
     combined with one all-gather per stage over the group's own communicator (`exchange` must be "nccl").  `propagation`
-    as ViewShardRunner.  Returns wall seconds per reference view."""
+    and `view_selection` as ViewShardRunner.  Returns wall seconds per reference view."""
     import time
     import torch
     import torch.distributed as dist
     from . import api
     _check_exchange(exchange)
     api.check_propagation(propagation)
+    _check_view_selection(view_selection)
     group_of, rank_in, members = hybrid_layout(world, shard)
     groups = [dist.new_group(ranks=m) if world > 1 else None for m in members]     # every rank creates every group
     my_group = group_of[rank]
@@ -146,18 +147,28 @@ def _check_exchange(exchange: str):
         raise ValueError(f"unknown exchange {exchange!r}: the source-view shard exchanges with NCCL only")
 
 
+def _check_view_selection(view_selection: str):
+    from . import api
+    api.view_sel(view_selection)
+    if view_selection != "off":
+        raise ValueError("view_selection=%r: the source-view shard has no joint view selection (its exchange carries top-n "
+                         "lists, not per-view costs)" % (view_selection,))
+
+
 class ViewShardRunner:
     """One reference view, source views sharded over `world` ranks.  All device work runs behind the C-ABI
     (gpm_shard_run): one stage kernel + ncclAllGather per exchange stage.  `exchange` must be "nccl"; the attribute of
     the same name is "nccl", or "none" for a single rank.  torch.distributed is only used at set-up, to pass the NCCL
     unique id around.  `propagation` ("fixed" or "adaptive", api.Context.set_propagation) is set on every rank's context;
-    all ranks must pass the same."""
+    all ranks must pass the same.  `view_selection` must be "off": the exchange carries each rank's top-n lists, not the
+    per-view costs joint view selection needs (DESIGN.md §17)."""
 
     def __init__(self, scene, rank: int, world: int, device: int = 0, seed: int = 0xC0FFEE, group=None, options=None,
-                 exchange: str = "nccl", propagation: str = "fixed"):
+                 exchange: str = "nccl", propagation: str = "fixed", view_selection: str = "off"):
         from . import api
         _check_exchange(exchange)
         api.check_propagation(propagation)
+        _check_view_selection(view_selection)
         self.scene, self.rank, self.world, self.group = scene, rank, world, group
         self.local = partition_views(scene.n_views, world)[rank]
         if not self.local:

@@ -130,6 +130,39 @@ int gpm_set_photometric(gpm_ctx* ctx, int kind, float min_std);
 enum { GPM_PROP_FIXED = 0, GPM_PROP_ADAPTIVE = 1 };
 int gpm_set_propagation(gpm_ctx* ctx, int kind);
 
+/* ---- view selection (DESIGN.md §17) ------------------------------------------------------------------------------------
+ * GPM_VSEL_OFF (the default) scores every hypothesis by the combination rule of gpm_params (cost_comb, n_best): each
+ * hypothesis picks its own views.  GPM_VSEL_JOINT is the multi-hypothesis joint view selection of ACMH (Xu & Tao, CVPR
+ * 2019): per pixel and launch, the per-view NCC costs m[k][j] of the offered in-range candidates k decide one weight per
+ * view j.  With good_j = #{k : m < tau_t}, bad_j = #{k : m > tau_bad} and s_j the sum of exp(-m^2 / (2 beta^2)) over the good
+ * entries, w_j = s_j / good_j if good_j >= n_good and bad_j < n_bad; else w_keep if view j was selected at this pixel by the
+ * last JVS launch and bad_j < n_bad; else 0.  tau_t = tau_init * exp(-t^2 / alpha), where t counts the iterations of
+ * gpm_sweep since gpm_init or gpm_set_state.  Every hypothesis of the pixel, the current plane included, then costs
+ * sum_j w_j c_j / sum_j w_j (c_j = m_j + g_j with the geometric term), or the combination rule where every w_j is 0.  The
+ * selected-views masks are cleared by gpm_init, gpm_set_state and a switch from OFF to JOINT; a switch either way marks the
+ * stored costs stale.  NCC cost, grey images and the 8-neighbour sweep only; fixed or adaptive propagation, with or without
+ * the geometric term.
+ * Refused with GPM_E_ARG: a NULL `vsel`, an unknown kind; for JOINT, tau_init, alpha, tau_bad or beta not finite or <= 0,
+ * w_keep not finite or < 0, n_good outside 1..8, n_bad outside 1..9; JOINT with the PM cost, on a context holding colour
+ * images, or with option neighbours = 20 (and, while JOINT is on, gpm_set_photometric(GPM_PHOTO_PM), a colour image upload
+ * and neighbours = 20).  With GPM_E_STATE: every gpm_shard_* call taking a context while JOINT is on.  A refused call
+ * changes nothing. */
+enum { GPM_VSEL_OFF = 0, GPM_VSEL_JOINT = 1 };
+typedef struct gpm_view_sel {
+    int kind;                          /* GPM_VSEL_OFF or GPM_VSEL_JOINT */
+    float tau_init;                    /* starting good threshold (ACMH: 0.8) */
+    float alpha;                       /* how fast the good threshold shrinks (90) */
+    float tau_bad;                     /* bad threshold (1.2) */
+    int n_good;                        /* a view needs at least n_good good candidates (3) */
+    int n_bad;                         /* ... and fewer than n_bad bad ones (3) */
+    float beta;                        /* width of the confidence function (0.3) */
+    float w_keep;                      /* weight of a remembered view (0.2) */
+} gpm_view_sel;
+int gpm_set_view_selection(gpm_ctx* ctx, const gpm_view_sel* vsel);
+/* The selected-views mask of every pixel ([height*width], bit j = view j), host memory; all zero before the first JOINT
+ * launch. */
+int gpm_get_view_masks(gpm_ctx* ctx, unsigned long long* masks);
+
 /* Seed of the per-pixel curand_init(seed, y, x) at initialisation (gipuma.cu:1019; the reference uses
  * clock64()) and the refinement RNG mode. */
 int gpm_set_rng(gpm_ctx* ctx, unsigned long long seed, int mode);
@@ -318,6 +351,15 @@ typedef struct gpm_job_opts {
 } gpm_job_opts;
 int gpm_batch_run_opts(const gpm_batch_desc* desc, const gpm_job_opts* opts, gpm_batch_stats* stats);
 int gpm_geo_batch_run_opts(const gpm_geo_batch_desc* desc, const gpm_job_opts* opts, gpm_geo_batch_stats* stats);
+
+/* The batch drivers with a view selection (DESIGN.md §17): every job's context also gets gpm_set_view_selection(vsel) in
+ * the per-view setup (both passes of the geometric driver; pass 2 starts at t = 0 after its gpm_set_state).  vsel = NULL
+ * is GPM_VSEL_OFF: the _opts drivers are these with NULL.  Refused with GPM_E_ARG before any CUDA call, besides what the
+ * _opts drivers refuse: what gpm_set_view_selection refuses for its arguments, and JOINT with GPM_PHOTO_PM or with
+ * channels = 4. */
+int gpm_batch_run_vsel(const gpm_batch_desc* desc, const gpm_job_opts* opts, const gpm_view_sel* vsel, gpm_batch_stats* stats);
+int gpm_geo_batch_run_vsel(const gpm_geo_batch_desc* desc, const gpm_job_opts* opts, const gpm_view_sel* vsel,
+                           gpm_geo_batch_stats* stats);
 
 /* ---- depth-map fusion: the per-view world-frame outputs (norm4 of gpm_batch_run, or its .dmb files) -> one point cloud;
  * what the reference's scripts hand to the external `fusibile` (scripts/dtu_fast.sh:56-57).  Deterministic: the same inputs

@@ -1,9 +1,9 @@
 """Fused-cloud quality, convergence and sweep speed of adaptive checkerboard sampling (DESIGN.md §16) against the reference's
-fixed neighbours; prints one JSON line.
+fixed neighbours, and of joint view selection (§17) against the combination rule; prints one JSON line.
 
     python tools/acs_bench.py [--rows 600] [--cols 800] [--cams 16] [--iterations 6] [--geo-iterations 2]
                               [--converge 2,3,4,6] [--scenes smooth,hard,lit] [--costs pm,ncc] [--speed-iterations 4]
-                              [--dtu-preset]
+                              [--vsel off,joint] [--dtu-preset]
 
 Quality: tools/ncc_bench.py's workload (the first `--cams` DTU cameras at `--cols` x `--rows`, every second camera a reference
 view, box 11, n_best 3, depth 300..800, views at 5..45 degrees, at most 6 per reference; the same fusion and evaluate_cloud
@@ -16,7 +16,10 @@ Speed: sweep ms per iteration from CUDA events on gpm_stream around gpm_sweep(`-
 one-iteration warm-up, fixed against adaptive, PM and NCC, at 1600 x 1200 and 800 x 600 (10 views, box 15), with
 gpm_get_stats' hypotheses offered, skipped and (view, sample) pairs evaluated of the timed sweep.
 --dtu-preset adds a DTU-size batch: 49 cameras at 1600 x 1200, every camera a reference view, PM, one worker, fixed against
-adaptive, total sweep seconds.  Needs a CUDA device; there is no CPU path.
+adaptive, total sweep seconds.
+--vsel: the view selections to run with the NCC cost ("off", "joint" at api.JVS_DEFAULTS; PM runs "off" only): every NCC
+quality and speed row is repeated per view selection (keys "<cost> <propagation>" and "<cost> <propagation> joint"), and
+--dtu-preset adds NCC fixed without and with joint view selection.  Needs a CUDA device; there is no CPU path.
 """
 import argparse
 import json
@@ -43,6 +46,7 @@ def main():
     ap.add_argument("--scenes", default="smooth,hard,lit")
     ap.add_argument("--costs", default="pm,ncc")
     ap.add_argument("--speed-iterations", type=int, default=4)
+    ap.add_argument("--vsel", default="off")
     ap.add_argument("--dtu-preset", action="store_true")
     a = ap.parse_args()
     import torch
@@ -64,6 +68,12 @@ def main():
     converge = [int(x) for x in a.converge.split(",") if x]
     costs = {"pm": {}, "ncc": dict(photometric="ncc", ncc_min_std=api.NCC_MIN_STD)}
     costs = {k: costs[k] for k in a.costs.split(",") if k}
+    vsels = [v for v in a.vsel.split(",") if v]
+
+    def runs(cost):
+        """(key, propagation, view selection) of one cost: joint view selection is built for NCC only"""
+        return [("%s %s%s" % (cost, mode, "" if v == "off" else " " + v), mode, v) for mode in MODES
+                for v in (vsels if cost == "ncc" else ["off"])]
 
     def params(iterations):
         p = S.AlgorithmParameters(box_hsize=11, box_vsize=11, iterations=iterations, n_best=3, cost_comb=S.COMB_BEST_N, gamma=10.0)
@@ -102,21 +112,21 @@ def main():
                     "completeness_mean_units": round(s["completeness_mean"] / unit, 4), "f_score": [round(f, 4) for f in s["f_score"]]}
 
         for cost, photo in costs.items():
-            for mode in MODES:
+            for key, mode, vsel in runs(cost):
                 r = {}
                 for it in sorted(set(converge + [a.iterations])):
-                    n4, _, st = api.batch_run(images, Ps, params(it), refs, propagation=mode, **kw, **photo)
+                    n4, _, st = api.batch_run(images, Ps, params(it), refs, propagation=mode, view_selection=vsel, **kw, **photo)
                     sc = score(n4)
                     if it == a.iterations:
                         r["photometric"] = dict(sc, sweep_ms_per_iteration=round(st["sweep_ms_total"] / it, 2))
                     if it in converge:
                         r.setdefault("f_score_1unit_after_iterations", {})[it] = sc["f_score"][2]
                 n4, _, info = api.geometric_pass(images, Ps, params(a.iterations - a.geo_iterations), refs,
-                                                 geo_iterations=a.geo_iterations, propagation=mode, **kw, **photo)
+                                                 geo_iterations=a.geo_iterations, propagation=mode, view_selection=vsel, **kw, **photo)
                 r["with_geometric"] = dict(score(n4), pass2_sweep_ms_per_iteration=round(
                     1e3 * sum(info["pass2_sweep_s"]) / max(1, a.geo_iterations), 2))
-                res["%s %s" % (cost, mode)] = r
-                log("%s %s %s: %s" % (scene, cost, mode, r))
+                res[key] = r
+                log("%s %s: %s" % (scene, key, r))
         out[scene] = res
 
     speed = {}
@@ -125,12 +135,13 @@ def main():
         sc.params.box_hsize = sc.params.box_vsize = 15
         row = {}
         for cost in costs:
-            for mode in MODES:
+            for key, mode, vsel in runs(cost):
                 with api.Context(cols, rows, len(sc.subset)) as ctx:
                     ctx.load_scene(sc)
                     if cost == "ncc":
                         ctx.set_photometric("ncc", api.NCC_MIN_STD)
                     ctx.set_propagation(mode)
+                    ctx.set_view_selection(vsel)
                     ctx.init()
                     ctx.sweep(1)
                     stream = torch.cuda.ExternalStream(ctx.stream)
@@ -141,10 +152,14 @@ def main():
                     e1.record(stream)
                     e1.synchronize()
                     st = ctx.stats()
-                    row["%s %s" % (cost, mode)] = {"ms_per_iteration": round(e0.elapsed_time(e1) / a.speed_iterations, 3),
+                    row[key] = {"ms_per_iteration": round(e0.elapsed_time(e1) / a.speed_iterations, 3),
                                                    "offered": st["hypotheses"], "skipped": st["skipped"], "pairs": st["pairs"]}
             row["%s adaptive_over_fixed" % cost] = round(row["%s adaptive" % cost]["ms_per_iteration"] /
                                                          row["%s fixed" % cost]["ms_per_iteration"], 3)
+            if cost == "ncc" and "joint" in vsels:
+                for mode in MODES:
+                    row["ncc %s joint_over_off" % mode] = round(row["ncc %s joint" % mode]["ms_per_iteration"] /
+                                                                row["ncc %s" % mode]["ms_per_iteration"], 3)
         speed["%dx%d, 10 views, box 15" % (cols, rows)] = row
         log("speed %dx%d: %s" % (cols, rows, row))
     out["speed"] = speed
@@ -161,6 +176,15 @@ def main():
                                      max_angle=45.0, max_views=6, seed=4242, want_outputs=False, propagation=mode)
             dtu[mode] = {"sweep_s_total": round(st["sweep_ms_total"] / 1e3, 3), "wall_s": round(time.perf_counter() - t0, 2)}
         dtu["adaptive_over_fixed"] = round(dtu["adaptive"]["sweep_s_total"] / dtu["fixed"]["sweep_s_total"], 3)
+        if "joint" in vsels:
+            for vsel in ("off", "joint"):
+                t0 = time.perf_counter()
+                _, _, st = api.batch_run(images, allP, params(a.iterations), list(range(n)), cam_scale=1.0, min_angle=5.0,
+                                         max_angle=45.0, max_views=6, seed=4242, want_outputs=False, photometric="ncc",
+                                         ncc_min_std=api.NCC_MIN_STD, view_selection=vsel)
+                dtu["ncc fixed " + vsel] = {"sweep_s_total": round(st["sweep_ms_total"] / 1e3, 3),
+                                            "wall_s": round(time.perf_counter() - t0, 2)}
+            dtu["ncc joint_over_off"] = round(dtu["ncc fixed joint"]["sweep_s_total"] / dtu["ncc fixed off"]["sweep_s_total"], 3)
         out["dtu_preset"] = dict(dtu, workload="%d views at 1600x1200, PM, %d iterations, one worker" % (n, a.iterations))
         log("DTU preset: %s" % dtu)
     print(json.dumps(out))
