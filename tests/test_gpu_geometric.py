@@ -10,6 +10,7 @@
 - every refusal leaves the launch count and the state untouched;
 - the two-pass driver runs on the fusion test's dataset and its output fuses and scores."""
 import ctypes
+import time
 
 import numpy as np
 import pytest
@@ -25,8 +26,11 @@ WEIGHT, MAX_ERR = 0.3, 6.0
 
 
 def make_scene(rows, cols, views, box=9, color=False):
+    """A rendered scene: the DTU rig up to 10 source views, the templeRing rig (any number of views) above.  At 40 x 60 the
+    64-view synthetic rig (config 5) accepts almost no refinement, in every mode; the templeRing rig accepts thousands."""
     from gipuma_b200 import scene as S
-    sc = S.make_config(2, rows=rows, cols=cols, n_views=views, iterations=2, seed=rows * 1000 + cols)
+    cfg = 2 if views <= 10 else 4
+    sc = S.make_config(cfg, rows=rows, cols=cols, n_views=views, iterations=2, seed=rows * 1000 + cols)
     sc.params.box_hsize = sc.params.box_vsize = box
     return S.colorize(sc) if color else sc
 
@@ -127,13 +131,20 @@ def learn_rcp(k, s, combined):
     return rcp
 
 
-@pytest.mark.parametrize("rows,cols,color,comb,n_best", [(53, 75, False, 1, 2), (31, 33, False, 0, 2), (97, 65, False, 3, 2),
-                                                           (53, 75, True, 1, 3), (29, 41, True, 0, 2)])
-def test_cost_of_many_views_equals_the_restatement(rows, cols, color, comb, n_best):
+# rows, cols, views, colour, cost_comb, n_best: 33 and 64 views put a second view in every lane (views lane + 32)
+MANY = [(53, 75, 4, False, 1, 2), (31, 33, 4, False, 0, 2), (97, 65, 4, False, 3, 2), (53, 75, 4, True, 1, 3),
+        (29, 41, 4, True, 0, 2), (40, 60, 33, False, 1, 3), (40, 60, 33, True, 3, 2), (40, 60, 64, False, 0, 2),
+        (40, 60, 64, False, 3, 2), (40, 60, 64, True, 1, 40)]
+
+
+@pytest.mark.parametrize("rows,cols,views,color,comb,n_best", MANY)
+def test_cost_of_many_views_equals_the_restatement(rows, cols, views, color, comb, n_best):
     from oracle import pygeo
-    sc = make_scene(rows, cols, 4, color=color)
+    t0 = time.perf_counter()
+    sc = make_scene(rows, cols, views, color=color)
     sc.params.cost_comb, sc.params.n_best = comb, n_best
     depths = depth_maps(sc, rows + 7)
+    n_near = 0
     for planes in planes_to_score(sc, rows):
         photo = []
         for v in range(sc.n_views):
@@ -147,23 +158,38 @@ def test_cost_of_many_views_equals_the_restatement(rows, cols, color, comb, n_be
         s0, k0 = pygeo.combine_sum(photo, comb, n_best, sc.params.good_factor)
         rcp = learn_rcp(k0, s0, c0)
         assert bits_equal(pygeo.combine(photo, comb, n_best, sc.params.good_factor, rcp), c0) == 0
-        sums = np.stack([(photo[v] + restated_g(sc, planes, depths, v)).astype(f32) for v in range(sc.n_views)])
+        g = np.stack([restated_g(sc, planes, depths, v) for v in range(sc.n_views)])
+        sums = (photo + g).astype(f32)
         want = pygeo.combine(sums, comb, n_best, sc.params.good_factor, rcp)
         known = ~np.isnan(want)
         assert known.mean() > 0.98, known.mean()
         assert bits_equal(got[known], want[known]) == 0, (rows, cols, comb, np.argwhere((got != want) & known)[:5])
+        n_near += int((g[32:] < f32(WEIGHT) * f32(MAX_ERR)).sum())
+    if views > 32:
+        assert n_near > 0                         # views lane + 32 are scored by an actual reprojection error
+    print("\ngeometric cost, %dx%d, %d views, colour %s, comb %d, n_best %d: %d near views >= 32, %.2f s" %
+          (rows, cols, views, color, comb, n_best, n_near, time.perf_counter() - t0))
 
 
-@pytest.mark.parametrize("rows,cols,color", [(53, 75, False), (97, 65, False), (53, 75, True), (31, 33, True)])
-def test_sweep_decisions_exact(rows, cols, color):
+# box 15: 64 samples, two rounds, so the lower bound is tested; box 25: six rounds; box 3: one round of 4 samples, the
+# lower bound has nothing to cut short
+@pytest.mark.parametrize("rows,cols,views,box,color", [(53, 75, 4, 15, False), (97, 65, 4, 15, False), (53, 75, 4, 15, True),
+                                                       (31, 33, 4, 15, True), (40, 60, 33, 3, False), (40, 60, 33, 25, False),
+                                                       (40, 60, 64, 3, False), (40, 60, 64, 25, False), (40, 60, 64, 25, True)])
+def test_sweep_decisions_exact(rows, cols, views, box, color):
     from oracle import pypropagate as pp
-    sc = make_scene(rows, cols, 4, box=15, color=color)         # 64 samples: two rounds, so the lower bound is tested
+    t0 = time.perf_counter()
+    sc = make_scene(rows, cols, views, box=box, color=color)
     depths = depth_maps(sc, 3)
     seed = 4000 + rows + cols
     ctxs = [open_ctx(sc, seed, depths, WEIGHT),
             open_ctx(sc, seed, depths, WEIGHT, options={"memo": 0, "prune": 0, "dedupe": 0}),
             open_ctx(sc, seed, depths, WEIGHT)]
+    # at many views or the largest window the host picks fewer than 16 warps: a twin at another count holds the same bits
+    if views > 32 or box == 25:
+        ctxs.append(open_ctx(sc, seed, depths, WEIGHT, options={"nwarps": 3 if views == 64 else 7}))
     A = ctxs[0]
+    stepped = ctxs[1:2] + ctxs[3:]
     f = cost_of(A)
     cam = sc.cameras[0]
     ys, xs = np.mgrid[0:sc.rows, 0:sc.cols]
@@ -183,8 +209,12 @@ def test_sweep_decisions_exact(rows, cols, color):
                         want_p, want_c, amb = pp.expected(before[0], before[1], colour, mask, f, cam, sc.params.depthMin,
                                                           sc.params.depthMax, color_images=color)
                     A.phase(colour, mask)
-                    ctxs[1].phase(colour, mask)
                     after = A.get_state()
+                    for other in stepped:
+                        other.phase(colour, mask)
+                    for other in ctxs[3:]:                          # the warp-count twin, launch by launch
+                        p, c = other.get_state()
+                        assert bits_equal(p, after[0]) == 0 and bits_equal(c, after[1]) == 0, ("nwarps", colour, mask)
                     if mask != 4:
                         bad = ((after[0].view(np.uint32) != want_p.view(np.uint32)).any(axis=-1) |
                                (after[1].view(np.uint32) != want_c.view(np.uint32))) & ~amb
@@ -206,9 +236,15 @@ def test_sweep_decisions_exact(rows, cols, color):
         for ctx in ctxs:
             ctx.close()
     share = stats["ambiguous"] / max(1, stats["compared"] + stats["ambiguous"])
-    print("\ngeometric %dx%d colour=%s: %s, ambiguous %.4f, pruned %d of %d" % (rows, cols, color, stats, share, st["pruned"], st["hypotheses"]))
+    print("\ngeometric %dx%d, %d views, box %d, colour=%s: %s, ambiguous %.4f, pruned %d of %d, %.2f s" %
+          (rows, cols, views, box, color, stats, share, st["pruned"], st["hypotheses"], time.perf_counter() - t0))
     assert stats["accepted"] > 0 and stats["refined"] > 0 and share <= 0.005
-    assert st["pruned"] > 0                       # the lower bound with the geometric term does cut hypotheses short
+    ns = ((box - 1) // 2 + 1) ** 2
+    assert st["pairs_full"] == st["hypotheses"] * views * ns           # box 25: 169 samples, 5 x 32 + 9, six rounds
+    if ns > 32:
+        assert st["pruned"] > 0                   # the lower bound with the geometric term does cut hypotheses short
+    else:
+        assert st["pruned"] == 0                  # one round: the bound is the final cost
 
 
 def test_refusals_leave_launch_count_and_state_untouched():

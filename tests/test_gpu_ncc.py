@@ -14,6 +14,7 @@
   one is test_gpu_geometric_batch's restatement on NCC contexts), on the fusion test's dataset and a ragged one, with one and
   two workers, and the NCC cloud beats the PM cloud on the fusion test's dataset under a per-view gain and offset."""
 import ctypes
+import time
 from types import SimpleNamespace
 
 import numpy as np
@@ -92,7 +93,19 @@ def translation_cam(sx, sy):
     return g, ns
 
 
-SHIFTS = [(4, 0), (-8, 4), (0, -4), (12, 8)]
+def _rig(n=64, seed=2024):
+    """Shifts and (gain, offset) of up to GPM_MAX_VIEWS = 64 views: four fixed ones, then distinct even shifts in
+    [-8, 8]^2 (even: the d = -2 and -0.5 planes stay on integer texels) with a seeded gain and offset each."""
+    rng = np.random.default_rng(seed)
+    shifts = [(4, 0), (-8, 4), (0, -4), (12, 8)]
+    light = [(1.0, 0.0), (2.0, -60.0), (0.5, 17.0), (1.0, 0.0)]
+    pool = [(x, y) for x in range(-8, 9, 2) for y in range(-8, 9, 2) if (x, y) != (0, 0) and (x, y) not in shifts]
+    shifts += [pool[i] for i in rng.permutation(len(pool))[:n - 4]]
+    light += [(float(rng.uniform(0.5, 2.0)), float(rng.uniform(-60.0, 40.0))) for _ in range(n - 4)]
+    return shifts, light
+
+
+SHIFTS, LIGHT = _rig()
 
 
 def translation_case(rows, cols, views, box, seed):
@@ -104,8 +117,8 @@ def translation_case(rows, cols, views, box, seed):
     for v in range(views):
         sx, sy = SHIFTS[v]
         src = ref[np.clip(ys - sy, 0, rows - 1), np.clip(xs - sx, 0, cols - 1)]          # content of ref moved by (sx, sy)
-        gain, off = [(1.0, 0.0), (2.0, -60.0), (0.5, 17.0), (1.0, 0.0)][v]
-        img = np.clip(gain * src + off + rng.integers(-20, 21, src.shape) * (v == 3), 0, 255)
+        gain, off = LIGHT[v]
+        img = np.clip(gain * src + off + rng.integers(-20, 21, src.shape) * (v % 4 == 3), 0, 255)       # noise on every 4th
         imgs.append(np.floor(img).astype(f32))
     p = S.AlgorithmParameters(box_hsize=box, box_vsize=box, iterations=1, n_best=2, cost_comb=S.COMB_BEST_N, gamma=1e30)
     p.depthMin, p.depthMax = 0.1, 100.0
@@ -144,7 +157,12 @@ def restated_translation(ref, imgs, planes, box, views, min_std=MIN_STD):
     return np.stack(out)
 
 
-@pytest.mark.parametrize("box", [11, 15])
+def ns_of(box):
+    """Samples of a propagation window: box 3 is one 4-sample round, 11 is 32 + 4, 15 is 32 + 32, 25 is 5 x 32 + 9."""
+    return ((box - 1) // 2 + 1) ** 2
+
+
+@pytest.mark.parametrize("box", [3, 11, 15, 25])
 def test_cost_of_one_view_is_bit_exact(box):
     ref, imgs, p, planes = translation_case(45, 70, 1, box, box)
     with translation_ctx(ref, imgs, p, 1) as ctx:
@@ -154,31 +172,44 @@ def test_cost_of_one_view_is_bit_exact(box):
     assert 0.05 < (want < 0.5).mean() < 0.999                          # correlated windows and others
 
 
-@pytest.mark.parametrize("box,comb,geo", [(15, 1, False), (11, 0, False), (15, 3, False), (11, 1, True)])
-def test_cost_of_many_views_is_bit_exact(box, comb, geo):
+# views, box, cost_comb, n_best, geometric term: 33 and 64 views put a second view in every lane (views lane + 32)
+MANY = [(4, 15, 1, 2, False), (4, 11, 0, 2, False), (4, 15, 3, 2, False), (4, 11, 1, 2, True),
+        (33, 3, 1, 2, False), (64, 25, 1, 3, False), (64, 11, 1, 40, False), (40, 15, 0, 2, False), (40, 15, 3, 2, False),
+        (64, 9, 1, 3, True), (33, 25, 0, 2, True)]
+
+
+@pytest.mark.parametrize("views,box,comb,n_best,geo", MANY)
+def test_cost_of_many_views_is_bit_exact(views, box, comb, n_best, geo):
     from oracle import pygeo
-    ref, imgs, p, planes = translation_case(45, 70, 4, box, 100 + box + comb)
-    p.cost_comb = comb
-    per_view = restated_translation(ref, imgs, planes, box, 4)
-    with translation_ctx(ref, imgs, p, 4) as ctx:
+    t0 = time.perf_counter()
+    ref, imgs, p, planes = translation_case(45, 70, views, box, 100 + box + comb + views)
+    p.cost_comb, p.n_best = comb, n_best
+    per_view = restated_translation(ref, imgs, planes, box, views)
+    if views > 32:          # a view read in place of its lane partner (j <-> j - 32) would change the sums
+        assert (per_view[32:] != per_view[:views - 32]).mean() > 0.5
+    with translation_ctx(ref, imgs, p, views) as ctx:
         c0 = ctx.cost_eval(planes)
-        s0, k0 = pygeo.combine_sum(per_view, comb, p.n_best, p.good_factor)
+        s0, k0 = pygeo.combine_sum(per_view, comb, n_best, p.good_factor)
         rcp = learn_rcp(k0, s0, c0)
-        assert bits_equal(pygeo.combine(per_view, comb, p.n_best, p.good_factor, rcp), c0) == 0
+        assert bits_equal(pygeo.combine(per_view, comb, n_best, p.good_factor, rcp), c0) == 0
         if geo:
-            depths = [np.full(ref.shape, 5.0, f32) * (1 + 0.1 * v) for v in range(4)]
+            depths = [np.full(ref.shape, 5.0, f32) * (1 + 0.1 * v) for v in range(views)]
             depths[1][::3] = 0.0
-            for v in range(4):
+            for v in range(views):
                 ctx.set_view_depth(v, depths[v])
             ctx.set_geometric(WEIGHT, MAX_ERR)
             got = ctx.cost_eval(planes)
             rc = translation_cam(0, 0)[1]
             g = np.stack([pygeo.geo_cost(planes, rc, translation_cam(*SHIFTS[v])[1], depths[v], WEIGHT, MAX_ERR,
-                                         p.depthMin, p.depthMax) for v in range(4)])
-            want = pygeo.combine((per_view + g).astype(f32), comb, p.n_best, p.good_factor, rcp)
+                                         p.depthMin, p.depthMax) for v in range(views)])
+            want = pygeo.combine((per_view + g).astype(f32), comb, n_best, p.good_factor, rcp)
             known = ~np.isnan(want)
             assert known.mean() > 0.98 and bits_equal(got[known], want[known]) == 0
             assert (g < f32(WEIGHT * MAX_ERR)).any()
+            if views > 32:
+                assert (g[32:] < f32(WEIGHT * MAX_ERR)).any()               # views lane + 32 score a real error
+    print("\nNCC translation rig, %d views, box %d, comb %d, n_best %d, geo %s: %.2f s" %
+          (views, box, comb, n_best, geo, time.perf_counter() - t0))
 
 
 # ---- 3, 4. general scenes: float64 tolerance and gain invariance ----------------------------------------------------
@@ -256,16 +287,23 @@ def test_gain_and_offset_move_ncc_within_tolerance_and_pm_far():
 
 
 # ---- 5. decisions ---------------------------------------------------------------------------------------------------
-@pytest.mark.parametrize("rows,cols,geo", [(53, 75, False), (97, 65, False), (53, 75, True), (31, 33, True)])
-def test_sweep_decisions_exact(rows, cols, geo):
+@pytest.mark.parametrize("rows,cols,views,box,geo", [(53, 75, 4, 15, False), (97, 65, 4, 15, False), (53, 75, 4, 15, True),
+                                                     (31, 33, 4, 15, True), (40, 60, 33, 3, False), (40, 60, 33, 25, True),
+                                                     (40, 60, 64, 3, True), (40, 60, 64, 25, False)])
+def test_sweep_decisions_exact(rows, cols, views, box, geo):
     from oracle import pypropagate as pp
-    sc = make_scene(rows, cols, 4, box=15)
+    t0 = time.perf_counter()
+    sc = make_scene(rows, cols, views, box=box)
     depths = depth_maps(sc, 3) if geo else None
     wgt = WEIGHT if geo else 0.0
     seed = 5000 + rows + cols
     ctxs = [ncc_ctx(sc, seed, depths, wgt), ncc_ctx(sc, seed, depths, wgt, options={"memo": 0, "dedupe": 0}),
             ncc_ctx(sc, seed, depths, wgt)]
+    # at many views or the largest window the host picks fewer than 16 warps: a twin at another count holds the same bits
+    if views > 32 or box == 25:
+        ctxs.append(ncc_ctx(sc, seed, depths, wgt, options={"nwarps": 3 if views == 64 else 7}))
     A = ctxs[0]
+    stepped = ctxs[1:2] + ctxs[3:]
     f = cost_of(A)
     cam = sc.cameras[0]
     ys, xs = np.mgrid[0:sc.rows, 0:sc.cols]
@@ -274,7 +312,9 @@ def test_sweep_decisions_exact(rows, cols, geo):
         for ctx in ctxs:
             ctx.init()
         n0, c0 = A.get_state()
-        assert np.all((c0 >= 0) & (c0 <= 2 + WEIGHT * MAX_ERR))
+        # an NCC cost in [0, 2] plus a geometric term in [0, weight * max_err], up to the float32 roundings of the sum and
+        # of the mean (at box 3 whole windows are flat, NCC 2, and project nowhere, g = weight * max_err)
+        assert np.all((c0 >= 0) & (c0 <= (2 + WEIGHT * MAX_ERR) * (1 + 2 ** -20)))
         for ctx in ctxs[1:]:
             assert bits_equal(ctx.get_state()[0], n0) == 0 and bits_equal(ctx.get_state()[1], c0) == 0
         A.reset_stats()
@@ -286,8 +326,12 @@ def test_sweep_decisions_exact(rows, cols, geo):
                         want_p, want_c, amb = pp.expected(before[0], before[1], colour, mask, f, cam, sc.params.depthMin,
                                                           sc.params.depthMax)
                     A.phase(colour, mask)
-                    ctxs[1].phase(colour, mask)
                     after = A.get_state()
+                    for other in stepped:
+                        other.phase(colour, mask)
+                    for other in ctxs[3:]:                          # the warp-count twin, launch by launch
+                        p, c = other.get_state()
+                        assert bits_equal(p, after[0]) == 0 and bits_equal(c, after[1]) == 0, ("nwarps", colour, mask)
                     if mask != 4:
                         bad = ((after[0].view(np.uint32) != want_p.view(np.uint32)).any(axis=-1) |
                                (after[1].view(np.uint32) != want_c.view(np.uint32))) & ~amb
@@ -309,9 +353,11 @@ def test_sweep_decisions_exact(rows, cols, geo):
         for ctx in ctxs:
             ctx.close()
     share = stats["ambiguous"] / max(1, stats["compared"] + stats["ambiguous"])
-    print("\nNCC %dx%d geo=%s: %s, ambiguous %.4f, %s" % (rows, cols, geo, stats, share, st))
+    print("\nNCC %dx%d, %d views, box %d, geo=%s: %s, ambiguous %.4f, %s, %.2f s" %
+          (rows, cols, views, box, geo, stats, share, st, time.perf_counter() - t0))
     assert stats["accepted"] > 0 and stats["refined"] > 0 and share <= 0.005
     assert st["pruned"] == 0 and st["pairs"] == st["pairs_full"]          # no early-out on NCC costs
+    assert st["pairs_full"] == st["hypotheses"] * views * ns_of(box)      # every hypothesis ran all rounds_of(box) rounds
 
 
 # ---- 6. refusals ----------------------------------------------------------------------------------------------------

@@ -24,11 +24,14 @@ EXACT = {"beta": 1e30}
 # is then off by a relative delta <= 2^-21 after the roundings; a weighted mean sum w c / sum w moves by at most
 # 2 delta max|c_j - mean| <= 2 delta * 4 (c_j = NCC + geometric term <= 2 + WEIGHT * MAX_ERR < 4), and the two sequential
 # sums of up to V terms, on inputs that differ in the last bits, may round differently by V ulp of 4.  With V <= 10:
-# 8 * 2^-21 + 10 * 4 * 2^-23 < 9e-6.  TOL keeps a factor of 10 on top.
+# 8 * 2^-21 + 10 * 4 * 2^-23 < 9e-6, a factor of 10 under TOL; at GPM_MAX_VIEWS = 64: 8 * 2^-21 + 64 * 4 * 2^-23 < 3.5e-5, a
+# factor of 2.9 under TOL.
 TOL = 1e-4
 REPORT = {}
 
-# id: (rows, cols, views, box, geometric term, adaptive propagation, sweeps before the checked launches)
+# id: (rows, cols, views, box, geometric term, adaptive propagation, sweeps before the checked launches[, parameters over
+# EXACT]).  33 and 64 views put a second view in every lane (views lane + 32) and the upper half in the 64-bit masks; at
+# 64 views and box 25 with the geometric term each warp keeps the largest scratch of any kernel.
 CASES = {
     "fixed_53x75": (53, 75, 4, 15, False, False, 0),
     "adaptive_53x75_t2": (53, 75, 4, 15, False, True, 2),
@@ -37,16 +40,37 @@ CASES = {
     "fixed_8x8": (8, 8, 2, 9, False, False, 0),
     "adaptive_31x33_t5": (31, 33, 3, 11, False, True, 5),
     "adaptive_550x1000_t1": (550, 1000, 3, 9, False, True, 1),
+    "fixed_33v_box25": (40, 60, 33, 25, False, False, 0),
+    "geo_adaptive_64v_box3": (40, 60, 64, 3, True, True, 0),
+    "geo_fixed_64v_box25": (40, 60, 64, 25, True, False, 0),
+    "fixed_1v_good1_t2": (53, 75, 1, 15, False, False, 2, {"n_good": 1}),
+    "fixed_1v_t2": (53, 75, 1, 15, False, False, 2),
 }
+MANY = ["fixed_33v_box25", "geo_adaptive_64v_box3", "geo_fixed_64v_box25"]
 TWINS = [{"memo": 0}, {"prune": 0}, {"dedupe": 0}]
 
 
 def make_scene(case):
-    from gipuma_b200 import scene as S
-    rows, cols, views, box = CASES[case][:4]
-    sc = S.make_config(2, rows=rows, cols=cols, n_views=views, iterations=2, seed=rows * 1000 + cols)
-    sc.params.box_hsize = sc.params.box_vsize = box
-    return sc
+    import test_gpu_geometric as tg
+    return tg.make_scene(*CASES[case][:4])
+
+
+def exact(case):
+    """EXACT with the case's own parameters on top."""
+    return dict(EXACT, **(CASES[case][7] if len(CASES[case]) > 7 else {}))
+
+
+def twins_of(case):
+    """The twins' options; at many views or the largest window the host picks fewer than 16 warps, so one more twin runs
+    at another warp count."""
+    views, box = CASES[case][2:4]
+    return TWINS + ([{"nwarps": 3 if views == 64 else 7}] if views > 32 or box == 25 else [])
+
+
+def upper_masks_reached(masks):
+    """Bits >= 32 set, and not the same set at every pixel."""
+    hi = np.asarray(masks, np.uint64) >> np.uint64(32)
+    return bool((hi != 0).any()) and len(np.unique(hi)) > 1
 
 
 def open_jvs(case, sc, seed, options=None, params=EXACT, kind="joint"):
@@ -153,11 +177,10 @@ def chain(case, sc, A, twins, rows, t, params=EXACT, tol=None, masks=(1, 2, 3, 4
             stats["compared"] += n
             stats["ambiguous"] += a
             stats["refined" if mask == 4 else "accepted"] += acc
+            ref = state(A)
             for ctx in twins:
                 ctx.phase(colour, mask)
-        ref = state(A)
-        for ctx in twins:
-            assert same_state(state(ctx), ref), ("twin", colour)
+                assert same_state(state(ctx), ref), ("twin", colour, mask)
     return stats
 
 
@@ -167,8 +190,8 @@ def test_jvs_launches_exact(case):
     sc = make_scene(case)
     sweeps = CASES[case][6]
     seed = 7000 + sc.rows + sc.cols
-    A = open_jvs(case, sc, seed)
-    twins = [open_jvs(case, sc, seed, o) for o in TWINS]
+    A = open_jvs(case, sc, seed, params=exact(case))
+    twins = [open_jvs(case, sc, seed, o, params=exact(case)) for o in twins_of(case)]
     rows = Rows(case, sc)
     try:
         for ctx in [A] + twins:
@@ -178,9 +201,11 @@ def test_jvs_launches_exact(case):
         if sweeps:
             assert A.view_masks().any()
         A.reset_stats()
-        st = chain(case, sc, A, twins, rows, sweeps)
+        st = chain(case, sc, A, twins, rows, sweeps, params=exact(case))
         s = A.stats()
         assert s["pruned"] == 0 and (s["skipped"] > 0 or sc.rows * sc.cols < 1000)
+        if sc.n_views > 32:
+            assert upper_masks_reached(A.view_masks())
     finally:
         rows.close()
         for ctx in [A] + twins:
@@ -205,11 +230,12 @@ def hostile(sc, A, rng):
     return pl, cost.astype(f32)
 
 
-@pytest.mark.parametrize("case", ["fixed_53x75", "adaptive_53x75_t2", "geo_adaptive_45x71"])
+@pytest.mark.parametrize("case", ["fixed_53x75", "adaptive_53x75_t2", "geo_adaptive_45x71"] + MANY)
 def test_jvs_launches_exact_on_adversarial_states(case):
+    t0 = time.perf_counter()
     sc = make_scene(case)
-    A = open_jvs(case, sc, 77)
-    twins = [open_jvs(case, sc, 77, o) for o in TWINS]
+    A = open_jvs(case, sc, 77, params=exact(case))
+    twins = [open_jvs(case, sc, 77, o, params=exact(case)) for o in twins_of(case)]
     rows = Rows(case, sc)
     try:
         A.init()
@@ -217,18 +243,20 @@ def test_jvs_launches_exact_on_adversarial_states(case):
         for ctx in [A] + twins:
             ctx.set_state(pl, cost)
         assert not A.view_masks().any()                      # gpm_set_state clears the masks (and t)
-        st = chain(case, sc, A, twins, rows, 0)
-        st2 = chain(case, sc, A, twins, rows, 0)             # now with remembered views
+        st = chain(case, sc, A, twins, rows, 0, params=exact(case))
+        if sc.n_views > 32:
+            assert upper_masks_reached(A.view_masks())
+        st2 = chain(case, sc, A, twins, rows, 0, params=exact(case))   # now with remembered views
     finally:
         rows.close()
         for ctx in [A] + twins:
             ctx.close()
     assert st["accepted"] + st2["accepted"] > 0
-    REPORT["adversarial_" + case] = (st, st2)
-    print("\nadversarial %s: %s %s" % (case, st, st2))
+    REPORT["adversarial_" + case] = (st, st2, round(time.perf_counter() - t0, 2))
+    print("\nadversarial %s: %s" % (case, REPORT["adversarial_" + case]))
 
 
-@pytest.mark.parametrize("case", ["fixed_53x75", "geo_adaptive_45x71"])
+@pytest.mark.parametrize("case", ["fixed_53x75", "geo_adaptive_45x71", "geo_adaptive_64v_box3"])
 def test_jvs_launches_within_the_ex2_tolerance(case):
     """beta = 0.3 (the default): the device's MUFU.EX2 and numpy's exp2 differ in the last bits, so costs agree within TOL
     and decisions wherever every pair of competing weighted costs is more than 2 TOL apart."""
@@ -244,7 +272,9 @@ def test_jvs_launches_within_the_ex2_tolerance(case):
         rows.close()
         A.close()
     total = st["compared"] + st["ambiguous"]
-    assert st["accepted"] > 0 and st["ambiguous"] <= 0.02 * total, st
+    # a weighted mean over 64 views puts competing scores closer together, so more decisions fall within 2 TOL of each
+    # other: 3.3 % of the pixels on an H100 80GB HBM3 (700 W) at 64 views, under 2 % at 4
+    assert st["accepted"] > 0 and st["ambiguous"] <= (0.05 if sc.n_views > 32 else 0.02) * total, st
     REPORT["tolerance_" + case] = st
     print("\ntolerance %s: %s" % (case, st))
 
