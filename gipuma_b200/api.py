@@ -311,14 +311,13 @@ def view_sel(kind: str = "off", **params) -> GpmViewSel:
                       int(p["n_bad"]), float(p["beta"]), float(p["w_keep"]))
 
 
-def check_view_selection(kind: str, photometric: str, channels: int = 1, **params) -> GpmViewSel:
-    """view_sel plus what the batch drivers refuse for the combination: "joint" needs the NCC cost and grey images."""
-    v = view_sel(kind, **params)
-    if kind == "joint" and photometric != "ncc":
+def check_modes(photometric: str, view_selection: str, channels: int = 1):
+    """The mode rules the batch drivers refuse a combination by (include/gipuma_b200.h, mode compatibility), checked before
+    any call into the library: "joint" view selection needs the NCC cost, and both need grey images (channels 1)."""
+    if view_selection == "joint" and photometric != "ncc":
         raise ValueError("view_selection='joint' is built for the NCC cost (photometric='ncc')")
-    if kind == "joint" and channels == 4:
-        raise ValueError("view_selection='joint' supports grey images only")
-    return v
+    if photometric == "ncc" and channels == 4:
+        raise ValueError("the NCC photometric cost supports grey images only")
 
 
 def job_opts(photometric: str = "pm", ncc_min_std: float = NCC_MIN_STD, propagation: str = "fixed") -> GpmJobOpts:
@@ -646,7 +645,8 @@ def batch_run(images, Ps, params, refs, devices=(0,), cam_scale: float = 1.0, mi
     (Context.set_view_selection; "joint" needs photometric="ncc").
     Returns (norm4 [len(refs), H, W, 4] or None, cost or None, stats dict)."""
     opts = job_opts(photometric, ncc_min_std, propagation)
-    vsel = check_view_selection(view_selection, photometric, 1, **(jvs_params or {}))
+    vsel = view_sel(view_selection, **(jvs_params or {}))
+    check_modes(photometric, view_selection, 1)
     lib = load_library()
     imgs = np.ascontiguousarray(images, dtype=np.float32)
     n, H, W = imgs.shape
@@ -691,9 +691,8 @@ def geometric_pass(images, Ps, params, refs, geo_iterations: int = 2, weight: fl
     imgs = np.ascontiguousarray(images, dtype=np.float32)
     if imgs.ndim not in (3, 4) or (imgs.ndim == 4 and imgs.shape[3] != 4):
         raise ValueError("images must be [n, H, W] or [n, H, W, 4]")
-    vsel = check_view_selection(view_selection, photometric, 4 if imgs.ndim == 4 else 1, **(jvs_params or {}))
-    if photometric == "ncc" and imgs.ndim == 4:
-        raise ValueError("the NCC photometric cost supports grey images only")
+    vsel = view_sel(view_selection, **(jvs_params or {}))
+    check_modes(photometric, view_selection, 4 if imgs.ndim == 4 else 1)
     n, H, W = imgs.shape[:3]
     if len(Ps) != n:
         raise ValueError("one projection matrix per image is needed (%d images, %d matrices)" % (n, len(Ps)))

@@ -16,12 +16,15 @@
 #include "gpm_kernels.cuh"
 
 #include <algorithm>
+#include <array>
 #include <cctype>
 #include <cmath>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
 #include <string>
+#include <type_traits>
+#include <utility>
 #include <vector>
 
 using namespace gpm;
@@ -170,11 +173,10 @@ int reset_state_tags(gpm_ctx* c, int prov)
     return GPM_OK;
 }
 
-// the geometric-consistency mode's own preconditions at weight `weight` (the fused sweep and a missing depth map)
-int check_geometric(const gpm_ctx* c, float weight)
+// the geometric-consistency mode's precondition at weight `weight`: a depth map for every used source view
+int check_depth_maps(const gpm_ctx* c, float weight)
 {
     if (weight <= 0.f) return GPM_OK;
-    if (c->opt_neighbours == 20) return fail(GPM_E_ARG, "the geometric-consistency mode supports the 8-neighbour sweep only (option neighbours = 8)");
     for (int v = 0; v < c->V; v++)
         if (!c->have_depth[v]) return fail(GPM_E_STATE, "geometric-consistency mode: source view " + std::to_string(v) + " has no depth map (gpm_set_view_depth)");
     return GPM_OK;
@@ -182,6 +184,35 @@ int check_geometric(const gpm_ctx* c, float weight)
 
 bool ncc_on(const gpm_ctx* c) { return c->photo == GPM_PHOTO_NCC; }
 bool jvs_on(const gpm_ctx* c) { return c->vsel.kind == GPM_VSEL_JOINT; }
+
+// The context's sweep mode.  Every setter of one of its fields refuses a change that mode_conflict() would not pass, so it
+// always names a mode with kernels.
+Mode ctx_mode(const gpm_ctx* c)
+{
+    return Mode{c->color == 1, c->opt_neighbours == 20, c->geo_weight > 0.f, ncc_on(c), c->propagation == GPM_PROP_ADAPTIVE, jvs_on(c)};
+}
+
+const char* conflict_text(ModeConflict k)
+{
+    switch (k) {
+    case ModeConflict::fused: return "the geometric-consistency mode, the NCC cost, adaptive sampling and joint view selection support the 8-neighbour sweep only (option neighbours = 8)";
+    case ModeConflict::jvs_needs_ncc_grey: return "joint view selection is built for the NCC cost (GPM_PHOTO_NCC) on grey images";
+    case ModeConflict::ncc_colour: return "the NCC photometric cost supports grey images only";
+    default: return nullptr;
+    }
+}
+
+// Refuses the call `fn` if setting `field` of the context's mode to `on` gives a mode mode_conflict() does not pass.  Such a
+// refusal is GPM_E_ARG, but GPM_E_STATE for a colour image upload while only the NCC cost is on (include/gipuma_b200.h).
+int refuse_change(const gpm_ctx* c, const char* fn, bool Mode::*field, bool on)
+{
+    Mode m = ctx_mode(c);
+    m.*field = on;
+    const ModeConflict k = mode_conflict(m);
+    if (k == ModeConflict::none) return GPM_OK;
+    return fail(field == &Mode::color && k == ModeConflict::ncc_colour ? GPM_E_STATE : GPM_E_ARG, std::string(fn) + ": " + conflict_text(k));
+}
+
 // per-warp floats of the JVS kernel variant the context launches (0 without view selection)
 int jvs_extra(const gpm_ctx* c) { return jvs_on(c) ? jvs_floats(c->V, c->geo_weight > 0.f) : 0; }
 
@@ -202,7 +233,7 @@ int build_kparams(gpm_ctx* c, bool init_phase, KParams& P, bool eval_call = fals
     if (c->V < 1) return fail(GPM_E_STATE, "no source views (gpm_set_num_views)");
     for (int v = 0; v < c->V; v++)
         if (!c->have_view[v]) return fail(GPM_E_STATE, "source view " + std::to_string(v) + " has not been set");
-    if (const int rc = check_geometric(c, c->geo_weight)) return rc;
+    if (const int rc = check_depth_maps(c, c->geo_weight)) return rc;
     if (c->inputs_dirty || c->memo_dirty) {     // one clearing for a whole scene upload instead of two memsets per setter
         const int rc = reset_state_tags(c, c->inputs_dirty ? GPM_PROV_UNKNOWN : PROV_KEEP);
         if (rc) return rc;
@@ -366,23 +397,32 @@ JvsParams jvs_params(const gpm_ctx* c)
     return J;
 }
 
+// Kernel tables: entry Mode::bits() is the family's kernel for that mode, nullptr (refused, never launched) where it has
+// none.  k_sweep and k_cost_eval exist for the modes mode_conflict() passes (k_cost_eval reads neither the propagation, the
+// view selection nor the fused sweep), k_shard_stage for those shard_supports() passes.
+template <class Entry, int... B>
+auto make_table(Entry entry, std::integer_sequence<int, B...>) { return std::array{entry(std::integral_constant<int, B>{})...}; }
+
+const auto kSweep = make_table([](auto b) -> decltype(&k_sweep<false, false>) {
+    constexpr Mode m = Mode::of(decltype(b)::value);
+    if constexpr (mode_conflict(m) == ModeConflict::none) return k_sweep<m.color, m.fused, m.geo, m.ncc, m.adaptive, m.jvs>; else return nullptr;
+}, std::make_integer_sequence<int, GPM_MODES>{});
+
+const auto kCostEval = make_table([](auto b) -> decltype(&k_cost_eval<false>) {
+    constexpr Mode m = Mode::of(decltype(b)::value);
+    if constexpr (mode_conflict(m) == ModeConflict::none) return k_cost_eval<m.color, m.geo, m.ncc>; else return nullptr;
+}, std::make_integer_sequence<int, GPM_MODES>{});
+
+const auto kShardStage = make_table([](auto b) -> decltype(&k_shard_stage<false>) {
+    constexpr Mode m = Mode::of(decltype(b)::value);
+    if constexpr (shard_supports(m)) return k_shard_stage<m.color, m.adaptive>; else return nullptr;
+}, std::make_integer_sequence<int, GPM_MODES>{});
+
 int launch_colour(gpm_ctx* c, const KParams& P, int colour, int mask)
 {
-    const bool ncc = ncc_on(c);          // grey images, 8 neighbours (gpm_set_photometric)
-    const bool geo = c->geo_weight > 0.f;
-    const bool adaptive = c->propagation == GPM_PROP_ADAPTIVE;
-    auto kern = jvs_on(c)                                                                           // NCC only (gpm_set_view_selection)
-              ? (adaptive ? (geo ? k_sweep<false, false, true, true, true, true> : k_sweep<false, false, false, true, true, true>)
-                          : (geo ? k_sweep<false, false, true, true, false, true> : k_sweep<false, false, false, true, false, true>))
-              : c->propagation == GPM_PROP_ADAPTIVE                                                  // 8 neighbours (gpm_set_propagation)
-              ? (ncc ? (geo ? k_sweep<false, false, true, true, true> : k_sweep<false, false, false, true, true>)
-                 : geo ? (P.color ? k_sweep<true, false, true, false, true> : k_sweep<false, false, true, false, true>)
-                       : (P.color ? k_sweep<true, false, false, false, true> : k_sweep<false, false, false, false, true>))
-              : ncc ? (geo ? k_sweep<false, false, true, true> : k_sweep<false, false, false, true>)
-              : geo ? (P.color ? k_sweep<true, false, true> : k_sweep<false, false, true>)    // 8 neighbours (check_geometric)
-              : P.ncand == 20 ? (P.color ? k_sweep<true, true> : k_sweep<false, true>)
-                              : (P.color ? k_sweep<true, false> : k_sweep<false, false>);
-    kern<<<tile_grid(c), P.nwarps * 32, block_smem_bytes(P, ncc, jvs_extra(c)), c->stream>>>(P, c->tmap, c->d_cams, c->srcTex, c->planes,
+    const auto kern = kSweep[ctx_mode(c).bits()];
+    if (!kern) return fail(GPM_E_STATE, "k_sweep has no kernel for this context's mode");
+    kern<<<tile_grid(c), P.nwarps * 32, block_smem_bytes(P, ncc_on(c), jvs_extra(c)), c->stream>>>(P, c->tmap, c->d_cams, c->srcTex, c->planes,
         c->cost, c->rng, c->prov, Memo{c->pid, c->seen, c->refseen, c->memo_mask, c->next_id}, colour, mask, c->d_stats, geo_params(c),
         jvs_params(c));
     c->launches++;
@@ -391,16 +431,15 @@ int launch_colour(gpm_ctx* c, const KParams& P, int colour, int mask)
 }
 
 // cost of `planes` at every pixel into `cost` (k_cost_eval: one block per tile, no slices)
-cudaError_t launch_cost_eval(gpm_ctx* c, const KParams& P, const float4* planes, float* cost)
+int launch_cost_eval(gpm_ctx* c, const KParams& P, const float4* planes, float* cost)
 {
+    const auto kern = kCostEval[ctx_mode(c).bits()];
+    if (!kern) return fail(GPM_E_STATE, "k_cost_eval has no kernel for this context's mode");
     dim3 grid((P.W + GPM_TILE - 1) / GPM_TILE, (P.H + GPM_TILE - 1) / GPM_TILE);
-    const bool ncc = ncc_on(c);
-    auto kern = ncc ? (c->geo_weight > 0.f ? k_cost_eval<false, true, true> : k_cost_eval<false, false, true>)
-              : c->geo_weight > 0.f ? (P.color ? k_cost_eval<true, true> : k_cost_eval<false, true>)
-                                    : (P.color ? k_cost_eval<true> : k_cost_eval<false>);
-    kern<<<grid, P.nwarps * 32, block_smem_bytes(P, ncc), c->stream>>>(P, c->tmap, c->d_cams, c->srcTex, planes, cost, nullptr, geo_params(c));
+    kern<<<grid, P.nwarps * 32, block_smem_bytes(P, ncc_on(c)), c->stream>>>(P, c->tmap, c->d_cams, c->srcTex, planes, cost, nullptr, geo_params(c));
     c->launches++;
-    return cudaGetLastError();
+    CU(cudaGetLastError());
+    return GPM_OK;
 }
 
 // random planes (gipuma.cu:1870-1875) and their identities; the XORWOW states are kept in GPM_RNG_STATEFUL mode
@@ -543,34 +582,11 @@ extern "C" int gpm_create(gpm_ctx** out, int device, int width, int height, int 
     if (err == cudaSuccess) {
         ok(cudaDeviceGetAttribute(&c->smem_optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, device));
         ok(cudaDeviceGetAttribute(&c->num_sms, cudaDevAttrMultiProcessorCount, device));
-        ok(cudaFuncSetAttribute(k_sweep<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, c->smem_optin));
-        ok(cudaFuncSetAttribute(k_sweep<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, c->smem_optin));
-        ok(cudaFuncSetAttribute(k_sweep<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, c->smem_optin));
-        ok(cudaFuncSetAttribute(k_sweep<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, c->smem_optin));
-        ok(cudaFuncSetAttribute(k_cost_eval<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, c->smem_optin));
-        ok(cudaFuncSetAttribute(k_cost_eval<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, c->smem_optin));
-        ok(cudaFuncSetAttribute(k_sweep<false, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, c->smem_optin));
-        ok(cudaFuncSetAttribute(k_sweep<true, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, c->smem_optin));
-        ok(cudaFuncSetAttribute(k_cost_eval<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, c->smem_optin));
-        ok(cudaFuncSetAttribute(k_cost_eval<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, c->smem_optin));
-        ok(cudaFuncSetAttribute(k_sweep<false, false, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, c->smem_optin));
-        ok(cudaFuncSetAttribute(k_sweep<false, false, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, c->smem_optin));
-        ok(cudaFuncSetAttribute(k_cost_eval<false, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, c->smem_optin));
-        ok(cudaFuncSetAttribute(k_cost_eval<false, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, c->smem_optin));
-        ok(cudaFuncSetAttribute(k_shard_stage<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, c->smem_optin));
-        ok(cudaFuncSetAttribute(k_shard_stage<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, c->smem_optin));
-        ok(cudaFuncSetAttribute(k_sweep<false, false, false, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, c->smem_optin));
-        ok(cudaFuncSetAttribute(k_sweep<true, false, false, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, c->smem_optin));
-        ok(cudaFuncSetAttribute(k_sweep<false, false, true, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, c->smem_optin));
-        ok(cudaFuncSetAttribute(k_sweep<true, false, true, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, c->smem_optin));
-        ok(cudaFuncSetAttribute(k_sweep<false, false, false, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, c->smem_optin));
-        ok(cudaFuncSetAttribute(k_sweep<false, false, true, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, c->smem_optin));
-        ok(cudaFuncSetAttribute(k_shard_stage<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, c->smem_optin));
-        ok(cudaFuncSetAttribute(k_shard_stage<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, c->smem_optin));
-        ok(cudaFuncSetAttribute(k_sweep<false, false, false, true, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, c->smem_optin));
-        ok(cudaFuncSetAttribute(k_sweep<false, false, true, true, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, c->smem_optin));
-        ok(cudaFuncSetAttribute(k_sweep<false, false, false, true, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, c->smem_optin));
-        ok(cudaFuncSetAttribute(k_sweep<false, false, true, true, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, c->smem_optin));
+        auto optin = [&](const auto& table) {
+            for (const auto kern : table)
+                if (kern) ok(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, c->smem_optin));
+        };
+        optin(kSweep);  optin(kCostEval);  optin(kShardStage);
     }
     if (err != cudaSuccess) {
         std::string m = std::string("gpm_create: ") + cudaGetErrorString(err);
@@ -637,21 +653,13 @@ extern "C" int gpm_set_rng(gpm_ctx* c, unsigned long long seed, int mode)
     return GPM_OK;
 }
 
-// the NCC cost and joint view selection have no colour variant: a colour upload while either is on is refused before
-// anything changes
-static int refuse_color_under_ncc(const char* fn, const gpm_ctx* c, bool color)
-{
-    if (color && jvs_on(c)) return fail(GPM_E_ARG, std::string(fn) + ": joint view selection supports grey images only (gpm_set_view_selection GPM_VSEL_OFF)");
-    return color && ncc_on(c) ? fail(GPM_E_STATE, std::string(fn) + ": the NCC photometric cost supports grey images only (gpm_set_photometric GPM_PHOTO_PM)") : GPM_OK;
-}
-
 // Image uploads, T = float (grey) or float4 (colour: the reference's -color_processing path, main.cpp:560-605).  Each
 // returns after a stream synchronisation: the caller may reuse its buffer.
 template <typename T>
 static int set_reference(const char* fn, gpm_ctx* c, const float* img, size_t pitch_bytes, int on_device, const gpm_camera* cam)
 {
     if (!c || !img || !cam) return fail(GPM_E_ARG, std::string(fn) + ": null argument");
-    if (const int rc = refuse_color_under_ncc(fn, c, sizeof(T) == sizeof(float4))) return rc;
+    if (const int rc = refuse_change(c, fn, &Mode::color, sizeof(T) == sizeof(float4))) return rc;
     DeviceGuard g(c->device);
     int rc = ensure_color(c, sizeof(T) == sizeof(float4));
     if (rc) return rc;
@@ -674,7 +682,7 @@ static int set_view(const char* fn, gpm_ctx* c, int v, const float* img, size_t 
     if (!c || !img || !cam) return fail(GPM_E_ARG, std::string(fn) + ": null argument");
     if (v < 0 || v >= c->maxV) return fail(GPM_E_ARG, std::string(fn) + ": view index out of range");
     constexpr bool color = sizeof(T) == sizeof(float4);
-    if (const int rc = refuse_color_under_ncc(fn, c, color)) return rc;
+    if (const int rc = refuse_change(c, fn, &Mode::color, color)) return rc;
     DeviceGuard g(c->device);
     int rc = ensure_color(c, color);
     if (rc) return rc;
@@ -750,53 +758,20 @@ extern "C" int gpm_set_view_depth(gpm_ctx* c, int v, const float* depth, size_t 
     return GPM_OK;
 }
 
-extern "C" int gpm_set_geometric(gpm_ctx* c, float weight, float max_err)
-{
-    if (!c) return fail(GPM_E_ARG, "gpm_set_geometric: null context");
-    if (!std::isfinite(weight) || weight < 0.f) return fail(GPM_E_ARG, "gpm_set_geometric: weight must be finite and >= 0");
-    if (!std::isfinite(max_err) || max_err <= 0.f) return fail(GPM_E_ARG, "gpm_set_geometric: max_err must be finite and > 0");
-    if (weight > 0.f) {
-        if (c->shard_world > 0) return fail(GPM_E_STATE, "gpm_set_geometric: view sharding does not support the geometric-consistency mode");
-        if (const int rc = check_geometric(c, weight)) return rc;
-    }
-    if (weight != c->geo_weight || max_err != c->geo_max_err) c->inputs_dirty = true;
-    c->geo_weight = weight;
-    c->geo_max_err = max_err;
-    return GPM_OK;
-}
-
-extern "C" int gpm_set_photometric(gpm_ctx* c, int kind, float min_std)
-{
-    if (!c) return fail(GPM_E_ARG, "gpm_set_photometric: null context");
-    if (kind != GPM_PHOTO_PM && kind != GPM_PHOTO_NCC) return fail(GPM_E_ARG, "gpm_set_photometric: kind must be GPM_PHOTO_PM or GPM_PHOTO_NCC");
-    if (kind == GPM_PHOTO_NCC) {
-        if (!std::isfinite(min_std) || min_std <= 0.f) return fail(GPM_E_ARG, "gpm_set_photometric: min_std must be finite and > 0");
-        if (c->color == 1) return fail(GPM_E_ARG, "gpm_set_photometric: the NCC cost supports grey images only; this context holds colour images");
-        if (c->opt_neighbours == 20) return fail(GPM_E_ARG, "gpm_set_photometric: the NCC cost supports the 8-neighbour sweep only (option neighbours = 8)");
-    } else {
-        if (jvs_on(c)) return fail(GPM_E_ARG, "gpm_set_photometric: joint view selection is built for the NCC cost (gpm_set_view_selection GPM_VSEL_OFF first)");
-        min_std = 0.f;                               // not read by the PM cost
-    }
-    if (kind != c->photo || min_std != c->ncc_min_std) c->inputs_dirty = true;
-    c->photo = kind;
-    c->ncc_min_std = min_std;
-    return GPM_OK;
-}
-
-// Only which plane is offered from each direction changes; the accept rule and cost(p, plane) do not, so stored costs, their
-// provenance and the memo stay valid across a switch.
-extern "C" int gpm_set_propagation(gpm_ctx* c, int kind)
-{
-    if (!c) return fail(GPM_E_ARG, "gpm_set_propagation: null context");
-    if (kind != GPM_PROP_FIXED && kind != GPM_PROP_ADAPTIVE) return fail(GPM_E_ARG, "gpm_set_propagation: kind must be GPM_PROP_FIXED or GPM_PROP_ADAPTIVE");
-    if (kind == GPM_PROP_ADAPTIVE && c->opt_neighbours == 20)
-        return fail(GPM_E_ARG, "gpm_set_propagation: adaptive sampling supports the 8-neighbour sweep only (option neighbours = 8)");
-    c->propagation = kind;
-    return GPM_OK;
-}
-
+// What the setters refuse for their arguments alone; the batch drivers check the same before any CUDA call (job_refusal).
 namespace gpm {
-// what gpm_set_view_selection refuses for its arguments alone (the batch drivers check the same before any CUDA call)
+const char* photometric_refusal(int kind, float min_std)
+{
+    if (kind != GPM_PHOTO_PM && kind != GPM_PHOTO_NCC) return "kind must be GPM_PHOTO_PM or GPM_PHOTO_NCC";
+    if (kind == GPM_PHOTO_NCC && !(std::isfinite(min_std) && min_std > 0.f)) return "min_std must be finite and > 0";
+    return nullptr;
+}
+
+const char* propagation_refusal(int kind)
+{
+    return kind != GPM_PROP_FIXED && kind != GPM_PROP_ADAPTIVE ? "propagation must be GPM_PROP_FIXED or GPM_PROP_ADAPTIVE" : nullptr;
+}
+
 const char* view_sel_refusal(const gpm_view_sel* v)
 {
     if (!v) return "vsel is NULL";
@@ -810,23 +785,68 @@ const char* view_sel_refusal(const gpm_view_sel* v)
     if (v->n_bad < 1 || v->n_bad > 9) return "n_bad must be 1..9";
     return nullptr;
 }
+
+// What the batch drivers refuse for a job's options before any CUDA call: the setters' argument checks and the mode rule,
+// for grey (channels 1) or colour (channels 4) images.
+const char* job_refusal(const gpm_job_opts* o, const gpm_view_sel* v, int channels)
+{
+    if (!o) return "opts is NULL";
+    if (const char* bad = photometric_refusal(o->photometric, o->ncc_min_std)) return bad;
+    if (const char* bad = propagation_refusal(o->propagation)) return bad;
+    if (const char* bad = view_sel_refusal(v)) return bad;
+    return conflict_text(mode_conflict(Mode{channels == 4, false, false, o->photometric == GPM_PHOTO_NCC,
+                                            o->propagation == GPM_PROP_ADAPTIVE, v->kind == GPM_VSEL_JOINT}));
+}
 }  // namespace gpm
+
+extern "C" int gpm_set_geometric(gpm_ctx* c, float weight, float max_err)
+{
+    if (!c) return fail(GPM_E_ARG, "gpm_set_geometric: null context");
+    if (!std::isfinite(weight) || weight < 0.f) return fail(GPM_E_ARG, "gpm_set_geometric: weight must be finite and >= 0");
+    if (!std::isfinite(max_err) || max_err <= 0.f) return fail(GPM_E_ARG, "gpm_set_geometric: max_err must be finite and > 0");
+    if (weight > 0.f && c->shard_world > 0) return fail(GPM_E_STATE, "gpm_set_geometric: view sharding does not support the geometric-consistency mode");
+    if (const int rc = refuse_change(c, "gpm_set_geometric", &Mode::geo, weight > 0.f)) return rc;
+    if (const int rc = check_depth_maps(c, weight)) return rc;
+    if (weight != c->geo_weight || max_err != c->geo_max_err) c->inputs_dirty = true;
+    c->geo_weight = weight;
+    c->geo_max_err = max_err;
+    return GPM_OK;
+}
+
+extern "C" int gpm_set_photometric(gpm_ctx* c, int kind, float min_std)
+{
+    if (!c) return fail(GPM_E_ARG, "gpm_set_photometric: null context");
+    if (const char* bad = photometric_refusal(kind, min_std)) return fail(GPM_E_ARG, std::string("gpm_set_photometric: ") + bad);
+    if (const int rc = refuse_change(c, "gpm_set_photometric", &Mode::ncc, kind == GPM_PHOTO_NCC)) return rc;
+    if (kind == GPM_PHOTO_PM) min_std = 0.f;         // not read by the PM cost
+    if (kind != c->photo || min_std != c->ncc_min_std) c->inputs_dirty = true;
+    c->photo = kind;
+    c->ncc_min_std = min_std;
+    return GPM_OK;
+}
+
+// Only which plane is offered from each direction changes; the accept rule and cost(p, plane) do not, so stored costs, their
+// provenance and the memo stay valid across a switch.
+extern "C" int gpm_set_propagation(gpm_ctx* c, int kind)
+{
+    if (!c) return fail(GPM_E_ARG, "gpm_set_propagation: null context");
+    if (const char* bad = propagation_refusal(kind)) return fail(GPM_E_ARG, std::string("gpm_set_propagation: ") + bad);
+    if (const int rc = refuse_change(c, "gpm_set_propagation", &Mode::adaptive, kind == GPM_PROP_ADAPTIVE)) return rc;
+    c->propagation = kind;
+    return GPM_OK;
+}
 
 // A switch either way changes what the stored costs mean (weighted or combined): they and the memo are marked stale.
 extern "C" int gpm_set_view_selection(gpm_ctx* c, const gpm_view_sel* vsel)
 {
     if (!c) return fail(GPM_E_ARG, "gpm_set_view_selection: null context");
     if (const char* bad = view_sel_refusal(vsel)) return fail(GPM_E_ARG, std::string("gpm_set_view_selection: ") + bad);
-    if (vsel->kind == GPM_VSEL_JOINT) {
-        if (!ncc_on(c)) return fail(GPM_E_ARG, "gpm_set_view_selection: joint view selection is built for the NCC cost (gpm_set_photometric GPM_PHOTO_NCC)");
-        if (c->color == 1) return fail(GPM_E_ARG, "gpm_set_view_selection: joint view selection supports grey images only; this context holds colour images");
-        if (c->opt_neighbours == 20) return fail(GPM_E_ARG, "gpm_set_view_selection: joint view selection supports the 8-neighbour sweep only (option neighbours = 8)");
-        if (!jvs_on(c)) {
-            DeviceGuard g(c->device);
-            if (!c->vsel_mask) CU(cudaMalloc(&c->vsel_mask, (size_t)c->W * c->H * sizeof(unsigned long long)));
-            const int rc = clear_vsel_masks(c);
-            if (rc) return rc;
-        }
+    if (const int rc = refuse_change(c, "gpm_set_view_selection", &Mode::jvs, vsel->kind == GPM_VSEL_JOINT)) return rc;
+    if (vsel->kind == GPM_VSEL_JOINT && !jvs_on(c)) {
+        DeviceGuard g(c->device);
+        if (!c->vsel_mask) CU(cudaMalloc(&c->vsel_mask, (size_t)c->W * c->H * sizeof(unsigned long long)));
+        const int rc = clear_vsel_masks(c);
+        if (rc) return rc;
     }
     if (vsel->kind != c->vsel.kind) c->inputs_dirty = true;
     c->vsel = *vsel;
@@ -888,7 +908,8 @@ static int do_init(gpm_ctx* c)
     if (rc) return rc;
     rc = init_planes(c, P);
     if (rc) return rc;
-    CU(launch_cost_eval(c, P, c->planes, c->cost));
+    rc = launch_cost_eval(c, P, c->planes, c->cost);
+    if (rc) return rc;
     rc = clear_vsel_masks(c);                      // view selection starts over: no view selected, t = 0
     if (rc) return rc;
     c->vsel_t = 0;
@@ -988,10 +1009,12 @@ extern "C" int gpm_cost_eval(gpm_ctx* c, const float* planes, float* out_cost, i
         if (e1 == cudaSuccess) e1 = cudaMemcpyAsync(d_pl, planes, n * sizeof(float4), cudaMemcpyHostToDevice, c->stream);
         if (e1 != cudaSuccess) { cudaFree(d_pl);  cudaFree(d_out);  return fail(GPM_E_CUDA, std::string("gpm_cost_eval: ") + cudaGetErrorString(e1)); }
     }
-    cudaError_t e = launch_cost_eval(c, P, d_pl, d_out);
-    if (e == cudaSuccess && !on_device) e = cudaMemcpyAsync(out_cost, d_out, n * sizeof(float), cudaMemcpyDeviceToHost, c->stream);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(c->stream);
+    rc = launch_cost_eval(c, P, d_pl, d_out);
+    cudaError_t e = cudaSuccess;
+    if (rc == GPM_OK && !on_device) e = cudaMemcpyAsync(out_cost, d_out, n * sizeof(float), cudaMemcpyDeviceToHost, c->stream);
+    if (rc == GPM_OK && e == cudaSuccess) e = cudaStreamSynchronize(c->stream);
     if (!on_device) { cudaFree(d_pl);  cudaFree(d_out); }
+    if (rc) return rc;
     if (e != cudaSuccess) return fail(GPM_E_CUDA, std::string("gpm_cost_eval: ") + cudaGetErrorString(e));
     return GPM_OK;
 }
@@ -1027,26 +1050,26 @@ static int shard_refine_steps(const gpm_params& p)
     return n;
 }
 
-// the source-view shard has no geometric-consistency, NCC or view-selection variant: refused before anything is launched
-static int shard_refuses_mode(gpm_ctx* c)
+// Every shard call taking a context refuses a mode shard_supports() does not pass, before anything is launched: with
+// GPM_E_STATE here, but the fused sweep only where it launches (shard_common), with GPM_E_ARG.
+static int shard_refuses_state(gpm_ctx* c)
 {
-    if (jvs_on(c)) return fail(GPM_E_STATE, "view sharding does not support joint view selection: the exchange carries top-n lists, not per-view costs (gpm_set_view_selection GPM_VSEL_OFF)");
-    if (c->geo_weight > 0.f) return fail(GPM_E_STATE, "view sharding does not support the geometric-consistency mode (gpm_set_geometric weight 0)");
-    if (ncc_on(c)) return fail(GPM_E_STATE, "view sharding does not support the NCC photometric cost (gpm_set_photometric GPM_PHOTO_PM)");
-    return GPM_OK;
+    Mode m = ctx_mode(c);
+    m.fused = false;
+    return shard_supports(m) ? GPM_OK : fail(GPM_E_STATE, "view sharding supports neither the geometric-consistency mode, the NCC cost nor joint view selection");
 }
 
 extern "C" int gpm_shard_num_stages(gpm_ctx* c)
 {
     if (!c || !c->have_params) { fail(GPM_E_STATE, "gpm_shard_num_stages: parameters not set");  return -1; }
-    if (shard_refuses_mode(c)) return -1;
+    if (shard_refuses_state(c)) return -1;
     return 2 + shard_refine_steps(c->prm);
 }
 
 extern "C" long long gpm_shard_stage_floats(gpm_ctx* c, int stage)
 {
     if (!c || !c->have_params || stage < 0) { fail(GPM_E_ARG, "gpm_shard_stage_floats: bad arguments");  return -1; }
-    if (shard_refuses_mode(c)) return -1;
+    if (shard_refuses_state(c)) return -1;
     const long long half = (long long)c->H * ((c->W + 1) / 2);
     const int slots = stage == 1 ? 8 : 1;
     return (stage == 0 ? 2 : 1) * half * slots * c->prm.n_best;
@@ -1054,9 +1077,9 @@ extern "C" long long gpm_shard_stage_floats(gpm_ctx* c, int stage)
 
 static int shard_common(gpm_ctx* c, int stage, KParams& P)
 {
-    if (const int rc = shard_refuses_mode(c)) return rc;
+    if (const int rc = shard_refuses_state(c)) return rc;
     if (c->prm.cost_comb != GPM_COMB_BEST_N) return fail(GPM_E_ARG, "view sharding supports cost_comb = best_n only");
-    if (c->opt_neighbours != 8) return fail(GPM_E_ARG, "view sharding supports the 8-neighbour sweep only (option neighbours = 8)");
+    if (!shard_supports(ctx_mode(c))) return fail(GPM_E_ARG, "view sharding supports the 8-neighbour sweep only (option neighbours = 8)");
     if (c->prm.n_best < 1 || c->prm.n_best > 32) return fail(GPM_E_ARG, "view sharding needs 1 <= n_best <= 32");
     if (c->rng_mode != GPM_RNG_REFERENCE) return fail(GPM_E_ARG, "view sharding implements the reference's zero-state refinement stream only (GPM_RNG_REFERENCE)");
     const int last = 1 + shard_refine_steps(c->prm);
@@ -1079,10 +1102,10 @@ static int shard_common(gpm_ctx* c, int stage, KParams& P)
 // enqueue one stage kernel (stage 0 .. last+1) on the context's stream
 static int shard_launch_stage(gpm_ctx* c, const KParams& P, int colour, int stage, const float* gathered_prev, int world, float* xchg)
 {
+    const auto kern = kShardStage[ctx_mode(c).bits()];
+    if (!kern) return fail(GPM_E_STATE, "k_shard_stage has no kernel for this context's mode");
     const int last = 1 + shard_refine_steps(c->prm);
     ShardState S{c->dispbuf, c->candbuf, c->canddepth, c->sflags};
-    auto kern = c->propagation == GPM_PROP_ADAPTIVE ? (P.color ? k_shard_stage<true, true> : k_shard_stage<false, true>)
-                                                    : (P.color ? k_shard_stage<true> : k_shard_stage<false>);
     kern<<<tile_grid(c), P.nwarps * 32, block_smem_bytes(P), c->stream>>>(P, c->tmap, c->d_cams,
         c->srcTex, c->planes, c->cost, c->prov, S, Memo{c->pid, c->seen, c->refseen, c->memo_mask, c->next_id}, colour, stage, last,
         gathered_prev, world, xchg, c->d_stats);
@@ -1207,7 +1230,7 @@ static int shard_alloc_exchange(gpm_ctx* c)
 extern "C" int gpm_shard_comm_init(gpm_ctx* c, const void* id128, int rank, int world)
 {
     if (!c || world < 1 || world > 8 || rank < 0 || rank >= world) return fail(GPM_E_ARG, "gpm_shard_comm_init: bad arguments (1 <= world <= 8)");
-    if (const int rc = shard_refuses_mode(c)) return rc;
+    if (const int rc = shard_refuses_state(c)) return rc;
     DeviceGuard g(c->device);
     gpm_shard_comm_destroy_(c);
     c->shard_rank = rank;  c->shard_world = world;
@@ -1225,7 +1248,7 @@ extern "C" int gpm_shard_comm_init(gpm_ctx* c, const void* id128, int rank, int 
 extern "C" int gpm_shard_comm_attach(gpm_ctx* c, void* nccl_comm, int rank, int world)
 {
     if (!c || world < 1 || world > 8 || rank < 0 || rank >= world || (world > 1 && !nccl_comm)) return fail(GPM_E_ARG, "gpm_shard_comm_attach: bad arguments");
-    if (const int rc = shard_refuses_mode(c)) return rc;
+    if (const int rc = shard_refuses_state(c)) return rc;
     if (world > 1 && !nccl_api()) return fail(GPM_E_STATE, "NCCL (libnccl.so.2) could not be loaded; set GPM_NCCL_LIB");
     gpm_shard_comm_destroy_(c);
     c->comm = nccl_comm;  c->shard_rank = rank;  c->shard_world = world;
@@ -1374,10 +1397,7 @@ extern "C" int gpm_set_option(gpm_ctx* c, const char* name, int value)
     }
     else if (n == "neighbours") {
         if (value != 8 && value != 20) return fail(GPM_E_ARG, "neighbours must be 8 (close + far kernels) or 20 (fused kernel)");
-        if (value == 20 && c->geo_weight > 0.f) return fail(GPM_E_ARG, "the geometric-consistency mode supports the 8-neighbour sweep only");
-        if (value == 20 && ncc_on(c)) return fail(GPM_E_ARG, "the NCC photometric cost supports the 8-neighbour sweep only");
-        if (value == 20 && c->propagation == GPM_PROP_ADAPTIVE) return fail(GPM_E_ARG, "adaptive checkerboard sampling supports the 8-neighbour sweep only");
-        if (value == 20 && jvs_on(c)) return fail(GPM_E_ARG, "joint view selection supports the 8-neighbour sweep only");
+        if (const int rc = refuse_change(c, "gpm_set_option", &Mode::fused, value == 20)) return rc;
         DeviceGuard g(c->device);
         const int slots = value == 20 ? 20 : 8;
         if (slots != c->seen_slots) {

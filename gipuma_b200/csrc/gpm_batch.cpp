@@ -27,7 +27,7 @@
 #include <sys/stat.h>
 
 namespace gpm {
-const char* view_sel_refusal(const gpm_view_sel* v);     // gpm_api.cu
+const char* job_refusal(const gpm_job_opts* o, const gpm_view_sel* v, int channels);     // gpm_api.cu
 }
 
 namespace {
@@ -77,21 +77,6 @@ bool plan_view(const gpm_batch_desc* d, int ref, ViewSetup& s)
 gpm_job_opts photo_opts(int kind, float min_std) { return gpm_job_opts{kind, min_std, GPM_PROP_FIXED}; }
 
 const gpm_view_sel kVselOff{GPM_VSEL_OFF, 0.f, 0.f, 0.f, 0, 0, 0.f, 0.f};
-
-// what gpm_set_photometric, gpm_set_propagation and gpm_set_view_selection refuse for their arguments, NCC on colour images
-// and joint view selection with the PM cost or colour images; nullptr if none
-const char* opts_refusal(const gpm_job_opts* o, const gpm_view_sel* v, int channels)
-{
-    if (!o) return "opts is NULL";
-    if (o->photometric != GPM_PHOTO_PM && o->photometric != GPM_PHOTO_NCC) return "kind must be GPM_PHOTO_PM or GPM_PHOTO_NCC";
-    if (o->photometric == GPM_PHOTO_NCC && !(std::isfinite(o->ncc_min_std) && o->ncc_min_std > 0.f)) return "min_std must be finite and > 0";
-    if (o->photometric == GPM_PHOTO_NCC && channels == 4) return "the NCC cost supports grey images only (channels 1)";
-    if (o->propagation != GPM_PROP_FIXED && o->propagation != GPM_PROP_ADAPTIVE) return "propagation must be GPM_PROP_FIXED or GPM_PROP_ADAPTIVE";
-    if (const char* bad = gpm::view_sel_refusal(v)) return bad;
-    if (v->kind == GPM_VSEL_JOINT && o->photometric != GPM_PHOTO_NCC) return "joint view selection is built for the NCC cost (GPM_PHOTO_NCC)";
-    if (v->kind == GPM_VSEL_JOINT && channels == 4) return "joint view selection supports grey images only (channels 1)";
-    return nullptr;
-}
 
 // The per-view setup of a job: photometric cost, propagation, view selection, parameters, reference and source images
 // (grey: channels 1, RGBA: 4), view count, RNG.
@@ -189,7 +174,7 @@ static int batch_run(const char* fn, const gpm_batch_desc* d, const gpm_job_opts
         set_err(std::string(fn) + ": bad arguments");
         return GPM_E_ARG;
     }
-    if (const char* bad = opts_refusal(opts, vsel, 1)) {
+    if (const char* bad = gpm::job_refusal(opts, vsel, 1)) {
         set_err(std::string(fn) + ": bad arguments: " + bad);
         return GPM_E_ARG;
     }
@@ -322,7 +307,7 @@ static int geo_batch_run(const char* fn, const gpm_geo_batch_desc* g, const gpm_
     else if (g->geo_iterations < 0) bad = "geo_iterations must be >= 0";
     else if (!std::isfinite(g->weight) || g->weight < 0.f) bad = "weight must be finite and >= 0";
     else if (!std::isfinite(g->max_err) || g->max_err <= 0.f) bad = "max_err must be finite and > 0";
-    else bad = opts_refusal(opts, vsel, g->channels);
+    else bad = gpm::job_refusal(opts, vsel, g->channels);
     if (bad) {
         set_err(std::string(fn) + ": bad arguments: " + bad);
         return GPM_E_ARG;

@@ -102,6 +102,36 @@ struct JvsParams {
 // current plane or the refinement candidate), as many geometric terms with GEO, and the V view weights
 __host__ __device__ inline int jvs_floats(int V, bool geo) { return (geo ? 18 : 9) * V + V; }
 
+// ---- sweep modes: which combinations have kernels --------------------------------------------------------------------
+// A context's mode: colour images, the fused 20-neighbour sweep (option neighbours = 20), the geometric-consistency term
+// (§14), the NCC cost (§15), adaptive checkerboard sampling (§16) and joint view selection (§17).  Kernels are instantiated
+// (gpm_api.cu, kernel tables) and setters accept a change (gpm_set_*) exactly for the modes mode_conflict() passes.
+struct Mode {
+    bool color, fused, geo, ncc, adaptive, jvs;
+    __host__ __device__ constexpr int bits() const { return color | fused << 1 | geo << 2 | ncc << 3 | adaptive << 4 | jvs << 5; }
+    __host__ __device__ static constexpr Mode of(int b) { return Mode{bool(b & 1), bool(b & 2), bool(b & 4), bool(b & 8), bool(b & 16), bool(b & 32)}; }
+};
+constexpr int GPM_MODES = 64;
+
+enum class ModeConflict { none, fused, jvs_needs_ncc_grey, ncc_colour };
+
+// The one rule: the fused sweep has none of the four modes; joint view selection needs the NCC cost (on grey images);
+// the NCC cost needs grey images.  The first conflict found is the reason a refusal gives.
+__host__ __device__ constexpr ModeConflict mode_conflict(Mode m)
+{
+    if (m.fused && (m.geo || m.ncc || m.adaptive || m.jvs)) return ModeConflict::fused;
+    if (m.jvs && (!m.ncc || m.color)) return ModeConflict::jvs_needs_ncc_grey;
+    if (m.ncc && m.color) return ModeConflict::ncc_colour;
+    return ModeConflict::none;
+}
+
+// The source-view shard (k_shard_stage) exchanges top-n lists of the 8-neighbour sweep's PM costs: no geometric term, NCC
+// cost, joint view selection or fused sweep.
+__host__ __device__ constexpr bool shard_supports(Mode m)
+{
+    return mode_conflict(m) == ModeConflict::none && !m.geo && !m.ncc && !m.jvs && !m.fused;
+}
+
 // ---- exact memo of rejected work: plane identities ------------------------------------------------------------
 // Every plane carries a 32-bit identity: pid[p] = p + 1 at initialisation, a fresh number (atomic counter) whenever a
 // refinement creates a new plane, and COPIED when a plane propagates to a neighbour (gipuma.cu:867-871 copies the plane
@@ -459,10 +489,7 @@ k_sweep(const __grid_constant__ KParams P, const __grid_constant__ CUtensorMap t
         unsigned* __restrict__ rng_state, unsigned char* __restrict__ prov, Memo M, int colour, int phase_mask,
         unsigned long long* __restrict__ stats, const __grid_constant__ GeoParams G, const JvsParams J)
 {
-    static_assert(!(FUSED && GEO), "the geometric term is built for the 8-neighbour sweep only");
-    static_assert(!JVS || NCC, "joint view selection is built for the NCC cost (8-neighbour sweep, grey images) only");
-    static_assert(!(NCC && (FUSED || COLOR)), "the NCC cost is built for the 8-neighbour sweep on grey images only");
-    static_assert(!(FUSED && ADAPTIVE), "adaptive checkerboard sampling is built for the 8-neighbour sweep only");
+    static_assert(mode_conflict(Mode{COLOR, FUSED, GEO, NCC, ADAPTIVE, JVS}) == ModeConflict::none, "no such sweep mode (mode_conflict)");
     const GeoParams* g = (GEO || NCC) ? &G : nullptr;
     extern __shared__ __align__(128) float smem[];
     float* tile = smem;

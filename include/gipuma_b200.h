@@ -88,6 +88,23 @@ int gpm_set_view_color(gpm_ctx* ctx, int v, const float* rgba, size_t pitch_byte
 /* Number of source views actually used (viewSelectionSubsetNumber, main.cpp:918). */
 int gpm_set_num_views(gpm_ctx* ctx, int n_views);
 
+/* ---- mode compatibility -------------------------------------------------------------------------------------------------
+ * A context sweeps in one mode of six fields: colour images (fixed by the first image upload), the fused 20-neighbour sweep
+ * (option "neighbours" = 20), the geometric-consistency term, the NCC cost, adaptive sampling and joint view selection
+ * (DESIGN.md §14–§17).  Every combination exists except:
+ *   - the fused sweep with the geometric term, the NCC cost, adaptive sampling or joint view selection;
+ *   - joint view selection without the NCC cost, and so with colour images;
+ *   - the NCC cost with colour images.
+ * A call that would make one of these is refused and changes nothing.  gpm_set_geometric, gpm_set_photometric,
+ * gpm_set_propagation, gpm_set_view_selection and gpm_set_option("neighbours") return GPM_E_ARG, whichever of the two
+ * fields is set last.  A colour image upload (gpm_set_reference_color, gpm_set_view_color) returns GPM_E_ARG while joint
+ * view selection is on and GPM_E_STATE while only the NCC cost is.  The batch drivers refuse the same combinations of their
+ * job options and image type with GPM_E_ARG before any CUDA call.
+ * The source-view shard runs neither the geometric term, the NCC cost nor joint view selection: while one is on, every
+ * gpm_shard_* call taking a context returns GPM_E_STATE (gpm_shard_num_stages and gpm_shard_stage_floats return -1), and
+ * gpm_set_geometric refuses to turn the term on with GPM_E_STATE once a shard communicator is set.  gpm_shard_stage,
+ * gpm_shard_finish_init and gpm_shard_run refuse the fused sweep with GPM_E_ARG. */
+
 /* ---- geometric consistency (DESIGN.md §14) ----------------------------------------------------------------------------
  * A second PatchMatch pass may score each hypothesis against the source views' own depth maps as well: with weight > 0 the
  * cost of view j becomes photo_j + g_j, g_j = weight * min(err, max_err), where err is the forward-backward reprojection
@@ -98,10 +115,8 @@ int gpm_set_num_views(gpm_ctx* ctx, int n_views);
  *   memory), each pixel's depth along view v's own optical axis as gpm_finalize writes it (0 = no depth).  The cameras are
  *   those of gpm_set_view (K^-1 included) and the reference's K.  Storage is allocated by the first call.
  * gpm_set_geometric: weight 0 (the default) turns the mode off and gives exactly the photometric cost.  Refused with
- *   GPM_E_ARG: weight negative or not finite, max_err not finite or <= 0, option neighbours = 20 (the fused sweep has no
- *   such variant); with GPM_E_STATE: a used view (0 .. n_views-1) without a depth map — also at the next launch, if
- *   gpm_set_num_views adds one.  The source-view shard (every gpm_shard_* call taking a context) has no such variant and
- *   refuses to run while the mode is on. */
+ *   GPM_E_ARG: weight negative or not finite, max_err not finite or <= 0; with GPM_E_STATE: a used view (0 .. n_views-1)
+ *   without a depth map — also at the next launch, if gpm_set_num_views adds one.  Other modes: "mode compatibility". */
 int gpm_set_view_depth(gpm_ctx* ctx, int v, const float* depth, size_t pitch_bytes, int on_device);
 int gpm_set_geometric(gpm_ctx* ctx, float weight, float max_err);
 
@@ -111,9 +126,8 @@ int gpm_set_geometric(gpm_ctx* ctx, float weight, float max_err);
  * source image leave unchanged; a window whose weighted standard deviation, in the reference or the source view, is below
  * min_std grey levels costs 2.  Grey images and the 8-neighbour sweep only.  With the geometric mode on, view j's cost is
  * ncc_j + g_j.  The lower-bound early-out (option "prune") has no effect on NCC costs.  min_std is ignored for PM.
- * Refused with GPM_E_ARG: an unknown kind; NCC with min_std not finite or <= 0, on a context holding colour images, or with
- * option neighbours = 20 (and neighbours = 20 while NCC is on).  With GPM_E_STATE: a colour image upload while NCC is on, and
- * every gpm_shard_* call taking a context.  A refused call changes nothing. */
+ * Refused with GPM_E_ARG: an unknown kind; NCC with min_std not finite or <= 0.  Other modes: "mode compatibility".  A
+ * refused call changes nothing. */
 enum { GPM_PHOTO_PM = 0, GPM_PHOTO_NCC = 1 };
 int gpm_set_photometric(gpm_ctx* ctx, int kind, float min_std);
 
@@ -125,8 +139,7 @@ int gpm_set_photometric(gpm_ctx* ctx, int kind, float min_std);
  * costs count as +inf and a tie goes to the earliest pixel of the region's scan order.  The accept rule, the refinement and
  * every cost are unchanged, so the mode may be switched at any point of a run and works with every cost mode, grey or
  * colour, and with the source-view shard (gpm_shard_*).
- * Refused with GPM_E_ARG: an unknown kind; ADAPTIVE with option neighbours = 20 (and neighbours = 20 while ADAPTIVE is
- * on).  A refused call changes nothing. */
+ * Refused with GPM_E_ARG: an unknown kind.  Other modes: "mode compatibility".  A refused call changes nothing. */
 enum { GPM_PROP_FIXED = 0, GPM_PROP_ADAPTIVE = 1 };
 int gpm_set_propagation(gpm_ctx* ctx, int kind);
 
@@ -143,9 +156,7 @@ int gpm_set_propagation(gpm_ctx* ctx, int kind);
  * stored costs stale.  NCC cost, grey images and the 8-neighbour sweep only; fixed or adaptive propagation, with or without
  * the geometric term.
  * Refused with GPM_E_ARG: a NULL `vsel`, an unknown kind; for JOINT, tau_init, alpha, tau_bad or beta not finite or <= 0,
- * w_keep not finite or < 0, n_good outside 1..8, n_bad outside 1..9; JOINT with the PM cost, on a context holding colour
- * images, or with option neighbours = 20 (and, while JOINT is on, gpm_set_photometric(GPM_PHOTO_PM), a colour image upload
- * and neighbours = 20).  With GPM_E_STATE: every gpm_shard_* call taking a context while JOINT is on.  A refused call
+ * w_keep not finite or < 0, n_good outside 1..8, n_bad outside 1..9.  Other modes: "mode compatibility".  A refused call
  * changes nothing. */
 enum { GPM_VSEL_OFF = 0, GPM_VSEL_JOINT = 1 };
 typedef struct gpm_view_sel {
@@ -336,14 +347,14 @@ int gpm_geo_batch_run(const gpm_geo_batch_desc* desc, gpm_geo_batch_stats* stats
 /* The batch drivers with a choice of photometric cost: every job's context gets gpm_set_photometric(kind, min_std) in the
  * per-view setup (both passes of the geometric driver).  gpm_batch_run and gpm_geo_batch_run are these with GPM_PHOTO_PM.
  * Refused with GPM_E_ARG before any CUDA call, besides what those refuse: what gpm_set_photometric refuses for its
- * arguments, and channels = 4 with GPM_PHOTO_NCC. */
+ * arguments, and the combinations "mode compatibility" excludes. */
 int gpm_batch_run_photo(const gpm_batch_desc* desc, int kind, float min_std, gpm_batch_stats* stats);
 int gpm_geo_batch_run_photo(const gpm_geo_batch_desc* desc, int kind, float min_std, gpm_geo_batch_stats* stats);
 
 /* The batch drivers with per-job options: every job's context gets gpm_set_photometric(photometric, ncc_min_std) and
  * gpm_set_propagation(propagation) in the per-view setup (both passes of the geometric driver).  The _photo twins are these
  * with GPM_PROP_FIXED.  Refused with GPM_E_ARG before any CUDA call, besides what those refuse: what the two setters refuse
- * for their arguments, channels = 4 with GPM_PHOTO_NCC, and a NULL `opts`. */
+ * for their arguments, and a NULL `opts`. */
 typedef struct gpm_job_opts {
     int photometric;                   /* GPM_PHOTO_PM or GPM_PHOTO_NCC */
     float ncc_min_std;                 /* as gpm_set_photometric (ignored for PM) */
@@ -355,8 +366,7 @@ int gpm_geo_batch_run_opts(const gpm_geo_batch_desc* desc, const gpm_job_opts* o
 /* The batch drivers with a view selection (DESIGN.md §17): every job's context also gets gpm_set_view_selection(vsel) in
  * the per-view setup (both passes of the geometric driver; pass 2 starts at t = 0 after its gpm_set_state).  vsel = NULL
  * is GPM_VSEL_OFF: the _opts drivers are these with NULL.  Refused with GPM_E_ARG before any CUDA call, besides what the
- * _opts drivers refuse: what gpm_set_view_selection refuses for its arguments, and JOINT with GPM_PHOTO_PM or with
- * channels = 4. */
+ * _opts drivers refuse: what gpm_set_view_selection refuses for its arguments. */
 int gpm_batch_run_vsel(const gpm_batch_desc* desc, const gpm_job_opts* opts, const gpm_view_sel* vsel, gpm_batch_stats* stats);
 int gpm_geo_batch_run_vsel(const gpm_geo_batch_desc* desc, const gpm_job_opts* opts, const gpm_view_sel* vsel,
                            gpm_geo_batch_stats* stats);
