@@ -71,6 +71,19 @@ class GpmViewSel(C.Structure):
                 ("n_good", C.c_int), ("n_bad", C.c_int), ("beta", C.c_float), ("w_keep", C.c_float)]
 
 
+class GpmPriorBuild(C.Structure):
+    _fields_ = [("step", C.c_int), ("support_cost", C.c_float)]
+
+
+class GpmPriorInfo(C.Structure):
+    _fields_ = [("support", C.c_longlong), ("triangles", C.c_longlong), ("with_prior", C.c_longlong)]
+
+
+class GpmPriorOpts(C.Structure):
+    _fields_ = [("weight", C.c_float), ("depth_sigma", C.c_float), ("normal_sigma_deg", C.c_float), ("step", C.c_int),
+                ("support_cost", C.c_float), ("iterations", C.c_int), ("info", C.POINTER(GpmPriorInfo))]
+
+
 class GpmFuseCamera(C.Structure):
     _fields_ = [("M_inv", C.c_float * 9), ("P", C.c_float * 12), ("f", C.c_float)]
 
@@ -175,6 +188,15 @@ def load_library():
     L.gpm_batch_run_vsel.argtypes = [C.POINTER(GpmBatchDesc), C.POINTER(GpmJobOpts), C.POINTER(GpmViewSel), C.POINTER(GpmBatchStats)]
     L.gpm_geo_batch_run_vsel.argtypes = [C.POINTER(GpmGeoBatchDesc), C.POINTER(GpmJobOpts), C.POINTER(GpmViewSel),
                                          C.POINTER(GpmGeoBatchStats)]
+    L.gpm_set_planar_prior.argtypes = [vp, vp, C.c_size_t, C.c_int]
+    L.gpm_get_planar_prior.argtypes = [vp, vp, C.c_int]
+    L.gpm_build_planar_prior.argtypes = [vp, C.POINTER(GpmPriorBuild), C.POINTER(GpmPriorInfo)]
+    L.gpm_set_prior.argtypes = [vp, C.c_float, C.c_float, C.c_float]
+    L.gpm_offer_prior.argtypes = [vp]
+    L.gpm_batch_run_prior.argtypes = [C.POINTER(GpmBatchDesc), C.POINTER(GpmJobOpts), C.POINTER(GpmViewSel),
+                                      C.POINTER(GpmPriorOpts), C.POINTER(GpmBatchStats)]
+    L.gpm_geo_batch_run_prior.argtypes = [C.POINTER(GpmGeoBatchDesc), C.POINTER(GpmJobOpts), C.POINTER(GpmViewSel),
+                                          C.POINTER(GpmPriorOpts), C.POINTER(GpmGeoBatchStats)]
     L.gpm_batch_last_error.restype = C.c_char_p
     L.gpm_stream.restype = vp
     L.gpm_fuse_cameras.argtypes = [C.POINTER(C.c_double), C.c_int, C.c_double, C.POINTER(GpmFuseCamera)]
@@ -188,7 +210,9 @@ def load_library():
                  "gpm_init_planes", "gpm_shard_num_stages", "gpm_shard_stage", "gpm_shard_finish_init", "gpm_shard_unique_id",
                  "gpm_shard_comm_init", "gpm_shard_comm_attach", "gpm_shard_run", "gpm_measure_fetch_peak", "gpm_batch_run",
                  "gpm_geo_batch_run", "gpm_batch_run_photo", "gpm_geo_batch_run_photo", "gpm_batch_run_opts", "gpm_geo_batch_run_opts",
-                 "gpm_batch_run_vsel", "gpm_geo_batch_run_vsel",
+                 "gpm_batch_run_vsel", "gpm_geo_batch_run_vsel", "gpm_set_planar_prior", "gpm_get_planar_prior",
+                 "gpm_build_planar_prior", "gpm_set_prior", "gpm_offer_prior", "gpm_batch_run_prior",
+                 "gpm_geo_batch_run_prior",
                  "gpm_prepare_cameras", "gpm_select_views", "gpm_write_dmb", "gpm_read_dmb", "gpm_write_result_dmb",
                  "gpm_fuse_cameras", "gpm_fuse", "gpm_write_ply", "gpm_nearest_dist"):
         getattr(L, name).restype = C.c_int
@@ -311,13 +335,68 @@ def view_sel(kind: str = "off", **params) -> GpmViewSel:
                       int(p["n_bad"]), float(p["beta"]), float(p["w_keep"]))
 
 
-def check_modes(photometric: str, view_selection: str, channels: int = 1):
+# Planar prior (DESIGN.md §18): ACMP's scales, sigma_d = (depthMax - depthMin) / 64 (None here: it depends on the scene)
+# and sigma_n = 5 degrees; step and support_cost of the prior's construction.  The weight per photometric cost is the best of
+# the grid measured with tools/acs_bench.py --prior (§18's table).
+PRIOR_DEFAULTS = {"weight": {"pm": 2.0, "ncc": 0.1}, "depth_sigma": None, "normal_sigma_deg": 5.0, "step": 5, "support_cost": 0.5}
+
+
+def check_prior(weight: float, depth_sigma: float, normal_sigma_deg: float):
+    """The argument rules of gpm_set_prior, checked before any call into the library."""
+    if not (isinstance(weight, (int, float, np.floating, np.integer)) and np.isfinite(weight) and weight >= 0):
+        raise ValueError("weight must be finite and >= 0 (got %r)" % (weight,))
+    if not (isinstance(depth_sigma, (int, float, np.floating, np.integer)) and np.isfinite(depth_sigma) and depth_sigma > 0):
+        raise ValueError("depth_sigma must be finite and > 0 (got %r)" % (depth_sigma,))
+    if not (isinstance(normal_sigma_deg, (int, float, np.floating, np.integer)) and 0 < normal_sigma_deg <= 90):
+        raise ValueError("normal_sigma_deg must be in (0, 90] (got %r)" % (normal_sigma_deg,))
+
+
+def check_prior_build(step: int, support_cost: float):
+    """The argument rules of gpm_build_planar_prior, checked before any call into the library."""
+    if int(step) != step or not 1 <= step <= 64:
+        raise ValueError("step must be an integer in 1..64 (got %r)" % (step,))
+    if support_cost != support_cost:
+        raise ValueError("support_cost must not be NaN")
+
+
+def check_modes(photometric: str, view_selection: str, channels: int = 1, planar_prior: Optional[dict] = None):
     """The mode rules the batch drivers refuse a combination by (include/gipuma_b200.h, mode compatibility), checked before
-    any call into the library: "joint" view selection needs the NCC cost, and both need grey images (channels 1)."""
+    any call into the library: "joint" view selection needs the NCC cost, and both need grey images (channels 1); a planar
+    prior (a dict, see prior_opts) needs grey images and excludes joint view selection."""
     if view_selection == "joint" and photometric != "ncc":
         raise ValueError("view_selection='joint' is built for the NCC cost (photometric='ncc')")
     if photometric == "ncc" and channels == 4:
         raise ValueError("the NCC photometric cost supports grey images only")
+    if planar_prior is not None and (channels == 4 or view_selection == "joint"):
+        raise ValueError("the planar prior supports grey images without joint view selection")
+
+
+def prior_opts(planar_prior: Optional[dict], params, n_jobs: int, photometric: str = "pm"):
+    """gpm_prior_opts of the batch drivers' prior stage from `planar_prior` (None: no stage; a dict overriding
+    PRIOR_DEFAULTS, plus "iterations", the sweeps with the prior, 2 by default), every argument checked before any call into
+    the library.  depth_sigma None: (depthMax - depthMin) / 64 of `params`.  Returns (opts or None, the per-job info array)."""
+    if planar_prior is None:
+        return None, None
+    unknown = sorted(set(planar_prior) - set(PRIOR_DEFAULTS) - {"iterations"})
+    if unknown:
+        raise ValueError("unknown planar-prior parameters %s (known: %s)" % (unknown, sorted(PRIOR_DEFAULTS) + ["iterations"]))
+    p = dict(PRIOR_DEFAULTS, iterations=2)
+    p.update(planar_prior)
+    if isinstance(p["weight"], dict):
+        p["weight"] = p["weight"][photometric]
+    if p["depth_sigma"] is None:
+        p["depth_sigma"] = (float(params.depthMax) - float(params.depthMin)) / 64.0 if params is not None else 1.0
+    check_prior(p["weight"], p["depth_sigma"], p["normal_sigma_deg"])
+    check_prior_build(p["step"], p["support_cost"])
+    if int(p["iterations"]) != p["iterations"] or p["iterations"] < 0:
+        raise ValueError("iterations must be an integer >= 0 (got %r)" % (p["iterations"],))
+    info = (GpmPriorInfo * max(n_jobs, 1))()
+    return GpmPriorOpts(float(p["weight"]), float(p["depth_sigma"]), float(p["normal_sigma_deg"]), int(p["step"]),
+                        float(p["support_cost"]), int(p["iterations"]), info), info
+
+
+def _prior_info(info, k):
+    return [{"support": i.support, "triangles": i.triangles, "with_prior": i.with_prior} for i in info[:k]] if info else None
 
 
 def job_opts(photometric: str = "pm", ncc_min_std: float = NCC_MIN_STD, propagation: str = "fixed") -> GpmJobOpts:
@@ -423,6 +502,39 @@ class Context:
         the 8-neighbour sweep."""
         v = view_sel(kind, **params)
         self._check(self.lib.gpm_set_view_selection(self.h, C.byref(v)))
+
+    def set_prior(self, weight: float, depth_sigma: float, normal_sigma_deg: float = PRIOR_DEFAULTS["normal_sigma_deg"]):
+        """Planar prior term of every cost (DESIGN.md §18): weight * q / (1 + q) with q = (depth offset / depth_sigma)^2 +
+        (1 - cos of the normal angle) / (1 - cos normal_sigma_deg), against the pixel's prior plane; weight 0 turns it
+        off.  Needs a prior map (set_planar_prior or build_planar_prior), grey images and no joint view selection."""
+        check_prior(weight, depth_sigma, normal_sigma_deg)
+        self._check(self.lib.gpm_set_prior(self.h, float(weight), float(depth_sigma), float(normal_sigma_deg)))
+
+    def set_planar_prior(self, planes):
+        """Prior map [H, W, 4] (n.xyz, d per pixel; all-zero: no prior), numpy or torch, host or device."""
+        if tuple(planes.shape) != (self.H, self.W, 4):
+            raise ValueError("prior map must be [%d, %d, 4], got %s" % (self.H, self.W, tuple(planes.shape)))
+        if isinstance(planes, np.ndarray):
+            planes = np.ascontiguousarray(planes, dtype=np.float32)
+        ptr, dev = _ptr(planes)
+        self._check(self.lib.gpm_set_planar_prior(self.h, ptr, 0, dev))
+
+    def planar_prior(self) -> np.ndarray:
+        m = np.empty((self.H, self.W, 4), dtype=np.float32)
+        self._check(self.lib.gpm_get_planar_prior(self.h, C.c_void_p(m.ctypes.data), 0))
+        return m
+
+    def build_planar_prior(self, step: int = PRIOR_DEFAULTS["step"], support_cost: float = PRIOR_DEFAULTS["support_cost"]) -> dict:
+        """Prior map from the stored state: the cheapest pixel of each step x step cell whose cost < support_cost, the
+        Delaunay triangulation of those pixels and each triangle's plane.  Returns the counts."""
+        check_prior_build(step, support_cost)
+        b, info = GpmPriorBuild(int(step), float(support_cost)), GpmPriorInfo()
+        self._check(self.lib.gpm_build_planar_prior(self.h, C.byref(b), C.byref(info)))
+        return {"support": info.support, "triangles": info.triangles, "with_prior": info.with_prior}
+
+    def offer_prior(self):
+        """Every pixel with a prior takes its prior plane where that plane costs strictly less than the stored one."""
+        self._check(self.lib.gpm_offer_prior(self.h))
 
     def view_masks(self) -> np.ndarray:
         """[H, W] uint64: bit j set where the last joint-view-selection launch selected view j."""
@@ -637,16 +749,18 @@ def _job_stats(n_refs):
 def batch_run(images, Ps, params, refs, devices=(0,), cam_scale: float = 1.0, min_angle: float = 10.0, max_angle: float = 30.0,
               max_views: int = 9, seed: int = 0xC0FFEE, out_dir: Optional[str] = None, want_outputs: bool = True,
               photometric: str = "pm", ncc_min_std: float = NCC_MIN_STD, propagation: str = "fixed",
-              view_selection: str = "off", jvs_params: Optional[dict] = None):
-    """Reference-view batch in ONE process (gpm_batch_run_vsel): `images` [n, H, W] float32 (shared, page-locked once), `Ps`
+              view_selection: str = "off", jvs_params: Optional[dict] = None, planar_prior: Optional[dict] = None):
+    """Reference-view batch in ONE process (gpm_batch_run_prior): `images` [n, H, W] float32 (shared, page-locked once), `Ps`
     n 3x4 projections, `refs` the reference views to process, `devices` the CUDA ordinals to use (one worker thread each),
     `photometric` the cost, "pm" or "ncc" with min_std `ncc_min_std` (Context.set_photometric), `propagation` "fixed" or
     "adaptive" (Context.set_propagation), `view_selection` "off" or "joint" with `jvs_params` overriding JVS_DEFAULTS
-    (Context.set_view_selection; "joint" needs photometric="ncc").
+    (Context.set_view_selection; "joint" needs photometric="ncc"), `planar_prior` None or a dict (prior_opts): a prior stage
+    after the params.iterations sweeps of every job (DESIGN.md §18), whose counts come back per job in stats["prior"].
     Returns (norm4 [len(refs), H, W, 4] or None, cost or None, stats dict)."""
     opts = job_opts(photometric, ncc_min_std, propagation)
     vsel = view_sel(view_selection, **(jvs_params or {}))
-    check_modes(photometric, view_selection, 1)
+    check_modes(photometric, view_selection, 1, planar_prior)
+    prior, pinfo = prior_opts(planar_prior, params, len(refs), photometric)
     lib = load_library()
     imgs = np.ascontiguousarray(images, dtype=np.float32)
     n, H, W = imgs.shape
@@ -654,19 +768,19 @@ def batch_run(images, Ps, params, refs, devices=(0,), cam_scale: float = 1.0, mi
     cc = np.empty((len(refs), H, W), np.float32) if want_outputs else None
     d, _keep = _batch_desc(imgs, Ps, params, refs, devices, cam_scale, min_angle, max_angle, max_views, seed, out_dir, n4, cc)
     st = _job_stats(len(refs))
-    rc = lib.gpm_batch_run_vsel(C.byref(d), C.byref(opts), C.byref(vsel), C.byref(st))
+    rc = lib.gpm_batch_run_prior(C.byref(d), C.byref(opts), C.byref(vsel), C.byref(prior) if prior else None, C.byref(st))
     if rc != 0:
         raise GipumaError("gpm_batch_run failed (%d): %s" % (rc, lib.gpm_batch_last_error().decode()))
     k = len(refs)
     return n4, cc, {"jobs_done": st.jobs_done, "sweep_ms_total": st.sweep_ms_total, "sweep_ms": st.per_job_sweep_ms[:k],
-                    "views": st.per_job_views[:k], "device": st.per_job_device[:k]}
+                    "views": st.per_job_views[:k], "device": st.per_job_device[:k], "prior": _prior_info(pinfo, k)}
 
 
 def geometric_pass(images, Ps, params, refs, geo_iterations: int = 2, weight: float = GEO_WEIGHT, max_err: float = GEO_MAX_ERR,
                    cam_scale: float = 1.0, min_angle: float = 10.0, max_angle: float = 30.0, max_views: int = 9,
                    seed: int = 0xC0FFEE, devices=(0,), out_dir: Optional[str] = None, photometric: str = "pm",
                    ncc_min_std: float = NCC_MIN_STD, propagation: str = "fixed", view_selection: str = "off",
-                   jvs_params: Optional[dict] = None):
+                   jvs_params: Optional[dict] = None, planar_prior: Optional[dict] = None):
     """PatchMatch with a geometric-consistency second pass (DESIGN.md §14) for the reference views `refs`, run by the
     native two-pass batch driver (gpm_geo_batch_run) over the worker pool of `devices` (one worker thread and context each;
     a device may be listed more than once).
@@ -679,7 +793,8 @@ def geometric_pass(images, Ps, params, refs, geo_iterations: int = 2, weight: fl
     arguments as batch_run; out_dir: None, or where <ref, 8 digits>/{disp,normals}.dmb of the pass-2 results are written;
     photometric / ncc_min_std: the photometric cost of both passes, as batch_run ("ncc": grey images only); propagation:
     the propagation mode of both passes, as batch_run; view_selection / jvs_params: the view selection of both passes, as
-    batch_run (pass 2 starts over at t = 0).
+    batch_run (pass 2 starts over at t = 0); planar_prior: a prior stage in pass 1 only, as batch_run (info["prior"]: the
+    counts per pass-1 view, in info["pass1_views"]' order).
     Returns (norm4 [len(refs), H, W, 4], cost [len(refs), H, W], info) with norm4 as batch_run returns it, so fuse and
     evaluate_cloud take it unchanged; info: "pass1_views" (the views pass 1 ran, ascending), "pass1_sweep_s" (in that order)
     and "pass2_sweep_s" (per reference view): CUDA-event seconds of each view's sweep call on its context's stream;
@@ -692,8 +807,9 @@ def geometric_pass(images, Ps, params, refs, geo_iterations: int = 2, weight: fl
     if imgs.ndim not in (3, 4) or (imgs.ndim == 4 and imgs.shape[3] != 4):
         raise ValueError("images must be [n, H, W] or [n, H, W, 4]")
     vsel = view_sel(view_selection, **(jvs_params or {}))
-    check_modes(photometric, view_selection, 4 if imgs.ndim == 4 else 1)
+    check_modes(photometric, view_selection, 4 if imgs.ndim == 4 else 1, planar_prior)
     n, H, W = imgs.shape[:3]
+    prior, pinfo = prior_opts(planar_prior, params, n, photometric)
     if len(Ps) != n:
         raise ValueError("one projection matrix per image is needed (%d images, %d matrices)" % (n, len(Ps)))
     refs = [int(r) for r in refs]
@@ -711,14 +827,14 @@ def geometric_pass(images, Ps, params, refs, geo_iterations: int = 2, weight: fl
     ref_views = (C.c_int * (k * int(max_views)))()
     jobs = _job_stats(k)                                   # owns the per-job arrays st.batch points into
     st = GpmGeoBatchStats(jobs, 0, p1_views, p1_ms, ref_views)
-    rc = lib.gpm_geo_batch_run_vsel(C.byref(g), C.byref(opts), C.byref(vsel), C.byref(st))
+    rc = lib.gpm_geo_batch_run_prior(C.byref(g), C.byref(opts), C.byref(vsel), C.byref(prior) if prior else None, C.byref(st))
     if rc != 0:
         raise GipumaError("gpm_geo_batch_run failed (%d): %s" % (rc, lib.gpm_batch_last_error().decode()))
     m = st.n_pass1
     views = [[v for v in ref_views[j * max_views:(j + 1) * max_views] if v >= 0] for j in range(k)]
     info = {"pass1_views": p1_views[:m], "pass1_sweep_s": [t / 1e3 for t in p1_ms[:m]],
             "pass2_sweep_s": [t / 1e3 for t in st.batch.per_job_sweep_ms[:k]], "views": views,
-            "device": st.batch.per_job_device[:k]}
+            "device": st.batch.per_job_device[:k], "prior": _prior_info(pinfo, m)}
     return n4, cc, info
 
 

@@ -42,7 +42,7 @@ def _run(cmd):
 
 def build_library(force: bool = False) -> str:
     src = [os.path.join(HERE, "csrc", f) for f in ("gpm_api.cu", "gpm_host.cpp", "gpm_batch.cpp", "gpm_fuse.cu", "gpm_cloud.cu",
-                                                   "gpm_kernels.cuh", "gpm_device.cuh")]
+                                                   "gpm_kernels.cuh", "gpm_device.cuh", "gpm_prior.cpp")]
     src.append(os.path.join(ROOT, "include", "gipuma_b200.h"))
     out = os.path.join(HERE, "libgipuma_b200.so")
     stamp = out + ".sig"
@@ -53,7 +53,7 @@ def build_library(force: bool = False) -> str:
         ieee_objs = [os.path.join(tmp, os.path.basename(s)[:-3] + ".o") for s in src[3:5]]
         for s, o in zip(src[3:5], ieee_objs):
             _run([NVCC] + FUSE + ["-o", o, s])
-        _run([NVCC] + COMMON + ["-o", out, src[0], src[1], src[2]] + ieee_objs + ["-lpthread"])
+        _run([NVCC] + COMMON + ["-o", out, src[0], src[1], src[2], src[7]] + ieee_objs + ["-lpthread"])
     with open(stamp, "w") as fh:
         fh.write(sig)
     return out

@@ -121,6 +121,11 @@ struct gpm_ctx {
     gpm_view_sel vsel{GPM_VSEL_OFF, 0.f, 0.f, 0.f, 0, 0, 0.f, 0.f};
     unsigned long long* vsel_mask = nullptr;   // [H*W] selected-views masks, allocated by the first switch to JOINT
     int vsel_t = 0;                            // iterations of gpm_sweep since gpm_init / gpm_set_state
+    // planar prior (DESIGN.md §18): on while prior_weight > 0 (gpm_set_prior); the map is uploaded or built
+    float4* prior_map = nullptr;               // [H*W], allocated by the first gpm_set_planar_prior / gpm_build_planar_prior
+    float* prior_cost = nullptr;               // [H*W] gpm_offer_prior's costs of the prior planes
+    float prior_weight = 0.f, prior_depth_sigma = 1.f, prior_normal_deg = 5.f;
+    bool have_state = false;                   // gpm_init, gpm_run or gpm_set_state has given every pixel a plane and a cost
 };
 
 namespace {
@@ -189,15 +194,17 @@ bool jvs_on(const gpm_ctx* c) { return c->vsel.kind == GPM_VSEL_JOINT; }
 // always names a mode with kernels.
 Mode ctx_mode(const gpm_ctx* c)
 {
-    return Mode{c->color == 1, c->opt_neighbours == 20, c->geo_weight > 0.f, ncc_on(c), c->propagation == GPM_PROP_ADAPTIVE, jvs_on(c)};
+    return Mode{c->color == 1, c->opt_neighbours == 20, c->geo_weight > 0.f, ncc_on(c), c->propagation == GPM_PROP_ADAPTIVE, jvs_on(c),
+                c->prior_weight > 0.f};
 }
 
 const char* conflict_text(ModeConflict k)
 {
     switch (k) {
-    case ModeConflict::fused: return "the geometric-consistency mode, the NCC cost, adaptive sampling and joint view selection support the 8-neighbour sweep only (option neighbours = 8)";
+    case ModeConflict::fused: return "the geometric-consistency mode, the NCC cost, adaptive sampling, joint view selection and the planar prior support the 8-neighbour sweep only (option neighbours = 8)";
     case ModeConflict::jvs_needs_ncc_grey: return "joint view selection is built for the NCC cost (GPM_PHOTO_NCC) on grey images";
     case ModeConflict::ncc_colour: return "the NCC photometric cost supports grey images only";
+    case ModeConflict::prior: return "the planar prior supports grey images without joint view selection";
     default: return nullptr;
     }
 }
@@ -211,6 +218,17 @@ int refuse_change(const gpm_ctx* c, const char* fn, bool Mode::*field, bool on)
     const ModeConflict k = mode_conflict(m);
     if (k == ModeConflict::none) return GPM_OK;
     return fail(field == &Mode::color && k == ModeConflict::ncc_colour ? GPM_E_STATE : GPM_E_ARG, std::string(fn) + ": " + conflict_text(k));
+}
+
+// The planar prior's bound (DESIGN.md §18): the largest valid cost of parameters p (PM: ns at the initialisation window
+// times the largest dissimilarity; NCC: 2) plus the geometric term's largest value plus the prior's weight stays below
+// MAXCOST, so that a valid cost with the term never reaches MAXCOST.  Checked by every setter that changes one of them.
+bool prior_bound_ok(const gpm_params& p, bool ncc, float geo_weight, float geo_max_err, float prior_weight)
+{
+    if (prior_weight <= 0.f) return true;
+    const int nside = p.box_hsize / 2 + 1;
+    const float top = ncc ? 2.0f : (float)(nside * nside) * ((1.0f - p.alpha) * p.tau_color + p.alpha * p.tau_gradient);
+    return top + geo_weight * geo_max_err + prior_weight < GPM_MAXCOST;
 }
 
 // per-warp floats of the JVS kernel variant the context launches (0 without view selection)
@@ -297,7 +315,8 @@ int build_kparams(gpm_ctx* c, bool init_phase, KParams& P, bool eval_call = fals
     // The lower bound counts a view as valid from its PARTIAL cost; a view whose final cost reaches MAXCOST (then excluded,
     // gipuma.cu:771-774) would make the bound exceed the final value.  Unreachable while ns * max dissimilarity < MAXCOST.
     // The geometric term adds at most weight * max_err to a view's final cost (0 outside that mode).
-    if ((float)P.ns * ((1.0f - p.alpha) * p.tau_color + p.alpha * p.tau_gradient) + c->geo_weight * c->geo_max_err >= GPM_MAXCOST) P.prune = 0;
+    // The planar prior adds less than its weight (DESIGN.md §18).
+    if ((float)P.ns * ((1.0f - p.alpha) * p.tau_color + p.alpha * p.tau_gradient) + c->geo_weight * c->geo_max_err + c->prior_weight >= GPM_MAXCOST) P.prune = 0;
     if (ncc_on(c)) P.prune = 0;                             // partial NCC sums bound nothing (DESIGN.md §15)
     P.dedupe_self = c->opt_dedupe ? 1 : 0;
     // rounding variant of k_cost_eval: at initialisation the reference's binary is y-first for float, x-first for float4;
@@ -397,6 +416,17 @@ JvsParams jvs_params(const gpm_ctx* c)
     return J;
 }
 
+// the planar prior's parameters (DESIGN.md §18): 1 - cos(sigma_n) in double, rounded once
+PriorParams prior_params(const gpm_ctx* c)
+{
+    PriorParams R{};
+    R.map = c->prior_map;
+    R.weight = c->prior_weight;
+    R.depth_sigma = c->prior_depth_sigma;
+    R.normal_scale = (float)(1.0 - std::cos((double)c->prior_normal_deg * 3.14159265358979323846 / 180.0));
+    return R;
+}
+
 // Kernel tables: entry Mode::bits() is the family's kernel for that mode, nullptr (refused, never launched) where it has
 // none.  k_sweep and k_cost_eval exist for the modes mode_conflict() passes (k_cost_eval reads neither the propagation, the
 // view selection nor the fused sweep), k_shard_stage for those shard_supports() passes.
@@ -405,12 +435,12 @@ auto make_table(Entry entry, std::integer_sequence<int, B...>) { return std::arr
 
 const auto kSweep = make_table([](auto b) -> decltype(&k_sweep<false, false>) {
     constexpr Mode m = Mode::of(decltype(b)::value);
-    if constexpr (mode_conflict(m) == ModeConflict::none) return k_sweep<m.color, m.fused, m.geo, m.ncc, m.adaptive, m.jvs>; else return nullptr;
+    if constexpr (mode_conflict(m) == ModeConflict::none) return k_sweep<m.color, m.fused, m.geo, m.ncc, m.adaptive, m.jvs, m.prior>; else return nullptr;
 }, std::make_integer_sequence<int, GPM_MODES>{});
 
 const auto kCostEval = make_table([](auto b) -> decltype(&k_cost_eval<false>) {
     constexpr Mode m = Mode::of(decltype(b)::value);
-    if constexpr (mode_conflict(m) == ModeConflict::none) return k_cost_eval<m.color, m.geo, m.ncc>; else return nullptr;
+    if constexpr (mode_conflict(m) == ModeConflict::none) return k_cost_eval<m.color, m.geo, m.ncc, m.prior>; else return nullptr;
 }, std::make_integer_sequence<int, GPM_MODES>{});
 
 const auto kShardStage = make_table([](auto b) -> decltype(&k_shard_stage<false>) {
@@ -424,7 +454,7 @@ int launch_colour(gpm_ctx* c, const KParams& P, int colour, int mask)
     if (!kern) return fail(GPM_E_STATE, "k_sweep has no kernel for this context's mode");
     kern<<<tile_grid(c), P.nwarps * 32, block_smem_bytes(P, ncc_on(c), jvs_extra(c)), c->stream>>>(P, c->tmap, c->d_cams, c->srcTex, c->planes,
         c->cost, c->rng, c->prov, Memo{c->pid, c->seen, c->refseen, c->memo_mask, c->next_id}, colour, mask, c->d_stats, geo_params(c),
-        jvs_params(c));
+        jvs_params(c), prior_params(c));
     c->launches++;
     CU(cudaGetLastError());
     return GPM_OK;
@@ -436,7 +466,8 @@ int launch_cost_eval(gpm_ctx* c, const KParams& P, const float4* planes, float* 
     const auto kern = kCostEval[ctx_mode(c).bits()];
     if (!kern) return fail(GPM_E_STATE, "k_cost_eval has no kernel for this context's mode");
     dim3 grid((P.W + GPM_TILE - 1) / GPM_TILE, (P.H + GPM_TILE - 1) / GPM_TILE);
-    kern<<<grid, P.nwarps * 32, block_smem_bytes(P, ncc_on(c)), c->stream>>>(P, c->tmap, c->d_cams, c->srcTex, planes, cost, nullptr, geo_params(c));
+    kern<<<grid, P.nwarps * 32, block_smem_bytes(P, ncc_on(c)), c->stream>>>(P, c->tmap, c->d_cams, c->srcTex, planes, cost, nullptr, geo_params(c),
+                                                                            prior_params(c));
     c->launches++;
     CU(cudaGetLastError());
     return GPM_OK;
@@ -609,6 +640,7 @@ extern "C" void gpm_destroy(gpm_ctx* c)
     if (c->srcArr) cudaFreeArray(c->srcArr);
     cudaFree(c->planar);
     cudaFree(c->planes);  cudaFree(c->cost);  cudaFree(c->prov);  cudaFree(c->seen);  cudaFree(c->refseen);  cudaFree(c->pid);  cudaFree(c->next_id);  cudaFree(c->memo_mask);  cudaFree(c->rng);  cudaFree(c->dispbuf);  cudaFree(c->candbuf);  cudaFree(c->canddepth);  cudaFree(c->sflags);  cudaFree(c->xchg);  cudaFree(c->gath);  cudaFree(c->refpad);  cudaFree(c->staging);  cudaFree(c->geo_depth);  cudaFree(c->geo_kinv);  cudaFree(c->vsel_mask);
+    cudaFree(c->prior_map);  cudaFree(c->prior_cost);
     cudaFree(c->d_cams);  cudaFree(c->d_stats);
     if (c->ev0) cudaEventDestroy(c->ev0);
     if (c->ev1) cudaEventDestroy(c->ev1);
@@ -625,6 +657,8 @@ extern "C" int gpm_set_params(gpm_ctx* c, const gpm_params* p)
         return fail(GPM_E_ARG, "box size must be odd, 3.." + std::to_string(GPM_MAX_BOX));
     if (p->cost_comb < 0 || p->cost_comb > 3) return fail(GPM_E_ARG, "cost_comb must be 0..3");
     if (p->iterations < 0) return fail(GPM_E_ARG, "iterations must be >= 0");
+    if (!prior_bound_ok(*p, ncc_on(c), c->geo_weight, c->geo_max_err, c->prior_weight))
+        return fail(GPM_E_ARG, "gpm_set_params: with the planar prior's weight a valid cost could reach MAXCOST");
     c->prm = *p;
     c->have_params = true;
     c->inputs_dirty = true;                          // the cost function depends on the parameters: stored costs / memo are stale
@@ -786,16 +820,30 @@ const char* view_sel_refusal(const gpm_view_sel* v)
     return nullptr;
 }
 
+const char* prior_refusal(float weight, float depth_sigma, float normal_sigma_deg);
+const char* prior_build_refusal(const gpm_prior_build* b);
+
+// The batch drivers' prior stage (NULL: none): gpm_set_prior's and gpm_build_planar_prior's argument rules, and iterations.
+const char* prior_opts_refusal(const gpm_prior_opts* p)
+{
+    if (!p) return nullptr;
+    if (const char* bad = prior_refusal(p->weight, p->depth_sigma, p->normal_sigma_deg)) return bad;
+    const gpm_prior_build b{p->step, p->support_cost};
+    if (const char* bad = prior_build_refusal(&b)) return bad;
+    return p->iterations < 0 ? "prior iterations must be >= 0" : nullptr;
+}
+
 // What the batch drivers refuse for a job's options before any CUDA call: the setters' argument checks and the mode rule,
-// for grey (channels 1) or colour (channels 4) images.
-const char* job_refusal(const gpm_job_opts* o, const gpm_view_sel* v, int channels)
+// for grey (channels 1) or colour (channels 4) images; a prior stage counts as the planar-prior mode.
+const char* job_refusal(const gpm_job_opts* o, const gpm_view_sel* v, const gpm_prior_opts* prior, int channels)
 {
     if (!o) return "opts is NULL";
     if (const char* bad = photometric_refusal(o->photometric, o->ncc_min_std)) return bad;
     if (const char* bad = propagation_refusal(o->propagation)) return bad;
     if (const char* bad = view_sel_refusal(v)) return bad;
+    if (const char* bad = prior_opts_refusal(prior)) return bad;
     return conflict_text(mode_conflict(Mode{channels == 4, false, false, o->photometric == GPM_PHOTO_NCC,
-                                            o->propagation == GPM_PROP_ADAPTIVE, v->kind == GPM_VSEL_JOINT}));
+                                            o->propagation == GPM_PROP_ADAPTIVE, v->kind == GPM_VSEL_JOINT, prior != nullptr}));
 }
 }  // namespace gpm
 
@@ -807,6 +855,8 @@ extern "C" int gpm_set_geometric(gpm_ctx* c, float weight, float max_err)
     if (weight > 0.f && c->shard_world > 0) return fail(GPM_E_STATE, "gpm_set_geometric: view sharding does not support the geometric-consistency mode");
     if (const int rc = refuse_change(c, "gpm_set_geometric", &Mode::geo, weight > 0.f)) return rc;
     if (const int rc = check_depth_maps(c, weight)) return rc;
+    if (c->have_params && !prior_bound_ok(c->prm, ncc_on(c), weight, max_err, c->prior_weight))
+        return fail(GPM_E_ARG, "gpm_set_geometric: with the planar prior's weight a valid cost could reach MAXCOST");
     if (weight != c->geo_weight || max_err != c->geo_max_err) c->inputs_dirty = true;
     c->geo_weight = weight;
     c->geo_max_err = max_err;
@@ -818,6 +868,8 @@ extern "C" int gpm_set_photometric(gpm_ctx* c, int kind, float min_std)
     if (!c) return fail(GPM_E_ARG, "gpm_set_photometric: null context");
     if (const char* bad = photometric_refusal(kind, min_std)) return fail(GPM_E_ARG, std::string("gpm_set_photometric: ") + bad);
     if (const int rc = refuse_change(c, "gpm_set_photometric", &Mode::ncc, kind == GPM_PHOTO_NCC)) return rc;
+    if (c->have_params && !prior_bound_ok(c->prm, kind == GPM_PHOTO_NCC, c->geo_weight, c->geo_max_err, c->prior_weight))
+        return fail(GPM_E_ARG, "gpm_set_photometric: with the planar prior's weight a valid cost could reach MAXCOST");
     if (kind == GPM_PHOTO_PM) min_std = 0.f;         // not read by the PM cost
     if (kind != c->photo || min_std != c->ncc_min_std) c->inputs_dirty = true;
     c->photo = kind;
@@ -864,6 +916,184 @@ extern "C" int gpm_get_view_masks(gpm_ctx* c, unsigned long long* masks)
     return GPM_OK;
 }
 
+// ---- planar prior (DESIGN.md §18) ---------------------------------------------------------------------------------
+namespace gpm {
+std::vector<std::array<int, 3>> delaunay(const std::vector<int>& xy);
+std::array<float, 4> triangle_plane(const float* Kinv, const int* x, const int* y, const float* const* plane);
+
+const char* prior_refusal(float weight, float depth_sigma, float normal_sigma_deg)
+{
+    if (!std::isfinite(weight) || weight < 0.f) return "weight must be finite and >= 0";
+    if (!std::isfinite(depth_sigma) || depth_sigma <= 0.f) return "depth_sigma must be finite and > 0";
+    if (!std::isfinite(normal_sigma_deg) || normal_sigma_deg <= 0.f || normal_sigma_deg > 90.f) return "normal_sigma_deg must be in (0, 90]";
+    return nullptr;
+}
+
+const char* prior_build_refusal(const gpm_prior_build* b)
+{
+    if (!b) return "build is NULL";
+    if (b->step < 1 || b->step > 64) return "step must be 1..64";
+    if (b->support_cost != b->support_cost) return "support_cost must not be NaN";
+    return nullptr;
+}
+}  // namespace gpm
+
+static int ensure_prior_map(gpm_ctx* c)
+{
+    if (c->prior_map) return GPM_OK;
+    const size_t n = (size_t)c->W * c->H;
+    CU(cudaMalloc(&c->prior_map, n * sizeof(float4)));
+    CU(cudaMemsetAsync(c->prior_map, 0, n * sizeof(float4), c->stream));
+    return GPM_OK;
+}
+
+extern "C" int gpm_set_planar_prior(gpm_ctx* c, const float* planes, size_t pitch_bytes, int on_device)
+{
+    if (!c || !planes) return fail(GPM_E_ARG, "gpm_set_planar_prior: null argument");
+    const size_t row = (size_t)c->W * sizeof(float4);
+    if (pitch_bytes == 0) pitch_bytes = row;
+    if (pitch_bytes < row) return fail(GPM_E_ARG, "gpm_set_planar_prior: pitch_bytes is smaller than a row");
+    DeviceGuard g(c->device);
+    if (const int rc = ensure_prior_map(c)) return rc;
+    CU(cudaMemcpy2DAsync(c->prior_map, row, planes, pitch_bytes, row, c->H, on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice,
+                         c->stream));
+    CU(cudaStreamSynchronize(c->stream));
+    if (c->prior_weight > 0.f) c->inputs_dirty = true;     // the cost function reads the map: stored costs / memo are stale
+    return GPM_OK;
+}
+
+extern "C" int gpm_get_planar_prior(gpm_ctx* c, float* planes, int on_device)
+{
+    if (!c || !planes) return fail(GPM_E_ARG, "gpm_get_planar_prior: null argument");
+    if (!c->prior_map) return fail(GPM_E_STATE, "gpm_get_planar_prior: no prior map (gpm_set_planar_prior or gpm_build_planar_prior)");
+    DeviceGuard g(c->device);
+    CU(cudaMemcpyAsync(planes, c->prior_map, (size_t)c->W * c->H * sizeof(float4), on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost,
+                       c->stream));
+    CU(cudaStreamSynchronize(c->stream));
+    return GPM_OK;
+}
+
+extern "C" int gpm_set_prior(gpm_ctx* c, float weight, float depth_sigma, float normal_sigma_deg)
+{
+    if (!c) return fail(GPM_E_ARG, "gpm_set_prior: null context");
+    if (const char* bad = prior_refusal(weight, depth_sigma, normal_sigma_deg)) return fail(GPM_E_ARG, std::string("gpm_set_prior: ") + bad);
+    if (weight > 0.f && c->shard_world > 0) return fail(GPM_E_STATE, "gpm_set_prior: view sharding does not support the planar prior");
+    if (const int rc = refuse_change(c, "gpm_set_prior", &Mode::prior, weight > 0.f)) return rc;
+    if (weight > 0.f && !c->prior_map) return fail(GPM_E_STATE, "gpm_set_prior: no prior map (gpm_set_planar_prior or gpm_build_planar_prior)");
+    if (c->have_params && !prior_bound_ok(c->prm, ncc_on(c), c->geo_weight, c->geo_max_err, weight))
+        return fail(GPM_E_ARG, "gpm_set_prior: weight would let a valid cost reach MAXCOST");
+    if (weight != c->prior_weight || (weight > 0.f && (depth_sigma != c->prior_depth_sigma || normal_sigma_deg != c->prior_normal_deg)))
+        c->inputs_dirty = true;
+    c->prior_weight = weight;
+    c->prior_depth_sigma = depth_sigma;
+    c->prior_normal_deg = normal_sigma_deg;
+    return GPM_OK;
+}
+
+// Support points (GPU), Delaunay triangulation and triangle planes (host), rasterisation (GPU), from the stored state.
+extern "C" int gpm_build_planar_prior(gpm_ctx* c, const gpm_prior_build* b, gpm_prior_info* info)
+{
+    if (!c) return fail(GPM_E_ARG, "gpm_build_planar_prior: null context");
+    if (const char* bad = prior_build_refusal(b)) return fail(GPM_E_ARG, std::string("gpm_build_planar_prior: ") + bad);
+    if (c->W > 4097 || c->H > 4097) return fail(GPM_E_ARG, "gpm_build_planar_prior: images wider or taller than 4097 pixels are not supported");
+    if (!c->have_params || !c->have_ref) return fail(GPM_E_STATE, "gpm_build_planar_prior: gpm_set_params and gpm_set_reference first");
+    if (!c->have_state) return fail(GPM_E_STATE, "gpm_build_planar_prior: no state to build from (gpm_init, gpm_run or gpm_set_state)");
+    DeviceGuard g(c->device);
+    KParams P{};
+    P.W = c->W;  P.H = c->H;
+    P.ref = c->ref;
+    P.ref.depthMin = c->prm.depthMin;  P.ref.depthMax = c->prm.depthMax;
+    const int step = b->step, cells_x = (c->W + step - 1) / step, cells_y = (c->H + step - 1) / step, ncell = cells_x * cells_y;
+    int* d_at = nullptr;
+    float4* d_pl = nullptr;
+    int* d_tri = nullptr;
+    float4* d_tpl = nullptr;
+    unsigned long long* d_cnt = nullptr;
+    auto release = [&]() { cudaFree(d_at);  cudaFree(d_pl);  cudaFree(d_tri);  cudaFree(d_tpl);  cudaFree(d_cnt); };
+    auto cuda = [&](cudaError_t e, const char* what) -> int {
+        if (e == cudaSuccess) return GPM_OK;
+        release();
+        return fail(GPM_E_CUDA, std::string("gpm_build_planar_prior: ") + what + ": " + cudaGetErrorString(e));
+    };
+    if (int rc = ensure_prior_map(c)) return rc;
+    if (int rc = cuda(cudaMalloc(&d_at, ncell * sizeof(int)), "cudaMalloc")) return rc;
+    if (int rc = cuda(cudaMalloc(&d_pl, ncell * sizeof(float4)), "cudaMalloc")) return rc;
+    if (int rc = cuda(cudaMalloc(&d_cnt, sizeof(unsigned long long)), "cudaMalloc")) return rc;
+    dim3 blk(16, 16), grd((cells_x + 15) / 16, (cells_y + 15) / 16);
+    k_prior_support<<<grd, blk, 0, c->stream>>>(P, c->planes, c->cost, step, b->support_cost, cells_x, cells_y, d_at, d_pl);
+    c->launches++;
+    if (int rc = cuda(cudaGetLastError(), "k_prior_support")) return rc;
+    std::vector<int> at(ncell);
+    std::vector<float4> pl(ncell);
+    if (int rc = cuda(cudaMemcpyAsync(at.data(), d_at, ncell * sizeof(int), cudaMemcpyDeviceToHost, c->stream), "cudaMemcpy")) return rc;
+    if (int rc = cuda(cudaMemcpyAsync(pl.data(), d_pl, ncell * sizeof(float4), cudaMemcpyDeviceToHost, c->stream), "cudaMemcpy")) return rc;
+    if (int rc = cuda(cudaStreamSynchronize(c->stream), "support points")) return rc;
+    std::vector<int> xy;
+    std::vector<float4> spl;
+    for (int k = 0; k < ncell; k++)
+        if (at[k] >= 0) { xy.push_back(at[k] % c->W);  xy.push_back(at[k] / c->W);  spl.push_back(pl[k]); }
+    std::vector<std::array<int, 3>> tris;
+    try { tris = delaunay(xy); } catch (const std::exception& e) { release();  return fail(GPM_E_STATE, std::string("gpm_build_planar_prior: triangulation failed: ") + e.what()); }
+    const int ntri = (int)tris.size();
+    std::vector<int> tv(6 * (size_t)std::max(ntri, 1));
+    std::vector<float4> tp(std::max(ntri, 1));
+    for (int t = 0; t < ntri; t++) {
+        int x[3], y[3];
+        const float* pp[3];
+        for (int i = 0; i < 3; i++) {
+            x[i] = xy[2 * tris[t][i]];  y[i] = xy[2 * tris[t][i] + 1];
+            pp[i] = &spl[tris[t][i]].x;
+            tv[6 * t + 2 * i] = x[i];  tv[6 * t + 2 * i + 1] = y[i];
+        }
+        const std::array<float, 4> q = triangle_plane(c->ref.K_inv, x, y, pp);
+        tp[t] = make_float4(q[0], q[1], q[2], q[3]);
+    }
+    if (int rc = cuda(cudaMemsetAsync(c->prior_map, 0, (size_t)c->W * c->H * sizeof(float4), c->stream), "cudaMemset")) return rc;
+    if (int rc = cuda(cudaMemsetAsync(d_cnt, 0, sizeof(unsigned long long), c->stream), "cudaMemset")) return rc;
+    if (ntri > 0) {
+        if (int rc = cuda(cudaMalloc(&d_tri, tv.size() * sizeof(int)), "cudaMalloc")) return rc;
+        if (int rc = cuda(cudaMalloc(&d_tpl, tp.size() * sizeof(float4)), "cudaMalloc")) return rc;
+        if (int rc = cuda(cudaMemcpyAsync(d_tri, tv.data(), tv.size() * sizeof(int), cudaMemcpyHostToDevice, c->stream), "cudaMemcpy")) return rc;
+        if (int rc = cuda(cudaMemcpyAsync(d_tpl, tp.data(), tp.size() * sizeof(float4), cudaMemcpyHostToDevice, c->stream), "cudaMemcpy")) return rc;
+        k_prior_raster<<<(ntri + 127) / 128, 128, 0, c->stream>>>(P, d_tri, d_tpl, ntri, c->prior_map, d_cnt);
+        c->launches++;
+        if (int rc = cuda(cudaGetLastError(), "k_prior_raster")) return rc;
+    }
+    unsigned long long with = 0;
+    if (int rc = cuda(cudaMemcpyAsync(&with, d_cnt, sizeof(with), cudaMemcpyDeviceToHost, c->stream), "cudaMemcpy")) return rc;
+    if (int rc = cuda(cudaStreamSynchronize(c->stream), "rasterisation")) return rc;
+    release();
+    if (c->prior_weight > 0.f) c->inputs_dirty = true;
+    if (info) { info->support = (long long)spl.size();  info->triangles = ntri;  info->with_prior = (long long)with; }
+    return GPM_OK;
+}
+
+// Every pixel with a prior takes its prior plane where that plane's cost under the context's mode is strictly lower.
+extern "C" int gpm_offer_prior(gpm_ctx* c)
+{
+    if (!c) return fail(GPM_E_ARG, "gpm_offer_prior: null context");
+    if (!c->prior_map) return fail(GPM_E_STATE, "gpm_offer_prior: no prior map (gpm_set_planar_prior or gpm_build_planar_prior)");
+    DeviceGuard g(c->device);
+    KParams P;
+    int rc = build_kparams(c, false, P);
+    if (rc) return rc;
+    rc = sync_cams(c);
+    if (rc) return rc;
+    if (!c->prior_cost) CU(cudaMalloc(&c->prior_cost, (size_t)c->W * c->H * sizeof(float)));
+    rc = launch_cost_eval(c, P, c->prior_map, c->prior_cost);
+    if (rc) return rc;
+    dim3 b(16, 16), gr((c->W + 15) / 16, (c->H + 15) / 16);
+    // provenance: the rounding variant k_cost_eval just used (bit 0 x-first, bit 1 gradient folding), or NCC's own tag
+    const unsigned site = ncc_on(c) ? GPM_PROV_NCC : (unsigned)(P.cost_variant | (P.grad_variant << 1));
+    k_offer_prior<<<gr, b, 0, c->stream>>>(P, c->prior_map, c->prior_cost, c->planes, c->cost, c->prov, site, c->pid, c->next_id);
+    c->launches++;
+    CU(cudaGetLastError());
+    k_advance_ids<<<1, 1, 0, c->stream>>>(c->next_id, (unsigned)((size_t)c->W * c->H));
+    CU(cudaGetLastError());
+    CU(cudaStreamSynchronize(c->stream));
+    return GPM_OK;
+}
+
 extern "C" int gpm_set_state(gpm_ctx* c, const float* norm4, const float* cost, int on_device)
 {
     if (!c) return fail(GPM_E_ARG, "gpm_set_state: null context");
@@ -876,6 +1106,7 @@ extern "C" int gpm_set_state(gpm_ctx* c, const float* norm4, const float* cost, 
         if (rc) return rc;
     }
     if (cost) CU(cudaMemcpyAsync(c->cost, cost, n * sizeof(float), k, c->stream));
+    if (norm4 && cost) c->have_state = true;
     // provenance of the supplied costs is unknown (GPM_PROV_UNKNOWN) unless the caller vouches that they came from an
     // initialisation / refinement evaluation of exactly these planes ("trust_state": 0)
     int rc = reset_state_tags(c, c->opt_trust_state ? init_prov(c) : GPM_PROV_UNKNOWN);
@@ -913,6 +1144,7 @@ static int do_init(gpm_ctx* c)
     rc = clear_vsel_masks(c);                      // view selection starts over: no view selected, t = 0
     if (rc) return rc;
     c->vsel_t = 0;
+    c->have_state = true;
     return reset_state_tags(c, init_prov(c));     // costs now come from the init-variant evaluation (float4: x-first + gradient folding 1; NCC: its own)
 }
 
@@ -1056,7 +1288,7 @@ static int shard_refuses_state(gpm_ctx* c)
 {
     Mode m = ctx_mode(c);
     m.fused = false;
-    return shard_supports(m) ? GPM_OK : fail(GPM_E_STATE, "view sharding supports neither the geometric-consistency mode, the NCC cost nor joint view selection");
+    return shard_supports(m) ? GPM_OK : fail(GPM_E_STATE, "view sharding supports neither the geometric-consistency mode, the NCC cost, joint view selection nor the planar prior");
 }
 
 extern "C" int gpm_shard_num_stages(gpm_ctx* c)

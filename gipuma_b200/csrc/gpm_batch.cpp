@@ -8,7 +8,8 @@
 // (gpm_run) and hands back / writes the result (disp.dmb + normals.dmb, main.cpp:1002-1003, for the external fusibile).
 // gpm_geo_batch_run runs the two-pass geometric-consistency flow (DESIGN.md §14) on the same pool and image cache.  The
 // _photo twins of both choose the photometric cost (DESIGN.md §15), the _opts ones every per-job option (gpm_job_opts):
-// the photometric cost and the propagation mode (§16), and the _vsel ones the view selection besides (§17).
+// the photometric cost and the propagation mode (§16), the _vsel ones the view selection besides (§17), and the _prior
+// ones a planar-prior stage in every photometric job besides (§18).
 // Host C++ over the C-ABI; the only CUDA calls are page-locking, the geometric driver's host store and its sweep events.
 #include "../../include/gipuma_b200.h"
 
@@ -27,7 +28,7 @@
 #include <sys/stat.h>
 
 namespace gpm {
-const char* job_refusal(const gpm_job_opts* o, const gpm_view_sel* v, int channels);     // gpm_api.cu
+const char* job_refusal(const gpm_job_opts* o, const gpm_view_sel* v, const gpm_prior_opts* prior, int channels);     // gpm_api.cu
 }
 
 namespace {
@@ -166,79 +167,6 @@ extern "C" const char* gpm_batch_last_error(void)
     return copy.c_str();
 }
 
-// gpm_batch_run and its _photo / _opts / _vsel twins; `fn` names the entry point in error messages
-static int batch_run(const char* fn, const gpm_batch_desc* d, const gpm_job_opts* opts, const gpm_view_sel* vsel, gpm_batch_stats* stats)
-{
-    clear_err();
-    if (!batch_desc_ok(d)) {
-        set_err(std::string(fn) + ": bad arguments");
-        return GPM_E_ARG;
-    }
-    if (const char* bad = gpm::job_refusal(opts, vsel, 1)) {
-        set_err(std::string(fn) + ": bad arguments: " + bad);
-        return GPM_E_ARG;
-    }
-    const int n = d->n_images, W = d->width, H = d->height;
-    const size_t pitch = d->pitch_bytes ? d->pitch_bytes : (size_t)W * sizeof(float);
-    const size_t npix = (size_t)W * H;
-    PinnedImages pinned(d, pitch * H);
-
-    std::atomic<int> next(0), failed(0);
-    std::vector<double> sweep_ms(d->n_refs, 0.0);
-    std::vector<int> views_used(d->n_refs, 0), device_of(d->n_refs, -1);
-    run_workers(d, failed, [&](gpm_ctx* ctx, int dev) {
-        ViewSetup s;
-        std::vector<float> n4;
-        take_jobs(next, d->n_refs, failed, [&](int job) {
-            const int ref = d->ref_indices ? d->ref_indices[job] : job;
-            if (ref < 0 || ref >= n) { set_err(std::string(fn) + ": reference index out of range");  return false; }
-            if (!plan_view(d, ref, s)) { set_err(std::string(fn) + ": no source view passes the angle filter for reference " + std::to_string(ref));  return false; }
-            int rc = load_view(ctx, d, 1, pitch, s, *opts, *vsel);
-            float ms = 0.f;
-            if (rc == GPM_OK) rc = gpm_run(ctx, &ms);
-            if (rc != GPM_OK) { set_err(std::string("reference view ") + std::to_string(ref) + ": " + gpm_last_error());  return false; }
-            sweep_ms[job] = ms;  views_used[job] = s.nv;  device_of[job] = dev;
-            float* o4 = d->out_norm4 ? d->out_norm4 + (size_t)job * npix * 4 : nullptr;
-            float* oc = d->out_cost ? d->out_cost + (size_t)job * npix : nullptr;
-            if (d->out_dir && !o4) { n4.resize(npix * 4);  o4 = n4.data(); }
-            if (o4 || oc) rc = gpm_get_state(ctx, o4, oc, 0);
-            if (rc == GPM_OK && d->out_dir) rc = write_result(d->out_dir, ref, o4, H, W);
-            if (rc != GPM_OK) { set_err(std::string(fn) + ": could not store the result of reference view " + std::to_string(ref));  return false; }
-            return true;
-        });
-    });
-    if (stats) {
-        stats->jobs_done = 0;  stats->sweep_ms_total = 0.0;
-        for (int j = 0; j < d->n_refs; j++) if (device_of[j] >= 0) { stats->jobs_done++;  stats->sweep_ms_total += sweep_ms[j]; }
-        if (stats->per_job_sweep_ms) for (int j = 0; j < d->n_refs; j++) stats->per_job_sweep_ms[j] = (float)sweep_ms[j];
-        if (stats->per_job_views) for (int j = 0; j < d->n_refs; j++) stats->per_job_views[j] = views_used[j];
-        if (stats->per_job_device) for (int j = 0; j < d->n_refs; j++) stats->per_job_device[j] = device_of[j];
-    }
-    return failed.load() ? GPM_E_STATE : GPM_OK;
-}
-
-extern "C" int gpm_batch_run(const gpm_batch_desc* d, gpm_batch_stats* stats)
-{
-    const gpm_job_opts o = photo_opts(GPM_PHOTO_PM, 0.f);
-    return batch_run("gpm_batch_run", d, &o, &kVselOff, stats);
-}
-
-extern "C" int gpm_batch_run_photo(const gpm_batch_desc* d, int kind, float min_std, gpm_batch_stats* stats)
-{
-    const gpm_job_opts o = photo_opts(kind, min_std);
-    return batch_run("gpm_batch_run_photo", d, &o, &kVselOff, stats);
-}
-
-extern "C" int gpm_batch_run_opts(const gpm_batch_desc* d, const gpm_job_opts* opts, gpm_batch_stats* stats)
-{
-    return batch_run("gpm_batch_run_opts", d, opts, &kVselOff, stats);
-}
-
-extern "C" int gpm_batch_run_vsel(const gpm_batch_desc* d, const gpm_job_opts* opts, const gpm_view_sel* vsel, gpm_batch_stats* stats)
-{
-    return batch_run("gpm_batch_run_vsel", d, opts, vsel ? vsel : &kVselOff, stats);
-}
-
 // ---- two-pass geometric-consistency batch (DESIGN.md §14) -----------------------------------------------------------------
 namespace {
 // Page-locked host memory (portable: every device's context may copy from it) for the lifetime of this object.
@@ -294,11 +222,126 @@ private:
     int cuda_fail() { error = std::string("sweep event: ") + cudaGetErrorString(cudaGetLastError());  return GPM_E_CUDA; }
     cudaEvent_t a_ = nullptr, b_ = nullptr;
 };
+
+// The prior stage of a photometric job (DESIGN.md §18), after its params.iterations sweeps: the prior map built from the
+// state, the term on, the state re-scored under it (gpm_cost_eval + gpm_set_state), the prior planes offered, and
+// prior->iterations more sweeps.  The caller finalizes and then turns the term off (prior_off).
+int prior_stage(gpm_ctx* ctx, const gpm_prior_opts* p, gpm_prior_info* info, std::vector<float>& n4, std::vector<float>& cost,
+                SweepTimer& timer, float* ms)
+{
+    const gpm_prior_build b{p->step, p->support_cost};
+    int rc = gpm_build_planar_prior(ctx, &b, info);
+    if (rc == GPM_OK) rc = gpm_set_prior(ctx, p->weight, p->depth_sigma, p->normal_sigma_deg);
+    if (rc == GPM_OK) rc = gpm_get_state(ctx, n4.data(), nullptr, 0);
+    if (rc == GPM_OK) rc = gpm_cost_eval(ctx, n4.data(), cost.data(), 0);
+    if (rc == GPM_OK) rc = gpm_set_state(ctx, n4.data(), cost.data(), 0);
+    if (rc == GPM_OK) rc = gpm_offer_prior(ctx);
+    if (rc == GPM_OK) rc = timer.sweep(ctx, p->iterations, ms);
+    return rc;
+}
+int prior_off(gpm_ctx* ctx, const gpm_prior_opts* p) { return gpm_set_prior(ctx, 0.f, p->depth_sigma, p->normal_sigma_deg); }
 }  // namespace
+
+// gpm_batch_run and its _photo / _opts / _vsel / _prior twins; `fn` names the entry point in error messages
+static int batch_run(const char* fn, const gpm_batch_desc* d, const gpm_job_opts* opts, const gpm_view_sel* vsel,
+                     const gpm_prior_opts* prior, gpm_batch_stats* stats)
+{
+    clear_err();
+    if (!batch_desc_ok(d)) {
+        set_err(std::string(fn) + ": bad arguments");
+        return GPM_E_ARG;
+    }
+    if (const char* bad = gpm::job_refusal(opts, vsel, prior, 1)) {
+        set_err(std::string(fn) + ": bad arguments: " + bad);
+        return GPM_E_ARG;
+    }
+    const int n = d->n_images, W = d->width, H = d->height;
+    const size_t pitch = d->pitch_bytes ? d->pitch_bytes : (size_t)W * sizeof(float);
+    const size_t npix = (size_t)W * H;
+    PinnedImages pinned(d, pitch * H);
+
+    std::atomic<int> next(0), failed(0);
+    std::vector<double> sweep_ms(d->n_refs, 0.0);
+    std::vector<int> views_used(d->n_refs, 0), device_of(d->n_refs, -1);
+    run_workers(d, failed, [&](gpm_ctx* ctx, int dev) {
+        if (ctx && prior) cudaSetDevice(dev);            // the prior stage's sweep events live on the context's device
+        ViewSetup s;
+        SweepTimer timer;
+        std::vector<float> n4, cost(ctx && prior ? npix : 0);
+        if (ctx && prior) n4.resize(npix * 4);
+        take_jobs(next, d->n_refs, failed, [&](int job) {
+            const int ref = d->ref_indices ? d->ref_indices[job] : job;
+            if (ref < 0 || ref >= n) { set_err(std::string(fn) + ": reference index out of range");  return false; }
+            if (!plan_view(d, ref, s)) { set_err(std::string(fn) + ": no source view passes the angle filter for reference " + std::to_string(ref));  return false; }
+            int rc = load_view(ctx, d, 1, pitch, s, *opts, *vsel);
+            float ms = 0.f, ms2 = 0.f;
+            if (!prior) {
+                if (rc == GPM_OK) rc = gpm_run(ctx, &ms);
+            } else {                                     // gpm_run's steps with the prior stage before the finalize
+                if (rc == GPM_OK) rc = gpm_init(ctx);
+                if (rc == GPM_OK) rc = timer.sweep(ctx, d->params.iterations, &ms);
+                if (rc == GPM_OK) rc = prior_stage(ctx, prior, prior->info ? prior->info + job : nullptr, n4, cost, timer, &ms2);
+                if (rc == GPM_OK) rc = gpm_finalize(ctx);
+                if (rc == GPM_OK) rc = prior_off(ctx, prior);
+                ms += ms2;
+            }
+            if (rc != GPM_OK) {
+                set_err(std::string("reference view ") + std::to_string(ref) + ": " +
+                        (rc == GPM_E_CUDA && !timer.error.empty() ? timer.error : std::string(gpm_last_error())));
+                return false;
+            }
+            sweep_ms[job] = ms;  views_used[job] = s.nv;  device_of[job] = dev;
+            float* o4 = d->out_norm4 ? d->out_norm4 + (size_t)job * npix * 4 : nullptr;
+            float* oc = d->out_cost ? d->out_cost + (size_t)job * npix : nullptr;
+            if (d->out_dir && !o4) { n4.resize(npix * 4);  o4 = n4.data(); }
+            if (o4 || oc) rc = gpm_get_state(ctx, o4, oc, 0);
+            if (rc == GPM_OK && d->out_dir) rc = write_result(d->out_dir, ref, o4, H, W);
+            if (rc != GPM_OK) { set_err(std::string(fn) + ": could not store the result of reference view " + std::to_string(ref));  return false; }
+            return true;
+        });
+    });
+    if (stats) {
+        stats->jobs_done = 0;  stats->sweep_ms_total = 0.0;
+        for (int j = 0; j < d->n_refs; j++) if (device_of[j] >= 0) { stats->jobs_done++;  stats->sweep_ms_total += sweep_ms[j]; }
+        if (stats->per_job_sweep_ms) for (int j = 0; j < d->n_refs; j++) stats->per_job_sweep_ms[j] = (float)sweep_ms[j];
+        if (stats->per_job_views) for (int j = 0; j < d->n_refs; j++) stats->per_job_views[j] = views_used[j];
+        if (stats->per_job_device) for (int j = 0; j < d->n_refs; j++) stats->per_job_device[j] = device_of[j];
+    }
+    return failed.load() ? GPM_E_STATE : GPM_OK;
+}
+
+extern "C" int gpm_batch_run(const gpm_batch_desc* d, gpm_batch_stats* stats)
+{
+    const gpm_job_opts o = photo_opts(GPM_PHOTO_PM, 0.f);
+    return batch_run("gpm_batch_run", d, &o, &kVselOff, nullptr, stats);
+}
+
+extern "C" int gpm_batch_run_photo(const gpm_batch_desc* d, int kind, float min_std, gpm_batch_stats* stats)
+{
+    const gpm_job_opts o = photo_opts(kind, min_std);
+    return batch_run("gpm_batch_run_photo", d, &o, &kVselOff, nullptr, stats);
+}
+
+extern "C" int gpm_batch_run_opts(const gpm_batch_desc* d, const gpm_job_opts* opts, gpm_batch_stats* stats)
+{
+    return batch_run("gpm_batch_run_opts", d, opts, &kVselOff, nullptr, stats);
+}
+
+extern "C" int gpm_batch_run_vsel(const gpm_batch_desc* d, const gpm_job_opts* opts, const gpm_view_sel* vsel, gpm_batch_stats* stats)
+{
+    return batch_run("gpm_batch_run_vsel", d, opts, vsel ? vsel : &kVselOff, nullptr, stats);
+}
+
+extern "C" int gpm_batch_run_prior(const gpm_batch_desc* d, const gpm_job_opts* opts, const gpm_view_sel* vsel, const gpm_prior_opts* prior,
+                                   gpm_batch_stats* stats)
+{
+    return batch_run("gpm_batch_run_prior", d, opts, vsel ? vsel : &kVselOff, prior, stats);
+}
+
 
 // gpm_geo_batch_run and its _photo / _opts / _vsel twins; `fn` names the entry point in error messages
 static int geo_batch_run(const char* fn, const gpm_geo_batch_desc* g, const gpm_job_opts* opts, const gpm_view_sel* vsel,
-                         gpm_geo_batch_stats* stats)
+                         const gpm_prior_opts* prior, gpm_geo_batch_stats* stats)
 {
     clear_err();
     const char* bad = nullptr;
@@ -307,7 +350,7 @@ static int geo_batch_run(const char* fn, const gpm_geo_batch_desc* g, const gpm_
     else if (g->geo_iterations < 0) bad = "geo_iterations must be >= 0";
     else if (!std::isfinite(g->weight) || g->weight < 0.f) bad = "weight must be finite and >= 0";
     else if (!std::isfinite(g->max_err) || g->max_err <= 0.f) bad = "max_err must be finite and > 0";
-    else bad = gpm::job_refusal(opts, vsel, g->channels);
+    else bad = gpm::job_refusal(opts, vsel, prior, g->channels);
     if (bad) {
         set_err(std::string(fn) + ": bad arguments: " + bad);
         return GPM_E_ARG;
@@ -383,8 +426,12 @@ static int geo_batch_run(const char* fn, const gpm_geo_batch_desc* g, const gpm_
             int rc = load_view(ctx, d, g->channels, pitch, setup[r], *opts, *vsel);
             if (rc == GPM_OK) rc = gpm_init(ctx);
             if (rc == GPM_OK) rc = timer.sweep(ctx, d->params.iterations, &pass1_ms[job]);
+            float ms2 = 0.f;
+            if (rc == GPM_OK && prior) rc = prior_stage(ctx, prior, prior->info ? prior->info + job : nullptr, n4, cost, timer, &ms2);
+            pass1_ms[job] += ms2;
             if (rc == GPM_OK && raw_slot[r] >= 0) rc = gpm_get_state(ctx, raw_store + (size_t)raw_slot[r] * npix * 4, nullptr, 0);
             if (rc == GPM_OK) rc = gpm_finalize(ctx);
+            if (rc == GPM_OK && prior) rc = prior_off(ctx, prior);     // pass 2 has no prior
             if (rc == GPM_OK) rc = gpm_get_state(ctx, n4.data(), nullptr, 0);
             if (rc != GPM_OK) return fail_at("pass 1 of", r, rc);
             float* dep = depth_store + (size_t)depth_slot[r] * npix;
@@ -439,22 +486,28 @@ static int geo_batch_run(const char* fn, const gpm_geo_batch_desc* g, const gpm_
 extern "C" int gpm_geo_batch_run(const gpm_geo_batch_desc* g, gpm_geo_batch_stats* stats)
 {
     const gpm_job_opts o = photo_opts(GPM_PHOTO_PM, 0.f);
-    return geo_batch_run("gpm_geo_batch_run", g, &o, &kVselOff, stats);
+    return geo_batch_run("gpm_geo_batch_run", g, &o, &kVselOff, nullptr, stats);
 }
 
 extern "C" int gpm_geo_batch_run_photo(const gpm_geo_batch_desc* g, int kind, float min_std, gpm_geo_batch_stats* stats)
 {
     const gpm_job_opts o = photo_opts(kind, min_std);
-    return geo_batch_run("gpm_geo_batch_run_photo", g, &o, &kVselOff, stats);
+    return geo_batch_run("gpm_geo_batch_run_photo", g, &o, &kVselOff, nullptr, stats);
 }
 
 extern "C" int gpm_geo_batch_run_opts(const gpm_geo_batch_desc* g, const gpm_job_opts* opts, gpm_geo_batch_stats* stats)
 {
-    return geo_batch_run("gpm_geo_batch_run_opts", g, opts, &kVselOff, stats);
+    return geo_batch_run("gpm_geo_batch_run_opts", g, opts, &kVselOff, nullptr, stats);
 }
 
 extern "C" int gpm_geo_batch_run_vsel(const gpm_geo_batch_desc* g, const gpm_job_opts* opts, const gpm_view_sel* vsel,
                                       gpm_geo_batch_stats* stats)
 {
-    return geo_batch_run("gpm_geo_batch_run_vsel", g, opts, vsel ? vsel : &kVselOff, stats);
+    return geo_batch_run("gpm_geo_batch_run_vsel", g, opts, vsel ? vsel : &kVselOff, nullptr, stats);
+}
+
+extern "C" int gpm_geo_batch_run_prior(const gpm_geo_batch_desc* g, const gpm_job_opts* opts, const gpm_view_sel* vsel,
+                                       const gpm_prior_opts* prior, gpm_geo_batch_stats* stats)
+{
+    return geo_batch_run("gpm_geo_batch_run_prior", g, opts, vsel ? vsel : &kVselOff, prior, stats);
 }

@@ -330,6 +330,45 @@ __device__ __forceinline__ float ncc_cost(float Wsum, float Sr, float Srr, float
     return x < 0.0f ? 0.0f : (x > 2.0f ? 2.0f : x);
 }
 
+// ---- planar prior — DESIGN.md §18 --------------------------------------------------------------------------------
+// What the k_sweep / k_cost_eval variants with PRIOR = true read besides KParams: one plane per pixel (the prior map,
+// n.xyz and d in the state's layout; a pixel has a prior where the plane's depth is in [depthMin, depthMax]) and the term's
+// parameters.  A kernel parameter of its own, so that KParams, GeoParams and JvsParams keep their layout.
+struct PriorParams {
+    const float4* map;          // [H*W]
+    float weight;               // the term's saturation value
+    float depth_sigma;          // sigma_d, in depth units
+    float normal_scale;         // 1 - cos(sigma_n), rounded once from double on the host
+};
+
+// a stored or evaluated cost with the prior term: MAXCOST (no valid view) stays MAXCOST
+__device__ __forceinline__ float with_prior(float c, float prior) { return c == GPM_MAXCOST ? c : fadd(c, prior); }
+
+// Depth of plane (n, d) at pixel p by plane_depth's formula, in IEEE round-to-nearest multiply, add and divide (no FMA, no
+// approximate reciprocal), so that the prior's depths, its has-a-prior test and the support points' depth test are
+// reproducible bit for bit in float32 numpy.  A NaN d gives NaN, which is in no depth range.
+__device__ __forceinline__ float prior_depth(const RefCam& c, float nx, float ny, float nz, float d, float px, float py)
+{
+    const float t = __fadd_rn(__fadd_rn(__fmul_rn(nx, __fsub_rn(px, c.K2)), __fmul_rn(c.alpha, __fmul_rn(ny, __fsub_rn(py, c.K5)))),
+                              __fmul_rn(nz, c.fx));
+    return __fdiv_rn(__fmul_rn(d, -c.fx), t);
+}
+
+// prior(p, h) = weight * q / (1 + q), q = ((depth_h - depth_pi) / sigma_d)^2 + max(0, 1 - n_h . n_pi) / (1 - cos sigma_n):
+// a bounded Geman-McClure penalty, 0 at the prior plane, saturating at weight (also where q is not finite).  IEEE
+// round-to-nearest multiply, add, subtract and divide only, the dot product as (a0 b0 + a1 b1) + a2 b2, so that a float32
+// numpy restatement reproduces every bit (oracle/pyprior.py).  pd: the prior plane's prior_depth at the pixel, hd: the
+// hypothesis'.
+__device__ __forceinline__ float prior_cost(const PriorParams& R, const float4& pi, float pd, float nx, float ny, float nz, float hd)
+{
+    const float delta = __fdiv_rn(__fsub_rn(hd, pd), R.depth_sigma);
+    const float dot = __fadd_rn(__fadd_rn(__fmul_rn(nx, pi.x), __fmul_rn(ny, pi.y)), __fmul_rn(nz, pi.z));
+    const float off = __fsub_rn(1.0f, dot);
+    const float a = __fdiv_rn(off > 0.0f ? off : 0.0f, R.normal_scale);
+    const float q = __fadd_rn(__fmul_rn(delta, delta), a);
+    return __fmul_rn(R.weight, q < 1e30f ? __fdiv_rn(q, __fadd_rn(1.0f, q)) : 1.0f);
+}
+
 // ---- cost of one plane hypothesis at the warp's pixel ---------------------------------------
 // pmCostMultiview_cu (gipuma.cu:720-806) over pmCost_shared (:585-680) / pmCostComputation_shared (:223-277).
 // Returns the exact combined cost, or — if `bound` is finite and an exact lower bound of the final cost
@@ -346,12 +385,14 @@ __device__ __forceinline__ float ncc_cost(float Wsum, float Sr, float Srr, float
 // ignored: every call site uses one rounding variant.  No bound is tested (partial sums bound nothing); `bound` is ignored.
 // ROWS (NCC only; joint view selection, DESIGN.md §17): nothing is combined; view v's NCC cost goes to per_view0[v] and,
 // with GEO, its geometric term to per_view1[v] (written by lanes v and v + 32), and the result is 0.
-template <int XF, bool COLOR, bool GEO = false, bool NCC = false, bool ROWS = false>
+// PRIOR (planar prior, DESIGN.md §18): the result is with_prior(cost, prior), and the bound test compares fadd(b, prior):
+// prior >= 0 and a rounded add is monotone, so that stays an exact lower bound of the final value.
+template <int XF, bool COLOR, bool GEO = false, bool NCC = false, bool ROWS = false, bool PRIOR = false>
 __device__ __forceinline__ float eval_plane(const KParams& P, const float* __restrict__ sCam, const WarpScratch& ws,
                                             cudaTextureObject_t src, float nx, float ny, float nz, float d,
                                             float bound, unsigned lane, WarpStats& st,
                                             float* per_view0 = nullptr, float* per_view1 = nullptr, unsigned rt = 0u,
-                                            const GeoParams* G = nullptr, float gpx = 0.0f, float gpy = 0.0f)
+                                            const GeoParams* G = nullptr, float gpx = 0.0f, float gpy = 0.0f, float prior = 0.0f)
 {
     static_assert(!ROWS || NCC, "per-view cost rows are built for the NCC cost only");
     // XF = 0 / 1: compile-time variant; XF = 2: per call, rt bit 0 = x-term first, bit 1 = gradient folding variant,
@@ -471,7 +512,8 @@ __device__ __forceinline__ float eval_plane(const KParams& P, const float* __res
             if ((int)lane + 32 < P.V) { per_view0[lane + 32] = c1;  if (GEO) per_view1[lane + 32] = g1; }
             return 0.0f;
         }
-        if constexpr (GEO) return combine_views(P, fadd(c0, g0), fadd(c1, g1), lane);
+        if constexpr (PRIOR) return with_prior(GEO ? combine_views(P, fadd(c0, g0), fadd(c1, g1), lane) : combine_views(P, c0, c1, lane), prior);
+        else if constexpr (GEO) return combine_views(P, fadd(c0, g0), fadd(c1, g1), lane);
         else return combine_views(P, c0, c1, lane);
     }
 
@@ -657,7 +699,10 @@ __device__ __forceinline__ float eval_plane(const KParams& P, const float* __res
             float b;
             if constexpr (GEO) b = combine_views(P, fadd(c0, g0), fadd(c1, g1), lane);
             else b = combine_views(P, c0, c1, lane);
-            if (last) return b;
+            if constexpr (PRIOR) {
+                if (last) return with_prior(b, prior);
+                b = fadd(b, prior);
+            } else if (last) return b;
             if (b >= bound) { st.pruned++; return b; }
         }
         s0 = s1;

@@ -104,32 +104,35 @@ __host__ __device__ inline int jvs_floats(int V, bool geo) { return (geo ? 18 : 
 
 // ---- sweep modes: which combinations have kernels --------------------------------------------------------------------
 // A context's mode: colour images, the fused 20-neighbour sweep (option neighbours = 20), the geometric-consistency term
-// (§14), the NCC cost (§15), adaptive checkerboard sampling (§16) and joint view selection (§17).  Kernels are instantiated
-// (gpm_api.cu, kernel tables) and setters accept a change (gpm_set_*) exactly for the modes mode_conflict() passes.
+// (§14), the NCC cost (§15), adaptive checkerboard sampling (§16), joint view selection (§17) and the planar prior (§18).
+// Kernels are instantiated (gpm_api.cu, kernel tables) and setters accept a change (gpm_set_*) exactly for the modes
+// mode_conflict() passes.
 struct Mode {
-    bool color, fused, geo, ncc, adaptive, jvs;
-    __host__ __device__ constexpr int bits() const { return color | fused << 1 | geo << 2 | ncc << 3 | adaptive << 4 | jvs << 5; }
-    __host__ __device__ static constexpr Mode of(int b) { return Mode{bool(b & 1), bool(b & 2), bool(b & 4), bool(b & 8), bool(b & 16), bool(b & 32)}; }
+    bool color, fused, geo, ncc, adaptive, jvs, prior;
+    __host__ __device__ constexpr int bits() const { return color | fused << 1 | geo << 2 | ncc << 3 | adaptive << 4 | jvs << 5 | prior << 6; }
+    __host__ __device__ static constexpr Mode of(int b) { return Mode{bool(b & 1), bool(b & 2), bool(b & 4), bool(b & 8), bool(b & 16), bool(b & 32), bool(b & 64)}; }
 };
-constexpr int GPM_MODES = 64;
+constexpr int GPM_MODES = 128;
 
-enum class ModeConflict { none, fused, jvs_needs_ncc_grey, ncc_colour };
+enum class ModeConflict { none, fused, jvs_needs_ncc_grey, ncc_colour, prior };
 
-// The one rule: the fused sweep has none of the four modes; joint view selection needs the NCC cost (on grey images);
-// the NCC cost needs grey images.  The first conflict found is the reason a refusal gives.
+// The one rule: the fused sweep has none of the five modes; joint view selection needs the NCC cost (on grey images);
+// the NCC cost needs grey images; the planar prior needs grey images and excludes joint view selection.  The first
+// conflict found is the reason a refusal gives.
 __host__ __device__ constexpr ModeConflict mode_conflict(Mode m)
 {
-    if (m.fused && (m.geo || m.ncc || m.adaptive || m.jvs)) return ModeConflict::fused;
+    if (m.fused && (m.geo || m.ncc || m.adaptive || m.jvs || m.prior)) return ModeConflict::fused;
     if (m.jvs && (!m.ncc || m.color)) return ModeConflict::jvs_needs_ncc_grey;
     if (m.ncc && m.color) return ModeConflict::ncc_colour;
+    if (m.prior && (m.color || m.jvs)) return ModeConflict::prior;
     return ModeConflict::none;
 }
 
 // The source-view shard (k_shard_stage) exchanges top-n lists of the 8-neighbour sweep's PM costs: no geometric term, NCC
-// cost, joint view selection or fused sweep.
+// cost, joint view selection, planar prior or fused sweep.
 __host__ __device__ constexpr bool shard_supports(Mode m)
 {
-    return mode_conflict(m) == ModeConflict::none && !m.geo && !m.ncc && !m.jvs && !m.fused;
+    return mode_conflict(m) == ModeConflict::none && !m.geo && !m.ncc && !m.jvs && !m.prior && !m.fused;
 }
 
 // ---- exact memo of rejected work: plane identities ------------------------------------------------------------
@@ -189,18 +192,39 @@ __global__ void k_init_planes(const __grid_constant__ KParams P, unsigned long l
     }
 }
 
+// ---- planar prior at one pixel (DESIGN.md §18) ------------------------------------------------------------------------
+// The pixel's prior plane and its depth (prior_depth), read once per pixel; of() is the term of a hypothesis, 0 where the
+// pixel has no prior (the prior plane's depth is not in [depthMin, depthMax]; an all-zero entry never is).
+struct PixelPrior {
+    float4 pi;
+    float pd;
+    bool has;
+    __device__ __forceinline__ float of(const KParams& P, const PriorParams& R, const float4& h, float fpx, float fpy) const
+    {
+        return has ? prior_cost(R, pi, pd, h.x, h.y, h.z, prior_depth(P.ref, h.x, h.y, h.z, h.w, fpx, fpy)) : 0.0f;
+    }
+};
+__device__ __forceinline__ PixelPrior pixel_prior(const KParams& P, const PriorParams& R, size_t at, float fpx, float fpy)
+{
+    PixelPrior q;
+    q.pi = R.map[at];
+    q.pd = prior_depth(P.ref, q.pi.x, q.pi.y, q.pi.z, q.pi.w, fpx, fpy);
+    q.has = q.pd >= P.ref.depthMin && q.pd <= P.ref.depthMax;
+    return q;
+}
+
 // ---- cost of the stored (or supplied) plane at every pixel — gipuma.cu:1040-1049 and gpm_cost_eval ----
 #ifndef GPM_LB_THREADS
 #define GPM_LB_THREADS 512       // max threads per block of the warp-per-pixel kernels (16 warps)
 #define GPM_LB_BLOCKS 1
 #endif
 // GEO: the cost with the geometric-consistency term (DESIGN.md §14); NCC: the NCC photometric cost (§15, grey only).
-// G is only read in those variants.
-template <bool COLOR, bool GEO = false, bool NCC = false>
+// G is only read in those variants.  PRIOR: with the planar prior's term (§18, grey only); R is only read there.
+template <bool COLOR, bool GEO = false, bool NCC = false, bool PRIOR = false>
 __global__ void __launch_bounds__(GPM_LB_THREADS, GPM_LB_BLOCKS)
 k_cost_eval(const __grid_constant__ KParams P, const __grid_constant__ CUtensorMap tmap, const ViewCam* __restrict__ cams,
             cudaTextureObject_t src, const float4* __restrict__ planes, float* __restrict__ cost, unsigned long long* __restrict__ stats,
-            const __grid_constant__ GeoParams G)
+            const __grid_constant__ GeoParams G, const PriorParams R)
 {
     extern __shared__ __align__(128) float smem[];
     float* tile = smem;
@@ -220,11 +244,13 @@ k_cost_eval(const __grid_constant__ KParams P, const __grid_constant__ CUtensorM
         const float inf = __int_as_float(0x7f800000);
         const GeoParams* g = (GEO || NCC) ? &G : nullptr;
         const float fpx = __int2float_rn(px), fpy = __int2float_rn(py);
+        float pr = 0.0f;
+        if constexpr (PRIOR) pr = pixel_prior(P, R, (size_t)py * P.W + px, fpx, fpy).of(P, R, n, fpx, fpy);
         float c;
-        if constexpr (NCC) c = eval_plane<1, COLOR, GEO, true>(P, sCam, ws, src, n.x, n.y, n.z, n.w, inf, lane, st, nullptr, nullptr, 0u, g, fpx, fpy);
-        else c = (P.cost_rt & 12) ? eval_plane<2, COLOR, GEO>(P, sCam, ws, src, n.x, n.y, n.z, n.w, inf, lane, st, nullptr, nullptr, (unsigned)P.cost_rt, g, fpx, fpy)
-                 : P.cost_variant ? eval_plane<1, COLOR, GEO>(P, sCam, ws, src, n.x, n.y, n.z, n.w, inf, lane, st, nullptr, nullptr, 0u, g, fpx, fpy)
-                                  : eval_plane<0, COLOR, GEO>(P, sCam, ws, src, n.x, n.y, n.z, n.w, inf, lane, st, nullptr, nullptr, 0u, g, fpx, fpy);
+        if constexpr (NCC) c = eval_plane<1, COLOR, GEO, true, false, PRIOR>(P, sCam, ws, src, n.x, n.y, n.z, n.w, inf, lane, st, nullptr, nullptr, 0u, g, fpx, fpy, pr);
+        else c = (P.cost_rt & 12) ? eval_plane<2, COLOR, GEO, false, false, PRIOR>(P, sCam, ws, src, n.x, n.y, n.z, n.w, inf, lane, st, nullptr, nullptr, (unsigned)P.cost_rt, g, fpx, fpy, pr)
+                 : P.cost_variant ? eval_plane<1, COLOR, GEO, false, false, PRIOR>(P, sCam, ws, src, n.x, n.y, n.z, n.w, inf, lane, st, nullptr, nullptr, 0u, g, fpx, fpy, pr)
+                                  : eval_plane<0, COLOR, GEO, false, false, PRIOR>(P, sCam, ws, src, n.x, n.y, n.z, n.w, inf, lane, st, nullptr, nullptr, 0u, g, fpx, fpy, pr);
         if (lane == 0) cost[(size_t)py * P.W + px] = c;
     }
     flush_stats(stats, st, lane);
@@ -481,15 +507,16 @@ __device__ __forceinline__ void jvs_pixel(const KParams& P, const JvsParams& J, 
 // GEO: the cost with the geometric-consistency term (DESIGN.md §14; 8-neighbour sweep only); NCC: the NCC photometric cost
 // (§15; 8-neighbour sweep, grey images only).  G is only read in those variants.  ADAPTIVE: adaptive checkerboard sampling
 // (§16; 8-neighbour sweep), candidate k is acs_neighbour's choice instead of the fixed neighbour.  JVS: joint view
-// selection (§17; NCC only), every pixel goes through jvs_pixel; J is only read in those variants.
-template <bool COLOR, bool FUSED, bool GEO = false, bool NCC = false, bool ADAPTIVE = false, bool JVS = false>
+// selection (§17; NCC only), every pixel goes through jvs_pixel; J is only read in those variants.  PRIOR: every
+// hypothesis' cost carries the planar prior's term (§18; grey, no joint view selection); R is only read there.
+template <bool COLOR, bool FUSED, bool GEO = false, bool NCC = false, bool ADAPTIVE = false, bool JVS = false, bool PRIOR = false>
 __global__ void __launch_bounds__(GPM_LB_THREADS, GPM_LB_BLOCKS)
 k_sweep(const __grid_constant__ KParams P, const __grid_constant__ CUtensorMap tmap, const ViewCam* __restrict__ cams,
         cudaTextureObject_t src, float4* __restrict__ planes, float* __restrict__ cost,
         unsigned* __restrict__ rng_state, unsigned char* __restrict__ prov, Memo M, int colour, int phase_mask,
-        unsigned long long* __restrict__ stats, const __grid_constant__ GeoParams G, const JvsParams J)
+        unsigned long long* __restrict__ stats, const __grid_constant__ GeoParams G, const JvsParams J, const PriorParams R)
 {
-    static_assert(mode_conflict(Mode{COLOR, FUSED, GEO, NCC, ADAPTIVE, JVS}) == ModeConflict::none, "no such sweep mode (mode_conflict)");
+    static_assert(mode_conflict(Mode{COLOR, FUSED, GEO, NCC, ADAPTIVE, JVS, PRIOR}) == ModeConflict::none, "no such sweep mode (mode_conflict)");
     const GeoParams* g = (GEO || NCC) ? &G : nullptr;
     extern __shared__ __align__(128) float smem[];
     float* tile = smem;
@@ -530,6 +557,8 @@ k_sweep(const __grid_constant__ KParams P, const __grid_constant__ CUtensorMap t
             float disp_now = plane_depth(cam, norm_now.x, norm_now.y, norm_now.z, norm_now.w, fpx, fpy);   // :1530
             // which rounding variant of the cost function produced cost_now: eval_plane's rt (0 = y-first, 1 = x-first, ...), 0xff = unknown
             int prov_now = prov[center];
+            PixelPrior pp{};
+            if constexpr (PRIOR) pp = pixel_prior(P, R, center, fpx, fpy);
 
             // candidate k lives in lane k: 0..3 = up, down, left, right at 1 px (:1571-1582), 4..7 at 5 px (:1450-1462);
             // fused kernel: the 20 candidates of gipuma.cu:1236-1330 in source order
@@ -588,9 +617,11 @@ k_sweep(const __grid_constant__ KParams P, const __grid_constant__ CUtensorMap t
                 const bool dup = __any_sync(GPM_FULL, same_mine);
                 if (!in_range || same_now || dup) { st.skip++; continue; }
                 if (!window_ready) { setup_window<COLOR, NCC>(P, tile + P.tile_xo, ws, px, py, tile_x0, tile_y0, lane);  window_ready = true; }
+                float pr = 0.0f;
+                if constexpr (PRIOR) pr = pp.of(P, R, nb, fpx, fpy);
                 const float c = FUSED ? eval_plane<2, COLOR>(P, sCam, ws, src, nb.x, nb.y, nb.z, nb.w, cost_now, lane, st, nullptr, nullptr, site)
-                                      : eval_plane<(COLOR ? 0 : 1), COLOR, GEO, NCC>(P, sCam, ws, src, nb.x, nb.y, nb.z, nb.w, cost_now, lane, st,
-                                                                                nullptr, nullptr, 0u, g, fpx, fpy);
+                                      : eval_plane<(COLOR ? 0 : 1), COLOR, GEO, NCC, false, PRIOR>(P, sCam, ws, src, nb.x, nb.y, nb.z, nb.w, cost_now, lane, st,
+                                                                                nullptr, nullptr, 0u, g, fpx, fpy, pr);
                 if (c < cost_now) {                                                              // :867-871
                     disp_now = disp_before;
                     norm_now = nb;
@@ -646,9 +677,11 @@ k_sweep(const __grid_constant__ KParams P, const __grid_constant__ CUtensorMap t
                     if (dot3(cand.x, cand.y, cand.z, vx, vy, vz) > 0.0f) { cand.x = -cand.x;  cand.y = -cand.y;  cand.z = -cand.z; }
                     cand.w = plane_d(cam, cand.x, cand.y, cand.z, fpx, fpy, depth_new);   // :969
                     const unsigned rsite = NCC ? GPM_PROV_NCC : FUSED ? (unsigned)P.site[20] : 0u;
+                    float pr = 0.0f;
+                    if constexpr (PRIOR) pr = pp.of(P, R, cand, fpx, fpy);
                     const float c = FUSED ? eval_plane<2, COLOR>(P, sCam, ws, src, cand.x, cand.y, cand.z, cand.w, cost_now, lane, st, nullptr, nullptr, rsite)
-                                          : eval_plane<0, COLOR, GEO, NCC>(P, sCam, ws, src, cand.x, cand.y, cand.z, cand.w, cost_now, lane, st,
-                                                                      nullptr, nullptr, 0u, g, fpx, fpy);
+                                          : eval_plane<0, COLOR, GEO, NCC, false, PRIOR>(P, sCam, ws, src, cand.x, cand.y, cand.z, cand.w, cost_now, lane, st,
+                                                                      nullptr, nullptr, 0u, g, fpx, fpy, pr);
                     if (c < cost_now) {                                                          // :986-990 (no depth-range test)
                         prov_now = (int)rsite;
                         any_accept = true;
@@ -983,6 +1016,85 @@ __global__ void k_shard_accept0(const __grid_constant__ KParams P, float* __rest
         prov[center] = P.color ? 3 : 0;          // initialisation variant
     }
 }
+
+// ---- planar prior construction and offer (DESIGN.md §18) ------------------------------------------------------------
+// Support point of each step x step cell (one thread per cell): the pixel with the smallest stored cost, NaN never winning
+// and a tie going to the lower (y, x), kept when its cost < support_cost and its plane's prior_depth is in range.
+// at[cell] = its pixel index or -1, plane[cell] = its plane.
+__global__ void k_prior_support(const __grid_constant__ KParams P, const float4* __restrict__ planes, const float* __restrict__ cost,
+                                int step, float support_cost, int cells_x, int cells_y, int* __restrict__ at, float4* __restrict__ plane)
+{
+    const int cx = blockIdx.x * blockDim.x + threadIdx.x, cy = blockIdx.y * blockDim.y + threadIdx.y;
+    if (cx >= cells_x || cy >= cells_y) return;
+    int best = -1;
+    float best_c = 0.0f;
+    for (int y = cy * step; y < min(P.H, cy * step + step); y++)
+        for (int x = cx * step; x < min(P.W, cx * step + step); x++) {
+            const float c = cost[(size_t)y * P.W + x];
+            if (c == c && (best < 0 || c < best_c)) { best = y * P.W + x;  best_c = c; }
+        }
+    int keep = -1;
+    float4 pl = make_float4(0.f, 0.f, 0.f, 0.f);
+    if (best >= 0 && best_c < support_cost) {
+        pl = planes[best];
+        const float dep = prior_depth(P.ref, pl.x, pl.y, pl.z, pl.w, __int2float_rn(best % P.W), __int2float_rn(best / P.W));
+        if (dep >= P.ref.depthMin && dep <= P.ref.depthMax) keep = best;
+    }
+    at[cy * cells_x + cx] = keep;
+    plane[cy * cells_x + cx] = pl;
+}
+
+// Rasterisation of the triangles (one thread per triangle over its bounding box).  tri[t] = three counter-clockwise
+// (orient > 0) integer vertices x0 y0 x1 y1 x2 y2.  Pixel p belongs to a triangle when every edge a -> b has
+// orient(a, b, p) > 0, or = 0 and the edge is top-left (b.y > a.y, or b.y == a.y and b.x < a.x): an interior edge is
+// top-left in exactly one of its two triangles, so every pixel inside the hull belongs to exactly one triangle.  The pixel
+// gets the triangle's plane where that plane's prior_depth is in range (counted in *with_prior), and stays all-zero else.
+__global__ void k_prior_raster(const __grid_constant__ KParams P, const int* __restrict__ tri, const float4* __restrict__ tri_plane,
+                               int ntri, float4* __restrict__ map, unsigned long long* __restrict__ with_prior)
+{
+    const int t = blockIdx.x * blockDim.x + threadIdx.x;
+    if (t >= ntri) return;
+    const int* v = tri + 6 * t;
+    const float4 pl = tri_plane[t];
+    if (pl.x == 0.f && pl.y == 0.f && pl.z == 0.f && pl.w == 0.f) return;            // no plane (degenerate triangle)
+    const int x0 = min(v[0], min(v[2], v[4])), x1 = max(v[0], max(v[2], v[4]));
+    const int y0 = min(v[1], min(v[3], v[5])), y1 = max(v[1], max(v[3], v[5]));
+    unsigned long long n = 0;
+    for (int y = y0; y <= y1; y++)
+        for (int x = x0; x <= x1; x++) {
+            bool in = true;
+            for (int e = 0; e < 3 && in; e++) {
+                const long long ax = v[2 * e], ay = v[2 * e + 1], bx = v[(2 * e + 2) % 6], by = v[(2 * e + 3) % 6];
+                const long long o = (bx - ax) * ((long long)y - ay) - (by - ay) * ((long long)x - ax);
+                in = o > 0 || (o == 0 && (by > ay || (by == ay && bx < ax)));
+            }
+            if (!in) continue;
+            const float dep = prior_depth(P.ref, pl.x, pl.y, pl.z, pl.w, __int2float_rn(x), __int2float_rn(y));
+            if (dep >= P.ref.depthMin && dep <= P.ref.depthMax) { map[(size_t)y * P.W + x] = pl;  n++; }
+        }
+    if (n) atomicAdd(with_prior, n);
+}
+
+// gpm_offer_prior: pixel p with a prior takes its prior plane when that plane's cost c_prior[p] (k_cost_eval under the
+// context's mode) is strictly below the stored cost.  An accepted plane gets the fresh identity *next_id + p; the caller
+// then advances the counter by W*H, so the identities do not depend on the order in which the threads run.
+__global__ void k_offer_prior(const __grid_constant__ KParams P, const float4* __restrict__ map, const float* __restrict__ c_prior,
+                              float4* __restrict__ planes, float* __restrict__ cost, unsigned char* __restrict__ prov, unsigned site,
+                              unsigned* __restrict__ pid, const unsigned* __restrict__ next_id)
+{
+    const int x = blockIdx.x * blockDim.x + threadIdx.x, y = blockIdx.y * blockDim.y + threadIdx.y;
+    if (x >= P.W || y >= P.H) return;
+    const size_t at = (size_t)y * P.W + x;
+    const float4 pi = map[at];
+    const float dep = prior_depth(P.ref, pi.x, pi.y, pi.z, pi.w, __int2float_rn(x), __int2float_rn(y));
+    if (!(dep >= P.ref.depthMin && dep <= P.ref.depthMax) || !(c_prior[at] < cost[at])) return;
+    planes[at] = pi;
+    cost[at] = c_prior[at];
+    prov[at] = (unsigned char)site;
+    pid[at] = *next_id + (unsigned)at;
+}
+
+__global__ void k_advance_ids(unsigned* __restrict__ next_id, unsigned n) { *next_id += n; }
 
 // ---- final depth / world normal — gipuma_compute_disp, gipuma.cu:1080-1103 ------------------
 __global__ void k_finalize(const __grid_constant__ KParams P, float4* __restrict__ planes, const float* __restrict__ cost)

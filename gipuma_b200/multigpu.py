@@ -106,7 +106,7 @@ def hybrid_layout(world: int, shard: int):
 
 def run_hybrid(make_scene: Callable[[int], object], n_reference_views: int, rank: int, world: int, shard: int,
                device: int = 0, on_result: Optional[Callable] = None, exchange: str = "nccl",
-               propagation: str = "fixed", view_selection: str = "off") -> List[float]:
+               propagation: str = "fixed", view_selection: str = "off", planar_prior=None) -> List[float]:
     """Reference views are dealt round-robin to world/shard groups; inside a group the source views are sharded and
     combined with one all-gather per stage over the group's own communicator (`exchange` must be "nccl").  `propagation`
     and `view_selection` as ViewShardRunner.  Returns wall seconds per reference view."""
@@ -117,6 +117,7 @@ def run_hybrid(make_scene: Callable[[int], object], n_reference_views: int, rank
     _check_exchange(exchange)
     api.check_propagation(propagation)
     _check_view_selection(view_selection)
+    _check_planar_prior(planar_prior)
     group_of, rank_in, members = hybrid_layout(world, shard)
     groups = [dist.new_group(ranks=m) if world > 1 else None for m in members]     # every rank creates every group
     my_group = group_of[rank]
@@ -155,6 +156,12 @@ def _check_view_selection(view_selection: str):
                          "lists, not per-view costs)" % (view_selection,))
 
 
+def _check_planar_prior(planar_prior):
+    if planar_prior is not None:
+        raise ValueError("planar_prior: the source-view shard has no planar prior (its exchange carries top-n lists of the "
+                         "photometric cost)")
+
+
 class ViewShardRunner:
     """One reference view, source views sharded over `world` ranks.  All device work runs behind the C-ABI
     (gpm_shard_run): one stage kernel + ncclAllGather per exchange stage.  `exchange` must be "nccl"; the attribute of
@@ -164,11 +171,12 @@ class ViewShardRunner:
     per-view costs joint view selection needs (DESIGN.md §17)."""
 
     def __init__(self, scene, rank: int, world: int, device: int = 0, seed: int = 0xC0FFEE, group=None, options=None,
-                 exchange: str = "nccl", propagation: str = "fixed", view_selection: str = "off"):
+                 exchange: str = "nccl", propagation: str = "fixed", view_selection: str = "off", planar_prior=None):
         from . import api
         _check_exchange(exchange)
         api.check_propagation(propagation)
         _check_view_selection(view_selection)
+        _check_planar_prior(planar_prior)
         self.scene, self.rank, self.world, self.group = scene, rank, world, group
         self.local = partition_views(scene.n_views, world)[rank]
         if not self.local:

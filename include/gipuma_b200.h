@@ -89,18 +89,20 @@ int gpm_set_view_color(gpm_ctx* ctx, int v, const float* rgba, size_t pitch_byte
 int gpm_set_num_views(gpm_ctx* ctx, int n_views);
 
 /* ---- mode compatibility -------------------------------------------------------------------------------------------------
- * A context sweeps in one mode of six fields: colour images (fixed by the first image upload), the fused 20-neighbour sweep
- * (option "neighbours" = 20), the geometric-consistency term, the NCC cost, adaptive sampling and joint view selection
- * (DESIGN.md §14–§17).  Every combination exists except:
- *   - the fused sweep with the geometric term, the NCC cost, adaptive sampling or joint view selection;
+ * A context sweeps in one mode of seven fields: colour images (fixed by the first image upload), the fused 20-neighbour
+ * sweep (option "neighbours" = 20), the geometric-consistency term, the NCC cost, adaptive sampling, joint view selection
+ * and the planar prior (DESIGN.md §14–§18).  Every combination exists except:
+ *   - the fused sweep with the geometric term, the NCC cost, adaptive sampling, joint view selection or the planar prior;
  *   - joint view selection without the NCC cost, and so with colour images;
- *   - the NCC cost with colour images.
+ *   - the NCC cost with colour images;
+ *   - the planar prior with colour images or with joint view selection.
  * A call that would make one of these is refused and changes nothing.  gpm_set_geometric, gpm_set_photometric,
- * gpm_set_propagation, gpm_set_view_selection and gpm_set_option("neighbours") return GPM_E_ARG, whichever of the two
- * fields is set last.  A colour image upload (gpm_set_reference_color, gpm_set_view_color) returns GPM_E_ARG while joint
- * view selection is on and GPM_E_STATE while only the NCC cost is.  The batch drivers refuse the same combinations of their
- * job options and image type with GPM_E_ARG before any CUDA call.
- * The source-view shard runs neither the geometric term, the NCC cost nor joint view selection: while one is on, every
+ * gpm_set_propagation, gpm_set_view_selection, gpm_set_prior and gpm_set_option("neighbours") return GPM_E_ARG, whichever
+ * of the two fields is set last.  A colour image upload (gpm_set_reference_color, gpm_set_view_color) returns GPM_E_ARG
+ * while joint view selection or the planar prior is on and GPM_E_STATE while only the NCC cost is.  The batch drivers
+ * refuse the same combinations of their job options and image type with GPM_E_ARG before any CUDA call.
+ * The source-view shard runs neither the geometric term, the NCC cost, joint view selection nor the planar prior: while one
+ * is on, every
  * gpm_shard_* call taking a context returns GPM_E_STATE (gpm_shard_num_stages and gpm_shard_stage_floats return -1), and
  * gpm_set_geometric refuses to turn the term on with GPM_E_STATE once a shard communicator is set.  gpm_shard_stage,
  * gpm_shard_finish_init and gpm_shard_run refuse the fused sweep with GPM_E_ARG. */
@@ -459,6 +461,60 @@ int gpm_nearest_dist(const gpm_nn_desc* desc, gpm_nn_result* result);
 
 const char* gpm_last_error(void);
 const char* gpm_version(void);
+
+/* ---- planar prior (DESIGN.md §18) -------------------------------------------------------------------------------------
+ * ACMP's planar prior (Xu & Tao, AAAI 2020) as an opt-in mode: a prior map holds one plane per pixel (float4 n.xyz, d in
+ * the state's layout; a pixel has a prior where that plane's depth lies in [depthMin, depthMax], so an all-zero entry has
+ * none).  While the mode is on (weight > 0), every cost the context computes (gpm_init, gpm_sweep, gpm_phase, gpm_cost_eval,
+ * gpm_run, gpm_offer_prior) is c + weight * q / (1 + q) at a pixel with a prior, q = ((depth_h - depth_prior) /
+ * depth_sigma)^2 + max(0, 1 - n_h . n_prior) / (1 - cos normal_sigma), and c where c = MAXCOST or the pixel has none.
+ * gpm_set_planar_prior: width x height float4 (pitch_bytes between rows, 0 = packed; host or device memory).
+ * gpm_get_planar_prior: the map (GPM_E_STATE if none was set or built).
+ * gpm_build_planar_prior: the map from the stored planes and costs: per step x step cell the pixel with the smallest cost,
+ *   kept if its cost < support_cost and its depth is in range; the Delaunay triangulation of those pixels; each triangle's
+ *   plane through the three pixels' points on their own planes, rasterised with the top-left rule.  `info` (may be NULL)
+ *   receives the counts.  Refused with GPM_E_ARG: step outside 1..64, support_cost NaN, an image wider or taller than 4097
+ *   pixels; with GPM_E_STATE: before gpm_set_params and gpm_set_reference.
+ * gpm_set_prior: weight 0 (the default) turns the mode off.  Refused with GPM_E_ARG: weight negative or not finite,
+ *   depth_sigma not finite or <= 0, normal_sigma_deg outside (0, 90], a weight with which a valid cost of the current
+ *   parameters could reach MAXCOST; with GPM_E_STATE: weight > 0 without a map.  Other modes: "mode compatibility".
+ * gpm_offer_prior: every pixel with a prior takes its prior plane (with a fresh identity) where that plane's cost under
+ *   the context's mode is strictly below the stored cost.  GPM_E_STATE without a map.
+ * A refused call changes nothing. */
+typedef struct gpm_prior_build {
+    int   step;                        /* cell size in pixels (5) */
+    float support_cost;                /* a cell's cheapest pixel is a support point when its cost is below this */
+} gpm_prior_build;
+typedef struct gpm_prior_info {
+    long long support;                 /* support points */
+    long long triangles;
+    long long with_prior;              /* pixels with a prior */
+} gpm_prior_info;
+int gpm_set_planar_prior(gpm_ctx* ctx, const float* planes, size_t pitch_bytes, int on_device);
+int gpm_get_planar_prior(gpm_ctx* ctx, float* planes, int on_device);
+int gpm_build_planar_prior(gpm_ctx* ctx, const gpm_prior_build* build, gpm_prior_info* info);
+int gpm_set_prior(gpm_ctx* ctx, float weight, float depth_sigma, float normal_sigma_deg);
+int gpm_offer_prior(gpm_ctx* ctx);
+
+/* The batch drivers' prior stage (DESIGN.md §18).  In every photometric job (each job of gpm_batch_run_prior, pass 1 of
+ * gpm_geo_batch_run_prior), after params.iterations sweeps: gpm_build_planar_prior (step, support_cost), gpm_set_prior
+ * (weight, depth_sigma, normal_sigma_deg), gpm_cost_eval + gpm_set_state of the current planes, gpm_offer_prior,
+ * gpm_sweep(iterations); then gpm_finalize and the term off.  Pass 2 of the geometric driver has no prior.  info (may be
+ * NULL): one gpm_prior_info per job (gpm_batch_run_prior) or per pass-1 view, in stats->pass1_views' order
+ * (gpm_geo_batch_run_prior).  Refused with GPM_E_ARG before any CUDA call: gpm_set_prior's and gpm_build_planar_prior's
+ * argument rules, iterations < 0, and the planar prior's mode conflicts (colour images, joint view selection).  The
+ * _vsel drivers are these with prior = NULL. */
+typedef struct gpm_prior_opts {
+    float weight, depth_sigma, normal_sigma_deg;
+    int   step;
+    float support_cost;
+    int   iterations;                  /* sweeps with the prior */
+    gpm_prior_info* info;
+} gpm_prior_opts;
+int gpm_batch_run_prior(const gpm_batch_desc* desc, const gpm_job_opts* opts, const gpm_view_sel* vsel, const gpm_prior_opts* prior,
+                        gpm_batch_stats* stats);
+int gpm_geo_batch_run_prior(const gpm_geo_batch_desc* desc, const gpm_job_opts* opts, const gpm_view_sel* vsel,
+                            const gpm_prior_opts* prior, gpm_geo_batch_stats* stats);
 
 #ifdef __cplusplus
 }

@@ -20,6 +20,13 @@ adaptive, total sweep seconds.
 --vsel: the view selections to run with the NCC cost ("off", "joint" at api.JVS_DEFAULTS; PM runs "off" only): every NCC
 quality and speed row is repeated per view selection (keys "<cost> <propagation>" and "<cost> <propagation> joint"), and
 --dtu-preset adds NCC fixed without and with joint view selection.  Needs a CUDA device; there is no CPU path.
+--prior PM_WEIGHTS/NCC_WEIGHTS (e.g. 1,4,16/0.1,0.3,1): the planar-prior study (DESIGN.md §18) instead of the above.  On the
+same quality workload, per scene, cost and propagation, `--iterations` photometric iterations (batch_run) against
+`--iterations` - 2 photometric plus 2 with the prior (planar_prior: sigma_d = (800 - 300) / 64, sigma_n 5 degrees, step 5,
+support_cost 0.5 for NCC and 3 for PM) at each weight; on the hard scene also the scores restricted to its texture-less band
+(ground-truth points with |Y - 180 unit| < 70 unit, the height field's band rule, and the vertices in the same band).  Then
+the build time of gpm_build_planar_prior and sweep ms per iteration without and with the prior, at 800 x 600 and
+1600 x 1200 (10 views, box 15, CUDA events on gpm_stream).
 """
 import argparse
 import json
@@ -48,6 +55,7 @@ def main():
     ap.add_argument("--speed-iterations", type=int, default=4)
     ap.add_argument("--vsel", default="off")
     ap.add_argument("--dtu-preset", action="store_true")
+    ap.add_argument("--prior", default="")
     a = ap.parse_args()
     import torch
     if not torch.cuda.is_available():
@@ -93,6 +101,10 @@ def main():
     fPs = [Ps[r] for r in refs]
     kw = dict(cam_scale=scale, min_angle=5.0, max_angle=45.0, max_views=6, seed=4242)
     fuse_kw = dict(depth_min=300.0, depth_max=800.0, disp_thresh=0.1, normal_thresh=30.0, num_consistent=2)
+    if a.prior:
+        out["prior"] = prior_study(a, api, S, torch, costs, render, params, Ps, scale, refs, fPs, kw, fuse_kw, log)
+        print(json.dumps(out))
+        return
     for scene in [x for x in a.scenes.split(",") if x]:                    # --scenes "": speed only
         log("%s: rendering" % scene)
         hf, images = render(Ps, scale, a.rows, a.cols, scene == "hard")
@@ -188,6 +200,89 @@ def main():
         out["dtu_preset"] = dict(dtu, workload="%d views at 1600x1200, PM, %d iterations, one worker" % (n, a.iterations))
         log("DTU preset: %s" % dtu)
     print(json.dumps(out))
+
+
+def prior_study(a, api, S, torch, costs, render, params, Ps, scale, refs, fPs, kw, fuse_kw, log):
+    pm_w, ncc_w = a.prior.split("/")
+    weights = {"pm": [float(x) for x in pm_w.split(",") if x], "ncc": [float(x) for x in ncc_w.split(",") if x]}
+    support = {"pm": 3.0, "ncc": 0.5}
+    sigma_d = (800.0 - 300.0) / 64.0
+    res = {}
+    for scene in [x for x in a.scenes.split(",") if x]:
+        log("prior %s: rendering" % scene)
+        hf, images = render(Ps, scale, a.rows, a.cols, scene == "hard")
+        if scene == "lit":
+            rng = np.random.default_rng(2024)
+            images = np.clip(np.stack([rng.uniform(0.6, 1.4) * im + rng.uniform(-40, 40) for im in images]), 0, 255).astype(np.float32)
+        gt = S.gt_points(fPs, scale, a.rows, a.cols, hf, stride=2)
+        unit = hf.unit
+        in_band = lambda p: np.abs(p[:, 1] - 180.0 * unit) < 70.0 * unit          # noqa: E731  (HeightField's band rule)
+
+        def score(n4):
+            v, _ = api.fuse(n4, fPs, cam_scale=scale, **fuse_kw)
+            s = api.evaluate_cloud(v, gt, max_dist=10 * unit, taus=(0.25 * unit, 0.5 * unit, unit))
+            r = {"f_score_1unit": round(s["f_score"][2], 4), "completeness_mean_units": round(s["completeness_mean"] / unit, 4)}
+            if scene == "hard":
+                v = np.stack([v["x"], v["y"], v["z"]], axis=1).astype(np.float32)
+                vb = np.ascontiguousarray(v[in_band(v)])
+                b = api.evaluate_cloud(vb, np.ascontiguousarray(gt[in_band(gt)]), max_dist=10 * unit, taus=(unit,))
+                r["band_f_score_1unit"] = round(b["f_score"][0], 4)
+                r["band_completeness_mean_units"] = round(b["completeness_mean"] / unit, 4)
+            return r
+
+        row = {}
+        for cost, photo in costs.items():
+            for mode in MODES:
+                key = "%s %s" % (cost, mode)
+                n4, _, st = api.batch_run(images, Ps, params(a.iterations), refs, propagation=mode, **kw, **photo)
+                r = {"photometric %d" % a.iterations: score(n4)}
+                for w in weights[cost]:
+                    prior = {"weight": w, "depth_sigma": sigma_d, "support_cost": support[cost], "iterations": 2}
+                    n4, _, st = api.batch_run(images, Ps, params(a.iterations - 2), refs, propagation=mode, planar_prior=prior,
+                                              **kw, **photo)
+                    r["%d + 2 prior, weight %g" % (a.iterations - 2, w)] = dict(
+                        score(n4), with_prior_share=round(float(np.mean([p["with_prior"] for p in st["prior"]])) / (a.rows * a.cols), 3))
+                row[key] = r
+                log("prior %s %s: %s" % (scene, key, r))
+        res[scene] = row
+
+    speed = {}
+    for rows, cols in ((600, 800), (1200, 1600)):
+        sc = S.make_config(2, rows=rows, cols=cols, n_views=10, iterations=1, seed=7)
+        sc.params.box_hsize = sc.params.box_vsize = 15
+        row = {}
+        for cost in costs:
+            with api.Context(cols, rows, len(sc.subset)) as ctx:
+                ctx.load_scene(sc)
+                if cost == "ncc":
+                    ctx.set_photometric("ncc", api.NCC_MIN_STD)
+                ctx.init()
+                ctx.sweep(2)
+                _, c = ctx.get_state()
+                torch.cuda.synchronize()
+                t = []
+                for _ in range(3):
+                    t0 = time.perf_counter()
+                    info = ctx.build_planar_prior(5, float(np.nanpercentile(c, 50)))
+                    t.append(time.perf_counter() - t0)
+                stream = torch.cuda.ExternalStream(ctx.stream)
+                r = {"build_ms": round(1e3 * min(t), 2), "build_counts": info}
+                for label, w in (("without", 0.0), ("with", 1.0 if cost == "pm" else 0.3)):
+                    ctx.set_prior(w, (sc.params.depthMax - sc.params.depthMin) / 64.0, 5.0)
+                    p, _ = ctx.get_state()
+                    ctx.set_state(p, ctx.cost_eval(p))
+                    ctx.sweep(1)
+                    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+                    e0.record(stream)
+                    ctx.sweep(a.speed_iterations)
+                    e1.record(stream)
+                    e1.synchronize()
+                    r["sweep_ms_per_iteration_%s_prior" % label] = round(e0.elapsed_time(e1) / a.speed_iterations, 3)
+                row[cost] = r
+        speed["%dx%d, 10 views, box 15" % (cols, rows)] = row
+        log("prior speed %dx%d: %s" % (cols, rows, row))
+    res["speed"] = speed
+    return res
 
 
 if __name__ == "__main__":
