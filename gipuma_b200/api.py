@@ -84,6 +84,22 @@ class GpmPriorOpts(C.Structure):
                 ("support_cost", C.c_float), ("iterations", C.c_int), ("info", C.POINTER(GpmPriorInfo))]
 
 
+class GpmJbuParams(C.Structure):
+    _fields_ = [("radius", C.c_int), ("sigma_space", C.c_float), ("sigma_range", C.c_float)]
+
+
+class GpmMsBatchDesc(C.Structure):
+    _fields_ = [("geo", GpmGeoBatchDesc), ("levels", C.c_int), ("jbu", GpmJbuParams)]
+
+
+MS_MAX_LEVELS = 4
+
+
+class GpmMsBatchStats(C.Structure):
+    _fields_ = [("batch", GpmBatchStats), ("n_views", C.c_int), ("views", C.POINTER(C.c_int)),
+                ("level_sweep_ms", C.c_double * MS_MAX_LEVELS), ("level_upsample_ms", C.c_double * MS_MAX_LEVELS)]
+
+
 class GpmFuseCamera(C.Structure):
     _fields_ = [("M_inv", C.c_float * 9), ("P", C.c_float * 12), ("f", C.c_float)]
 
@@ -199,6 +215,10 @@ def load_library():
                                           C.POINTER(GpmPriorOpts), C.POINTER(GpmGeoBatchStats)]
     L.gpm_batch_last_error.restype = C.c_char_p
     L.gpm_stream.restype = vp
+    L.gpm_downsample.argtypes = [C.c_int, vp, C.c_size_t, C.c_int, C.c_int, C.c_int, vp, C.c_int]
+    L.gpm_upsample_planes.argtypes = [vp, vp, C.c_int, C.c_int, C.c_int, C.POINTER(GpmJbuParams), vp, vp]
+    L.gpm_ms_batch_run.argtypes = [C.POINTER(GpmMsBatchDesc), C.POINTER(GpmJobOpts), C.POINTER(GpmViewSel),
+                                   C.POINTER(GpmMsBatchStats)]
     L.gpm_fuse_cameras.argtypes = [C.POINTER(C.c_double), C.c_int, C.c_double, C.POINTER(GpmFuseCamera)]
     L.gpm_fuse.argtypes = [C.POINTER(GpmFuseDesc), C.POINTER(GpmFuseResult)]
     L.gpm_write_ply.argtypes = [C.c_char_p, vp, C.c_longlong]
@@ -212,7 +232,7 @@ def load_library():
                  "gpm_geo_batch_run", "gpm_batch_run_photo", "gpm_geo_batch_run_photo", "gpm_batch_run_opts", "gpm_geo_batch_run_opts",
                  "gpm_batch_run_vsel", "gpm_geo_batch_run_vsel", "gpm_set_planar_prior", "gpm_get_planar_prior",
                  "gpm_build_planar_prior", "gpm_set_prior", "gpm_offer_prior", "gpm_batch_run_prior",
-                 "gpm_geo_batch_run_prior",
+                 "gpm_geo_batch_run_prior", "gpm_downsample", "gpm_upsample_planes", "gpm_ms_batch_run",
                  "gpm_prepare_cameras", "gpm_select_views", "gpm_write_dmb", "gpm_read_dmb", "gpm_write_result_dmb",
                  "gpm_fuse_cameras", "gpm_fuse", "gpm_write_ply", "gpm_nearest_dist"):
         getattr(L, name).restype = C.c_int
@@ -397,6 +417,69 @@ def prior_opts(planar_prior: Optional[dict], params, n_jobs: int, photometric: s
 
 def _prior_info(info, k):
     return [{"support": i.support, "triangles": i.triangles, "with_prior": i.with_prior} for i in info[:k]] if info else None
+
+
+# Joint bilateral upsampling of planes between pyramid levels (DESIGN.md §19): candidates within `radius` coarse pixels,
+# a Gaussian spatial weight of sigma_space fine pixels and a Cauchy range weight of sigma_range grey levels.  MS_LEVELS and
+# MS_GEO_ITERATIONS are multiscale_pass's default pyramid depth and sweeps per level.  These are the settings measured with
+# tools/ms_bench.py (§19's table), not the result of a search.
+JBU_DEFAULTS = {"radius": 2, "sigma_space": 2.0, "sigma_range": 10.0}
+MS_LEVELS, MS_GEO_ITERATIONS = 3, 2
+
+
+def jbu_params(radius: int = JBU_DEFAULTS["radius"], sigma_space: float = JBU_DEFAULTS["sigma_space"],
+               sigma_range: float = JBU_DEFAULTS["sigma_range"]) -> GpmJbuParams:
+    """gpm_jbu_params, every argument checked before any call into the library by the rules of gpm_upsample_planes."""
+    if isinstance(radius, bool) or int(radius) != radius or not 0 <= radius <= 4:
+        raise ValueError("radius must be an integer in 0..4 (got %r)" % (radius,))
+    for name, v in (("sigma_space", sigma_space), ("sigma_range", sigma_range)):
+        if not (isinstance(v, (int, float, np.floating, np.integer)) and np.isfinite(v) and v > 0):
+            raise ValueError("%s must be finite and > 0 (got %r)" % (name, v))
+    return GpmJbuParams(int(radius), float(sigma_space), float(sigma_range))
+
+
+def level_size(n: int, level: int) -> int:
+    """Pixels along one side at pyramid level `level` of a side of n pixels: each level halves it, rounding up."""
+    for _ in range(level):
+        n = (n + 1) // 2
+    return n
+
+
+def downsample(img, device: int = 0):
+    """One pyramid level on the GPU (gpm_downsample): [H, W] grey or [H, W, 4] RGBA float32, numpy or a CUDA tensor, to
+    [(H + 1) // 2, (W + 1) // 2(, 4)] of the same kind.  Coarse pixel (xc, yc) is the separable [1, 2, 1] / 4 average
+    around fine pixel (2 xc, 2 yc) with replicated borders, which is what K / 2 describes (DESIGN.md §19)."""
+    shape = tuple(img.shape)
+    if len(shape) not in (2, 3) or (len(shape) == 3 and shape[2] != 4):
+        raise ValueError("images must be [H, W] or [H, W, 4]")
+    if shape[0] < 1 or shape[1] < 1:
+        raise ValueError("images must have at least one pixel")
+    H, W = shape[:2]
+    ch = 1 if len(shape) == 2 else 4
+    out_shape = ((H + 1) // 2, (W + 1) // 2) + shape[2:]
+    if isinstance(img, np.ndarray):
+        img = np.ascontiguousarray(img, dtype=np.float32)
+        out = np.empty(out_shape, np.float32)
+    else:
+        import torch
+        out = torch.empty(out_shape, dtype=torch.float32, device=img.device)
+        device = img.device.index if img.is_cuda else device
+    src, dev = _ptr(img)
+    dst, _ = _ptr(out)
+    lib = load_library()
+    if lib.gpm_downsample(int(device), src, 0, W, H, ch, dst, dev) != 0:
+        raise GipumaError("gpm_downsample: %s" % lib.gpm_last_error().decode())
+    return out
+
+
+def pyramid(img, levels: int, device: int = 0):
+    """[img, downsample(img), ...]: `levels` images, full size first."""
+    if isinstance(levels, bool) or int(levels) != levels or levels < 1:
+        raise ValueError("levels must be an integer >= 1 (got %r)" % (levels,))
+    out = [img]
+    for _ in range(int(levels) - 1):
+        out.append(downsample(out[-1], device))
+    return out
 
 
 def job_opts(photometric: str = "pm", ncc_min_std: float = NCC_MIN_STD, propagation: str = "fixed") -> GpmJobOpts:
@@ -602,6 +685,27 @@ class Context:
         out = np.empty((self.H, self.W), dtype=np.float32)
         self._check(self.lib.gpm_cost_eval(self.h, C.c_void_p(pl.ctypes.data), C.c_void_p(out.ctypes.data), 0))
         return out
+
+    def upsample_planes(self, coarse, radius: int = JBU_DEFAULTS["radius"], sigma_space: float = JBU_DEFAULTS["sigma_space"],
+                        sigma_range: float = JBU_DEFAULTS["sigma_range"]):
+        """Joint bilateral upsampling (gpm_upsample_planes, DESIGN.md §19) of a coarse level's raw planes coarse
+        [(H + 1) // 2, (W + 1) // 2, 4] (numpy, or a CUDA tensor) to this context's level, guided by its reference image,
+        with its parameters' depth range and its reference camera.  Returns (planes [H, W, 4], depth [H, W]) of the input's
+        kind; depth 0 where no coarse plane could be used.  The context's state is not touched."""
+        jbu = jbu_params(radius, sigma_space, sigma_range)
+        Hc, Wc = (self.H + 1) // 2, (self.W + 1) // 2
+        if tuple(coarse.shape) != (Hc, Wc, 4):
+            raise ValueError("coarse planes must be [%d, %d, 4] for a %dx%d context (got %s)" % (Hc, Wc, self.W, self.H, tuple(coarse.shape)))
+        if isinstance(coarse, np.ndarray):
+            coarse = np.ascontiguousarray(coarse, dtype=np.float32)
+            planes, depth = np.empty((self.H, self.W, 4), np.float32), np.empty((self.H, self.W), np.float32)
+        else:
+            import torch
+            planes = torch.empty((self.H, self.W, 4), dtype=torch.float32, device=coarse.device)
+            depth = torch.empty((self.H, self.W), dtype=torch.float32, device=coarse.device)
+        pc, dev = _ptr(coarse)
+        self._check(self.lib.gpm_upsample_planes(self.h, pc, Wc, Hc, dev, C.byref(jbu), _ptr(planes)[0], _ptr(depth)[0]))
+        return planes, depth
 
     def run(self) -> float:
         """init + params.iterations sweeps + finalize; returns the sweep time in ms (reference's timed span)."""
@@ -835,6 +939,71 @@ def geometric_pass(images, Ps, params, refs, geo_iterations: int = 2, weight: fl
     info = {"pass1_views": p1_views[:m], "pass1_sweep_s": [t / 1e3 for t in p1_ms[:m]],
             "pass2_sweep_s": [t / 1e3 for t in st.batch.per_job_sweep_ms[:k]], "views": views,
             "device": st.batch.per_job_device[:k], "prior": _prior_info(pinfo, m)}
+    return n4, cc, info
+
+
+def multiscale_pass(images, Ps, params, refs, levels: int = MS_LEVELS, geo_iterations: int = MS_GEO_ITERATIONS,
+                    weight: float = GEO_WEIGHT, max_err: float = GEO_MAX_ERR, jbu: Optional[dict] = None,
+                    cam_scale: float = 1.0, min_angle: float = 10.0, max_angle: float = 30.0, max_views: int = 9,
+                    seed: int = 0xC0FFEE, devices=(0,), out_dir: Optional[str] = None, photometric: str = "pm",
+                    ncc_min_std: float = NCC_MIN_STD, propagation: str = "fixed", view_selection: str = "off",
+                    jvs_params: Optional[dict] = None):
+    """Coarse-to-fine multi-scale PatchMatch (ACMM; DESIGN.md §19) for the reference views `refs`, run by the native
+    multi-level batch driver (gpm_ms_batch_run) over the worker pool of `devices`.
+
+    V, the views refined, is the transitive closure of the references' view selections; each view keeps its level-0
+    selection and depth range at every level.  Level l has the images downsampled l times (downsample) and K / 2^l.  At the
+    coarsest level every view of V runs init, params.iterations photometric sweeps and finalize, then geo_iterations sweeps
+    with the geometric term against the other views' depth maps of that level.  Each finer level upsamples every view's
+    planes (Context.upsample_planes with `jbu`, a dict overriding JBU_DEFAULTS) into planes and a depth map, and then
+    refines (at level 0 only the references) with geo_iterations sweeps against those depth maps.  levels = 1 is
+    geometric_pass over V.  The other arguments are geometric_pass's (there is no planar prior here).
+    Returns (norm4 [len(refs), H, W, 4], cost [len(refs), H, W], info) with norm4 as batch_run returns it, so fuse and
+    evaluate_cloud take it unchanged; info: "views" (V, ascending), "level_sweep_s" (CUDA-event sweep seconds summed over
+    the views, per level, full size first), "level_upsample_s" (host seconds of the upsampling calls, per level), "sweep_s"
+    (each reference's level-0 sweep seconds), "device" (the device that refined it at level 0)."""
+    check_geometric(weight, max_err)
+    opts = job_opts(photometric, ncc_min_std, propagation)
+    if isinstance(levels, bool) or int(levels) != levels or not 1 <= levels <= MS_MAX_LEVELS:
+        raise ValueError("levels must be an integer in 1..%d (got %r)" % (MS_MAX_LEVELS, levels))
+    if int(geo_iterations) != geo_iterations or geo_iterations < 0:
+        raise ValueError("geo_iterations must be an integer >= 0")
+    unknown = sorted(set(jbu or {}) - set(JBU_DEFAULTS))
+    if unknown:
+        raise ValueError("unknown JBU parameters %s (known: %s)" % (unknown, sorted(JBU_DEFAULTS)))
+    jp = jbu_params(**dict(JBU_DEFAULTS, **(jbu or {})))
+    imgs = np.ascontiguousarray(images, dtype=np.float32)
+    if imgs.ndim not in (3, 4) or (imgs.ndim == 4 and imgs.shape[3] != 4):
+        raise ValueError("images must be [n, H, W] or [n, H, W, 4]")
+    vsel = view_sel(view_selection, **(jvs_params or {}))
+    check_modes(photometric, view_selection, 4 if imgs.ndim == 4 else 1)
+    n, H, W = imgs.shape[:3]
+    if min(level_size(W, levels - 1), level_size(H, levels - 1)) < 8:
+        raise ValueError("the coarsest level of %d levels of %dx%d images is %dx%d, below 8x8" %
+                         (levels, W, H, level_size(W, levels - 1), level_size(H, levels - 1)))
+    if len(Ps) != n:
+        raise ValueError("one projection matrix per image is needed (%d images, %d matrices)" % (n, len(Ps)))
+    refs = [int(r) for r in refs]
+    if not refs or any(r < 0 or r >= n for r in refs):
+        raise ValueError("reference views must be image indices in 0..%d" % (n - 1))
+    if not 1 <= max_views <= 64:
+        raise ValueError("max_views must be 1..64")
+    lib = load_library()
+    k = len(refs)
+    n4 = np.empty((k, H, W, 4), np.float32)
+    cc = np.empty((k, H, W), np.float32)
+    d, _keep = _batch_desc(imgs, Ps, params, refs, devices, cam_scale, min_angle, max_angle, max_views, seed, out_dir, n4, cc)
+    m = GpmMsBatchDesc(GpmGeoBatchDesc(d, 1 if imgs.ndim == 3 else 4, int(geo_iterations), float(weight), float(max_err)),
+                       int(levels), jp)
+    views = (C.c_int * n)()
+    jobs = _job_stats(k)                                   # owns the per-job arrays st.batch points into
+    st = GpmMsBatchStats(jobs, 0, views)
+    rc = lib.gpm_ms_batch_run(C.byref(m), C.byref(opts), C.byref(vsel), C.byref(st))
+    if rc != 0:
+        raise GipumaError("gpm_ms_batch_run failed (%d): %s" % (rc, lib.gpm_batch_last_error().decode()))
+    info = {"views": views[:st.n_views], "level_sweep_s": [t / 1e3 for t in st.level_sweep_ms[:levels]],
+            "level_upsample_s": [t / 1e3 for t in st.level_upsample_ms[:levels]],
+            "sweep_s": [t / 1e3 for t in st.batch.per_job_sweep_ms[:k]], "device": st.batch.per_job_device[:k]}
     return n4, cc, info
 
 

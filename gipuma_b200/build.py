@@ -20,9 +20,10 @@ ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 # --use_fast_math: same arithmetic mode as the reference's build (CMakeLists.txt:23); the kernels pin every
 # operation with explicit .rn.ftz intrinsics on top of it (gpm_device.cuh).
 COMMON = ["-O3", "--use_fast_math", "-std=c++17", "-lineinfo", "-Xcompiler", "-fPIC", "-shared"] + ARCH
-# The fusion (gpm_fuse.cu) and the cloud distances (gpm_cloud.cu) are compiled on their own in IEEE mode: denormals kept, no
-# contraction, so that the fusion's decisions are exactly those of the scalar restatement oracle/fusion_oracle.c (DESIGN.md
-# §12) and every distance is exactly that of the brute-force restatement oracle/pycloud.py (§13).
+# The fusion (gpm_fuse.cu), the cloud distances (gpm_cloud.cu) and the pyramid / plane upsampling (gpm_scale.cu) are compiled
+# on their own in IEEE mode: denormals kept, no contraction, so that the fusion's decisions are exactly those of the scalar
+# restatement oracle/fusion_oracle.c (DESIGN.md §12), every distance is exactly that of the brute-force restatement
+# oracle/pycloud.py (§13) and every pyramid and upsampled value that of oracle/pyscale.py (§19).
 FUSE = ["-O3", "-std=c++17", "-lineinfo", "-Xcompiler", "-fPIC", "-ftz=false", "-prec-div=true", "-prec-sqrt=true",
         "-fmad=false", "-c"] + ARCH
 
@@ -41,19 +42,20 @@ def _run(cmd):
 
 
 def build_library(force: bool = False) -> str:
-    src = [os.path.join(HERE, "csrc", f) for f in ("gpm_api.cu", "gpm_host.cpp", "gpm_batch.cpp", "gpm_fuse.cu", "gpm_cloud.cu",
-                                                   "gpm_kernels.cuh", "gpm_device.cuh", "gpm_prior.cpp")]
-    src.append(os.path.join(ROOT, "include", "gipuma_b200.h"))
+    csrc = lambda *names: [os.path.join(HERE, "csrc", f) for f in names]
+    fast = csrc("gpm_api.cu", "gpm_host.cpp", "gpm_batch.cpp", "gpm_prior.cpp")
+    ieee = csrc("gpm_fuse.cu", "gpm_cloud.cu", "gpm_scale.cu")
+    headers = csrc("gpm_kernels.cuh", "gpm_device.cuh", "gpm_scale.cuh") + [os.path.join(ROOT, "include", "gipuma_b200.h")]
     out = os.path.join(HERE, "libgipuma_b200.so")
     stamp = out + ".sig"
-    sig = _sig(src, " ".join(COMMON + FUSE))
+    sig = _sig(fast + ieee + headers, " ".join(COMMON + FUSE))
     if not force and os.path.exists(out) and os.path.exists(stamp) and open(stamp).read() == sig:
         return out
     with tempfile.TemporaryDirectory() as tmp:
-        ieee_objs = [os.path.join(tmp, os.path.basename(s)[:-3] + ".o") for s in src[3:5]]
-        for s, o in zip(src[3:5], ieee_objs):
+        ieee_objs = [os.path.join(tmp, os.path.basename(s)[:-3] + ".o") for s in ieee]
+        for s, o in zip(ieee, ieee_objs):
             _run([NVCC] + FUSE + ["-o", o, s])
-        _run([NVCC] + COMMON + ["-o", out, src[0], src[1], src[2], src[7]] + ieee_objs + ["-lpthread"])
+        _run([NVCC] + COMMON + ["-o", out] + fast + ieee_objs + ["-lpthread"])
     with open(stamp, "w") as fh:
         fh.write(sig)
     return out

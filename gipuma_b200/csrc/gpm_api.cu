@@ -14,6 +14,7 @@
 // No CPU fallback exists: every entry point needs a CUDA device and reports GPM_E_CUDA otherwise.
 #include "../../include/gipuma_b200.h"
 #include "gpm_kernels.cuh"
+#include "gpm_scale.cuh"
 
 #include <algorithm>
 #include <array>
@@ -1127,6 +1128,59 @@ extern "C" int gpm_get_state(gpm_ctx* c, float* norm4, float* cost, int on_devic
     if (norm4) CU(cudaMemcpyAsync(norm4, c->planes, n * sizeof(float4), k, c->stream));
     if (cost) CU(cudaMemcpyAsync(cost, c->cost, n * sizeof(float), k, c->stream));
     CU(cudaStreamSynchronize(c->stream));
+    return GPM_OK;
+}
+
+// Joint bilateral upsampling (DESIGN.md §19): reads the parameters' depth range, the reference's K^-1 and the reference image
+// as staged for the sweep; the state, costs, memo and counters are left as they are.
+extern "C" int gpm_upsample_planes(gpm_ctx* c, const float* coarse, int coarse_w, int coarse_h, int on_device,
+                                   const gpm_jbu_params* jbu, float* planes, float* depth)
+{
+    if (!c || !coarse || !jbu) return fail(GPM_E_ARG, "gpm_upsample_planes: null argument");
+    if (coarse_w != (c->W + 1) / 2 || coarse_h != (c->H + 1) / 2)
+        return fail(GPM_E_ARG, "gpm_upsample_planes: the coarse level must be ((W + 1) / 2) x ((H + 1) / 2) of the context's");
+    if (jbu->radius < 0 || jbu->radius > kJbuMaxRadius) return fail(GPM_E_ARG, "gpm_upsample_planes: radius must be 0..4");
+    if (!(std::isfinite(jbu->sigma_space) && jbu->sigma_space > 0.f) || !(std::isfinite(jbu->sigma_range) && jbu->sigma_range > 0.f))
+        return fail(GPM_E_ARG, "gpm_upsample_planes: sigma_space and sigma_range must be finite and > 0");
+    if (!c->have_params || !c->have_ref) return fail(GPM_E_STATE, "gpm_upsample_planes: gpm_set_params and gpm_set_reference first");
+    DeviceGuard g(c->device);
+    JbuArgs a{};
+    a.Wc = coarse_w;  a.Hc = coarse_h;  a.W = c->W;  a.H = c->H;  a.radius = jbu->radius;
+    a.guide = c->refpad;  a.guide_pitch = c->refpitch;  a.apron = GPM_APRON;  a.color = c->color == 1;
+    memcpy(a.kinv, c->ref.K_inv, sizeof(a.kinv));
+    a.depth_min = c->prm.depthMin;  a.depth_max = c->prm.depthMax;
+    const double ss = jbu->sigma_space, sr = jbu->sigma_range;
+    a.k_range = (float)(1.0 / (sr * sr));
+    for (int by = 0; by < 2; by++)
+        for (int bx = 0; bx < 2; bx++)
+            for (int j = -kJbuMaxRadius; j <= kJbuMaxRadius; j++)
+                for (int i = -kJbuMaxRadius; i <= kJbuMaxRadius; i++) {
+                    const double dx = 2 * i - bx, dy = 2 * j - by;       // (2 q - p) in fine pixels
+                    a.ws[((by * 2 + bx) * kJbuSide + j + kJbuMaxRadius) * kJbuSide + i + kJbuMaxRadius] =
+                        (float)std::exp(-(dx * dx + dy * dy) / (2.0 * ss * ss));
+                }
+    const size_t nc = (size_t)coarse_w * coarse_h, n = (size_t)c->W * c->H;
+    void *d_coarse = nullptr, *d_planes = nullptr, *d_depth = nullptr;
+    cudaError_t e = cudaSuccess;
+    if (on_device) {
+        a.coarse = reinterpret_cast<const float4*>(coarse);
+        a.planes = reinterpret_cast<float4*>(planes);
+        a.depth = depth;
+    } else {
+        e = cudaMalloc(&d_coarse, nc * sizeof(float4));
+        if (e == cudaSuccess && planes) e = cudaMalloc(&d_planes, n * sizeof(float4));
+        if (e == cudaSuccess && depth) e = cudaMalloc(&d_depth, n * sizeof(float));
+        if (e == cudaSuccess) e = cudaMemcpyAsync(d_coarse, coarse, nc * sizeof(float4), cudaMemcpyHostToDevice, c->stream);
+        a.coarse = static_cast<const float4*>(d_coarse);
+        a.planes = static_cast<float4*>(d_planes);
+        a.depth = static_cast<float*>(d_depth);
+    }
+    if (e == cudaSuccess) e = launch_jbu(a, c->stream);
+    if (e == cudaSuccess && !on_device && planes) e = cudaMemcpyAsync(planes, d_planes, n * sizeof(float4), cudaMemcpyDeviceToHost, c->stream);
+    if (e == cudaSuccess && !on_device && depth) e = cudaMemcpyAsync(depth, d_depth, n * sizeof(float), cudaMemcpyDeviceToHost, c->stream);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(c->stream);
+    cudaFree(d_coarse);  cudaFree(d_planes);  cudaFree(d_depth);
+    if (e != cudaSuccess) return fail(GPM_E_CUDA, std::string("gpm_upsample_planes: ") + cudaGetErrorString(e));
     return GPM_OK;
 }
 

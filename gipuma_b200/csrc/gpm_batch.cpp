@@ -9,14 +9,16 @@
 // gpm_geo_batch_run runs the two-pass geometric-consistency flow (DESIGN.md §14) on the same pool and image cache.  The
 // _photo twins of both choose the photometric cost (DESIGN.md §15), the _opts ones every per-job option (gpm_job_opts):
 // the photometric cost and the propagation mode (§16), the _vsel ones the view selection besides (§17), and the _prior
-// ones a planar-prior stage in every photometric job besides (§18).
-// Host C++ over the C-ABI; the only CUDA calls are page-locking, the geometric driver's host store and its sweep events.
+// ones a planar-prior stage in every photometric job besides (§18).  gpm_ms_batch_run runs the coarse-to-fine multi-scale
+// flow (§19) on the same pool: a pyramid of the images, then per level a Jacobi step of upsampling and geometric refinement.
+// Host C++ over the C-ABI; the only CUDA calls are page-locking, the geometric drivers' host stores and their sweep events.
 #include "../../include/gipuma_b200.h"
 
 #include <cuda_runtime.h>
 
 #include <algorithm>
 #include <atomic>
+#include <chrono>
 #include <cmath>
 #include <condition_variable>
 #include <cstdio>
@@ -80,9 +82,9 @@ gpm_job_opts photo_opts(int kind, float min_std) { return gpm_job_opts{kind, min
 const gpm_view_sel kVselOff{GPM_VSEL_OFF, 0.f, 0.f, 0.f, 0, 0, 0.f, 0.f};
 
 // The per-view setup of a job: photometric cost, propagation, view selection, parameters, reference and source images
-// (grey: channels 1, RGBA: 4), view count, RNG.
-int load_view(gpm_ctx* ctx, const gpm_batch_desc* d, int channels, size_t pitch, const ViewSetup& s, const gpm_job_opts& o,
-              const gpm_view_sel& v)
+// (images[i]: image i, grey: channels 1, RGBA: 4), view count, RNG.
+int load_view(gpm_ctx* ctx, const gpm_batch_desc* d, const float* const* images, int channels, size_t pitch, const ViewSetup& s,
+              const gpm_job_opts& o, const gpm_view_sel& v)
 {
     auto set_reference = channels == 4 ? gpm_set_reference_color : gpm_set_reference;
     auto set_view = channels == 4 ? gpm_set_view_color : gpm_set_view;
@@ -90,8 +92,8 @@ int load_view(gpm_ctx* ctx, const gpm_batch_desc* d, int channels, size_t pitch,
     if (rc == GPM_OK) rc = gpm_set_propagation(ctx, o.propagation);
     if (rc == GPM_OK) rc = gpm_set_view_selection(ctx, &v);
     if (rc == GPM_OK) rc = gpm_set_params(ctx, &s.p);
-    if (rc == GPM_OK) rc = set_reference(ctx, d->images[s.order[0]], pitch, 0, &s.cams[0]);
-    for (int v = 0; v < s.nv && rc == GPM_OK; v++) rc = set_view(ctx, v, d->images[s.source(v)], pitch, 0, &s.cams[s.subset[v]]);
+    if (rc == GPM_OK) rc = set_reference(ctx, images[s.order[0]], pitch, 0, &s.cams[0]);
+    for (int v = 0; v < s.nv && rc == GPM_OK; v++) rc = set_view(ctx, v, images[s.source(v)], pitch, 0, &s.cams[s.subset[v]]);
     if (rc == GPM_OK) rc = gpm_set_num_views(ctx, s.nv);
     if (rc == GPM_OK) rc = gpm_set_rng(ctx, d->seed, GPM_RNG_REFERENCE);
     return rc;
@@ -181,20 +183,24 @@ private:
     void* p_ = nullptr;
 };
 
-// Every worker of the pool waits in arrive_and_wait until all of them have arrived.
+// Every worker of the pool waits in arrive_and_wait until all of them have arrived; the barrier may be passed any number of
+// times (each pass is one generation).
 class Barrier {
 public:
-    explicit Barrier(int n) : left_(n) {}
+    explicit Barrier(int n) : n_(n), left_(n) {}
     void arrive_and_wait()
     {
         std::unique_lock<std::mutex> l(m_);
-        if (--left_ == 0) cv_.notify_all();
-        else cv_.wait(l, [&] { return left_ == 0; });
+        const unsigned gen = gen_;
+        if (--left_ == 0) { left_ = n_;  gen_++;  cv_.notify_all(); }
+        else cv_.wait(l, [&] { return gen_ != gen; });
     }
 private:
     std::mutex m_;
     std::condition_variable cv_;
+    const int n_;
     int left_;
+    unsigned gen_ = 0;
 };
 
 // CUDA-event time of one gpm_sweep, from an event recorded on the context's stream before it to one recorded after it.
@@ -273,7 +279,7 @@ static int batch_run(const char* fn, const gpm_batch_desc* d, const gpm_job_opts
             const int ref = d->ref_indices ? d->ref_indices[job] : job;
             if (ref < 0 || ref >= n) { set_err(std::string(fn) + ": reference index out of range");  return false; }
             if (!plan_view(d, ref, s)) { set_err(std::string(fn) + ": no source view passes the angle filter for reference " + std::to_string(ref));  return false; }
-            int rc = load_view(ctx, d, 1, pitch, s, *opts, *vsel);
+            int rc = load_view(ctx, d, d->images, 1, pitch, s, *opts, *vsel);
             float ms = 0.f, ms2 = 0.f;
             if (!prior) {
                 if (rc == GPM_OK) rc = gpm_run(ctx, &ms);
@@ -339,19 +345,38 @@ extern "C" int gpm_batch_run_prior(const gpm_batch_desc* d, const gpm_job_opts* 
 }
 
 
+namespace {
+// What the geometric and the multi-level drivers refuse in a descriptor, or NULL; is_ref[i] = 1 for every reference view i.
+// Every reference index must be an image (without ref_indices: n_refs <= n_images); with out_dir each must be listed once,
+// or two workers would write the same files.
+const char* geo_desc_refusal(const gpm_geo_batch_desc* g, const gpm_job_opts* opts, const gpm_view_sel* vsel,
+                             const gpm_prior_opts* prior, std::vector<char>& is_ref)
+{
+    if (!g || !batch_desc_ok(&g->batch)) return "the batch descriptor is refused as gpm_batch_run refuses it";
+    if (g->channels != 1 && g->channels != 4) return "channels must be 1 or 4";
+    if (g->geo_iterations < 0) return "geo_iterations must be >= 0";
+    if (!std::isfinite(g->weight) || g->weight < 0.f) return "weight must be finite and >= 0";
+    if (!std::isfinite(g->max_err) || g->max_err <= 0.f) return "max_err must be finite and > 0";
+    if (const char* bad = gpm::job_refusal(opts, vsel, prior, g->channels)) return bad;
+    const gpm_batch_desc* d = &g->batch;
+    is_ref.assign(d->n_images, 0);
+    for (int j = 0; j < d->n_refs; j++) {
+        const int r = d->ref_indices ? d->ref_indices[j] : j;
+        if (r < 0 || r >= d->n_images) return "reference index out of range";
+        if (is_ref[r] && d->out_dir) return "a reference view is listed twice while out_dir is set";
+        is_ref[r] = 1;
+    }
+    return nullptr;
+}
+}  // namespace
+
 // gpm_geo_batch_run and its _photo / _opts / _vsel twins; `fn` names the entry point in error messages
 static int geo_batch_run(const char* fn, const gpm_geo_batch_desc* g, const gpm_job_opts* opts, const gpm_view_sel* vsel,
                          const gpm_prior_opts* prior, gpm_geo_batch_stats* stats)
 {
     clear_err();
-    const char* bad = nullptr;
-    if (!g || !batch_desc_ok(&g->batch)) bad = "the batch descriptor is refused as gpm_batch_run refuses it";
-    else if (g->channels != 1 && g->channels != 4) bad = "channels must be 1 or 4";
-    else if (g->geo_iterations < 0) bad = "geo_iterations must be >= 0";
-    else if (!std::isfinite(g->weight) || g->weight < 0.f) bad = "weight must be finite and >= 0";
-    else if (!std::isfinite(g->max_err) || g->max_err <= 0.f) bad = "max_err must be finite and > 0";
-    else bad = gpm::job_refusal(opts, vsel, prior, g->channels);
-    if (bad) {
+    std::vector<char> is_ref;
+    if (const char* bad = geo_desc_refusal(g, opts, vsel, prior, is_ref)) {
         set_err(std::string(fn) + ": bad arguments: " + bad);
         return GPM_E_ARG;
     }
@@ -360,19 +385,7 @@ static int geo_batch_run(const char* fn, const gpm_geo_batch_desc* g, const gpm_
     const size_t pitch = d->pitch_bytes ? d->pitch_bytes : (size_t)W * sizeof(float) * g->channels;
     const size_t npix = (size_t)W * H;
     auto ref_of = [&](int job) { return d->ref_indices ? d->ref_indices[job] : job; };
-    // Every reference index must be an image (without ref_indices: n_refs <= n_images); with out_dir each must be listed
-    // once, or two workers would write the same files.
-    std::vector<char> is_ref(n, 0), in_pass1(n, 0);
-    for (int j = 0; j < n_refs && !bad; j++) {
-        const int r = ref_of(j);
-        if (r < 0 || r >= n) bad = "reference index out of range";
-        else if (is_ref[r] && d->out_dir) bad = "a reference view is listed twice while out_dir is set";
-        else is_ref[r] = 1;
-    }
-    if (bad) {
-        set_err(std::string(fn) + ": bad arguments: " + bad);
-        return GPM_E_ARG;
-    }
+    std::vector<char> in_pass1(n, 0);
 
     // Pass-1 set: the reference views and every view their selection picks (not recursive), planned on the host before
     // anything runs, so that a view without source views is refused before any CUDA call.
@@ -423,7 +436,7 @@ static int geo_batch_run(const char* fn, const gpm_geo_batch_desc* g, const gpm_
         };
         take_jobs(next1, n_pass1, failed, [&](int job) {          // pass 1: photometric
             const int r = pass1[job];
-            int rc = load_view(ctx, d, g->channels, pitch, setup[r], *opts, *vsel);
+            int rc = load_view(ctx, d, d->images, g->channels, pitch, setup[r], *opts, *vsel);
             if (rc == GPM_OK) rc = gpm_init(ctx);
             if (rc == GPM_OK) rc = timer.sweep(ctx, d->params.iterations, &pass1_ms[job]);
             float ms2 = 0.f;
@@ -443,7 +456,7 @@ static int geo_batch_run(const char* fn, const gpm_geo_batch_desc* g, const gpm_
             const int r = ref_of(job);
             const ViewSetup& s = setup[r];
             const float* raw = raw_store + (size_t)raw_slot[r] * npix * 4;
-            int rc = load_view(ctx, d, g->channels, pitch, s, *opts, *vsel);
+            int rc = load_view(ctx, d, d->images, g->channels, pitch, s, *opts, *vsel);
             for (int v = 0; v < s.nv && rc == GPM_OK; v++) rc = gpm_set_view_depth(ctx, v, depth_store + (size_t)depth_slot[s.source(v)] * npix, 0, 0);
             if (rc == GPM_OK) rc = gpm_set_geometric(ctx, g->weight, g->max_err);
             if (rc == GPM_OK) rc = gpm_cost_eval(ctx, raw, cost.data(), 0);
@@ -510,4 +523,234 @@ extern "C" int gpm_geo_batch_run_prior(const gpm_geo_batch_desc* g, const gpm_jo
                                        const gpm_prior_opts* prior, gpm_geo_batch_stats* stats)
 {
     return geo_batch_run("gpm_geo_batch_run_prior", g, opts, vsel ? vsel : &kVselOff, prior, stats);
+}
+
+
+// ---- coarse-to-fine multi-scale batch (DESIGN.md §19) ---------------------------------------------------------------------
+namespace {
+int level_size(int s, int level) { for (int k = 0; k < level; k++) s = (s + 1) / 2;  return s; }
+
+// A view's setup at a coarser level: the level-0 selection, order and depth range, the cameras at `cam_scale` and the
+// disparities of their f.
+bool rescale_view(const ViewSetup& s0, int n, double cam_scale, ViewSetup& s)
+{
+    s = s0;
+    if (gpm_prepare_cameras(s.P.data(), n, cam_scale, s.cams.data()) != GPM_OK) return false;
+    s.p.min_disparity = s.cams[0].f * s.cams[0].baseline / s.p.depthMax;
+    s.p.max_disparity = s.cams[0].f * s.cams[0].baseline / s.p.depthMin;
+    return true;
+}
+
+const char* ms_refusal(const gpm_ms_batch_desc* m, const gpm_job_opts* opts, const gpm_view_sel* vsel, std::vector<char>& is_ref)
+{
+    if (!m) return "null descriptor";
+    if (const char* bad = geo_desc_refusal(&m->geo, opts, vsel, nullptr, is_ref)) return bad;
+    if (m->levels < 1 || m->levels > GPM_MS_MAX_LEVELS) return "levels must be 1..4";
+    if (level_size(m->geo.batch.width, m->levels - 1) < 8 || level_size(m->geo.batch.height, m->levels - 1) < 8)
+        return "the coarsest level is below 8 x 8 pixels";
+    if (m->jbu.radius < 0 || m->jbu.radius > 4) return "jbu.radius must be 0..4";
+    if (!(std::isfinite(m->jbu.sigma_space) && m->jbu.sigma_space > 0.f) || !(std::isfinite(m->jbu.sigma_range) && m->jbu.sigma_range > 0.f))
+        return "jbu.sigma_space and jbu.sigma_range must be finite and > 0";
+    return nullptr;
+}
+}  // namespace
+
+extern "C" int gpm_ms_batch_run(const gpm_ms_batch_desc* m, const gpm_job_opts* opts, const gpm_view_sel* vsel,
+                                gpm_ms_batch_stats* stats)
+{
+    const std::string fn = "gpm_ms_batch_run";
+    clear_err();
+    if (!vsel) vsel = &kVselOff;
+    std::vector<char> is_ref;
+    if (const char* bad = ms_refusal(m, opts, vsel, is_ref)) {
+        set_err(fn + ": bad arguments: " + bad);
+        return GPM_E_ARG;
+    }
+    const gpm_geo_batch_desc* g = &m->geo;
+    const gpm_batch_desc* d = &g->batch;
+    const int n = d->n_images, n_refs = d->n_refs, ch = g->channels, L = m->levels, top = L - 1;
+    auto ref_of = [&](int job) { return d->ref_indices ? d->ref_indices[job] : job; };
+
+    // V: the transitive closure of the references' selections, planned at level 0 before any CUDA call.
+    std::vector<ViewSetup> setup0(n);
+    std::vector<char> in_v(n, 0);
+    std::vector<int> queue;
+    for (int i = 0; i < n; i++) if (is_ref[i]) { in_v[i] = 1;  queue.push_back(i); }
+    for (size_t q = 0; q < queue.size(); q++) {
+        const int i = queue[q];
+        if (!plan_view(d, i, setup0[i])) {
+            set_err(fn + ": no source view passes the angle filter for " + (is_ref[i] ? "reference view " : "source view ") + std::to_string(i));
+            return GPM_E_STATE;
+        }
+        for (int v = 0; v < setup0[i].nv; v++) {
+            const int s = setup0[i].source(v);
+            if (!in_v[s]) { in_v[s] = 1;  queue.push_back(s); }
+        }
+    }
+    std::vector<int> views, slot(n, -1), refs;
+    for (int i = 0; i < n; i++) {
+        if (in_v[i]) { slot[i] = (int)views.size();  views.push_back(i); }
+        if (is_ref[i]) refs.push_back(i);
+    }
+    const int nV = (int)views.size(), nR = (int)refs.size();
+
+    // Per level: size, setups (selection and depth range of level 0; cameras and disparities of the level), image pitch.
+    const double scale0 = d->cam_scale > 0 ? d->cam_scale : 1.0;
+    std::vector<int> Wl(L), Hl(L);
+    std::vector<size_t> npix(L), pitch(L);
+    std::vector<std::vector<ViewSetup>> setup(L);
+    for (int l = 0; l < L; l++) {
+        Wl[l] = level_size(d->width, l);  Hl[l] = level_size(d->height, l);
+        npix[l] = (size_t)Wl[l] * Hl[l];
+        pitch[l] = l == 0 && d->pitch_bytes ? d->pitch_bytes : (size_t)Wl[l] * ch * sizeof(float);
+        if (l == 0) { setup[0] = std::move(setup0);  continue; }
+        setup[l].resize(n);
+        for (int i : views)
+            if (!rescale_view(setup[0][i], n, scale0 * (double)(1 << l), setup[l][i])) {
+                set_err(fn + ": bad arguments: the cameras cannot be prepared at level " + std::to_string(l));
+                return GPM_E_ARG;
+            }
+    }
+
+    // The host store: the pyramid levels 1 .. L-1 of every view of V; the raw planes of even levels (level-0 size) and of odd
+    // levels (level-1 size), so that a level's upsampling reads the next coarser level's planes while it writes its own; one
+    // depth map per view of V, of the current level.
+    std::vector<size_t> pyr_off(L, 0);
+    size_t floats = 0;
+    for (int l = 1; l < L; l++) { pyr_off[l] = floats;  floats += (size_t)nV * npix[l] * ch; }
+    const size_t raw_even = floats;
+    floats += (size_t)nV * npix[0] * 4;
+    const size_t raw_odd = floats;
+    if (L > 1) floats += (size_t)nV * npix[1] * 4;
+    const size_t depth_off = floats;
+    floats += (size_t)nV * npix[0];
+    PinnedImages pinned(d, pitch[0] * d->height);
+    PinnedStore store(floats);
+    if (!store.get()) {
+        set_err(fn + ": cannot allocate the page-locked host store: " + cudaGetErrorString(cudaGetLastError()));
+        return GPM_E_CUDA;
+    }
+    float* const base = store.get();
+    auto pyr = [&](int l, int k) { return base + pyr_off[l] + (size_t)k * npix[l] * ch; };
+    auto raw = [&](int l, int k) { return base + (l % 2 ? raw_odd + (size_t)k * npix[1] * 4 : raw_even + (size_t)k * npix[0] * 4); };
+    auto dep = [&](int k) { return base + depth_off + (size_t)k * npix[0]; };
+    std::vector<std::vector<const float*>> imgs(L, std::vector<const float*>(n, nullptr));
+    for (int i = 0; i < n; i++) imgs[0][i] = d->images[i];
+    for (int l = 1; l < L; l++) for (int k = 0; k < nV; k++) imgs[l][views[k]] = pyr(l, k);
+
+    const int n_stages = 2 + 2 * L;
+    std::vector<std::atomic<int>> next(n_stages);
+    for (auto& a : next) a.store(0);
+    std::atomic<int> failed(0);
+    std::vector<std::vector<float>> sweep_ms(L, std::vector<float>(nV, 0.f)), up_ms(L, std::vector<float>(nV, 0.f));
+    std::vector<int> device_of(n_refs, -1);
+    std::vector<float> job_ms(n_refs, 0.f);
+    Barrier barrier(d->n_devices);
+    run_workers(d, failed, [&](gpm_ctx* ctx, int dev) {
+        if (ctx) cudaSetDevice(dev);                     // a worker thread of its own: the sweep events live on its device
+        std::vector<gpm_ctx*> lc(L, nullptr);            // one context per level
+        lc[0] = ctx;
+        for (int l = 1; l < L && ctx; l++)
+            if (gpm_create(&lc[l], dev, Wl[l], Hl[l], d->max_views) != GPM_OK) {
+                set_err(fn + ": gpm_create at level " + std::to_string(l) + ": " + gpm_last_error());
+                failed++;
+                lc[l] = nullptr;
+            }
+        SweepTimer timer;
+        std::vector<float> n4(ctx ? npix[0] * 4 : 0), cost(ctx ? npix[0] : 0);
+        auto fail_at = [&](const char* stage, int l, int view, int rc) {
+            set_err(fn + ": level " + std::to_string(l) + " " + stage + " of view " + std::to_string(view) + ": " +
+                    (rc == GPM_E_CUDA && !timer.error.empty() ? timer.error : std::string(gpm_last_error())));
+            return false;
+        };
+        take_jobs(next[0], L > 1 ? nV : 0, failed, [&](int k) {              // 1. the pyramid
+            const float* src = d->images[views[k]];
+            for (int l = 1; l < L; l++) {
+                const int rc = gpm_downsample(dev, src, pitch[l - 1], Wl[l - 1], Hl[l - 1], ch, pyr(l, k), 0);
+                if (rc != GPM_OK) return fail_at("pyramid", l, views[k], rc);
+                src = pyr(l, k);
+            }
+            return true;
+        });
+        barrier.arrive_and_wait();
+        take_jobs(next[1], nV, failed, [&](int k) {                           // 2. coarsest level, photometric
+            const int i = views[k];
+            gpm_ctx* c = lc[top];
+            int rc = load_view(c, d, imgs[top].data(), ch, pitch[top], setup[top][i], *opts, *vsel);
+            if (rc == GPM_OK) rc = gpm_init(c);
+            if (rc == GPM_OK) rc = timer.sweep(c, d->params.iterations, &sweep_ms[top][k]);
+            if (rc == GPM_OK) rc = gpm_get_state(c, raw(top, k), nullptr, 0);
+            if (rc == GPM_OK) rc = gpm_finalize(c);
+            if (rc == GPM_OK) rc = gpm_get_state(c, n4.data(), nullptr, 0);
+            if (rc != GPM_OK) return fail_at("photometric stage", top, i, rc);
+            float* D = dep(k);
+            for (size_t p = 0; p < npix[top]; p++) D[p] = n4[p * 4 + 3];
+            return true;
+        });
+        barrier.arrive_and_wait();
+        for (int l = top; l >= 0; l--) {
+            if (l < top) {
+                take_jobs(next[2 + 2 * l], nV, failed, [&](int k) {           // upsampling of level l + 1 into level l
+                    const int i = views[k];
+                    const ViewSetup& s = setup[l][i];
+                    auto set_reference = ch == 4 ? gpm_set_reference_color : gpm_set_reference;
+                    int rc = gpm_set_params(lc[l], &s.p);
+                    if (rc == GPM_OK) rc = set_reference(lc[l], imgs[l][i], pitch[l], 0, &s.cams[0]);
+                    const auto t0 = std::chrono::steady_clock::now();
+                    if (rc == GPM_OK) rc = gpm_upsample_planes(lc[l], raw(l + 1, k), Wl[l + 1], Hl[l + 1], 0, &m->jbu, raw(l, k), dep(k));
+                    up_ms[l][k] = std::chrono::duration<float, std::milli>(std::chrono::steady_clock::now() - t0).count();
+                    return rc == GPM_OK ? true : fail_at("upsampling", l, i, rc);
+                });
+                barrier.arrive_and_wait();                                    // every D_l exists before any view refines
+            }
+            const int n_jobs = l == 0 ? nR : nV;                              // at level 0 only the references' results are read
+            take_jobs(next[3 + 2 * l], n_jobs, failed, [&](int job) {         // geometric stage of level l
+                const int i = l == 0 ? refs[job] : views[job], k = slot[i];
+                const ViewSetup& s = setup[l][i];
+                gpm_ctx* c = lc[l];
+                float ms = 0.f;
+                int rc = load_view(c, d, imgs[l].data(), ch, pitch[l], s, *opts, *vsel);
+                for (int v = 0; v < s.nv && rc == GPM_OK; v++) rc = gpm_set_view_depth(c, v, dep(slot[s.source(v)]), 0, 0);
+                if (rc == GPM_OK) rc = gpm_set_geometric(c, g->weight, g->max_err);
+                if (rc == GPM_OK) rc = gpm_cost_eval(c, raw(l, k), cost.data(), 0);
+                if (rc == GPM_OK) rc = gpm_set_state(c, raw(l, k), cost.data(), 0);
+                if (rc == GPM_OK) rc = timer.sweep(c, g->geo_iterations, &ms);
+                sweep_ms[l][k] += ms;
+                if (rc == GPM_OK && l > 0) rc = gpm_get_state(c, raw(l, k), nullptr, 0);
+                if (rc == GPM_OK && l == 0) {
+                    rc = gpm_finalize(c);
+                    if (rc == GPM_OK) rc = gpm_get_state(c, n4.data(), cost.data(), 0);
+                    for (int j = 0; j < n_refs && rc == GPM_OK; j++) {
+                        if (ref_of(j) != i) continue;
+                        if (d->out_norm4) memcpy(d->out_norm4 + (size_t)j * npix[0] * 4, n4.data(), npix[0] * 4 * sizeof(float));
+                        if (d->out_cost) memcpy(d->out_cost + (size_t)j * npix[0], cost.data(), npix[0] * sizeof(float));
+                        device_of[j] = dev;  job_ms[j] = ms;
+                    }
+                    if (rc == GPM_OK && d->out_dir && write_result(d->out_dir, i, n4.data(), d->height, d->width) != GPM_OK) {
+                        set_err(fn + ": could not store the result of reference view " + std::to_string(i));
+                        return false;
+                    }
+                }
+                if (rc == GPM_OK) rc = gpm_set_geometric(c, 0.f, g->max_err);
+                return rc == GPM_OK ? true : fail_at("geometric stage", l, i, rc);
+            });
+            barrier.arrive_and_wait();
+        }
+        for (int l = 1; l < L; l++) if (lc[l]) gpm_destroy(lc[l]);
+    });
+    if (stats) {
+        gpm_batch_stats* b = &stats->batch;
+        b->jobs_done = 0;  b->sweep_ms_total = 0.0;
+        for (int j = 0; j < n_refs; j++) if (device_of[j] >= 0) { b->jobs_done++;  b->sweep_ms_total += job_ms[j]; }
+        if (b->per_job_sweep_ms) for (int j = 0; j < n_refs; j++) b->per_job_sweep_ms[j] = job_ms[j];
+        if (b->per_job_views) for (int j = 0; j < n_refs; j++) b->per_job_views[j] = setup[0][ref_of(j)].nv;
+        if (b->per_job_device) for (int j = 0; j < n_refs; j++) b->per_job_device[j] = device_of[j];
+        stats->n_views = nV;
+        if (stats->views) std::copy(views.begin(), views.end(), stats->views);
+        for (int l = 0; l < GPM_MS_MAX_LEVELS; l++) {
+            stats->level_sweep_ms[l] = stats->level_upsample_ms[l] = 0.0;
+            for (int k = 0; l < L && k < nV; k++) { stats->level_sweep_ms[l] += sweep_ms[l][k];  stats->level_upsample_ms[l] += up_ms[l][k]; }
+        }
+    }
+    return failed.load() ? GPM_E_STATE : GPM_OK;
 }

@@ -516,6 +516,78 @@ int gpm_batch_run_prior(const gpm_batch_desc* desc, const gpm_job_opts* opts, co
 int gpm_geo_batch_run_prior(const gpm_geo_batch_desc* desc, const gpm_job_opts* opts, const gpm_view_sel* vsel,
                             const gpm_prior_opts* prior, gpm_geo_batch_stats* stats);
 
+/* ---- coarse-to-fine multi-scale PatchMatch (DESIGN.md §19) ------------------------------------------------------------
+ * ACMM's multi-scale scheme (Xu & Tao, CVPR 2019): solve a coarse copy of the images, carry the planes up one level at a
+ * time with joint bilateral upsampling, and refine with the geometric term at every level.  Every arithmetic step below is
+ * one IEEE fp32 round-to-nearest operation, without contraction, so oracle/pyscale.py restates it bit for bit.
+ *
+ * gpm_downsample: one pyramid level.  The coarse image is ((width + 1) / 2) x ((height + 1) / 2); coarse pixel (xc, yc) is
+ *   centred on fine pixel (2 xc, 2 yc), which is what K / 2 (cam_scale * 2 of gpm_prepare_cameras) describes.  Per channel,
+ *   a separable [1, 2, 1] / 4 filter with replicated borders: the horizontal pass of each source row, then the vertical pass,
+ *   each (0.25 a + 0.5 b) + 0.25 c.  channels 1 (grey) or 4 (RGBA float4, w filtered like the others); src has pitch_bytes
+ *   between rows (0 = packed), dst is packed.  Host or device memory (on_device), on `device`.  Uses its own stream, is
+ *   synchronous and frees what it allocates.  Refused with GPM_E_ARG: null pointers, sizes < 1, other channel counts, a pitch
+ *   below the row size or not a multiple of 4. */
+int gpm_downsample(int device, const float* src, size_t pitch_bytes, int width, int height, int channels, float* dst,
+                   int on_device);
+
+/* gpm_upsample_planes: joint bilateral upsampling of a coarse level's raw planes (gpm_get_state's layout, the reference
+ *   camera frame, which only K's scale distinguishes between levels) to the level of `ctx`, whose gpm_set_params and
+ *   reference (image and camera) give the depth range, the rays and the guide.  For fine pixel p = (x, y) with ray
+ *   r = K_inv (x, y, 1): candidates q = (x >> 1, y >> 1) + (i, j), |i|, |j| <= radius, inside the coarse image, visited j
+ *   outer, i inner; z_q = -d_q / (n_q . r), used when finite and in [depthMin, depthMax]; w_q = ws * wr with ws =
+ *   exp(-((2 q.x - x)^2 + (2 q.y - y)^2) / (2 sigma_space^2)) computed in double and rounded once, and wr = 1 / (1 + dI^2 k),
+ *   k = fp32(1 / sigma_range^2), dI = I(p) - I(2 q) in the reference image as uploaded (colour: dI^2 = (dx^2 + dy^2) + dz^2
+ *   of x, y, z).  Z = sum w z / sum w, N = sum w n, n = N / |N|, d = -(n . (Z r)); depth Z.  Where the weights sum to 0 (no
+ *   candidate) or |N| is not > 0, the pixel gets the plane of (x >> 1, y >> 1) unchanged and depth 0 ("no depth" for
+ *   gpm_set_view_depth).  `planes` (W x H float4) and `depth` (W x H float) are caller memory of the input's kind; either
+ *   may be NULL.  The context's state, costs, memo, modes and counters are not read or changed.  Refused with GPM_E_ARG:
+ *   coarse_w != (W + 1) / 2 or coarse_h != (H + 1) / 2, radius outside 0..4, a sigma not finite or <= 0; GPM_E_STATE:
+ *   before gpm_set_params and gpm_set_reference. */
+typedef struct gpm_jbu_params {
+    int   radius;                      /* coarse pixels either side, 0..4 */
+    float sigma_space;                 /* fine pixels, > 0 */
+    float sigma_range;                 /* grey levels, > 0 */
+} gpm_jbu_params;
+int gpm_upsample_planes(gpm_ctx* ctx, const float* coarse, int coarse_w, int coarse_h, int on_device, const gpm_jbu_params* jbu,
+                        float* planes, float* depth);
+
+/* gpm_ms_batch_run: the multi-level batch driver, on gpm_batch_run's worker pool and shared image cache.  Planned on the
+ * calling thread before any CUDA call: the view set V, the transitive closure of the references' selections (so every view
+ * refined at a level has its neighbours' maps of that level), and per view of V its selection and depth range, chosen once on
+ * the full-size images and kept at every level; the disparities follow each level's f.  Level l uses cam_scale * 2^l and
+ * images downsampled l times with gpm_downsample.  Run, with every worker finishing a stage before the next starts:
+ *   1. the pyramid of every image of V, into one page-locked host store;
+ *   2. coarsest level, every v in V: gpm_init, params.iterations sweeps, the raw planes kept, gpm_finalize, the depth kept;
+ *   3. coarsest level, every v in V: the neighbours' depth maps, gpm_set_geometric(weight, max_err), gpm_cost_eval +
+ *      gpm_set_state of the raw planes, geo_iterations sweeps, the raw planes kept;
+ *   4. each finer level l, every v in V: gpm_upsample_planes of v's level-(l + 1) planes into planes and a depth map D_l(v);
+ *      then every v in V (at level 0 the reference views only, since nothing reads the others' results) as in 3, against
+ *      the neighbours' D_l: a Jacobi step, so the result depends neither on scheduling nor on the number of workers.
+ * After level 0 each reference view is finalized into out_norm4 / out_cost and the .dmb files, as gpm_geo_batch_run leaves
+ * them.  One context per worker and level.  Host store: the raw planes of two adjacent levels, a depth map per view of V
+ * and the pyramid, about 1.25 * 16 + 4 + 1.33 * channels bytes per pixel and view.  Refused with GPM_E_ARG before any CUDA
+ * call: what gpm_geo_batch_run_vsel refuses, levels outside 1..4, a coarsest level below 8 x 8, gpm_upsample_planes' JBU
+ * rules; GPM_E_STATE: a view of V with no source view passing the angle filter, named in gpm_batch_last_error().  A failure
+ * during the run stops every worker with GPM_E_STATE, the failing view named; contexts, registrations and stores are
+ * released on every path. */
+#define GPM_MS_MAX_LEVELS 4
+typedef struct gpm_ms_batch_desc {
+    gpm_geo_batch_desc geo;            /* batch.params.iterations: photometric sweeps at the coarsest level; geo_iterations:
+                                          sweeps with the term at every level; out_* receive the level-0 results */
+    int levels;                        /* 1..GPM_MS_MAX_LEVELS; 1 is gpm_geo_batch_run over V */
+    gpm_jbu_params jbu;
+} gpm_ms_batch_desc;
+typedef struct gpm_ms_batch_stats {
+    gpm_batch_stats batch;             /* per reference job: level-0 sweep ms, views selected, device */
+    int n_views;                       /* |V| */
+    int* views;                        /* NULL or n_images entries: V, ascending */
+    double level_sweep_ms[GPM_MS_MAX_LEVELS];     /* CUDA-event sweep time summed over the views, per level (0 = full size) */
+    double level_upsample_ms[GPM_MS_MAX_LEVELS];  /* host time of the gpm_upsample_planes calls, summed, per level */
+} gpm_ms_batch_stats;
+int gpm_ms_batch_run(const gpm_ms_batch_desc* desc, const gpm_job_opts* opts, const gpm_view_sel* vsel,
+                     gpm_ms_batch_stats* stats);
+
 #ifdef __cplusplus
 }
 #endif
