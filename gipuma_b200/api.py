@@ -100,6 +100,11 @@ class GpmMsBatchStats(C.Structure):
                 ("level_sweep_ms", C.c_double * MS_MAX_LEVELS), ("level_upsample_ms", C.c_double * MS_MAX_LEVELS)]
 
 
+class GpmMsPriorOpts(C.Structure):
+    _fields_ = [("photometric", C.POINTER(GpmPriorOpts)), ("geometric", C.POINTER(GpmPriorOpts)),
+                ("level_build_ms", C.c_double * MS_MAX_LEVELS)]
+
+
 class GpmFuseCamera(C.Structure):
     _fields_ = [("M_inv", C.c_float * 9), ("P", C.c_float * 12), ("f", C.c_float)]
 
@@ -219,6 +224,8 @@ def load_library():
     L.gpm_upsample_planes.argtypes = [vp, vp, C.c_int, C.c_int, C.c_int, C.POINTER(GpmJbuParams), vp, vp]
     L.gpm_ms_batch_run.argtypes = [C.POINTER(GpmMsBatchDesc), C.POINTER(GpmJobOpts), C.POINTER(GpmViewSel),
                                    C.POINTER(GpmMsBatchStats)]
+    L.gpm_ms_batch_run_prior.argtypes = [C.POINTER(GpmMsBatchDesc), C.POINTER(GpmJobOpts), C.POINTER(GpmViewSel),
+                                         C.POINTER(GpmMsPriorOpts), C.POINTER(GpmMsBatchStats)]
     L.gpm_fuse_cameras.argtypes = [C.POINTER(C.c_double), C.c_int, C.c_double, C.POINTER(GpmFuseCamera)]
     L.gpm_fuse.argtypes = [C.POINTER(GpmFuseDesc), C.POINTER(GpmFuseResult)]
     L.gpm_write_ply.argtypes = [C.c_char_p, vp, C.c_longlong]
@@ -232,7 +239,7 @@ def load_library():
                  "gpm_geo_batch_run", "gpm_batch_run_photo", "gpm_geo_batch_run_photo", "gpm_batch_run_opts", "gpm_geo_batch_run_opts",
                  "gpm_batch_run_vsel", "gpm_geo_batch_run_vsel", "gpm_set_planar_prior", "gpm_get_planar_prior",
                  "gpm_build_planar_prior", "gpm_set_prior", "gpm_offer_prior", "gpm_batch_run_prior",
-                 "gpm_geo_batch_run_prior", "gpm_downsample", "gpm_upsample_planes", "gpm_ms_batch_run",
+                 "gpm_geo_batch_run_prior", "gpm_downsample", "gpm_upsample_planes", "gpm_ms_batch_run", "gpm_ms_batch_run_prior",
                  "gpm_prepare_cameras", "gpm_select_views", "gpm_write_dmb", "gpm_read_dmb", "gpm_write_result_dmb",
                  "gpm_fuse_cameras", "gpm_fuse", "gpm_write_ply", "gpm_nearest_dist"):
         getattr(L, name).restype = C.c_int
@@ -419,12 +426,33 @@ def _prior_info(info, k):
     return [{"support": i.support, "triangles": i.triangles, "with_prior": i.with_prior} for i in info[:k]] if info else None
 
 
+MAXCOST = 1000.0
+
+
+def check_prior_bound(params, photometric: str, geo_weight: float, geo_max_err: float, prior_weight: float):
+    """The planar prior's bound (DESIGN.md §18), in the library's float32 order, checked before any call into the library:
+    the largest valid cost of `params` (PM: ns at the initialisation window times the largest dissimilarity; NCC: 2) plus
+    geo_weight * geo_max_err plus the prior's weight must stay below MAXCOST."""
+    f = np.float32
+    if prior_weight <= 0:
+        return
+    nside = int(params.box_hsize) // 2 + 1
+    top = f(2.0) if photometric == "ncc" else \
+        f(nside * nside) * ((f(1.0) - f(params.alpha)) * f(params.tau_color) + f(params.alpha) * f(params.tau_gradient))
+    if not (top + f(geo_weight) * f(geo_max_err)) + f(prior_weight) < f(MAXCOST):
+        raise ValueError("with the prior's weight %r a valid cost could reach MAXCOST (largest cost %g, geometric term %g)" %
+                         (prior_weight, top, f(geo_weight) * f(geo_max_err)))
+
+
 # Joint bilateral upsampling of planes between pyramid levels (DESIGN.md §19): candidates within `radius` coarse pixels,
 # a Gaussian spatial weight of sigma_space fine pixels and a Cauchy range weight of sigma_range grey levels.  MS_LEVELS and
 # MS_GEO_ITERATIONS are multiscale_pass's default pyramid depth and sweeps per level.  These are the settings measured with
 # tools/ms_bench.py (§19's table), not the result of a search.
 JBU_DEFAULTS = {"radius": 2, "sigma_space": 2.0, "sigma_range": 10.0}
 MS_LEVELS, MS_GEO_ITERATIONS = 3, 2
+# multiscale_pass's geometric prior stage (DESIGN.md §20) picks support points by costs that include the geometric term:
+# its default support_cost, the better of the two values measured with tools/ms_bench.py --prior.
+MS_GEO_PRIOR_SUPPORT_COST = PRIOR_DEFAULTS["support_cost"]
 
 
 def jbu_params(radius: int = JBU_DEFAULTS["radius"], sigma_space: float = JBU_DEFAULTS["sigma_space"],
@@ -947,9 +975,9 @@ def multiscale_pass(images, Ps, params, refs, levels: int = MS_LEVELS, geo_itera
                     cam_scale: float = 1.0, min_angle: float = 10.0, max_angle: float = 30.0, max_views: int = 9,
                     seed: int = 0xC0FFEE, devices=(0,), out_dir: Optional[str] = None, photometric: str = "pm",
                     ncc_min_std: float = NCC_MIN_STD, propagation: str = "fixed", view_selection: str = "off",
-                    jvs_params: Optional[dict] = None):
+                    jvs_params: Optional[dict] = None, planar_prior: Optional[dict] = None, geo_prior: Optional[dict] = None):
     """Coarse-to-fine multi-scale PatchMatch (ACMM; DESIGN.md §19) for the reference views `refs`, run by the native
-    multi-level batch driver (gpm_ms_batch_run) over the worker pool of `devices`.
+    multi-level batch driver (gpm_ms_batch_run_prior) over the worker pool of `devices`.
 
     V, the views refined, is the transitive closure of the references' view selections; each view keeps its level-0
     selection and depth range at every level.  Level l has the images downsampled l times (downsample) and K / 2^l.  At the
@@ -957,11 +985,18 @@ def multiscale_pass(images, Ps, params, refs, levels: int = MS_LEVELS, geo_itera
     with the geometric term against the other views' depth maps of that level.  Each finer level upsamples every view's
     planes (Context.upsample_planes with `jbu`, a dict overriding JBU_DEFAULTS) into planes and a depth map, and then
     refines (at level 0 only the references) with geo_iterations sweeps against those depth maps.  levels = 1 is
-    geometric_pass over V.  The other arguments are geometric_pass's (there is no planar prior here).
+    geometric_pass over V.  The other arguments are geometric_pass's.
+    The planar prior (ACMMP; DESIGN.md §20), each None (no stage) or a dict as batch_run's planar_prior (prior_opts):
+    planar_prior runs a prior stage at the coarsest level after the photometric sweeps, so the coarsest geometric sweeps
+    read depth maps made with it; geo_prior runs one at every level after the geo_iterations sweeps, with support points
+    chosen by costs that include the geometric term (its support_cost defaults to MS_GEO_PRIOR_SUPPORT_COST, in those
+    units).  Both need grey images and exclude joint view selection.
     Returns (norm4 [len(refs), H, W, 4], cost [len(refs), H, W], info) with norm4 as batch_run returns it, so fuse and
     evaluate_cloud take it unchanged; info: "views" (V, ascending), "level_sweep_s" (CUDA-event sweep seconds summed over
-    the views, per level, full size first), "level_upsample_s" (host seconds of the upsampling calls, per level), "sweep_s"
-    (each reference's level-0 sweep seconds), "device" (the device that refined it at level 0)."""
+    the views, per level, full size first, prior sweeps included), "level_upsample_s" (host seconds of the upsampling calls,
+    per level), "sweep_s" (each reference's level-0 sweep seconds), "device" (the device that refined it at level 0);
+    "prior": {"photometric": per image index, "geometric": per level, per image index} of the prior's counts (None for a
+    stage not run; zeros where a view ran no stage), "level_build_ms" (host milliseconds of the prior builds, per level)."""
     check_geometric(weight, max_err)
     opts = job_opts(photometric, ncc_min_std, propagation)
     if isinstance(levels, bool) or int(levels) != levels or not 1 <= levels <= MS_MAX_LEVELS:
@@ -976,11 +1011,25 @@ def multiscale_pass(images, Ps, params, refs, levels: int = MS_LEVELS, geo_itera
     if imgs.ndim not in (3, 4) or (imgs.ndim == 4 and imgs.shape[3] != 4):
         raise ValueError("images must be [n, H, W] or [n, H, W, 4]")
     vsel = view_sel(view_selection, **(jvs_params or {}))
-    check_modes(photometric, view_selection, 4 if imgs.ndim == 4 else 1)
+    channels = 4 if imgs.ndim == 4 else 1
+    check_modes(photometric, view_selection, channels)
     n, H, W = imgs.shape[:3]
     if min(level_size(W, levels - 1), level_size(H, levels - 1)) < 8:
         raise ValueError("the coarsest level of %d levels of %dx%d images is %dx%d, below 8x8" %
                          (levels, W, H, level_size(W, levels - 1), level_size(H, levels - 1)))
+    stages = {}
+    for name, spec, geo_w, level, n_info in (("photometric", planar_prior, 0.0, levels - 1, n),
+                                              ("geometric", geo_prior, weight, 0, MS_MAX_LEVELS * n)):
+        if spec is None:
+            continue
+        check_modes(photometric, view_selection, channels, spec)
+        if name == "geometric":
+            spec = dict({"support_cost": MS_GEO_PRIOR_SUPPORT_COST}, **spec)
+        stages[name] = prior_opts(spec, params, n_info, photometric)
+        check_prior_bound(params, photometric, geo_w, max_err, stages[name][0].weight)
+        if max(level_size(W, level), level_size(H, level)) > 4097:
+            raise ValueError("the %s prior stage builds the prior at level %d, %dx%d, wider or taller than 4097 pixels" %
+                             (name, level, level_size(W, level), level_size(H, level)))
     if len(Ps) != n:
         raise ValueError("one projection matrix per image is needed (%d images, %d matrices)" % (n, len(Ps)))
     refs = [int(r) for r in refs]
@@ -998,12 +1047,18 @@ def multiscale_pass(images, Ps, params, refs, levels: int = MS_LEVELS, geo_itera
     views = (C.c_int * n)()
     jobs = _job_stats(k)                                   # owns the per-job arrays st.batch points into
     st = GpmMsBatchStats(jobs, 0, views)
-    rc = lib.gpm_ms_batch_run(C.byref(m), C.byref(opts), C.byref(vsel), C.byref(st))
+    po = GpmMsPriorOpts(*[C.pointer(stages[s][0]) if s in stages else None for s in ("photometric", "geometric")])
+    rc = lib.gpm_ms_batch_run_prior(C.byref(m), C.byref(opts), C.byref(vsel), C.byref(po), C.byref(st))
     if rc != 0:
         raise GipumaError("gpm_ms_batch_run failed (%d): %s" % (rc, lib.gpm_batch_last_error().decode()))
     info = {"views": views[:st.n_views], "level_sweep_s": [t / 1e3 for t in st.level_sweep_ms[:levels]],
             "level_upsample_s": [t / 1e3 for t in st.level_upsample_ms[:levels]],
-            "sweep_s": [t / 1e3 for t in st.batch.per_job_sweep_ms[:k]], "device": st.batch.per_job_device[:k]}
+            "sweep_s": [t / 1e3 for t in st.batch.per_job_sweep_ms[:k]], "device": st.batch.per_job_device[:k],
+            "level_build_ms": list(po.level_build_ms[:levels])}
+    pinfo = {s: stages[s][1] if s in stages else None for s in ("photometric", "geometric")}
+    info["prior"] = {"photometric": _prior_info(pinfo["photometric"], n),
+                     "geometric": [_prior_info(pinfo["geometric"][l * n:(l + 1) * n], n) for l in range(levels)]
+                     if pinfo["geometric"] else None}
     return n4, cc, info
 
 

@@ -40,6 +40,18 @@ static int fail(int code, const std::string& msg)
 
 namespace gpm {
 int set_last_error(int code, const std::string& msg) { return fail(code, msg); }     // for gpm_fuse.cu and gpm_cloud.cu
+
+// The planar prior's bound (DESIGN.md §18): the largest valid cost of parameters p (PM: ns at the initialisation window
+// times the largest dissimilarity; NCC: 2) plus the geometric term's largest value plus the prior's weight stays below
+// MAXCOST, so that a valid cost with the term never reaches MAXCOST.  Checked by every setter that changes one of them,
+// and by the multi-level driver before any CUDA call (gpm_batch.cpp).
+bool prior_bound_ok(const gpm_params& p, bool ncc, float geo_weight, float geo_max_err, float prior_weight)
+{
+    if (prior_weight <= 0.f) return true;
+    const int nside = p.box_hsize / 2 + 1;
+    const float top = ncc ? 2.0f : (float)(nside * nside) * ((1.0f - p.alpha) * p.tau_color + p.alpha * p.tau_gradient);
+    return top + geo_weight * geo_max_err + prior_weight < GPM_MAXCOST;
+}
 }
 
 #define CU(call)                                                                                      \
@@ -219,17 +231,6 @@ int refuse_change(const gpm_ctx* c, const char* fn, bool Mode::*field, bool on)
     const ModeConflict k = mode_conflict(m);
     if (k == ModeConflict::none) return GPM_OK;
     return fail(field == &Mode::color && k == ModeConflict::ncc_colour ? GPM_E_STATE : GPM_E_ARG, std::string(fn) + ": " + conflict_text(k));
-}
-
-// The planar prior's bound (DESIGN.md §18): the largest valid cost of parameters p (PM: ns at the initialisation window
-// times the largest dissimilarity; NCC: 2) plus the geometric term's largest value plus the prior's weight stays below
-// MAXCOST, so that a valid cost with the term never reaches MAXCOST.  Checked by every setter that changes one of them.
-bool prior_bound_ok(const gpm_params& p, bool ncc, float geo_weight, float geo_max_err, float prior_weight)
-{
-    if (prior_weight <= 0.f) return true;
-    const int nside = p.box_hsize / 2 + 1;
-    const float top = ncc ? 2.0f : (float)(nside * nside) * ((1.0f - p.alpha) * p.tau_color + p.alpha * p.tau_gradient);
-    return top + geo_weight * geo_max_err + prior_weight < GPM_MAXCOST;
 }
 
 // per-warp floats of the JVS kernel variant the context launches (0 without view selection)

@@ -10,7 +10,8 @@
 // _photo twins of both choose the photometric cost (DESIGN.md §15), the _opts ones every per-job option (gpm_job_opts):
 // the photometric cost and the propagation mode (§16), the _vsel ones the view selection besides (§17), and the _prior
 // ones a planar-prior stage in every photometric job besides (§18).  gpm_ms_batch_run runs the coarse-to-fine multi-scale
-// flow (§19) on the same pool: a pyramid of the images, then per level a Jacobi step of upsampling and geometric refinement.
+// flow (§19) on the same pool: a pyramid of the images, then per level a Jacobi step of upsampling and geometric refinement;
+// its _prior twin adds prior stages at the coarsest level's photometric stage and in every geometric stage (§20).
 // Host C++ over the C-ABI; the only CUDA calls are page-locking, the geometric drivers' host stores and their sweep events.
 #include "../../include/gipuma_b200.h"
 
@@ -31,6 +32,7 @@
 
 namespace gpm {
 const char* job_refusal(const gpm_job_opts* o, const gpm_view_sel* v, const gpm_prior_opts* prior, int channels);     // gpm_api.cu
+bool prior_bound_ok(const gpm_params& p, bool ncc, float geo_weight, float geo_max_err, float prior_weight);        // gpm_api.cu
 }
 
 namespace {
@@ -231,12 +233,15 @@ private:
 
 // The prior stage of a photometric job (DESIGN.md §18), after its params.iterations sweeps: the prior map built from the
 // state, the term on, the state re-scored under it (gpm_cost_eval + gpm_set_state), the prior planes offered, and
-// prior->iterations more sweeps.  The caller finalizes and then turns the term off (prior_off).
+// prior->iterations more sweeps.  The caller finalizes and then turns the term off (prior_off).  build_ms (may be NULL)
+// receives the host time of the build.
 int prior_stage(gpm_ctx* ctx, const gpm_prior_opts* p, gpm_prior_info* info, std::vector<float>& n4, std::vector<float>& cost,
-                SweepTimer& timer, float* ms)
+                SweepTimer& timer, float* ms, float* build_ms = nullptr)
 {
     const gpm_prior_build b{p->step, p->support_cost};
+    const auto t0 = std::chrono::steady_clock::now();
     int rc = gpm_build_planar_prior(ctx, &b, info);
+    if (build_ms) *build_ms = std::chrono::duration<float, std::milli>(std::chrono::steady_clock::now() - t0).count();
     if (rc == GPM_OK) rc = gpm_set_prior(ctx, p->weight, p->depth_sigma, p->normal_sigma_deg);
     if (rc == GPM_OK) rc = gpm_get_state(ctx, n4.data(), nullptr, 0);
     if (rc == GPM_OK) rc = gpm_cost_eval(ctx, n4.data(), cost.data(), 0);
@@ -553,12 +558,35 @@ const char* ms_refusal(const gpm_ms_batch_desc* m, const gpm_job_opts* opts, con
         return "jbu.sigma_space and jbu.sigma_range must be finite and > 0";
     return nullptr;
 }
+
+// What the multi-level driver refuses in its prior stages (DESIGN.md §20), after ms_refusal passed: each given stage's
+// options and mode rule; a weight with which a valid cost could reach MAXCOST, which gpm_set_prior would refuse only
+// during the run (photometric stage: without the geometric term; geometric stage: with weight * max_err); a level whose
+// build gpm_build_planar_prior refuses (photometric stage: the coarsest; geometric stage: level 0, the largest).
+std::string ms_prior_refusal(const gpm_ms_batch_desc* m, const gpm_job_opts* opts, const gpm_view_sel* vsel, const gpm_ms_prior_opts* prior)
+{
+    if (!prior) return "";
+    const gpm_geo_batch_desc* g = &m->geo;
+    const bool ncc = opts->photometric == GPM_PHOTO_NCC;
+    const struct { const char* name; const gpm_prior_opts* p; float geo_weight; int level; } stages[2] = {
+        {"photometric", prior->photometric, 0.f, m->levels - 1}, {"geometric", prior->geometric, g->weight, 0}};
+    for (const auto& s : stages) {
+        if (!s.p) continue;
+        if (const char* bad = gpm::job_refusal(opts, vsel, s.p, g->channels)) return std::string(s.name) + " prior stage: " + bad;
+        if (!gpm::prior_bound_ok(g->batch.params, ncc, s.geo_weight, g->max_err, s.p->weight))
+            return std::string(s.name) + " prior stage: with its weight a valid cost could reach MAXCOST";
+        if (level_size(g->batch.width, s.level) > 4097 || level_size(g->batch.height, s.level) > 4097)
+            return std::string(s.name) + " prior stage: its level " + std::to_string(s.level) + " is wider or taller than 4097 pixels";
+    }
+    return "";
+}
 }  // namespace
 
-extern "C" int gpm_ms_batch_run(const gpm_ms_batch_desc* m, const gpm_job_opts* opts, const gpm_view_sel* vsel,
-                                gpm_ms_batch_stats* stats)
+// gpm_ms_batch_run and gpm_ms_batch_run_prior; `fn` names the entry point in error messages
+static int ms_batch_run(const char* fn_name, const gpm_ms_batch_desc* m, const gpm_job_opts* opts, const gpm_view_sel* vsel,
+                        gpm_ms_prior_opts* prior, gpm_ms_batch_stats* stats)
 {
-    const std::string fn = "gpm_ms_batch_run";
+    const std::string fn = fn_name;
     clear_err();
     if (!vsel) vsel = &kVselOff;
     std::vector<char> is_ref;
@@ -566,9 +594,18 @@ extern "C" int gpm_ms_batch_run(const gpm_ms_batch_desc* m, const gpm_job_opts* 
         set_err(fn + ": bad arguments: " + bad);
         return GPM_E_ARG;
     }
+    const std::string bad_prior = ms_prior_refusal(m, opts, vsel, prior);
+    if (!bad_prior.empty()) {
+        set_err(fn + ": bad arguments: " + bad_prior);
+        return GPM_E_ARG;
+    }
+    const gpm_prior_opts* P_photo = prior ? prior->photometric : nullptr;
+    const gpm_prior_opts* P_geo = prior ? prior->geometric : nullptr;
     const gpm_geo_batch_desc* g = &m->geo;
     const gpm_batch_desc* d = &g->batch;
     const int n = d->n_images, n_refs = d->n_refs, ch = g->channels, L = m->levels, top = L - 1;
+    if (P_photo && P_photo->info) memset(P_photo->info, 0, (size_t)n * sizeof(gpm_prior_info));
+    if (P_geo && P_geo->info) memset(P_geo->info, 0, (size_t)GPM_MS_MAX_LEVELS * n * sizeof(gpm_prior_info));
     auto ref_of = [&](int job) { return d->ref_indices ? d->ref_indices[job] : job; };
 
     // V: the transitive closure of the references' selections, planned at level 0 before any CUDA call.
@@ -642,7 +679,8 @@ extern "C" int gpm_ms_batch_run(const gpm_ms_batch_desc* m, const gpm_job_opts* 
     std::vector<std::atomic<int>> next(n_stages);
     for (auto& a : next) a.store(0);
     std::atomic<int> failed(0);
-    std::vector<std::vector<float>> sweep_ms(L, std::vector<float>(nV, 0.f)), up_ms(L, std::vector<float>(nV, 0.f));
+    std::vector<std::vector<float>> sweep_ms(L, std::vector<float>(nV, 0.f)), up_ms(L, std::vector<float>(nV, 0.f)),
+        build_ms(L, std::vector<float>(nV, 0.f));
     std::vector<int> device_of(n_refs, -1);
     std::vector<float> job_ms(n_refs, 0.f);
     Barrier barrier(d->n_devices);
@@ -679,8 +717,13 @@ extern "C" int gpm_ms_batch_run(const gpm_ms_batch_desc* m, const gpm_job_opts* 
             int rc = load_view(c, d, imgs[top].data(), ch, pitch[top], setup[top][i], *opts, *vsel);
             if (rc == GPM_OK) rc = gpm_init(c);
             if (rc == GPM_OK) rc = timer.sweep(c, d->params.iterations, &sweep_ms[top][k]);
+            float ms2 = 0.f, bms = 0.f;                                       // the photometric prior stage (§20)
+            if (rc == GPM_OK && P_photo)
+                rc = prior_stage(c, P_photo, P_photo->info ? P_photo->info + i : nullptr, n4, cost, timer, &ms2, &bms);
+            sweep_ms[top][k] += ms2;  build_ms[top][k] += bms;
             if (rc == GPM_OK) rc = gpm_get_state(c, raw(top, k), nullptr, 0);
             if (rc == GPM_OK) rc = gpm_finalize(c);
+            if (rc == GPM_OK && P_photo) rc = prior_off(c, P_photo);
             if (rc == GPM_OK) rc = gpm_get_state(c, n4.data(), nullptr, 0);
             if (rc != GPM_OK) return fail_at("photometric stage", top, i, rc);
             float* D = dep(k);
@@ -715,7 +758,11 @@ extern "C" int gpm_ms_batch_run(const gpm_ms_batch_desc* m, const gpm_job_opts* 
                 if (rc == GPM_OK) rc = gpm_cost_eval(c, raw(l, k), cost.data(), 0);
                 if (rc == GPM_OK) rc = gpm_set_state(c, raw(l, k), cost.data(), 0);
                 if (rc == GPM_OK) rc = timer.sweep(c, g->geo_iterations, &ms);
-                sweep_ms[l][k] += ms;
+                float ms2 = 0.f, bms = 0.f;                                   // the geometric prior stage (§20)
+                if (rc == GPM_OK && P_geo)
+                    rc = prior_stage(c, P_geo, P_geo->info ? P_geo->info + (size_t)l * n + i : nullptr, n4, cost, timer, &ms2, &bms);
+                ms += ms2;
+                sweep_ms[l][k] += ms;  build_ms[l][k] += bms;
                 if (rc == GPM_OK && l > 0) rc = gpm_get_state(c, raw(l, k), nullptr, 0);
                 if (rc == GPM_OK && l == 0) {
                     rc = gpm_finalize(c);
@@ -731,6 +778,7 @@ extern "C" int gpm_ms_batch_run(const gpm_ms_batch_desc* m, const gpm_job_opts* 
                         return false;
                     }
                 }
+                if (rc == GPM_OK && P_geo) rc = prior_off(c, P_geo);
                 if (rc == GPM_OK) rc = gpm_set_geometric(c, 0.f, g->max_err);
                 return rc == GPM_OK ? true : fail_at("geometric stage", l, i, rc);
             });
@@ -752,5 +800,22 @@ extern "C" int gpm_ms_batch_run(const gpm_ms_batch_desc* m, const gpm_job_opts* 
             for (int k = 0; l < L && k < nV; k++) { stats->level_sweep_ms[l] += sweep_ms[l][k];  stats->level_upsample_ms[l] += up_ms[l][k]; }
         }
     }
+    if (prior)
+        for (int l = 0; l < GPM_MS_MAX_LEVELS; l++) {
+            prior->level_build_ms[l] = 0.0;
+            for (int k = 0; l < L && k < nV; k++) prior->level_build_ms[l] += build_ms[l][k];
+        }
     return failed.load() ? GPM_E_STATE : GPM_OK;
+}
+
+extern "C" int gpm_ms_batch_run(const gpm_ms_batch_desc* m, const gpm_job_opts* opts, const gpm_view_sel* vsel,
+                                gpm_ms_batch_stats* stats)
+{
+    return ms_batch_run("gpm_ms_batch_run", m, opts, vsel, nullptr, stats);
+}
+
+extern "C" int gpm_ms_batch_run_prior(const gpm_ms_batch_desc* m, const gpm_job_opts* opts, const gpm_view_sel* vsel,
+                                      gpm_ms_prior_opts* prior, gpm_ms_batch_stats* stats)
+{
+    return ms_batch_run("gpm_ms_batch_run_prior", m, opts, vsel, prior, stats);
 }

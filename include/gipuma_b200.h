@@ -588,6 +588,32 @@ typedef struct gpm_ms_batch_stats {
 int gpm_ms_batch_run(const gpm_ms_batch_desc* desc, const gpm_job_opts* opts, const gpm_view_sel* vsel,
                      gpm_ms_batch_stats* stats);
 
+/* gpm_ms_batch_run_prior: gpm_ms_batch_run with the planar prior (ACMMP: Xu, Kong, Zuo & Tao, TPAMI 2022; DESIGN.md §20).
+ * Each stage given is the batch drivers' prior stage (gpm_prior_opts above: build, gpm_set_prior, gpm_cost_eval +
+ * gpm_set_state of the current planes, gpm_offer_prior, `iterations` sweeps), and touches only its own view's context, so
+ * every level stays a Jacobi step.
+ *   photometric: at the coarsest level, in step 2 of gpm_ms_batch_run, after the params.iterations sweeps; then the raw planes
+ *     kept, gpm_finalize, the term off, the depth map kept: the coarsest geometric stage reads depth maps made with the prior.
+ *   geometric: at every level, in each geometric stage, after the geo_iterations sweeps with the geometric term; then the raw
+ *     planes kept (levels > 0) or gpm_finalize and the outputs (level 0); then the term off and the geometric term off.  Its
+ *     support points are chosen by the stored costs, which include the geometric term, so support_cost is in those units: a
+ *     pixel that is photometrically cheap but geometrically inconsistent is not a support point.
+ * info of a stage (NULL or caller memory): photometric n_images entries, by image index; geometric GPM_MS_MAX_LEVELS *
+ * n_images entries, [level * n_images + image].  Entries of views or levels that ran no stage are zeroed.  The prior
+ * sweeps count in stats->level_sweep_ms and the level-0 per-job sweep ms; level_build_ms receives the host time of the
+ * gpm_build_planar_prior calls of both stages, summed over the views, per level.  prior NULL, or both stages NULL, is
+ * gpm_ms_batch_run.  Refused with GPM_E_ARG before any CUDA call, besides what gpm_ms_batch_run refuses: per stage given,
+ * what gpm_batch_run_prior refuses of its options (so colour images and joint view selection), a weight with which a valid
+ * cost could reach MAXCOST (photometric: without the geometric term; geometric: with weight * max_err), and a level that
+ * gpm_build_planar_prior refuses, wider or taller than 4097 pixels (photometric: the coarsest; geometric: level 0). */
+typedef struct gpm_ms_prior_opts {
+    const gpm_prior_opts* photometric; /* NULL: no stage */
+    const gpm_prior_opts* geometric;   /* NULL: no stage */
+    double level_build_ms[GPM_MS_MAX_LEVELS];     /* out: host time of the gpm_build_planar_prior calls, summed, per level */
+} gpm_ms_prior_opts;
+int gpm_ms_batch_run_prior(const gpm_ms_batch_desc* desc, const gpm_job_opts* opts, const gpm_view_sel* vsel,
+                           gpm_ms_prior_opts* prior, gpm_ms_batch_stats* stats);
+
 #ifdef __cplusplus
 }
 #endif

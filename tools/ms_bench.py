@@ -3,6 +3,7 @@ prints one JSON line.
 
     python tools/ms_bench.py [--rows 600] [--cols 800] [--cams 16] [--scenes smooth,hard,lit] [--costs pm,ncc]
                              [--modes fixed,adaptive] [--levels 2,3] [--weights 0.5,0] [--jbu RADIUS,SIGMA_S,SIGMA_R] [--dtu-preset]
+                             [--prior]
 
 Quality: tools/acs_bench.py's workload (the first `--cams` DTU cameras at `--cols` x `--rows`, every second camera a
 reference view, box 11, n_best 3, depth 300..800, views at 5..45 degrees, at most 6 per reference; the same fusion and
@@ -12,8 +13,13 @@ geometric term at every level, at each of `--levels` and `--weights` (weight 0: 
 has the F-score at 0.25, 0.5 and 1 unit, mean accuracy and completeness (units), vertices and the sweep ms summed over every
 level and view (CUDA events on gpm_stream); on the hard scene also the scores on its texture-less band (acs_bench.py's
 prior_study band rule).  --dtu-preset adds 49 cameras at 1600 x 1200, every camera a reference view, PM, one worker:
-wall seconds and summed sweep seconds of geometric_pass 4 + 2 against multiscale_pass at each of `--levels`.  Needs a CUDA
-device; there is no CPU path.
+wall seconds and summed sweep seconds of geometric_pass 4 + 2 against multiscale_pass at each of `--levels`.
+--prior adds the planar prior inside the multi-level driver (DESIGN.md §20), each stage with PRIOR_DEFAULTS and 2 sweeps: per
+level count, multiscale_pass at weight GEO_WEIGHT with no stage, the photometric stage, the geometric stage and both, the
+geometric stage at two support costs (PRIOR_DEFAULTS["support_cost"] and that plus GEO_WEIGHT * 1 pixel, the geometric term
+of a pixel 1 pixel off), with the prior builds' host ms per level; and geometric_pass 4 + 2 with planar_prior as the
+single-scale comparison.  With --dtu-preset it adds multiscale_pass with both stages at each support cost to the preset.
+Needs a CUDA device; there is no CPU path.
 """
 import argparse
 import json
@@ -39,6 +45,7 @@ def main():
     ap.add_argument("--weights", default="0.5,0")
     ap.add_argument("--jbu", default="")
     ap.add_argument("--dtu-preset", action="store_true")
+    ap.add_argument("--prior", action="store_true")
     a = ap.parse_args()
     import torch
     if not torch.cuda.is_available():
@@ -63,6 +70,13 @@ def main():
     out = {"gpu": gpu, "jbu": jbu, "workload": "%d DTU cameras at %dx%d" % (a.cams, a.cols, a.rows)}
     costs = {"pm": {}, "ncc": dict(photometric="ncc", ncc_min_std=api.NCC_MIN_STD)}
     costs = {k: costs[k] for k in a.costs.split(",") if k}
+    s0 = api.PRIOR_DEFAULTS["support_cost"]
+    supports = [s0, s0 + api.GEO_WEIGHT * 1.0]
+    prior_rows = [("none", None, None), ("photometric", {}, None)]
+    prior_rows += [(name % s, photo, {"support_cost": s}) for s in supports
+                   for name, photo in (("geometric s=%g", None), ("both s=%g", {}))]
+    if a.prior:
+        out["prior_support_costs"] = supports
 
     def params(iterations):
         p = S.AlgorithmParameters(box_hsize=11, box_vsize=11, iterations=iterations, n_best=3, cost_comb=S.COMB_BEST_N, gamma=10.0)
@@ -123,6 +137,19 @@ def main():
                                         level_sweep_ms=[round(1e3 * t, 1) for t in info["level_sweep_s"]],
                                         level_upsample_ms=[round(1e3 * t, 1) for t in info["level_upsample_s"]])
                         log("%s %s %s %s: %s" % (scene, cost, mode, key, row[key]))
+                if a.prior:
+                    n4, _, info = api.geometric_pass(images, Ps, params(4), refs, geo_iterations=2, propagation=mode,
+                                                     planar_prior={}, **kw, **photo)
+                    row["geometric_pass 4 + 2, planar_prior"] = score(n4, 1e3 * (sum(info["pass1_sweep_s"]) + sum(info["pass2_sweep_s"])))
+                    for L in levels:
+                        for name, pp, gp in prior_rows:
+                            n4, _, info = api.multiscale_pass(images, Ps, params(4), refs, levels=L, geo_iterations=2, jbu=jbu,
+                                                              propagation=mode, planar_prior=pp, geo_prior=gp, **kw, **photo)
+                            key = "multiscale_pass levels %d, prior %s" % (L, name)
+                            row[key] = dict(score(n4, 1e3 * sum(info["level_sweep_s"])),
+                                            level_sweep_ms=[round(1e3 * t, 1) for t in info["level_sweep_s"]],
+                                            level_build_ms=[round(t, 1) for t in info["level_build_ms"]])
+                            log("%s %s %s %s: %s" % (scene, cost, mode, key, row[key]))
                 res["%s %s" % (cost, mode)] = row
                 log("%s %s %s: %s" % (scene, cost, mode, row))
         out[scene] = res
@@ -145,6 +172,14 @@ def main():
                                                    "sweep_s_total": round(sum(info["level_sweep_s"]), 3),
                                                    "level_sweep_s": [round(t, 3) for t in info["level_sweep_s"]],
                                                    "level_upsample_s": [round(t, 3) for t in info["level_upsample_s"]]}
+            for name, pp, gp in (prior_rows[-1:-4:-2] if a.prior else []):                # both stages, each support cost
+                t0 = time.perf_counter()
+                _, _, info = api.multiscale_pass(images, allP, params(4), list(range(n)), levels=L, geo_iterations=2, jbu=jbu,
+                                                 planar_prior=pp, geo_prior=gp, **dkw)
+                dtu["multiscale_pass levels %d, prior %s" % (L, name)] = {
+                    "wall_s": round(time.perf_counter() - t0, 2), "sweep_s_total": round(sum(info["level_sweep_s"]), 3),
+                    "level_sweep_s": [round(t, 3) for t in info["level_sweep_s"]],
+                    "level_build_s": [round(t / 1e3, 3) for t in info["level_build_ms"]]}
         out["dtu_preset"] = dict(dtu, workload="%d views at 1600x1200, PM, fixed, one worker, every view a reference" % n)
         log("DTU preset: %s" % dtu)
     print(json.dumps(out))
