@@ -236,6 +236,14 @@ int refuse_change(const gpm_ctx* c, const char* fn, bool Mode::*field, bool on)
 // per-warp floats of the JVS kernel variant the context launches (0 without view selection)
 int jvs_extra(const gpm_ctx* c) { return jvs_on(c) ? jvs_floats(c->V, c->geo_weight > 0.f) : 0; }
 
+// k_sweep's per-warp floats beyond the common scratch, and its shared memory per block: the JVS rows, or the plane-major
+// pass's scratch and candidate cost table in the mode that shares propagation samples (shares_samples)
+int sweep_extra(const gpm_ctx* c, const KParams& P) { return shares_samples(ctx_mode(c)) ? share_extra_floats(P) : jvs_extra(c); }
+size_t sweep_smem_bytes(const gpm_ctx* c, const KParams& P)
+{
+    return block_smem_bytes(P, ncc_on(c), sweep_extra(c, P)) + (shares_samples(ctx_mode(c)) ? GPM_SHARE_TABLE_BYTES : 0);
+}
+
 // selected-views masks back to "none selected" (gpm_init, gpm_set_state, a switch to JOINT)
 int clear_vsel_masks(gpm_ctx* c)
 {
@@ -345,15 +353,15 @@ int build_kparams(gpm_ctx* c, bool init_phase, KParams& P, bool eval_call = fals
     P.ref.depthMin = p.depthMin;  P.ref.depthMax = p.depthMax;
     // warps per block: as many as fit (<= 16).  The kernels use 128 registers per thread, so one 16-warp block fills an SM
     // anyway; shared memory may therefore be spent up to the per-block opt-in limit.
-    const size_t per_warp = (size_t)warp_scratch_floats(P.ns_pad, P.V, P.color, ncc_on(c), jvs_extra(c)) * sizeof(float);
-    const size_t fixed = ((size_t)fixed_smem_floats(P) + 4) * sizeof(float);
+    const size_t per_warp = (size_t)warp_scratch_floats(P.ns_pad, P.V, P.color, ncc_on(c), sweep_extra(c, P)) * sizeof(float);
+    const size_t fixed = ((size_t)fixed_smem_floats(P) + 4) * sizeof(float) + (shares_samples(ctx_mode(c)) ? GPM_SHARE_TABLE_BYTES : 0);
     int nw = GPM_LB_THREADS / 32;
     const size_t budget = (size_t)c->smem_optin > 16 * 1024 ? (size_t)c->smem_optin - 8 * 1024 : 40 * 1024;
     while (nw > 2 && fixed + nw * per_warp > budget) nw--;
     if (c->opt_nwarps > 0) nw = c->opt_nwarps;
     if (nw > GPM_LB_THREADS / 32) nw = GPM_LB_THREADS / 32;
     P.nwarps = nw;
-    if (block_smem_bytes(P, ncc_on(c), jvs_extra(c)) > (size_t)c->smem_optin)
+    if (sweep_smem_bytes(c, P) > (size_t)c->smem_optin)
         return fail(GPM_E_ARG, "configuration needs more shared memory per block than the device offers");
     return ensure_tensor_map(c, P);
 }
@@ -454,7 +462,7 @@ int launch_colour(gpm_ctx* c, const KParams& P, int colour, int mask)
 {
     const auto kern = kSweep[ctx_mode(c).bits()];
     if (!kern) return fail(GPM_E_STATE, "k_sweep has no kernel for this context's mode");
-    kern<<<tile_grid(c), P.nwarps * 32, block_smem_bytes(P, ncc_on(c), jvs_extra(c)), c->stream>>>(P, c->tmap, c->d_cams, c->srcTex, c->planes,
+    kern<<<tile_grid(c), P.nwarps * 32, sweep_smem_bytes(c, P), c->stream>>>(P, c->tmap, c->d_cams, c->srcTex, c->planes,
         c->cost, c->rng, c->prov, Memo{c->pid, c->seen, c->refseen, c->memo_mask, c->next_id}, colour, mask, c->d_stats, geo_params(c),
         jvs_params(c), prior_params(c));
     c->launches++;

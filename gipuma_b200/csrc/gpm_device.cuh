@@ -369,6 +369,73 @@ __device__ __forceinline__ float prior_cost(const PriorParams& R, const float4& 
     return __fmul_rn(R.weight, q < 1e30f ? __fdiv_rn(q, __fadd_rn(1.0f, q)) : 1.0f);
 }
 
+// homographies H_v = K_v (R_v - t_v n^T / d) K_ref^-1 of plane (n, d) for every view into H[v * 12 ...] (rows of 3,
+// 16-byte aligned) — getHomography_cu, gipuma.cu:339-356
+__device__ __forceinline__ void homographies(const KParams& P, const float* __restrict__ sCam, float* H, float nx, float ny, float nz,
+                                             float d, unsigned lane)
+{
+    const float rd = frcp(d);
+    const float* Ki = P.ref.K_inv;
+    for (int v = lane; v < P.V; v += 32) {
+        const float* K = sCam + v * GPM_VIEWCAM_FLOATS;
+        const float* R = K + 9;
+        const float* t = K + 18;
+        float A[9], T[9];
+#pragma unroll
+        for (int i = 0; i < 3; i++) {
+            A[3 * i + 0] = ffma(-fmul(t[i], nx), rd, R[3 * i + 0]);
+            A[3 * i + 1] = ffma(-fmul(t[i], ny), rd, R[3 * i + 1]);
+            A[3 * i + 2] = ffma(-fmul(t[i], nz), rd, R[3 * i + 2]);
+        }
+#pragma unroll
+        for (int i = 0; i < 3; i++)
+#pragma unroll
+            for (int j = 0; j < 3; j++)
+                T[3 * i + j] = ffma(A[3 * i + 2], Ki[6 + j], ffma(A[3 * i], Ki[j], fmul(A[3 * i + 1], Ki[3 + j])));
+        float* Hv = H + v * 12;
+#pragma unroll
+        for (int i = 0; i < 3; i++)
+#pragma unroll
+            for (int j = 0; j < 3; j++)
+                Hv[3 * i + j] = ffma(K[3 * i + 2], T[6 + j], ffma(K[3 * i], T[j], fmul(K[3 * i + 1], T[3 + j])));
+    }
+}
+
+// dissimilarity of one grey sample against one view — pmCostComputation_shared, gipuma.cu:253-274
+__device__ __forceinline__ float dissim_grey(const KParams& P, float one_minus_alpha, float gx1, float gy1, float left, float gx2,
+                                             float gy2, float t_c)
+{
+    const float gradX = fsub(gx1, gx2);
+    const float gradY = fsub(gy1, gy2);
+    const float gradDis = fmin_(P.tau_gradient, fmul(fadd(fabsf(gradX), fabsf(gradY)), 0.0625f));
+    const float colDis = fmin_(P.tau_color, fabsf(fsub(left, t_c)));
+    return ffma(colDis, one_minus_alpha, fmul(P.alpha, gradDis));
+}
+
+// getCorrespondingPoint_cu (gipuma.cu:207-217): H (x, y, 1)^T, then / z — the division's multiply is fused with
+// the +-1 / +0.5 texel offsets in the reference binary (FFMA X, rcp(Z), {0.5, 1, -1}); then the source-view taps
+// of gipuma.cu:251-253: gx2 = tex(x+1,y) - tex(x-1,y), gy2 = tex(x,y+1) - tex(x,y-1), centre.  The three flags are the
+// rounding variant of each row of H (see eval_plane).
+__device__ __forceinline__ void fetch_sample_grey(cudaTextureObject_t src, const float4& h0, const float4& h1, const float4& h2, float ax,
+                                                  float ay, int v, bool XFIRST, bool YFIRSTX, bool ZFIRSTX, float& gx2, float& gy2,
+                                                  float& t_c)
+{
+    const float X = XFIRST ? fadd(h0.z, ffma(h0.y, ay, fmul(h0.x, ax))) : fadd(h0.z, ffma(h0.x, ax, fmul(h0.y, ay)));
+    const float Y = YFIRSTX ? fadd(h1.y, ffma(h1.x, ay, fmul(h0.w, ax))) : fadd(h1.y, ffma(h0.w, ax, fmul(h1.x, ay)));
+    const float Z = ZFIRSTX ? fadd(h2.x, ffma(h1.w, ay, fmul(h1.z, ax))) : fadd(h2.x, ffma(h1.z, ax, fmul(h1.w, ay)));
+    const float r = frcp(Z);
+    const float cx = ffma(X, r, 0.5f), cy = ffma(Y, r, 0.5f);
+    const float cxp = fadd(ffma(X, r, 1.0f), 0.5f), cxm = fadd(ffma(X, r, -1.0f), 0.5f);
+    const float cyp = fadd(ffma(Y, r, 1.0f), 0.5f), cym = fadd(ffma(Y, r, -1.0f), 0.5f);
+    t_c = tex2DLayered<float>(src, cx, cy, v);
+    const float t_xp = tex2DLayered<float>(src, cxp, cy, v);
+    const float t_xm = tex2DLayered<float>(src, cxm, cy, v);
+    const float t_yp = tex2DLayered<float>(src, cx, cyp, v);
+    const float t_ym = tex2DLayered<float>(src, cx, cym, v);
+    gx2 = fsub(t_xp, t_xm);
+    gy2 = fsub(t_yp, t_ym);
+}
+
 // ---- cost of one plane hypothesis at the warp's pixel ---------------------------------------
 // pmCostMultiview_cu (gipuma.cu:720-806) over pmCost_shared (:585-680) / pmCostComputation_shared (:223-277).
 // Returns the exact combined cost, or — if `bound` is finite and an exact lower bound of the final cost
@@ -402,34 +469,7 @@ __device__ __forceinline__ float eval_plane(const KParams& P, const float* __res
     const bool ZFIRSTX = XF == 2 ? (((rt >> 3) ^ rt) & 1u) != 0u : XF == 1;
     const int grad_variant = XF == 2 ? (int)((rt >> 1) & 1u) : P.grad_variant;
 
-    // homographies H_v = K_v (R_v - t_v n^T / d) K_ref^-1 — getHomography_cu, gipuma.cu:339-356
-    {
-        const float rd = frcp(d);
-        const float* Ki = P.ref.K_inv;
-        for (int v = lane; v < P.V; v += 32) {
-            const float* K = sCam + v * GPM_VIEWCAM_FLOATS;
-            const float* R = K + 9;
-            const float* t = K + 18;
-            float A[9], T[9];
-#pragma unroll
-            for (int i = 0; i < 3; i++) {
-                A[3 * i + 0] = ffma(-fmul(t[i], nx), rd, R[3 * i + 0]);
-                A[3 * i + 1] = ffma(-fmul(t[i], ny), rd, R[3 * i + 1]);
-                A[3 * i + 2] = ffma(-fmul(t[i], nz), rd, R[3 * i + 2]);
-            }
-#pragma unroll
-            for (int i = 0; i < 3; i++)
-#pragma unroll
-                for (int j = 0; j < 3; j++)
-                    T[3 * i + j] = ffma(A[3 * i + 2], Ki[6 + j], ffma(A[3 * i], Ki[j], fmul(A[3 * i + 1], Ki[3 + j])));
-            float* H = ws.H + v * 12;
-#pragma unroll
-            for (int i = 0; i < 3; i++)
-#pragma unroll
-                for (int j = 0; j < 3; j++)
-                    H[3 * i + j] = ffma(K[3 * i + 2], T[6 + j], ffma(K[3 * i], T[j], fmul(K[3 * i + 1], T[3 + j])));
-        }
-    }
+    homographies(P, sCam, ws.H, nx, ny, nz, d, lane);
     __syncwarp();
     float g0 = 0.0f, g1 = 0.0f;          // geometric terms of views lane and lane + 32
     if constexpr (GEO) {
@@ -522,33 +562,12 @@ __device__ __forceinline__ float eval_plane(const KParams& P, const float* __res
     st.hyp++;
     st.pairs_full += (unsigned long long)P.V * P.ns;
 
-    // dissimilarity of one sample against one view — pmCostComputation_shared, gipuma.cu:253-274
     auto dissim = [&](float gx1, float gy1, float left, float gx2, float gy2, float t_c) {
-        const float gradX = fsub(gx1, gx2);
-        const float gradY = fsub(gy1, gy2);
-        const float gradDis = fmin_(P.tau_gradient, fmul(fadd(fabsf(gradX), fabsf(gradY)), 0.0625f));
-        const float colDis = fmin_(P.tau_color, fabsf(fsub(left, t_c)));
-        return ffma(colDis, one_minus_alpha, fmul(P.alpha, gradDis));
+        return dissim_grey(P, one_minus_alpha, gx1, gy1, left, gx2, gy2, t_c);
     };
-    // getCorrespondingPoint_cu (gipuma.cu:207-217): H (x, y, 1)^T, then / z — the division's multiply is fused with
-    // the +-1 / +0.5 texel offsets in the reference binary (FFMA X, rcp(Z), {0.5, 1, -1}); then the source-view taps
-    // of gipuma.cu:251-253: gx2 = tex(x+1,y) - tex(x-1,y), gy2 = tex(x,y+1) - tex(x,y-1), centre.
     auto fetch_sample = [&](const float4& h0, const float4& h1, const float4& h2, float ax, float ay, int v,
                             float& gx2, float& gy2, float& t_c) {
-        const float X = XFIRST ? fadd(h0.z, ffma(h0.y, ay, fmul(h0.x, ax))) : fadd(h0.z, ffma(h0.x, ax, fmul(h0.y, ay)));
-        const float Y = YFIRSTX ? fadd(h1.y, ffma(h1.x, ay, fmul(h0.w, ax))) : fadd(h1.y, ffma(h0.w, ax, fmul(h1.x, ay)));
-        const float Z = ZFIRSTX ? fadd(h2.x, ffma(h1.w, ay, fmul(h1.z, ax))) : fadd(h2.x, ffma(h1.z, ax, fmul(h1.w, ay)));
-        const float r = frcp(Z);
-        const float cx = ffma(X, r, 0.5f), cy = ffma(Y, r, 0.5f);
-        const float cxp = fadd(ffma(X, r, 1.0f), 0.5f), cxm = fadd(ffma(X, r, -1.0f), 0.5f);
-        const float cyp = fadd(ffma(Y, r, 1.0f), 0.5f), cym = fadd(ffma(Y, r, -1.0f), 0.5f);
-        t_c = tex2DLayered<float>(src, cx, cy, v);
-        const float t_xp = tex2DLayered<float>(src, cxp, cy, v);
-        const float t_xm = tex2DLayered<float>(src, cxm, cy, v);
-        const float t_yp = tex2DLayered<float>(src, cx, cyp, v);
-        const float t_ym = tex2DLayered<float>(src, cx, cym, v);
-        gx2 = fsub(t_xp, t_xm);
-        gy2 = fsub(t_yp, t_ym);
+        fetch_sample_grey(src, h0, h1, h2, ax, ay, v, XFIRST, YFIRSTX, ZFIRSTX, gx2, gy2, t_c);
     };
 
     // ---- colour (T = float4) variants: pmCostComputation_shared<float4>, l1_norm(float4) = (|x|+|y|+|z|) * 0.3333333f

@@ -327,6 +327,270 @@ __device__ __forceinline__ bool sweep_neighbour(int k, const int& px, const int&
     else return close_far_neighbour(k, px, py, W, H, qx, qy);
 }
 
+// ---- shared propagation samples (DESIGN.md §4) ------------------------------------------------------------------------
+// In the sweep mode with none of the options of Mode — grey images, PM cost, the fixed 8-neighbour sweep — k_sweep costs the
+// propagated candidates plane-major before its per-pixel loop.  A launch of colour c never writes a plane of colour 1 - c, and
+// each such plane q is offered to q +- (0, 1), q +- (0, 5) (its column group) and q +- (1, 0), q +- (5, 0) (its row group).
+// The four windows of a group lie on one stride-2 lattice, and a sample's dissimilarity against view v is a function of the
+// plane, the view and the sample's absolute texel alone (the propagation sites all use rounding variant 1), so one warp
+// fetches each lattice texel of a group once and runs every target pixel's own chain over it.
+__host__ __device__ constexpr bool shares_samples(Mode m) { return m.bits() == 0; }
+
+// Per-warp layout of the plane-major pass, in floats from the warp's scratch (which it overlays: the pass ends before the
+// per-pixel loop starts).  L texels of the union lattice (nside x (nside + 5)); A/left/pos: per fetched texel in fetch order,
+// its (x, y, gx1, gy1), its reference value and its place in D; lines: the lattice lines the needed windows cover; w: the
+// support weights of up to four targets; cv: their per-view costs; D: the dissimilarities of C views (views in chunks, so
+// that D does not grow with V).
+struct ShareLayout { int L, LS, WS, C, A, H, left, pos, lines, w, cv, D, total; };
+__host__ __device__ inline ShareLayout share_layout(const KParams& P)
+{
+    ShareLayout s;
+    s.L = P.nside * (P.nside + 5);
+    s.LS = s.L | 1;
+    s.WS = P.ns | 1;
+    const int chunks = (P.V + 7) / 8;
+    s.C = (P.V + chunks - 1) / chunks;
+    s.A = 0;
+    s.H = 4 * s.L;
+    s.left = s.H + 12 * P.V;
+    s.pos = s.left + s.L;
+    s.lines = s.pos + s.L;
+    s.w = s.lines + 20;
+    s.cv = s.w + 4 * s.WS;
+    s.D = s.cv + 4 * P.V;
+    s.total = s.D + s.C * s.LS;
+    return s;
+}
+// floats per warp the pass needs beyond the common warp scratch (block_smem_bytes' `extra`)
+__host__ __device__ inline int share_extra_floats(const KParams& P)
+{
+    const int d = share_layout(P).total - warp_scratch_floats(P.ns_pad, P.V, 0);
+    return d > 0 ? d : 0;
+}
+// after the block's usual shared memory: the costs cand_cost[pixel][k] of the tile's 512 pixels of the launch's colour,
+// then each pixel's need mask (bit k: candidate k is evaluated)
+#define GPM_SHARE_TABLE_BYTES (GPM_TILE * GPM_TILE / 2 * (8 * 4 + 1))
+
+__device__ __forceinline__ int nth_set_bit(unsigned m, int i)
+{
+    for (; i > 0; i--) m &= m - 1u;
+    return __ffs(m) - 1;
+}
+
+// Need masks of the slice's pixels, from the state at launch start only: candidate k of pixel p is evaluated unless it is
+// not offered (border guard, phase mask), one of p's 8 remembered identities (memo), its depth at p is out of range, it is
+// p's own plane with p's cost of the same rounding variant (dedupe_self), or an earlier candidate of p has its identity
+// (dedupe_cand).  Each skip is exact: cost(p, plane) is a pure function and p's cost only decreases, so a skipped candidate
+// could not be accepted at any point of p's candidate scan.  Lanes 8m..8m+7 hold the 8 candidates of pixel m of 4.
+__device__ __forceinline__ void share_need_masks(const KParams& P, const float4* __restrict__ planes, const unsigned char* __restrict__ prov,
+                                                 const Memo& M, int colour, int phase_mask, int idx_begin, int idx_end,
+                                                 unsigned char* need, unsigned lane, unsigned warp)
+{
+    const int j = (int)(lane & 7);
+    // two groups of 4 pixels per step, every load of a step issued before any is used (the pass is latency bound)
+    for (int base = idx_begin + 8 * (int)warp; base < idx_end; base += 8 * P.nwarps) {
+        int idx[2], px[2], py[2];
+        bool valid[2], offered[2];
+        unsigned id[2], old_id[2], own[2], mmask[2];
+        unsigned char pv[2];
+        float4 n[2];
+#pragma unroll
+        for (int u = 0; u < 2; u++) {
+            idx[u] = base + 4 * u + (int)(lane >> 3);
+            colour_pixel(idx[u], colour, px[u], py[u]);
+            valid[u] = idx[u] < idx_end && px[u] < P.W && py[u] < P.H;
+            const size_t center = valid[u] ? (size_t)py[u] * P.W + px[u] : 0;
+            int qx = px[u], qy = py[u];
+            offered[u] = valid[u] && ((phase_mask >> (j >> 2)) & 1) && close_far_neighbour(j, px[u], py[u], P.W, P.H, qx, qy);
+            const size_t at = (size_t)qy * P.W + qx;
+            id[u] = offered[u] ? M.pid[at] : 0u;
+            n[u] = offered[u] ? planes[at] : make_float4(0.f, 0.f, 0.f, 0.f);
+            mmask[u] = P.memo && valid[u] ? M.mask[center] : 0u;
+            old_id[u] = P.memo && valid[u] ? M.seen[center * 8 + j] : 0u;
+            own[u] = valid[u] ? M.pid[center] : 0u;
+            pv[u] = valid[u] ? prov[center] : (unsigned char)0;
+        }
+#pragma unroll
+        for (int u = 0; u < 2; u++) {
+            const bool old_ok = (mmask[u] >> j) & 1u;
+            bool known = false, dup = false;
+            for (int i = 0; i < 8; i++) {
+                const bool oi = __shfl_sync(GPM_FULL, old_ok, i, 8);
+                const unsigned idi = __shfl_sync(GPM_FULL, old_id[u], i, 8);
+                const bool ci = __shfl_sync(GPM_FULL, offered[u], i, 8);
+                const unsigned cid = __shfl_sync(GPM_FULL, id[u], i, 8);
+                known |= oi && idi == id[u];
+                dup |= i < j && ci && cid == id[u];
+            }
+            const float d = plane_depth(P.ref, n[u].x, n[u].y, n[u].z, n[u].w, __int2float_rn(px[u]), __int2float_rn(py[u]));   // gipuma.cu:829-830
+            const bool ok = offered[u] && !known && !(P.dedupe_cand && dup) && !(P.dedupe_self && pv[u] == 1 && id[u] == own[u]) &&
+                            d >= P.ref.depthMin && d <= P.ref.depthMax;
+            const unsigned b = __ballot_sync(GPM_FULL, ok);
+            if (j == 0 && idx[u] < idx_end) need[idx[u]] = (unsigned char)(b >> (lane & 24));
+        }
+    }
+}
+
+// The plane-major pass: every needed (pixel, candidate) of the slice gets its exact cost in table[idx * 8 + k].  Work items
+// are (plane q, group) over the other colour's pixels of the slice's rows plus the 5-pixel halo, taken dynamically by the
+// warps (counter).  `tile` is the staged reference window (already offset by tile_xo).
+__device__ __forceinline__ void share_costs(const KParams& P, const float* __restrict__ sCam, const float* __restrict__ tile,
+                                            float* wbase, cudaTextureObject_t src, const float4* __restrict__ planes, int colour,
+                                            int idx_begin, int idx_end, int tile_x0, int tile_y0, const unsigned char* need,
+                                            float* table, int* counter, unsigned long long* stats, unsigned lane, WarpStats& st)
+{
+    const ShareLayout S = share_layout(P);
+    float4* Ae = reinterpret_cast<float4*>(wbase + S.A);
+    float* Hs = wbase + S.H;
+    float* le = wbase + S.left;
+    int* pe = reinterpret_cast<int*>(wbase + S.pos);
+    int* lines = reinterpret_cast<int*>(wbase + S.lines);
+    float* wt = wbase + S.w;
+    float* cv = wbase + S.cv;
+    float* Dc = wbase + S.D;
+    const int nside = P.nside, rad = P.rad, tw = P.tile_stride, V = P.V;
+    const int bx0 = blockIdx.x * GPM_TILE, by0 = blockIdx.y * GPM_TILE;
+    // tile rows of the slice, and the items: column groups of its rows +- 5, then row groups of its rows (the row groups'
+    // columns run one lattice step past the halo on each side so that every row has 22 planes of the other colour)
+    const int ylo = by0 + 2 * (idx_begin >> 5), yhi = by0 + 2 * ((idx_end - 1) >> 5) + 1;
+    const int ncol = (yhi - ylo + 11) * 16, nitems = ncol + (yhi - ylo + 1) * 22;
+    const float nrg = -frcp(P.gamma);
+    const float one_minus_alpha = fsub(1.0f, P.alpha);
+    auto texel = [&](int x, int y) { return tile + (y - tile_y0) * tw + (x - tile_x0); };
+    auto plane_of = [&](int it, bool& col, int& qx, int& qy) {
+        col = it < ncol;
+        const int r = col ? it >> 4 : (it - ncol) / 22;
+        const int jq = col ? it & 15 : it - ncol - r * 22;
+        qy = col ? ylo - 5 + r : ylo + r;
+        qx = (col ? bx0 : bx0 - 6) + 2 * jq + ((1 + colour + qy) & 1);
+    };
+    // the warps take 8 items at a time; lane 4i + m tests target m of item i: q + off along the group's axis, of which q is
+    // candidate kk
+    int base = 8 * (int)(threadIdx.x >> 5);
+    while (base < nitems) {
+        const int m = (int)(lane & 3);
+        const int off = m == 0 ? -5 : m == 1 ? -1 : m == 2 ? 1 : 5;
+        int idx = 0, kk = 0;
+        bool mine = false;
+        if (base + (int)(lane >> 2) < nitems) {
+            bool col;
+            int qx, qy;
+            plane_of(base + (int)(lane >> 2), col, qx, qy);
+            kk = col ? (m == 0 ? 5 : m == 1 ? 1 : m == 2 ? 0 : 4) : (m == 0 ? 7 : m == 1 ? 3 : m == 2 ? 2 : 6);
+            const int tx = (col ? qx : qx + off) - bx0, ty = (col ? qy + off : qy) - by0;
+            idx = (ty >> 1) * GPM_TILE + tx;
+            mine = tx >= 0 && tx < GPM_TILE && ty >= 0 && ty < GPM_TILE && idx >= idx_begin && idx < idx_end && ((need[idx] >> kk) & 1);
+        }
+        for (unsigned bm = __ballot_sync(GPM_FULL, mine); bm; ) {
+            const int it = (__ffs(bm) - 1) >> 2;
+            const unsigned nm = (bm >> (4 * it)) & 15u;
+            bm &= ~(15u << (4 * it));
+            bool col;
+            int qx, qy;
+            plane_of(base + it, col, qx, qy);
+            const int nneed = __popc(nm);
+            const float4 pl = planes[(size_t)qy * P.W + qx];
+            homographies(P, sCam, Hs, pl.x, pl.y, pl.z, pl.w, lane);
+            unsigned lm = 0u;                                    // lattice lines covered by the needed windows
+            for (int i = 0; i < 4; i++)
+                if ((nm >> i) & 1u) lm |= ((1u << nside) - 1u) << (i == 0 ? 0 : i == 1 ? 2 : i == 2 ? 3 : 5);
+            const int nl = __popc(lm), NY = col ? nside + 5 : nside;
+            if ((int)lane < nside + 5 && ((lm >> lane) & 1u)) lines[__popc(lm & ((1u << lane) - 1u))] = (int)lane;
+            const int x0 = col ? qx - rad : qx - 5 - rad, y0 = col ? qy - 5 - rad : qy - rad;
+            __syncwarp();
+            // the fetch order: pairs of covered lines, 2 x 2 lattice blocks per hardware quad
+            const int n = nl * nside;
+            for (int e = (int)lane; e < n; e += 32) {
+                const int p2 = e / (2 * nside), rem = e - p2 * 2 * nside;
+                const bool pair = 2 * p2 + 1 < nl;
+                const int line = lines[pair ? 2 * p2 + (rem & 1) : 2 * p2], b = pair ? rem >> 1 : rem;
+                const int lx = col ? b : line, ly = col ? line : b;
+                const int x = x0 + 2 * lx, y = y0 + 2 * ly;
+                const float* t = texel(x, y);
+                Ae[e] = make_float4(__int2float_rn(x), __int2float_rn(y), fsub(t[1], t[-1]), fsub(t[tw], t[-tw]));   // as setup_window
+                le[e] = t[0];
+                pe[e] = lx * NY + ly;
+            }
+            for (int f = (int)lane; f < nneed * P.ns; f += 32) {  // support weights of the needed targets, as setup_window
+                const int i = f / P.ns, s = f - i * P.ns;
+                const int mi = nth_set_bit(nm, i);
+                const int o = mi == 0 ? -5 : mi == 1 ? -1 : mi == 2 ? 1 : 5;
+                const int cx = col ? qx : qx + o, cy = col ? qy + o : qy;
+                const int ii = s / nside, jj = s - ii * nside;
+                const float center = *texel(cx, cy), left = *texel(cx - rad + 2 * ii, cy - rad + 2 * jj);
+                wt[i * S.WS + s] = fex2(fmul(fmul(fabsf(fsub(left, center)), nrg), 1.4426950216293334961f));
+            }
+            __syncwarp();
+            const unsigned Mg = (1u << 20) / (unsigned)n + 1u;
+            for (int v0 = 0; v0 < V; v0 += S.C) {
+                const int Cc = min(S.C, V - v0), npairs = Cc * n;
+                // lane handles pair (view v0 + vi, texel e); N steps in flight before any result is consumed (as eval_plane)
+                auto fetch = [&](auto nconst, int q0) {
+                    constexpr int N = decltype(nconst)::value;
+                    float gx2[N], gy2[N], tc[N];
+                    float4 a[N];
+                    int dst[N], ei[N];
+#pragma unroll
+                    for (int u = 0; u < N; u++) {
+                        const int q = q0 + u * 32 + (int)lane;
+                        const int qc = min(q, npairs - 1);
+                        const int vi = (int)(((unsigned)qc * Mg) >> 20);           // qc / n
+                        const int e = qc - vi * n;
+                        const float4* H4 = reinterpret_cast<const float4*>(Hs + (v0 + vi) * 12);
+                        a[u] = Ae[e];
+                        ei[u] = e;
+                        dst[u] = q < npairs ? vi * S.LS + pe[e] : -1;
+                        fetch_sample_grey(src, H4[0], H4[1], H4[2], a[u].x, a[u].y, v0 + vi, true, true, true, gx2[u], gy2[u], tc[u]);
+                    }
+#pragma unroll
+                    for (int u = 0; u < N; u++) {
+                        const float dis = dissim_grey(P, one_minus_alpha, a[u].z, a[u].w, le[ei[u]], gx2[u], gy2[u], tc[u]);
+                        if (dst[u] >= 0) Dc[dst[u]] = dis;
+                    }
+                };
+                int q0 = 0;
+                for (; q0 + 32 < npairs; q0 += 64) fetch(std::integral_constant<int, 2>(), q0);
+                if (q0 < npairs) fetch(std::integral_constant<int, 1>(), q0);
+                __syncwarp();
+                // lane = (needed target i, view vi): the target's chain  c = c + w_s * D_s  in its own sample order
+                if ((int)lane < nneed * Cc) {
+                    const int i = (int)lane / Cc, vi = (int)lane - i * Cc;
+                    const int mi = nth_set_bit(nm, i);
+                    const int o = mi == 0 ? 0 : mi == 1 ? 2 : mi == 2 ? 3 : 5;
+                    const float* w = wt + i * S.WS;
+                    const float* D = Dc + vi * S.LS + (col ? o : o * nside);
+                    float c = 0.0f;
+                    for (int ii = 0; ii < nside; ii++)
+                        for (int jj = 0; jj < nside; jj++) c = ffma(w[ii * nside + jj], D[ii * NY + jj], c);
+                    cv[i * V + v0 + vi] = c;
+                }
+                __syncwarp();
+            }
+            for (int i = 0; i < nneed; i++) {
+                const float c0 = (int)lane < V ? cv[i * V + lane] : 0.0f;
+                const float c1 = (int)lane + 32 < V ? cv[i * V + lane + 32] : 0.0f;
+                const float c = combine_views(P, c0, c1, lane);
+                const int mi = nth_set_bit(nm, i);
+                const int ti = __shfl_sync(GPM_FULL, idx, 4 * it + mi), tk = __shfl_sync(GPM_FULL, kk, 4 * it + mi);
+                if (lane == 0) table[ti * 8 + tk] = c;
+            }
+            st.hyp += nneed;
+            st.pairs_full += (unsigned long long)nneed * V * P.ns;
+#ifndef GPM_SHARE_COUNT_FETCHES
+            st.pairs += (unsigned long long)nneed * V * P.ns;
+#else
+            // counting build of tools/share_bench.py: `pairs` counts the (view, texel) pairs really fetched, and slot 7 (no
+            // counter) the pass's pairs as `pairs` counts them otherwise
+            st.pairs += (unsigned long long)n * V;
+            if (lane == 0 && stats) atomicAdd(stats + 7, (unsigned long long)nneed * V * P.ns);
+#endif
+            __syncwarp();
+        }
+        if (lane == 0) base = atomicAdd(counter, 8);
+        base = __shfl_sync(GPM_FULL, base, 0);
+    }
+}
+
 // One pixel of a joint-view-selection launch (ACMH, Xu & Tao 2019; DESIGN.md §17): NCC cost, grey images, 8-neighbour
 // sweep.  The steps as §17 numbers them: (1) the per-view cost rows of the current plane and of every offered candidate
 // whose depth is in range (E), a candidate whose identity equals the current plane's or an earlier candidate's reusing
@@ -517,16 +781,18 @@ k_sweep(const __grid_constant__ KParams P, const __grid_constant__ CUtensorMap t
         unsigned long long* __restrict__ stats, const __grid_constant__ GeoParams G, const JvsParams J, const PriorParams R)
 {
     static_assert(mode_conflict(Mode{COLOR, FUSED, GEO, NCC, ADAPTIVE, JVS, PRIOR}) == ModeConflict::none, "no such sweep mode (mode_conflict)");
+    constexpr bool SHARE = shares_samples(Mode{COLOR, FUSED, GEO, NCC, ADAPTIVE, JVS, PRIOR});
     const GeoParams* g = (GEO || NCC) ? &G : nullptr;
     extern __shared__ __align__(128) float smem[];
     float* tile = smem;
     float* sCam = tile + tile_floats(P);
     float* scratch = smem + fixed_smem_floats(P);
-    const int extra = JVS ? jvs_floats(P.V, GEO) : 0;
+    const int extra = JVS ? jvs_floats(P.V, GEO) : SHARE ? share_extra_floats(P) : 0;
     int* counter = reinterpret_cast<int*>(scratch + (size_t)P.nwarps * warp_scratch_floats(P.ns_pad, P.V, P.color, NCC, extra));
     const unsigned lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const int tile_x0 = blockIdx.x * GPM_TILE - P.halo, tile_y0 = blockIdx.y * GPM_TILE - P.halo;
     if (threadIdx.x == 0) counter[0] = P.nwarps;
+    if constexpr (SHARE) if (threadIdx.x == 0) counter[1] = 8 * P.nwarps;
     stage_block(P, &tmap, cams, tile, sCam, tile_x0, tile_y0, 0u, NCC, extra);
     float* warp_base = scratch + (size_t)warp * warp_scratch_floats(P.ns_pad, P.V, P.color, NCC, extra);
     const WarpScratch ws = carve(warp_base, P.ns_pad, P.V, P.color, block_perm(P, smem, NCC, extra), NCC);
@@ -540,6 +806,16 @@ k_sweep(const __grid_constant__ KParams P, const __grid_constant__ CUtensorMap t
     const int per_slice = (GPM_TILE * GPM_TILE / 2 + (int)gridDim.z - 1) / (int)gridDim.z;
     const int idx_begin = (int)blockIdx.z * per_slice;
     const int idx_end = min(GPM_TILE * GPM_TILE / 2, idx_begin + per_slice);
+    // SHARE: the propagated candidates' costs come from the plane-major pass (share_costs) through cand_cost
+    float* const cand_cost = smem + block_smem_bytes(P, NCC, extra) / sizeof(float);
+    unsigned char* const cand_need = reinterpret_cast<unsigned char*>(cand_cost + GPM_TILE * GPM_TILE / 2 * 8);
+    if constexpr (SHARE) {
+        share_need_masks(P, planes, prov, M, colour, phase_mask, idx_begin, idx_end, cand_need, lane, warp);
+        __syncthreads();
+        share_costs(P, sCam, tile + P.tile_xo, warp_base, src, planes, colour, idx_begin, idx_end, tile_x0, tile_y0, cand_need, cand_cost,
+                    counter + 1, stats, lane, st);
+        __syncthreads();
+    }
     int idx = idx_begin + (int)warp;
     while (idx < idx_end) {
         int px, py;
@@ -593,9 +869,30 @@ k_sweep(const __grid_constant__ KParams P, const __grid_constant__ CUtensorMap t
             const bool old_ok = P.memo && lane < NC && ((mmask >> lane) & 1);
             const unsigned old_id = old_ok ? M.seen[center * NC + lane] : 0u;
             const bool memo_hit = old_ok && mine_ok && old_id == mine_id;
-            if (mine_ok && !memo_hit) mine = planes[mine_at];          // a remembered neighbour is skipped below without its plane
+            if (SHARE ? ((cand_need[idx] >> lane) & 1u) != 0u : mine_ok && !memo_hit) mine = planes[mine_at];   // a remembered neighbour is skipped below without its plane
             const unsigned cand_mask = __ballot_sync(GPM_FULL, mine_ok);
-            for (int k = 0; k < NC; k++) {
+            if constexpr (SHARE) {
+                // share_need_masks decided every skip from the launch-start state, share_costs evaluated the rest; the scan,
+                // in candidate order with strict <, is the one below.  A needed candidate whose identity the pixel took by an
+                // accept in this scan costs exactly cost_now, so taking its cost instead of skipping it decides the same.
+                const unsigned need = cand_need[idx];
+                for (int k = 0; k < NC; k++) {
+                    if (!((cand_mask >> k) & 1)) continue;
+                    if (!((need >> k) & 1)) { st.skip++; continue; }
+                    float4 nb;
+                    nb.x = __shfl_sync(GPM_FULL, mine.x, k);  nb.y = __shfl_sync(GPM_FULL, mine.y, k);
+                    nb.z = __shfl_sync(GPM_FULL, mine.z, k);  nb.w = __shfl_sync(GPM_FULL, mine.w, k);
+                    const unsigned cand_id = __shfl_sync(GPM_FULL, mine_id, k);
+                    const float c = cand_cost[idx * 8 + k];
+                    if (c < cost_now) {                                                          // :867-871
+                        disp_now = plane_depth(cam, nb.x, nb.y, nb.z, nb.w, fpx, fpy);
+                        norm_now = nb;
+                        cost_now = c;
+                        prov_now = 1;
+                        own_id = cand_id;
+                    }
+                }
+            } else for (int k = 0; k < NC; k++) {
                 if (!((cand_mask >> k) & 1)) continue;
                 // rounding variant of this call site: x-first for float images, y-first for float4 (DESIGN.md §2); the fused
                 // kernel's inlined sites are looked up (bit 0 = x-first, bit 1 = gradient folding)
