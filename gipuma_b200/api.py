@@ -105,6 +105,11 @@ class GpmMsPriorOpts(C.Structure):
                 ("level_build_ms", C.c_double * MS_MAX_LEVELS)]
 
 
+class GpmMsRestoreOpts(C.Structure):
+    _fields_ = [("photo_iterations", C.c_int), ("threshold", C.c_float), ("iterations", C.c_int),
+                ("restored", C.POINTER(C.c_int))]
+
+
 class GpmFuseCamera(C.Structure):
     _fields_ = [("M_inv", C.c_float * 9), ("P", C.c_float * 12), ("f", C.c_float)]
 
@@ -226,6 +231,9 @@ def load_library():
                                    C.POINTER(GpmMsBatchStats)]
     L.gpm_ms_batch_run_prior.argtypes = [C.POINTER(GpmMsBatchDesc), C.POINTER(GpmJobOpts), C.POINTER(GpmViewSel),
                                          C.POINTER(GpmMsPriorOpts), C.POINTER(GpmMsBatchStats)]
+    L.gpm_ms_batch_run_restore.argtypes = [C.POINTER(GpmMsBatchDesc), C.POINTER(GpmJobOpts), C.POINTER(GpmViewSel),
+                                           C.POINTER(GpmMsPriorOpts), C.POINTER(GpmMsRestoreOpts), C.POINTER(GpmMsBatchStats)]
+    L.gpm_set_geo_mask.argtypes = [vp, vp, C.c_size_t, C.c_int]
     L.gpm_fuse_cameras.argtypes = [C.POINTER(C.c_double), C.c_int, C.c_double, C.POINTER(GpmFuseCamera)]
     L.gpm_fuse.argtypes = [C.POINTER(GpmFuseDesc), C.POINTER(GpmFuseResult)]
     L.gpm_write_ply.argtypes = [C.c_char_p, vp, C.c_longlong]
@@ -240,6 +248,7 @@ def load_library():
                  "gpm_batch_run_vsel", "gpm_geo_batch_run_vsel", "gpm_set_planar_prior", "gpm_get_planar_prior",
                  "gpm_build_planar_prior", "gpm_set_prior", "gpm_offer_prior", "gpm_batch_run_prior",
                  "gpm_geo_batch_run_prior", "gpm_downsample", "gpm_upsample_planes", "gpm_ms_batch_run", "gpm_ms_batch_run_prior",
+                 "gpm_ms_batch_run_restore", "gpm_set_geo_mask",
                  "gpm_prepare_cameras", "gpm_select_views", "gpm_write_dmb", "gpm_read_dmb", "gpm_write_result_dmb",
                  "gpm_fuse_cameras", "gpm_fuse", "gpm_write_ply", "gpm_nearest_dist"):
         getattr(L, name).restype = C.c_int
@@ -455,6 +464,47 @@ MS_LEVELS, MS_GEO_ITERATIONS = 3, 2
 MS_GEO_PRIOR_SUPPORT_COST = PRIOR_DEFAULTS["support_cost"]
 
 
+# multiscale_pass's detail restorer (ACMM's, as the project's rule; DESIGN.md §21): detection threshold per photometric cost,
+# in that cost's units; photo_iterations None: params.iterations; iterations: sweeps after the restore.  The thresholds are
+# the best of the few measured with tools/ms_bench.py --restore (§21's table), not the result of a search.
+RESTORE_DEFAULTS = {"threshold": {"pm": 0.5, "ncc": 0.05}, "photo_iterations": None, "iterations": 2}
+
+
+def restore_opts(detail_restorer: Optional[dict], params, n_jobs: int, photometric: str = "pm"):
+    """gpm_ms_restore_opts from `detail_restorer` (None: no restorer; a dict overriding RESTORE_DEFAULTS), every argument
+    checked before any call into the library.  Returns (opts or None, the per-job restored-count array)."""
+    if detail_restorer is None:
+        return None, None
+    unknown = sorted(set(detail_restorer) - set(RESTORE_DEFAULTS))
+    if unknown:
+        raise ValueError("unknown detail-restorer parameters %s (known: %s)" % (unknown, sorted(RESTORE_DEFAULTS)))
+    r = dict(RESTORE_DEFAULTS)
+    r.update(detail_restorer)
+    if isinstance(r["threshold"], dict):
+        if photometric not in r["threshold"]:
+            raise ValueError("the threshold dict has no entry for photometric=%r (got %r)" % (photometric, r["threshold"]))
+        r["threshold"] = r["threshold"][photometric]
+    if r["photo_iterations"] is None:
+        r["photo_iterations"] = int(params.iterations)
+    t = r["threshold"]
+    # the library receives the threshold as float32: it must be finite after that rounding
+    t32 = np.float32(np.inf)
+    if not isinstance(t, bool) and isinstance(t, (int, float, np.floating, np.integer)):
+        with np.errstate(over="ignore"):
+            try:
+                t32 = np.float32(t)
+            except OverflowError:
+                pass
+    if not np.isfinite(t32):
+        raise ValueError("threshold must be a number that is finite in float32 (got %r)" % (t,))
+    for k, lo in (("photo_iterations", 1), ("iterations", 0)):
+        v = r[k]
+        if isinstance(v, bool) or not isinstance(v, (int, np.integer)) or not lo <= v <= 2 ** 31 - 1:
+            raise ValueError("%s must be an integer in %d..%d (got %r)" % (k, lo, 2 ** 31 - 1, v))
+    restored = (C.c_int * max(n_jobs, 1))()
+    return GpmMsRestoreOpts(int(r["photo_iterations"]), float(t32), int(r["iterations"]), restored), restored
+
+
 def jbu_params(radius: int = JBU_DEFAULTS["radius"], sigma_space: float = JBU_DEFAULTS["sigma_space"],
                sigma_range: float = JBU_DEFAULTS["sigma_range"]) -> GpmJbuParams:
     """gpm_jbu_params, every argument checked before any call into the library by the rules of gpm_upsample_planes."""
@@ -592,6 +642,25 @@ class Context:
         weight 0 turns it off."""
         check_geometric(weight, max_err)
         self._check(self.lib.gpm_set_geometric(self.h, float(weight), float(max_err)))
+
+    def set_geo_mask(self, mask):
+        """Per-pixel mask of the geometric term (DESIGN.md §21): [H, W] (numpy or torch, host or device; bool or uint8), nonzero
+        where the term is off; None clears it.  While the term is on, a masked pixel's costs are exactly those with the term
+        off.  Refused while the planar prior is on."""
+        if mask is None:
+            self._check(self.lib.gpm_set_geo_mask(self.h, None, 0, 0))
+            return
+        if tuple(mask.shape) != (self.H, self.W):
+            raise ValueError("mask must be [%d, %d], got %s" % (self.H, self.W, tuple(mask.shape)))
+        if isinstance(mask, np.ndarray):
+            m = np.ascontiguousarray(mask != 0, dtype=np.uint8)
+            self._check(self.lib.gpm_set_geo_mask(self.h, C.c_void_p(m.ctypes.data), 0, 0))
+            return
+        import torch
+        m = (mask != 0).to(torch.uint8).contiguous()
+        if m.is_cuda:
+            torch.cuda.current_stream(m.device).synchronize()     # the context works on its own stream
+        self._check(self.lib.gpm_set_geo_mask(self.h, C.c_void_p(m.data_ptr()), 0, 1 if m.is_cuda else 0))
 
     def set_photometric(self, kind: str = "pm", min_std: float = NCC_MIN_STD):
         """Photometric cost of every view (DESIGN.md §15): "pm", the reference's (the default), or "ncc", 1 - the
@@ -975,9 +1044,10 @@ def multiscale_pass(images, Ps, params, refs, levels: int = MS_LEVELS, geo_itera
                     cam_scale: float = 1.0, min_angle: float = 10.0, max_angle: float = 30.0, max_views: int = 9,
                     seed: int = 0xC0FFEE, devices=(0,), out_dir: Optional[str] = None, photometric: str = "pm",
                     ncc_min_std: float = NCC_MIN_STD, propagation: str = "fixed", view_selection: str = "off",
-                    jvs_params: Optional[dict] = None, planar_prior: Optional[dict] = None, geo_prior: Optional[dict] = None):
+                    jvs_params: Optional[dict] = None, planar_prior: Optional[dict] = None, geo_prior: Optional[dict] = None,
+                    detail_restorer: Optional[dict] = None):
     """Coarse-to-fine multi-scale PatchMatch (ACMM; DESIGN.md §19) for the reference views `refs`, run by the native
-    multi-level batch driver (gpm_ms_batch_run_prior) over the worker pool of `devices`.
+    multi-level batch driver (gpm_ms_batch_run_restore) over the worker pool of `devices`.
 
     V, the views refined, is the transitive closure of the references' view selections; each view keeps its level-0
     selection and depth range at every level.  Level l has the images downsampled l times (downsample) and K / 2^l.  At the
@@ -991,12 +1061,17 @@ def multiscale_pass(images, Ps, params, refs, levels: int = MS_LEVELS, geo_itera
     read depth maps made with it; geo_prior runs one at every level after the geo_iterations sweeps, with support points
     chosen by costs that include the geometric term (its support_cost defaults to MS_GEO_PRIOR_SUPPORT_COST, in those
     units).  Both need grey images and exclude joint view selection.
+    detail_restorer (DESIGN.md §21), None (off) or a dict overriding RESTORE_DEFAULTS: at level 0 each reference also runs a
+    photometric-only estimate (photo_iterations sweeps from init); after the geometric stage, pixels where the geometric
+    stage's plane costs photometrically more than `threshold` above the estimate's take the estimate's plane and sweep
+    without the geometric term (a per-pixel mask) for `iterations` more sweeps, while the rest keep it.
     Returns (norm4 [len(refs), H, W, 4], cost [len(refs), H, W], info) with norm4 as batch_run returns it, so fuse and
     evaluate_cloud take it unchanged; info: "views" (V, ascending), "level_sweep_s" (CUDA-event sweep seconds summed over
     the views, per level, full size first, prior sweeps included), "level_upsample_s" (host seconds of the upsampling calls,
     per level), "sweep_s" (each reference's level-0 sweep seconds), "device" (the device that refined it at level 0);
     "prior": {"photometric": per image index, "geometric": per level, per image index} of the prior's counts (None for a
-    stage not run; zeros where a view ran no stage), "level_build_ms" (host milliseconds of the prior builds, per level)."""
+    stage not run; zeros where a view ran no stage), "level_build_ms" (host milliseconds of the prior builds, per level);
+    "restored" (detail pixels per reference, None without the restorer)."""
     check_geometric(weight, max_err)
     opts = job_opts(photometric, ncc_min_std, propagation)
     if isinstance(levels, bool) or int(levels) != levels or not 1 <= levels <= MS_MAX_LEVELS:
@@ -1037,8 +1112,9 @@ def multiscale_pass(images, Ps, params, refs, levels: int = MS_LEVELS, geo_itera
         raise ValueError("reference views must be image indices in 0..%d" % (n - 1))
     if not 1 <= max_views <= 64:
         raise ValueError("max_views must be 1..64")
-    lib = load_library()
     k = len(refs)
+    ro, restored = restore_opts(detail_restorer, params, k, photometric)
+    lib = load_library()
     n4 = np.empty((k, H, W, 4), np.float32)
     cc = np.empty((k, H, W), np.float32)
     d, _keep = _batch_desc(imgs, Ps, params, refs, devices, cam_scale, min_angle, max_angle, max_views, seed, out_dir, n4, cc)
@@ -1048,13 +1124,14 @@ def multiscale_pass(images, Ps, params, refs, levels: int = MS_LEVELS, geo_itera
     jobs = _job_stats(k)                                   # owns the per-job arrays st.batch points into
     st = GpmMsBatchStats(jobs, 0, views)
     po = GpmMsPriorOpts(*[C.pointer(stages[s][0]) if s in stages else None for s in ("photometric", "geometric")])
-    rc = lib.gpm_ms_batch_run_prior(C.byref(m), C.byref(opts), C.byref(vsel), C.byref(po), C.byref(st))
+    rc = lib.gpm_ms_batch_run_restore(C.byref(m), C.byref(opts), C.byref(vsel), C.byref(po), C.byref(ro) if ro else None,
+                                      C.byref(st))
     if rc != 0:
         raise GipumaError("gpm_ms_batch_run failed (%d): %s" % (rc, lib.gpm_batch_last_error().decode()))
     info = {"views": views[:st.n_views], "level_sweep_s": [t / 1e3 for t in st.level_sweep_ms[:levels]],
             "level_upsample_s": [t / 1e3 for t in st.level_upsample_ms[:levels]],
             "sweep_s": [t / 1e3 for t in st.batch.per_job_sweep_ms[:k]], "device": st.batch.per_job_device[:k],
-            "level_build_ms": list(po.level_build_ms[:levels])}
+            "level_build_ms": list(po.level_build_ms[:levels]), "restored": restored[:k] if ro else None}
     pinfo = {s: stages[s][1] if s in stages else None for s in ("photometric", "geometric")}
     info["prior"] = {"photometric": _prior_info(pinfo["photometric"], n),
                      "geometric": [_prior_info(pinfo["geometric"][l * n:(l + 1) * n], n) for l in range(levels)]

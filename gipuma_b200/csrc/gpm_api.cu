@@ -139,6 +139,9 @@ struct gpm_ctx {
     float* prior_cost = nullptr;               // [H*W] gpm_offer_prior's costs of the prior planes
     float prior_weight = 0.f, prior_depth_sigma = 1.f, prior_normal_deg = 5.f;
     bool have_state = false;                   // gpm_init, gpm_run or gpm_set_state has given every pixel a plane and a cost
+    // the geometric term's per-pixel mask (DESIGN.md §21): nonzero bytes switch the term off; read while geo_mask_set
+    unsigned char* geo_mask = nullptr;         // [H*W], allocated by the first gpm_set_geo_mask
+    bool geo_mask_set = false;
 };
 
 namespace {
@@ -208,7 +211,7 @@ bool jvs_on(const gpm_ctx* c) { return c->vsel.kind == GPM_VSEL_JOINT; }
 Mode ctx_mode(const gpm_ctx* c)
 {
     return Mode{c->color == 1, c->opt_neighbours == 20, c->geo_weight > 0.f, ncc_on(c), c->propagation == GPM_PROP_ADAPTIVE, jvs_on(c),
-                c->prior_weight > 0.f};
+                c->prior_weight > 0.f, c->geo_weight > 0.f && c->geo_mask_set};
 }
 
 const char* conflict_text(ModeConflict k)
@@ -218,6 +221,7 @@ const char* conflict_text(ModeConflict k)
     case ModeConflict::jvs_needs_ncc_grey: return "joint view selection is built for the NCC cost (GPM_PHOTO_NCC) on grey images";
     case ModeConflict::ncc_colour: return "the NCC photometric cost supports grey images only";
     case ModeConflict::prior: return "the planar prior supports grey images without joint view selection";
+    case ModeConflict::geomask: return "the geometric term's mask and the planar prior exclude each other";
     default: return nullptr;
     }
 }
@@ -430,7 +434,8 @@ JvsParams jvs_params(const gpm_ctx* c)
 PriorParams prior_params(const gpm_ctx* c)
 {
     PriorParams R{};
-    R.map = c->prior_map;
+    if (ctx_mode(c).geomask) R.geo_mask = c->geo_mask;       // the masked variants read the mask in the map's place
+    else R.map = c->prior_map;
     R.weight = c->prior_weight;
     R.depth_sigma = c->prior_depth_sigma;
     R.normal_scale = (float)(1.0 - std::cos((double)c->prior_normal_deg * 3.14159265358979323846 / 180.0));
@@ -445,12 +450,13 @@ auto make_table(Entry entry, std::integer_sequence<int, B...>) { return std::arr
 
 const auto kSweep = make_table([](auto b) -> decltype(&k_sweep<false, false>) {
     constexpr Mode m = Mode::of(decltype(b)::value);
-    if constexpr (mode_conflict(m) == ModeConflict::none) return k_sweep<m.color, m.fused, m.geo, m.ncc, m.adaptive, m.jvs, m.prior>; else return nullptr;
+    if constexpr (mode_conflict(m) == ModeConflict::none) return k_sweep<m.color, m.fused, m.geo, m.ncc, m.adaptive, m.jvs, m.prior, m.geomask>;
+    else return nullptr;
 }, std::make_integer_sequence<int, GPM_MODES>{});
 
 const auto kCostEval = make_table([](auto b) -> decltype(&k_cost_eval<false>) {
     constexpr Mode m = Mode::of(decltype(b)::value);
-    if constexpr (mode_conflict(m) == ModeConflict::none) return k_cost_eval<m.color, m.geo, m.ncc, m.prior>; else return nullptr;
+    if constexpr (mode_conflict(m) == ModeConflict::none) return k_cost_eval<m.color, m.geo, m.ncc, m.prior, m.geomask>; else return nullptr;
 }, std::make_integer_sequence<int, GPM_MODES>{});
 
 const auto kShardStage = make_table([](auto b) -> decltype(&k_shard_stage<false>) {
@@ -650,7 +656,7 @@ extern "C" void gpm_destroy(gpm_ctx* c)
     if (c->srcArr) cudaFreeArray(c->srcArr);
     cudaFree(c->planar);
     cudaFree(c->planes);  cudaFree(c->cost);  cudaFree(c->prov);  cudaFree(c->seen);  cudaFree(c->refseen);  cudaFree(c->pid);  cudaFree(c->next_id);  cudaFree(c->memo_mask);  cudaFree(c->rng);  cudaFree(c->dispbuf);  cudaFree(c->candbuf);  cudaFree(c->canddepth);  cudaFree(c->sflags);  cudaFree(c->xchg);  cudaFree(c->gath);  cudaFree(c->refpad);  cudaFree(c->staging);  cudaFree(c->geo_depth);  cudaFree(c->geo_kinv);  cudaFree(c->vsel_mask);
-    cudaFree(c->prior_map);  cudaFree(c->prior_cost);
+    cudaFree(c->prior_map);  cudaFree(c->prior_cost);  cudaFree(c->geo_mask);
     cudaFree(c->d_cams);  cudaFree(c->d_stats);
     if (c->ev0) cudaEventDestroy(c->ev0);
     if (c->ev1) cudaEventDestroy(c->ev1);
@@ -873,6 +879,26 @@ extern "C" int gpm_set_geometric(gpm_ctx* c, float weight, float max_err)
     return GPM_OK;
 }
 
+// The mask is copied (W x H bytes, compacted); NULL clears it.  The masked kernels read it only while the term is on, so
+// only then does a change make stored costs and the memo stale.
+extern "C" int gpm_set_geo_mask(gpm_ctx* c, const unsigned char* mask, size_t pitch_bytes, int on_device)
+{
+    if (!c) return fail(GPM_E_ARG, "gpm_set_geo_mask: null context");
+    if (mask && c->prior_weight > 0.f) return fail(GPM_E_ARG, std::string("gpm_set_geo_mask: ") + conflict_text(ModeConflict::geomask));
+    if (pitch_bytes == 0) pitch_bytes = (size_t)c->W;
+    if (mask && pitch_bytes < (size_t)c->W) return fail(GPM_E_ARG, "gpm_set_geo_mask: pitch_bytes is smaller than a row");
+    if (mask) {
+        DeviceGuard g(c->device);
+        if (!c->geo_mask) CU(cudaMalloc(&c->geo_mask, (size_t)c->W * c->H));
+        CU(cudaMemcpy2DAsync(c->geo_mask, (size_t)c->W, mask, pitch_bytes, (size_t)c->W, c->H,
+                             on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, c->stream));
+        CU(cudaStreamSynchronize(c->stream));
+    }
+    if (c->geo_weight > 0.f && (mask || c->geo_mask_set)) c->inputs_dirty = true;
+    c->geo_mask_set = mask != nullptr;
+    return GPM_OK;
+}
+
 extern "C" int gpm_set_photometric(gpm_ctx* c, int kind, float min_std)
 {
     if (!c) return fail(GPM_E_ARG, "gpm_set_photometric: null context");
@@ -989,6 +1015,7 @@ extern "C" int gpm_set_prior(gpm_ctx* c, float weight, float depth_sigma, float 
     if (const char* bad = prior_refusal(weight, depth_sigma, normal_sigma_deg)) return fail(GPM_E_ARG, std::string("gpm_set_prior: ") + bad);
     if (weight > 0.f && c->shard_world > 0) return fail(GPM_E_STATE, "gpm_set_prior: view sharding does not support the planar prior");
     if (const int rc = refuse_change(c, "gpm_set_prior", &Mode::prior, weight > 0.f)) return rc;
+    if (weight > 0.f && c->geo_mask_set) return fail(GPM_E_ARG, std::string("gpm_set_prior: ") + conflict_text(ModeConflict::geomask));
     if (weight > 0.f && !c->prior_map) return fail(GPM_E_STATE, "gpm_set_prior: no prior map (gpm_set_planar_prior or gpm_build_planar_prior)");
     if (c->have_params && !prior_bound_ok(c->prm, ncc_on(c), c->geo_weight, c->geo_max_err, weight))
         return fail(GPM_E_ARG, "gpm_set_prior: weight would let a valid cost reach MAXCOST");

@@ -11,7 +11,8 @@
 // the photometric cost and the propagation mode (§16), the _vsel ones the view selection besides (§17), and the _prior
 // ones a planar-prior stage in every photometric job besides (§18).  gpm_ms_batch_run runs the coarse-to-fine multi-scale
 // flow (§19) on the same pool: a pyramid of the images, then per level a Jacobi step of upsampling and geometric refinement;
-// its _prior twin adds prior stages at the coarsest level's photometric stage and in every geometric stage (§20).
+// its _prior twin adds prior stages at the coarsest level's photometric stage and in every geometric stage (§20), and its
+// _restore twin the detail restorer at level 0 (§21).
 // Host C++ over the C-ABI; the only CUDA calls are page-locking, the geometric drivers' host stores and their sweep events.
 #include "../../include/gipuma_b200.h"
 
@@ -535,6 +536,26 @@ extern "C" int gpm_geo_batch_run_prior(const gpm_geo_batch_desc* g, const gpm_jo
 namespace {
 int level_size(int s, int level) { for (int k = 0; k < level; k++) s = (s + 1) / 2;  return s; }
 
+// The detail restorer's detection (DESIGN.md §21): pixel p is a detail pixel where the geometric stage's plane costs more
+// than `threshold` above the photometric-only plane, both costed photometrically: fsub(c_ms, c_ph) > threshold, one fp32
+// rounding (a NaN is never a detail pixel).  Returns the number of detail pixels.
+long long detect_details(const float* c_ms, const float* c_ph, float threshold, size_t n, unsigned char* detail)
+{
+    long long count = 0;
+    for (size_t p = 0; p < n; p++) {
+        detail[p] = c_ms[p] - c_ph[p] > threshold ? 1 : 0;
+        count += detail[p];
+    }
+    return count;
+}
+
+// planes <- the photometric-only plane at detail pixels, unchanged elsewhere
+void merge_planes(float* planes, const float* photo, const unsigned char* detail, size_t n)
+{
+    for (size_t p = 0; p < n; p++)
+        if (detail[p]) memcpy(planes + 4 * p, photo + 4 * p, 4 * sizeof(float));
+}
+
 // A view's setup at a coarser level: the level-0 selection, order and depth range, the cameras at `cam_scale` and the
 // disparities of their f.
 bool rescale_view(const ViewSetup& s0, int n, double cam_scale, ViewSetup& s)
@@ -580,11 +601,21 @@ std::string ms_prior_refusal(const gpm_ms_batch_desc* m, const gpm_job_opts* opt
     }
     return "";
 }
+
+// What the multi-level driver refuses of the detail restorer's options (DESIGN.md §21); NULL: no restorer.
+const char* ms_restore_refusal(const gpm_ms_restore_opts* r)
+{
+    if (!r) return nullptr;
+    if (r->photo_iterations < 1) return "detail restorer: photo_iterations must be >= 1";
+    if (r->iterations < 0) return "detail restorer: iterations must be >= 0";
+    if (!std::isfinite(r->threshold)) return "detail restorer: threshold must be finite";
+    return nullptr;
+}
 }  // namespace
 
-// gpm_ms_batch_run and gpm_ms_batch_run_prior; `fn` names the entry point in error messages
+// gpm_ms_batch_run, gpm_ms_batch_run_prior and gpm_ms_batch_run_restore; `fn` names the entry point in error messages
 static int ms_batch_run(const char* fn_name, const gpm_ms_batch_desc* m, const gpm_job_opts* opts, const gpm_view_sel* vsel,
-                        gpm_ms_prior_opts* prior, gpm_ms_batch_stats* stats)
+                        gpm_ms_prior_opts* prior, const gpm_ms_restore_opts* restore, gpm_ms_batch_stats* stats)
 {
     const std::string fn = fn_name;
     clear_err();
@@ -597,6 +628,10 @@ static int ms_batch_run(const char* fn_name, const gpm_ms_batch_desc* m, const g
     const std::string bad_prior = ms_prior_refusal(m, opts, vsel, prior);
     if (!bad_prior.empty()) {
         set_err(fn + ": bad arguments: " + bad_prior);
+        return GPM_E_ARG;
+    }
+    if (const char* bad = ms_restore_refusal(restore)) {
+        set_err(fn + ": bad arguments: " + bad);
         return GPM_E_ARG;
     }
     const gpm_prior_opts* P_photo = prior ? prior->photometric : nullptr;
@@ -681,7 +716,7 @@ static int ms_batch_run(const char* fn_name, const gpm_ms_batch_desc* m, const g
     std::atomic<int> failed(0);
     std::vector<std::vector<float>> sweep_ms(L, std::vector<float>(nV, 0.f)), up_ms(L, std::vector<float>(nV, 0.f)),
         build_ms(L, std::vector<float>(nV, 0.f));
-    std::vector<int> device_of(n_refs, -1);
+    std::vector<int> device_of(n_refs, -1), restored(n_refs, 0);
     std::vector<float> job_ms(n_refs, 0.f);
     Barrier barrier(d->n_devices);
     run_workers(d, failed, [&](gpm_ctx* ctx, int dev) {
@@ -696,6 +731,10 @@ static int ms_batch_run(const char* fn_name, const gpm_ms_batch_desc* m, const g
             }
         SweepTimer timer;
         std::vector<float> n4(ctx ? npix[0] * 4 : 0), cost(ctx ? npix[0] : 0);
+        // the detail restorer's buffers: the photometric-only planes, both detection costs and the detail mask
+        const bool rs = restore && ctx;
+        std::vector<float> ph4(rs ? npix[0] * 4 : 0), c_ms(rs ? npix[0] : 0), c_ph(rs ? npix[0] : 0);
+        std::vector<unsigned char> detail(rs ? npix[0] : 0);
         auto fail_at = [&](const char* stage, int l, int view, int rc) {
             set_err(fn + ": level " + std::to_string(l) + " " + stage + " of view " + std::to_string(view) + ": " +
                     (rc == GPM_E_CUDA && !timer.error.empty() ? timer.error : std::string(gpm_last_error())));
@@ -751,8 +790,21 @@ static int ms_batch_run(const char* fn_name, const gpm_ms_batch_desc* m, const g
                 const int i = l == 0 ? refs[job] : views[job], k = slot[i];
                 const ViewSetup& s = setup[l][i];
                 gpm_ctx* c = lc[l];
+                const bool restoring = restore && l == 0;
                 float ms = 0.f;
                 int rc = load_view(c, d, imgs[l].data(), ch, pitch[l], s, *opts, *vsel);
+                // restorer step 1 (§21): the photometric-only estimate, with the term off, in the view's context as loaded.
+                // The geometric stage below replaces the whole state (gpm_set_state), so the view is loaded once.  With one
+                // level this repeats the coarsest photometric stage when photo_iterations = params.iterations and there is
+                // no photometric prior stage; it is run anyway rather than special-cased.
+                if (rc == GPM_OK && restoring) {
+                    float ms1 = 0.f;
+                    rc = gpm_init(c);
+                    if (rc == GPM_OK) rc = timer.sweep(c, restore->photo_iterations, &ms1);
+                    if (rc == GPM_OK) rc = gpm_get_state(c, ph4.data(), nullptr, 0);
+                    ms += ms1;
+                    if (rc != GPM_OK) return fail_at("detail restorer's photometric estimate", l, i, rc);
+                }
                 for (int v = 0; v < s.nv && rc == GPM_OK; v++) rc = gpm_set_view_depth(c, v, dep(slot[s.source(v)]), 0, 0);
                 if (rc == GPM_OK) rc = gpm_set_geometric(c, g->weight, g->max_err);
                 if (rc == GPM_OK) rc = gpm_cost_eval(c, raw(l, k), cost.data(), 0);
@@ -762,6 +814,25 @@ static int ms_batch_run(const char* fn_name, const gpm_ms_batch_desc* m, const g
                 if (rc == GPM_OK && P_geo)
                     rc = prior_stage(c, P_geo, P_geo->info ? P_geo->info + (size_t)l * n + i : nullptr, n4, cost, timer, &ms2, &bms);
                 ms += ms2;
+                long long n_detail = 0;
+                if (rc == GPM_OK && restoring) {                              // restorer steps 2 (end) to 4 (§21)
+                    float ms4 = 0.f;
+                    if (P_geo) rc = prior_off(c, P_geo);
+                    if (rc == GPM_OK) rc = gpm_get_state(c, n4.data(), nullptr, 0);                 // the planes of the geometric stage
+                    if (rc == GPM_OK) rc = gpm_set_geometric(c, 0.f, g->max_err);                  // detection: photometric costs
+                    if (rc == GPM_OK) rc = gpm_cost_eval(c, n4.data(), c_ms.data(), 0);
+                    if (rc == GPM_OK) rc = gpm_cost_eval(c, ph4.data(), c_ph.data(), 0);
+                    if (rc == GPM_OK) {
+                        n_detail = detect_details(c_ms.data(), c_ph.data(), restore->threshold, npix[0], detail.data());
+                        merge_planes(n4.data(), ph4.data(), detail.data(), npix[0]);
+                        rc = gpm_set_geo_mask(c, detail.data(), 0, 0);
+                    }
+                    if (rc == GPM_OK) rc = gpm_set_geometric(c, g->weight, g->max_err);
+                    if (rc == GPM_OK) rc = gpm_cost_eval(c, n4.data(), cost.data(), 0);
+                    if (rc == GPM_OK) rc = gpm_set_state(c, n4.data(), cost.data(), 0);
+                    if (rc == GPM_OK) rc = timer.sweep(c, restore->iterations, &ms4);
+                    ms += ms4;
+                }
                 sweep_ms[l][k] += ms;  build_ms[l][k] += bms;
                 if (rc == GPM_OK && l > 0) rc = gpm_get_state(c, raw(l, k), nullptr, 0);
                 if (rc == GPM_OK && l == 0) {
@@ -771,14 +842,15 @@ static int ms_batch_run(const char* fn_name, const gpm_ms_batch_desc* m, const g
                         if (ref_of(j) != i) continue;
                         if (d->out_norm4) memcpy(d->out_norm4 + (size_t)j * npix[0] * 4, n4.data(), npix[0] * 4 * sizeof(float));
                         if (d->out_cost) memcpy(d->out_cost + (size_t)j * npix[0], cost.data(), npix[0] * sizeof(float));
-                        device_of[j] = dev;  job_ms[j] = ms;
+                        device_of[j] = dev;  job_ms[j] = ms;  restored[j] = (int)n_detail;
                     }
                     if (rc == GPM_OK && d->out_dir && write_result(d->out_dir, i, n4.data(), d->height, d->width) != GPM_OK) {
                         set_err(fn + ": could not store the result of reference view " + std::to_string(i));
                         return false;
                     }
                 }
-                if (rc == GPM_OK && P_geo) rc = prior_off(c, P_geo);
+                if (rc == GPM_OK && P_geo && !restoring) rc = prior_off(c, P_geo);
+                if (rc == GPM_OK && restoring) rc = gpm_set_geo_mask(c, nullptr, 0, 0);
                 if (rc == GPM_OK) rc = gpm_set_geometric(c, 0.f, g->max_err);
                 return rc == GPM_OK ? true : fail_at("geometric stage", l, i, rc);
             });
@@ -800,6 +872,7 @@ static int ms_batch_run(const char* fn_name, const gpm_ms_batch_desc* m, const g
             for (int k = 0; l < L && k < nV; k++) { stats->level_sweep_ms[l] += sweep_ms[l][k];  stats->level_upsample_ms[l] += up_ms[l][k]; }
         }
     }
+    if (restore && restore->restored) std::copy(restored.begin(), restored.end(), restore->restored);
     if (prior)
         for (int l = 0; l < GPM_MS_MAX_LEVELS; l++) {
             prior->level_build_ms[l] = 0.0;
@@ -811,11 +884,17 @@ static int ms_batch_run(const char* fn_name, const gpm_ms_batch_desc* m, const g
 extern "C" int gpm_ms_batch_run(const gpm_ms_batch_desc* m, const gpm_job_opts* opts, const gpm_view_sel* vsel,
                                 gpm_ms_batch_stats* stats)
 {
-    return ms_batch_run("gpm_ms_batch_run", m, opts, vsel, nullptr, stats);
+    return ms_batch_run("gpm_ms_batch_run", m, opts, vsel, nullptr, nullptr, stats);
 }
 
 extern "C" int gpm_ms_batch_run_prior(const gpm_ms_batch_desc* m, const gpm_job_opts* opts, const gpm_view_sel* vsel,
                                       gpm_ms_prior_opts* prior, gpm_ms_batch_stats* stats)
 {
-    return ms_batch_run("gpm_ms_batch_run_prior", m, opts, vsel, prior, stats);
+    return ms_batch_run("gpm_ms_batch_run_prior", m, opts, vsel, prior, nullptr, stats);
+}
+
+extern "C" int gpm_ms_batch_run_restore(const gpm_ms_batch_desc* m, const gpm_job_opts* opts, const gpm_view_sel* vsel,
+                                        gpm_ms_prior_opts* prior, const gpm_ms_restore_opts* restore, gpm_ms_batch_stats* stats)
+{
+    return ms_batch_run("gpm_ms_batch_run_restore", m, opts, vsel, prior, restore, stats);
 }

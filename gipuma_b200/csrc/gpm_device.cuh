@@ -334,8 +334,12 @@ __device__ __forceinline__ float ncc_cost(float Wsum, float Sr, float Srr, float
 // What the k_sweep / k_cost_eval variants with PRIOR = true read besides KParams: one plane per pixel (the prior map,
 // n.xyz and d in the state's layout; a pixel has a prior where the plane's depth is in [depthMin, depthMax]) and the term's
 // parameters.  A kernel parameter of its own, so that KParams, GeoParams and JvsParams keep their layout.
+// The variants with the geometric term's mask (DESIGN.md §21), which exclude the prior, read geo_mask in map's place.
 struct PriorParams {
-    const float4* map;          // [H*W]
+    union {
+        const float4* map;                  // [H*W]
+        const unsigned char* geo_mask;      // [H*W] nonzero: the geometric term is off at the pixel
+    };
     float weight;               // the term's saturation value
     float depth_sigma;          // sigma_d, in depth units
     float normal_scale;         // 1 - cos(sigma_n), rounded once from double on the host
@@ -454,12 +458,15 @@ __device__ __forceinline__ void fetch_sample_grey(cudaTextureObject_t src, const
 // with GEO, its geometric term to per_view1[v] (written by lanes v and v + 32), and the result is 0.
 // PRIOR (planar prior, DESIGN.md §18): the result is with_prior(cost, prior), and the bound test compares fadd(b, prior):
 // prior >= 0 and a rounded add is monotone, so that stays an exact lower bound of the final value.
+// geo_on false (GEO only; the pixel is masked, DESIGN.md §21): no geometric term is computed and the result is exactly that
+// of GEO = false; ROWS writes no geometric term.
 template <int XF, bool COLOR, bool GEO = false, bool NCC = false, bool ROWS = false, bool PRIOR = false>
 __device__ __forceinline__ float eval_plane(const KParams& P, const float* __restrict__ sCam, const WarpScratch& ws,
                                             cudaTextureObject_t src, float nx, float ny, float nz, float d,
                                             float bound, unsigned lane, WarpStats& st,
                                             float* per_view0 = nullptr, float* per_view1 = nullptr, unsigned rt = 0u,
-                                            const GeoParams* G = nullptr, float gpx = 0.0f, float gpy = 0.0f, float prior = 0.0f)
+                                            const GeoParams* G = nullptr, float gpx = 0.0f, float gpy = 0.0f, float prior = 0.0f,
+                                            bool geo_on = true)
 {
     static_assert(!ROWS || NCC, "per-view cost rows are built for the NCC cost only");
     // XF = 0 / 1: compile-time variant; XF = 2: per call, rt bit 0 = x-term first, bit 1 = gradient folding variant,
@@ -472,7 +479,7 @@ __device__ __forceinline__ float eval_plane(const KParams& P, const float* __res
     homographies(P, sCam, ws.H, nx, ny, nz, d, lane);
     __syncwarp();
     float g0 = 0.0f, g1 = 0.0f;          // geometric terms of views lane and lane + 32
-    if constexpr (GEO) {
+    if constexpr (GEO) if (geo_on) {
         if ((int)lane < P.V) g0 = geo_cost(P, *G, sCam + lane * GPM_VIEWCAM_FLOATS, (int)lane, nx, ny, nz, d, gpx, gpy);
         if ((int)lane + 32 < P.V) g1 = geo_cost(P, *G, sCam + (lane + 32) * GPM_VIEWCAM_FLOATS, (int)lane + 32, nx, ny, nz, d, gpx, gpy);
     }
@@ -548,12 +555,12 @@ __device__ __forceinline__ float eval_plane(const KParams& P, const float* __res
         const float c0 = ncc_cost(Wsum, Sr, Srr, St0, Stt0, Srt0, min_var);
         const float c1 = ncc_cost(Wsum, Sr, Srr, St1, Stt1, Srt1, min_var);
         if constexpr (ROWS) {
-            if ((int)lane < P.V) { per_view0[lane] = c0;  if (GEO) per_view1[lane] = g0; }
-            if ((int)lane + 32 < P.V) { per_view0[lane + 32] = c1;  if (GEO) per_view1[lane + 32] = g1; }
+            if ((int)lane < P.V) { per_view0[lane] = c0;  if (GEO && geo_on) per_view1[lane] = g0; }
+            if ((int)lane + 32 < P.V) { per_view0[lane + 32] = c1;  if (GEO && geo_on) per_view1[lane + 32] = g1; }
             return 0.0f;
         }
         if constexpr (PRIOR) return with_prior(GEO ? combine_views(P, fadd(c0, g0), fadd(c1, g1), lane) : combine_views(P, c0, c1, lane), prior);
-        else if constexpr (GEO) return combine_views(P, fadd(c0, g0), fadd(c1, g1), lane);
+        else if constexpr (GEO) return geo_on ? combine_views(P, fadd(c0, g0), fadd(c1, g1), lane) : combine_views(P, c0, c1, lane);
         else return combine_views(P, c0, c1, lane);
     }
 
@@ -716,7 +723,7 @@ __device__ __forceinline__ float eval_plane(const KParams& P, const float* __res
             if (last) { *per_view0 = c0;  *per_view1 = c1;  return 0.0f; }
         } else if (last || P.prune) {
             float b;
-            if constexpr (GEO) b = combine_views(P, fadd(c0, g0), fadd(c1, g1), lane);
+            if constexpr (GEO) b = geo_on ? combine_views(P, fadd(c0, g0), fadd(c1, g1), lane) : combine_views(P, c0, c1, lane);
             else b = combine_views(P, c0, c1, lane);
             if constexpr (PRIOR) {
                 if (last) return with_prior(b, prior);

@@ -104,27 +104,35 @@ __host__ __device__ inline int jvs_floats(int V, bool geo) { return (geo ? 18 : 
 
 // ---- sweep modes: which combinations have kernels --------------------------------------------------------------------
 // A context's mode: colour images, the fused 20-neighbour sweep (option neighbours = 20), the geometric-consistency term
-// (§14), the NCC cost (§15), adaptive checkerboard sampling (§16), joint view selection (§17) and the planar prior (§18).
+// (§14), the NCC cost (§15), adaptive checkerboard sampling (§16), joint view selection (§17), the planar prior (§18) and
+// the per-pixel mask of the geometric term (§21).
 // Kernels are instantiated (gpm_api.cu, kernel tables) and setters accept a change (gpm_set_*) exactly for the modes
 // mode_conflict() passes.
 struct Mode {
-    bool color, fused, geo, ncc, adaptive, jvs, prior;
-    __host__ __device__ constexpr int bits() const { return color | fused << 1 | geo << 2 | ncc << 3 | adaptive << 4 | jvs << 5 | prior << 6; }
-    __host__ __device__ static constexpr Mode of(int b) { return Mode{bool(b & 1), bool(b & 2), bool(b & 4), bool(b & 8), bool(b & 16), bool(b & 32), bool(b & 64)}; }
+    bool color, fused, geo, ncc, adaptive, jvs, prior, geomask;
+    __host__ __device__ constexpr int bits() const
+    {
+        return color | fused << 1 | geo << 2 | ncc << 3 | adaptive << 4 | jvs << 5 | prior << 6 | geomask << 7;
+    }
+    __host__ __device__ static constexpr Mode of(int b)
+    {
+        return Mode{bool(b & 1), bool(b & 2), bool(b & 4), bool(b & 8), bool(b & 16), bool(b & 32), bool(b & 64), bool(b & 128)};
+    }
 };
-constexpr int GPM_MODES = 128;
+constexpr int GPM_MODES = 256;
 
-enum class ModeConflict { none, fused, jvs_needs_ncc_grey, ncc_colour, prior };
+enum class ModeConflict { none, fused, jvs_needs_ncc_grey, ncc_colour, prior, geomask };
 
 // The one rule: the fused sweep has none of the five modes; joint view selection needs the NCC cost (on grey images);
-// the NCC cost needs grey images; the planar prior needs grey images and excludes joint view selection.  The first
-// conflict found is the reason a refusal gives.
+// the NCC cost needs grey images; the planar prior needs grey images and excludes joint view selection; the geometric
+// term's mask needs the term and excludes the planar prior.  The first conflict found is the reason a refusal gives.
 __host__ __device__ constexpr ModeConflict mode_conflict(Mode m)
 {
     if (m.fused && (m.geo || m.ncc || m.adaptive || m.jvs || m.prior)) return ModeConflict::fused;
     if (m.jvs && (!m.ncc || m.color)) return ModeConflict::jvs_needs_ncc_grey;
     if (m.ncc && m.color) return ModeConflict::ncc_colour;
     if (m.prior && (m.color || m.jvs)) return ModeConflict::prior;
+    if (m.geomask && (!m.geo || m.prior)) return ModeConflict::geomask;
     return ModeConflict::none;
 }
 
@@ -134,6 +142,12 @@ __host__ __device__ constexpr bool shard_supports(Mode m)
 {
     return mode_conflict(m) == ModeConflict::none && !m.geo && !m.ncc && !m.jvs && !m.prior && !m.fused;
 }
+
+// GEOMASK variants (§21): whether the geometric term is on at the pixel `at` — off where the mask byte is nonzero.  The mask
+// travels in PriorParams::geo_mask, which only the prior variants read otherwise: the mask excludes the prior
+// (mode_conflict), so every kernel keeps its parameter layout.
+template <bool GEOMASK>
+__device__ __forceinline__ bool geo_at(const PriorParams& R, size_t at) { return !GEOMASK || R.geo_mask[at] == 0; }
 
 // ---- exact memo of rejected work: plane identities ------------------------------------------------------------
 // Every plane carries a 32-bit identity: pid[p] = p + 1 at initialisation, a fresh number (atomic counter) whenever a
@@ -220,7 +234,8 @@ __device__ __forceinline__ PixelPrior pixel_prior(const KParams& P, const PriorP
 #endif
 // GEO: the cost with the geometric-consistency term (DESIGN.md §14); NCC: the NCC photometric cost (§15, grey only).
 // G is only read in those variants.  PRIOR: with the planar prior's term (§18, grey only); R is only read there.
-template <bool COLOR, bool GEO = false, bool NCC = false, bool PRIOR = false>
+// GEOMASK (with GEO): the term is off at the pixels R.geo_mask marks (§21).
+template <bool COLOR, bool GEO = false, bool NCC = false, bool PRIOR = false, bool GEOMASK = false>
 __global__ void __launch_bounds__(GPM_LB_THREADS, GPM_LB_BLOCKS)
 k_cost_eval(const __grid_constant__ KParams P, const __grid_constant__ CUtensorMap tmap, const ViewCam* __restrict__ cams,
             cudaTextureObject_t src, const float4* __restrict__ planes, float* __restrict__ cost, unsigned long long* __restrict__ stats,
@@ -246,11 +261,12 @@ k_cost_eval(const __grid_constant__ KParams P, const __grid_constant__ CUtensorM
         const float fpx = __int2float_rn(px), fpy = __int2float_rn(py);
         float pr = 0.0f;
         if constexpr (PRIOR) pr = pixel_prior(P, R, (size_t)py * P.W + px, fpx, fpy).of(P, R, n, fpx, fpy);
+        const bool gon = geo_at<GEOMASK>(R, (size_t)py * P.W + px);
         float c;
-        if constexpr (NCC) c = eval_plane<1, COLOR, GEO, true, false, PRIOR>(P, sCam, ws, src, n.x, n.y, n.z, n.w, inf, lane, st, nullptr, nullptr, 0u, g, fpx, fpy, pr);
-        else c = (P.cost_rt & 12) ? eval_plane<2, COLOR, GEO, false, false, PRIOR>(P, sCam, ws, src, n.x, n.y, n.z, n.w, inf, lane, st, nullptr, nullptr, (unsigned)P.cost_rt, g, fpx, fpy, pr)
-                 : P.cost_variant ? eval_plane<1, COLOR, GEO, false, false, PRIOR>(P, sCam, ws, src, n.x, n.y, n.z, n.w, inf, lane, st, nullptr, nullptr, 0u, g, fpx, fpy, pr)
-                                  : eval_plane<0, COLOR, GEO, false, false, PRIOR>(P, sCam, ws, src, n.x, n.y, n.z, n.w, inf, lane, st, nullptr, nullptr, 0u, g, fpx, fpy, pr);
+        if constexpr (NCC) c = eval_plane<1, COLOR, GEO, true, false, PRIOR>(P, sCam, ws, src, n.x, n.y, n.z, n.w, inf, lane, st, nullptr, nullptr, 0u, g, fpx, fpy, pr, gon);
+        else c = (P.cost_rt & 12) ? eval_plane<2, COLOR, GEO, false, false, PRIOR>(P, sCam, ws, src, n.x, n.y, n.z, n.w, inf, lane, st, nullptr, nullptr, (unsigned)P.cost_rt, g, fpx, fpy, pr, gon)
+                 : P.cost_variant ? eval_plane<1, COLOR, GEO, false, false, PRIOR>(P, sCam, ws, src, n.x, n.y, n.z, n.w, inf, lane, st, nullptr, nullptr, 0u, g, fpx, fpy, pr, gon)
+                                  : eval_plane<0, COLOR, GEO, false, false, PRIOR>(P, sCam, ws, src, n.x, n.y, n.z, n.w, inf, lane, st, nullptr, nullptr, 0u, g, fpx, fpy, pr, gon);
         if (lane == 0) cost[(size_t)py * P.W + px] = c;
     }
     flush_stats(stats, st, lane);
@@ -604,9 +620,11 @@ __device__ __forceinline__ void jvs_pixel(const KParams& P, const JvsParams& J, 
                                           const float* __restrict__ tile, const WarpScratch& ws, float* __restrict__ jv,
                                           cudaTextureObject_t src, float4* __restrict__ planes, float* __restrict__ cost,
                                           unsigned* __restrict__ rng_state, unsigned char* __restrict__ prov, const Memo& M,
-                                          int px, int py, int tile_x0, int tile_y0, int phase_mask, unsigned lane, WarpStats& st)
+                                          int px, int py, int tile_x0, int tile_y0, int phase_mask, unsigned lane, WarpStats& st,
+                                          bool geo_on = true)
 {
     const RefCam& cam = P.ref;
+    const bool with_geo = GEO && geo_on;            // false at a pixel the geometric term's mask marks (§21)
     const int W = P.W, H = P.H, V = P.V;
     const size_t center = (size_t)py * W + px;
     const float fpx = __int2float_rn(px), fpy = __int2float_rn(py);
@@ -641,7 +659,7 @@ __device__ __forceinline__ void jvs_pixel(const KParams& P, const JvsParams& J, 
 
     setup_window<false, true>(P, tile + P.tile_xo, ws, px, py, tile_x0, tile_y0, lane);
     auto eval_row = [&](float nx, float ny, float nz, float nd, int r) {
-        eval_plane<1, false, GEO, true, true>(P, sCam, ws, src, nx, ny, nz, nd, inf, lane, st, Mr + r * V, Gr + r * V, 0u, g, fpx, fpy);
+        eval_plane<1, false, GEO, true, true>(P, sCam, ws, src, nx, ny, nz, nd, inf, lane, st, Mr + r * V, Gr + r * V, 0u, g, fpx, fpy, 0.0f, geo_on);
     };
     // (1) rows: 4 bits per candidate k name the row that holds its costs
     eval_row(norm_now.x, norm_now.y, norm_now.z, norm_now.w, 8);
@@ -689,12 +707,12 @@ __device__ __forceinline__ void jvs_pixel(const KParams& P, const JvsParams& J, 
         const float* gr = Gr + r * V;
         if (wsum == 0.0f) {                          // no reliable view: today's NCC cost
             float c0 = 0.0f, c1 = 0.0f;
-            if ((int)lane < V) c0 = GEO ? fadd(m[lane], gr[lane]) : m[lane];
-            if ((int)lane + 32 < V) c1 = GEO ? fadd(m[lane + 32], gr[lane + 32]) : m[lane + 32];
+            if ((int)lane < V) c0 = with_geo ? fadd(m[lane], gr[lane]) : m[lane];
+            if ((int)lane + 32 < V) c1 = with_geo ? fadd(m[lane + 32], gr[lane + 32]) : m[lane + 32];
             return combine_views(P, c0, c1, lane);
         }
         float num = 0.0f;
-        if (lane == 0) for (int j = 0; j < V; j++) num = fadd(num, fmul(wv[j], GEO ? fadd(m[j], gr[j]) : m[j]));
+        if (lane == 0) for (int j = 0; j < V; j++) num = fadd(num, fmul(wv[j], with_geo ? fadd(m[j], gr[j]) : m[j]));
         return __shfl_sync(GPM_FULL, fdiv(num, wsum), 0);
     };
     // (5) the fold: strict <, candidates in k order (gipuma.cu:867-871)
@@ -772,16 +790,18 @@ __device__ __forceinline__ void jvs_pixel(const KParams& P, const JvsParams& J, 
 // (§15; 8-neighbour sweep, grey images only).  G is only read in those variants.  ADAPTIVE: adaptive checkerboard sampling
 // (§16; 8-neighbour sweep), candidate k is acs_neighbour's choice instead of the fixed neighbour.  JVS: joint view
 // selection (§17; NCC only), every pixel goes through jvs_pixel; J is only read in those variants.  PRIOR: every
-// hypothesis' cost carries the planar prior's term (§18; grey, no joint view selection); R is only read there.
-template <bool COLOR, bool FUSED, bool GEO = false, bool NCC = false, bool ADAPTIVE = false, bool JVS = false, bool PRIOR = false>
+// hypothesis' cost carries the planar prior's term (§18; grey, no joint view selection); R is only read there.  GEOMASK
+// (with GEO, without PRIOR): every hypothesis of a pixel R.geo_mask marks costs what it costs without the term (§21).
+template <bool COLOR, bool FUSED, bool GEO = false, bool NCC = false, bool ADAPTIVE = false, bool JVS = false, bool PRIOR = false,
+          bool GEOMASK = false>
 __global__ void __launch_bounds__(GPM_LB_THREADS, GPM_LB_BLOCKS)
 k_sweep(const __grid_constant__ KParams P, const __grid_constant__ CUtensorMap tmap, const ViewCam* __restrict__ cams,
         cudaTextureObject_t src, float4* __restrict__ planes, float* __restrict__ cost,
         unsigned* __restrict__ rng_state, unsigned char* __restrict__ prov, Memo M, int colour, int phase_mask,
         unsigned long long* __restrict__ stats, const __grid_constant__ GeoParams G, const JvsParams J, const PriorParams R)
 {
-    static_assert(mode_conflict(Mode{COLOR, FUSED, GEO, NCC, ADAPTIVE, JVS, PRIOR}) == ModeConflict::none, "no such sweep mode (mode_conflict)");
-    constexpr bool SHARE = shares_samples(Mode{COLOR, FUSED, GEO, NCC, ADAPTIVE, JVS, PRIOR});
+    static_assert(mode_conflict(Mode{COLOR, FUSED, GEO, NCC, ADAPTIVE, JVS, PRIOR, GEOMASK}) == ModeConflict::none, "no such sweep mode (mode_conflict)");
+    constexpr bool SHARE = shares_samples(Mode{COLOR, FUSED, GEO, NCC, ADAPTIVE, JVS, PRIOR, GEOMASK});
     const GeoParams* g = (GEO || NCC) ? &G : nullptr;
     extern __shared__ __align__(128) float smem[];
     float* tile = smem;
@@ -823,7 +843,8 @@ k_sweep(const __grid_constant__ KParams P, const __grid_constant__ CUtensorMap t
         if constexpr (JVS) {
             if (px < W && py < H)
                 jvs_pixel<GEO, ADAPTIVE>(P, J, g, sCam, tile, ws, warp_base + warp_scratch_floats(P.ns_pad, P.V, P.color, NCC), src, planes,
-                                         cost, rng_state, prov, M, px, py, tile_x0, tile_y0, phase_mask, lane, st);
+                                         cost, rng_state, prov, M, px, py, tile_x0, tile_y0, phase_mask, lane, st,
+                                         geo_at<GEOMASK>(R, (size_t)py * W + px));
         } else if (px < W && py < H) {
             const size_t center = (size_t)py * W + px;
             bool window_ready = false;          // the per-pixel window data is only built if something gets evaluated
@@ -835,6 +856,7 @@ k_sweep(const __grid_constant__ KParams P, const __grid_constant__ CUtensorMap t
             int prov_now = prov[center];
             PixelPrior pp{};
             if constexpr (PRIOR) pp = pixel_prior(P, R, center, fpx, fpy);
+            const bool gon = geo_at<GEOMASK>(R, center);
 
             // candidate k lives in lane k: 0..3 = up, down, left, right at 1 px (:1571-1582), 4..7 at 5 px (:1450-1462);
             // fused kernel: the 20 candidates of gipuma.cu:1236-1330 in source order
@@ -918,7 +940,7 @@ k_sweep(const __grid_constant__ KParams P, const __grid_constant__ CUtensorMap t
                 if constexpr (PRIOR) pr = pp.of(P, R, nb, fpx, fpy);
                 const float c = FUSED ? eval_plane<2, COLOR>(P, sCam, ws, src, nb.x, nb.y, nb.z, nb.w, cost_now, lane, st, nullptr, nullptr, site)
                                       : eval_plane<(COLOR ? 0 : 1), COLOR, GEO, NCC, false, PRIOR>(P, sCam, ws, src, nb.x, nb.y, nb.z, nb.w, cost_now, lane, st,
-                                                                                nullptr, nullptr, 0u, g, fpx, fpy, pr);
+                                                                                nullptr, nullptr, 0u, g, fpx, fpy, pr, gon);
                 if (c < cost_now) {                                                              // :867-871
                     disp_now = disp_before;
                     norm_now = nb;
@@ -978,7 +1000,7 @@ k_sweep(const __grid_constant__ KParams P, const __grid_constant__ CUtensorMap t
                     if constexpr (PRIOR) pr = pp.of(P, R, cand, fpx, fpy);
                     const float c = FUSED ? eval_plane<2, COLOR>(P, sCam, ws, src, cand.x, cand.y, cand.z, cand.w, cost_now, lane, st, nullptr, nullptr, rsite)
                                           : eval_plane<0, COLOR, GEO, NCC, false, PRIOR>(P, sCam, ws, src, cand.x, cand.y, cand.z, cand.w, cost_now, lane, st,
-                                                                      nullptr, nullptr, 0u, g, fpx, fpy, pr);
+                                                                      nullptr, nullptr, 0u, g, fpx, fpy, pr, gon);
                     if (c < cost_now) {                                                          // :986-990 (no depth-range test)
                         prov_now = (int)rsite;
                         any_accept = true;

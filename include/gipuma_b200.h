@@ -89,16 +89,18 @@ int gpm_set_view_color(gpm_ctx* ctx, int v, const float* rgba, size_t pitch_byte
 int gpm_set_num_views(gpm_ctx* ctx, int n_views);
 
 /* ---- mode compatibility -------------------------------------------------------------------------------------------------
- * A context sweeps in one mode of seven fields: colour images (fixed by the first image upload), the fused 20-neighbour
- * sweep (option "neighbours" = 20), the geometric-consistency term, the NCC cost, adaptive sampling, joint view selection
- * and the planar prior (DESIGN.md §14–§18).  Every combination exists except:
+ * A context sweeps in one mode of eight fields: colour images (fixed by the first image upload), the fused 20-neighbour
+ * sweep (option "neighbours" = 20), the geometric-consistency term, the NCC cost, adaptive sampling, joint view selection,
+ * the planar prior (DESIGN.md §14–§18) and the geometric term's per-pixel mask (§21; it counts while the term is on).
+ * Every combination exists except:
  *   - the fused sweep with the geometric term, the NCC cost, adaptive sampling, joint view selection or the planar prior;
  *   - joint view selection without the NCC cost, and so with colour images;
  *   - the NCC cost with colour images;
- *   - the planar prior with colour images or with joint view selection.
+ *   - the planar prior with colour images or with joint view selection;
+ *   - a geometric term's mask with the planar prior (whether the term is on or not).
  * A call that would make one of these is refused and changes nothing.  gpm_set_geometric, gpm_set_photometric,
- * gpm_set_propagation, gpm_set_view_selection, gpm_set_prior and gpm_set_option("neighbours") return GPM_E_ARG, whichever
- * of the two fields is set last.  A colour image upload (gpm_set_reference_color, gpm_set_view_color) returns GPM_E_ARG
+ * gpm_set_propagation, gpm_set_view_selection, gpm_set_prior, gpm_set_geo_mask and gpm_set_option("neighbours") return
+ * GPM_E_ARG, whichever of the two fields is set last.  A colour image upload (gpm_set_reference_color, gpm_set_view_color) returns GPM_E_ARG
  * while joint view selection or the planar prior is on and GPM_E_STATE while only the NCC cost is.  The batch drivers
  * refuse the same combinations of their job options and image type with GPM_E_ARG before any CUDA call.
  * The source-view shard runs neither the geometric term, the NCC cost, joint view selection nor the planar prior: while one
@@ -121,6 +123,15 @@ int gpm_set_num_views(gpm_ctx* ctx, int n_views);
  *   without a depth map — also at the next launch, if gpm_set_num_views adds one.  Other modes: "mode compatibility". */
 int gpm_set_view_depth(gpm_ctx* ctx, int v, const float* depth, size_t pitch_bytes, int on_device);
 int gpm_set_geometric(gpm_ctx* ctx, float weight, float max_err);
+
+/* gpm_set_geo_mask (DESIGN.md §21): a per-pixel mask of the geometric term, width x height bytes (pitch_bytes between rows,
+ * 0 = packed; host or device memory), copied.  While the term is on, every cost the context computes (gpm_init, gpm_sweep,
+ * gpm_phase, gpm_cost_eval, gpm_run) is at a pixel whose byte is nonzero exactly the cost with the term off, and elsewhere
+ * exactly the cost with it on.  NULL clears the mask (the default: no mask).  While the term is off the mask has no
+ * effect; while it is on, setting, changing or clearing the mask marks stored costs and the memo stale.  Refused with
+ * GPM_E_ARG: a mask while the planar prior is on, pitch_bytes smaller than width.  A refused call changes nothing;
+ * gpm_set_prior refuses to turn the prior on while a mask is set. */
+int gpm_set_geo_mask(gpm_ctx* ctx, const unsigned char* mask, size_t pitch_bytes, int on_device);
 
 /* ---- photometric cost (DESIGN.md §15) ---------------------------------------------------------------------------------
  * GPM_PHOTO_PM (the default) is the reference's adaptive-support-weight cost.  GPM_PHOTO_NCC replaces each view's cost by
@@ -613,6 +624,30 @@ typedef struct gpm_ms_prior_opts {
 } gpm_ms_prior_opts;
 int gpm_ms_batch_run_prior(const gpm_ms_batch_desc* desc, const gpm_job_opts* opts, const gpm_view_sel* vsel,
                            gpm_ms_prior_opts* prior, gpm_ms_batch_stats* stats);
+
+/* gpm_ms_batch_run_restore: gpm_ms_batch_run_prior with ACMM's detail restorer (Xu & Tao, CVPR 2019), as the project's own
+ * rule (DESIGN.md §21).  Only the level-0 job of each reference view changes, and all of it runs in that job's context:
+ *   1. photometric-only estimate: load_view with the geometric term off, gpm_init and photo_iterations sweeps, with the
+ *      setup and seed of gpm_geo_batch_run's pass 1 for the view; its raw planes PH kept;
+ *   2. the level-0 geometric stage as in gpm_ms_batch_run_prior, the geometric prior stage included; then the prior off
+ *      and the raw planes MS kept;
+ *   3. detection, with the geometric term off: gpm_cost_eval of MS and of PH gives c_ms and c_ph; a pixel is a detail pixel
+ *      where fsub(c_ms, c_ph) > threshold in fp32 (a NaN never is);
+ *   4. restore: PH at detail pixels, MS elsewhere; gpm_set_geo_mask of the detail pixels, the term on, gpm_cost_eval +
+ *      gpm_set_state of the merged planes, `iterations` sweeps;
+ *   5. gpm_finalize, the outputs and .dmb files as before; the mask cleared and the term off.
+ * The sweeps of steps 1 and 4 count in level_sweep_ms[0] and the job's sweep ms.  restore NULL is gpm_ms_batch_run_prior.
+ * Refused with GPM_E_ARG before any CUDA call, besides what gpm_ms_batch_run_prior refuses: photo_iterations < 1,
+ * iterations < 0, a threshold that is not finite.  Memory per worker: one W x H float4 buffer, two W x H cost buffers and
+ * the mask, on the host; the host store does not grow. */
+typedef struct gpm_ms_restore_opts {
+    int   photo_iterations;            /* sweeps of the photometric-only estimate, >= 1 */
+    float threshold;                   /* detection threshold, in units of the photometric cost */
+    int   iterations;                  /* sweeps after the restore, >= 0 */
+    int*  restored;                    /* out, NULL or n_refs entries: detail pixels per reference job */
+} gpm_ms_restore_opts;
+int gpm_ms_batch_run_restore(const gpm_ms_batch_desc* desc, const gpm_job_opts* opts, const gpm_view_sel* vsel,
+                             gpm_ms_prior_opts* prior, const gpm_ms_restore_opts* restore, gpm_ms_batch_stats* stats);
 
 #ifdef __cplusplus
 }

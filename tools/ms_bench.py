@@ -3,7 +3,7 @@ prints one JSON line.
 
     python tools/ms_bench.py [--rows 600] [--cols 800] [--cams 16] [--scenes smooth,hard,lit] [--costs pm,ncc]
                              [--modes fixed,adaptive] [--levels 2,3] [--weights 0.5,0] [--jbu RADIUS,SIGMA_S,SIGMA_R] [--dtu-preset]
-                             [--prior]
+                             [--prior] [--restore]
 
 Quality: tools/acs_bench.py's workload (the first `--cams` DTU cameras at `--cols` x `--rows`, every second camera a
 reference view, box 11, n_best 3, depth 300..800, views at 5..45 degrees, at most 6 per reference; the same fusion and
@@ -19,6 +19,11 @@ level count, multiscale_pass at weight GEO_WEIGHT with no stage, the photometric
 geometric stage at two support costs (PRIOR_DEFAULTS["support_cost"] and that plus GEO_WEIGHT * 1 pixel, the geometric term
 of a pixel 1 pixel off), with the prior builds' host ms per level; and geometric_pass 4 + 2 with planar_prior as the
 single-scale comparison.  With --dtu-preset it adds multiscale_pass with both stages at each support cost to the preset.
+--restore adds the detail restorer (DESIGN.md §21): per level count, multiscale_pass at weight GEO_WEIGHT without it and with
+it at each threshold of RESTORE_THRESHOLDS for the cost (RESTORE_DEFAULTS otherwise), with the share of level-0 pixels
+restored and the wall seconds of the call; on the hard scene every row also has the edge scores: F at 1 unit and mean
+completeness of the points within EDGE_UNITS units of a block wall (HeightField.height's block rule).  With --dtu-preset it
+adds multiscale_pass with the restorer at its defaults to the preset.
 Needs a CUDA device; there is no CPU path.
 """
 import argparse
@@ -31,6 +36,22 @@ import time
 import numpy as np
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+
+RESTORE_THRESHOLDS = {"pm": (0.5, 1.0, 2.0), "ncc": (0.05, 0.1, 0.2)}
+EDGE_UNITS = 3.0
+
+
+def near_wall(X, Y, unit, k=EDGE_UNITS):
+    """Points within k units of a block wall of HeightField.height: blocks are u < 0.33 and w < 0.33 of a 520-unit lattice,
+    u = X / 520 + 0.31, w = Y / 520 + 0.17 (mod 1)."""
+    L = 520.0 * unit
+    u, w = np.mod(X / L + 0.31, 1.0), np.mod(Y / L + 0.17, 1.0)
+    ku = k * unit / L
+
+    def dist(t):                                   # lattice distance to the nearest wall line, 0 or 0.33
+        return np.minimum(np.minimum(t, 1.0 - t), np.abs(t - 0.33))
+    inside = lambda t: (t < 0.33 + ku) | (t > 1.0 - ku)           # noqa: E731  (within the block's span, walls included)
+    return ((dist(u) < ku) & inside(w)) | ((dist(w) < ku) & inside(u))
 
 
 def main():
@@ -46,6 +67,7 @@ def main():
     ap.add_argument("--jbu", default="")
     ap.add_argument("--dtu-preset", action="store_true")
     ap.add_argument("--prior", action="store_true")
+    ap.add_argument("--restore", action="store_true")
     a = ap.parse_args()
     import torch
     if not torch.cuda.is_available():
@@ -118,6 +140,10 @@ def main():
                                        max_dist=10 * unit, taus=(unit,))
                 r["band_f_score_1unit"] = round(b["f_score"][0], 4)
                 r["band_completeness_mean_units"] = round(b["completeness_mean"] / unit, 4)
+                ev, eg = near_wall(v[:, 0], v[:, 1], unit), near_wall(gt[:, 0], gt[:, 1], unit)
+                e = api.evaluate_cloud(np.ascontiguousarray(v[ev]), np.ascontiguousarray(gt[eg]), max_dist=10 * unit, taus=(unit,))
+                r["edge_f_score_1unit"] = round(e["f_score"][0], 4)
+                r["edge_completeness_mean_units"] = round(e["completeness_mean"] / unit, 4)
             return r
 
         res = {}
@@ -150,6 +176,19 @@ def main():
                                             level_sweep_ms=[round(1e3 * t, 1) for t in info["level_sweep_s"]],
                                             level_build_ms=[round(t, 1) for t in info["level_build_ms"]])
                             log("%s %s %s %s: %s" % (scene, cost, mode, key, row[key]))
+                if a.restore:
+                    for L in levels:
+                        for t in (None,) + RESTORE_THRESHOLDS[cost]:
+                            t0 = time.perf_counter()
+                            n4, _, info = api.multiscale_pass(images, Ps, params(4), refs, levels=L, geo_iterations=2, jbu=jbu,
+                                                              propagation=mode, detail_restorer=None if t is None else {"threshold": t},
+                                                              **kw, **photo)
+                            wall = time.perf_counter() - t0
+                            key = "multiscale_pass levels %d, %s" % (L, "no restorer" if t is None else "restorer t=%g" % t)
+                            row[key] = dict(score(n4, 1e3 * sum(info["level_sweep_s"])), wall_s=round(wall, 2),
+                                            level_sweep_ms=[round(1e3 * x, 1) for x in info["level_sweep_s"]],
+                                            restored_share=None if t is None else round(sum(info["restored"]) / (len(refs) * a.rows * a.cols), 4))
+                            log("%s %s %s %s: %s" % (scene, cost, mode, key, row[key]))
                 res["%s %s" % (cost, mode)] = row
                 log("%s %s %s: %s" % (scene, cost, mode, row))
         out[scene] = res
@@ -180,6 +219,14 @@ def main():
                     "wall_s": round(time.perf_counter() - t0, 2), "sweep_s_total": round(sum(info["level_sweep_s"]), 3),
                     "level_sweep_s": [round(t, 3) for t in info["level_sweep_s"]],
                     "level_build_s": [round(t / 1e3, 3) for t in info["level_build_ms"]]}
+            if a.restore:
+                t0 = time.perf_counter()
+                _, _, info = api.multiscale_pass(images, allP, params(4), list(range(n)), levels=L, geo_iterations=2, jbu=jbu,
+                                                 detail_restorer={}, **dkw)
+                dtu["multiscale_pass levels %d, restorer" % L] = {
+                    "wall_s": round(time.perf_counter() - t0, 2), "sweep_s_total": round(sum(info["level_sweep_s"]), 3),
+                    "level_sweep_s": [round(t, 3) for t in info["level_sweep_s"]],
+                    "restored_share": round(sum(info["restored"]) / (n * 1600 * 1200), 4)}
         out["dtu_preset"] = dict(dtu, workload="%d views at 1600x1200, PM, fixed, one worker, every view a reference" % n)
         log("DTU preset: %s" % dtu)
     print(json.dumps(out))
