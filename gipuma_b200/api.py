@@ -121,6 +121,10 @@ class GpmFuseDesc(C.Structure):
                 ("num_consistent", C.c_int), ("device", C.c_int)]
 
 
+class GpmFuseRule(C.Structure):
+    _fields_ = [("kind", C.c_int), ("reproj_px", C.c_float), ("depth_rel", C.c_float)]
+
+
 class GpmFuseResult(C.Structure):
     _fields_ = [("count", C.c_longlong), ("capacity", C.c_longlong), ("vertices", C.c_void_p), ("source", C.c_void_p),
                 ("used", C.c_void_p), ("fuse_ms", C.c_float), ("upload_ms", C.c_float)]
@@ -236,6 +240,7 @@ def load_library():
     L.gpm_set_geo_mask.argtypes = [vp, vp, C.c_size_t, C.c_int]
     L.gpm_fuse_cameras.argtypes = [C.POINTER(C.c_double), C.c_int, C.c_double, C.POINTER(GpmFuseCamera)]
     L.gpm_fuse.argtypes = [C.POINTER(GpmFuseDesc), C.POINTER(GpmFuseResult)]
+    L.gpm_fuse_with_rule.argtypes = [C.POINTER(GpmFuseDesc), C.POINTER(GpmFuseRule), C.POINTER(GpmFuseResult)]
     L.gpm_write_ply.argtypes = [C.c_char_p, vp, C.c_longlong]
     L.gpm_nearest_dist.argtypes = [C.POINTER(GpmNnDesc), C.POINTER(GpmNnResult)]
     for name in ("gpm_create", "gpm_set_params", "gpm_set_reference", "gpm_set_view", "gpm_set_reference_color",
@@ -250,7 +255,7 @@ def load_library():
                  "gpm_geo_batch_run_prior", "gpm_downsample", "gpm_upsample_planes", "gpm_ms_batch_run", "gpm_ms_batch_run_prior",
                  "gpm_ms_batch_run_restore", "gpm_set_geo_mask",
                  "gpm_prepare_cameras", "gpm_select_views", "gpm_write_dmb", "gpm_read_dmb", "gpm_write_result_dmb",
-                 "gpm_fuse_cameras", "gpm_fuse", "gpm_write_ply", "gpm_nearest_dist"):
+                 "gpm_fuse_cameras", "gpm_fuse", "gpm_fuse_with_rule", "gpm_write_ply", "gpm_nearest_dist"):
         getattr(L, name).restype = C.c_int
     _lib = L
     return L
@@ -1166,7 +1171,31 @@ def write_result_dmb(depth_path: str, normal_path: str, norm4: np.ndarray):
         raise GipumaError("gpm_write_result_dmb failed")
 
 
-# ---- depth-map fusion (gpm_fuse; DESIGN.md §12) ----------------------------------------------------------------------
+# ---- depth-map fusion (gpm_fuse; DESIGN.md §12, §22) -----------------------------------------------------------------
+
+FUSE_RULES = {"disparity": 0, "reprojection": 1}                 # GPM_FUSE_DISPARITY, GPM_FUSE_REPROJECTION
+# The reprojection rule's thresholds: 2 pixels of reprojection error in the reference view and 1 % of relative depth, the
+# values COLMAP-style fusion is usually run with (measured against the disparity rule in DESIGN.md §22).
+FUSE_REPROJ_DEFAULTS = {"reproj_px": 2.0, "depth_rel": 0.01}
+
+
+def _fuse_rule(rule, reproj_px, depth_rel) -> GpmFuseRule:
+    """The gpm_fuse_rule of fuse's arguments; ValueError for what gpm_fuse_with_rule would refuse."""
+    if rule not in FUSE_RULES:
+        raise ValueError("rule must be one of %s, not %r" % (sorted(FUSE_RULES), rule))
+    if rule == "disparity":
+        if reproj_px is not None or depth_rel is not None:
+            raise ValueError("reproj_px and depth_rel apply to rule='reprojection' only")
+        return GpmFuseRule(FUSE_RULES[rule], 0.0, 0.0)
+    t = dict(FUSE_REPROJ_DEFAULTS)
+    for k, v in (("reproj_px", reproj_px), ("depth_rel", depth_rel)):
+        if v is not None:
+            t[k] = v
+        f = C.c_float(float(t[k])).value                            # the float the C-ABI receives
+        if not (np.isfinite(f) and f > 0):
+            raise ValueError("%s must be finite and > 0, not %r" % (k, t[k]))
+    return GpmFuseRule(FUSE_RULES[rule], t["reproj_px"], t["depth_rel"])
+
 
 def fuse_cameras(Ps, cam_scale: float = 1.0):
     """The fusion's per-view cameras (gpm_fuse_cameras): un-rebased world frame, K scaled by cam_scale."""
@@ -1179,14 +1208,19 @@ def fuse_cameras(Ps, cam_scale: float = 1.0):
 
 
 def fuse(norm4, Ps, depth_min: float, depth_max: float, disp_thresh: float = 0.1, normal_thresh: float = 30.0,
-         num_consistent: int = 3, images=None, cam_scale: float = 1.0, device: int = 0):
-    """Fuse N views' world-frame outputs into one point cloud on the GPU (gpm_fuse).
+         num_consistent: int = 3, images=None, cam_scale: float = 1.0, device: int = 0, rule: str = "disparity",
+         reproj_px: float = None, depth_rel: float = None):
+    """Fuse N views' world-frame outputs into one point cloud on the GPU (gpm_fuse_with_rule).
 
     norm4: [N, H, W, 4] float32 (world normal xyz + depth, 0 = invalid; what batch_run returns), numpy or torch (host or
     CUDA); Ps: the N 3x4 projection matrices of those views (as passed to batch_run); images: None, [N, H, W] grey or
     [N, H, W, 4] RGBA float in [0, 255], in the same memory as norm4.  The defaults of the thresholds are the reference's
-    DTU script's (scripts/dtu_fast.sh:23-26).  Returns (vertices: PLY_VERTEX array in (view, y, x) order, info dict with
-    count, source [count, 2] int32 (view, y*W + x), used [N, H, W] uint8 masks, fuse_ms, upload_ms)."""
+    DTU script's (scripts/dtu_fast.sh:23-26).  rule: "disparity" (the default: |f_j 0.54 / z - f_j 0.54 / d_j| <
+    disp_thresh, a threshold tied to DTU's scale) or "reprojection" (the scale-free rule of DESIGN.md §22: the target's
+    point reprojects into the reference view within reproj_px pixels and depth_rel relative depth; disp_thresh is not read;
+    None takes FUSE_REPROJ_DEFAULTS).  Returns (vertices: PLY_VERTEX array in (view, y, x) order, info dict with count,
+    source [count, 2] int32 (view, y*W + x), used [N, H, W] uint8 masks, fuse_ms, upload_ms)."""
+    fr = _fuse_rule(rule, reproj_px, depth_rel)
     lib = load_library()
     shape = tuple(norm4.shape)
     if len(shape) != 4 or shape[3] != 4 or len(Ps) != shape[0]:
@@ -1212,17 +1246,19 @@ def fuse(norm4, Ps, depth_min: float, depth_max: float, disp_thresh: float = 0.1
     d = GpmFuseDesc(n, W, H, p4, pi, ch, dev, P.ctypes.data_as(C.POINTER(C.c_double)), float(cam_scale), float(depth_min),
                     float(depth_max), float(disp_thresh), float(normal_thresh), int(num_consistent), int(device))
     r = GpmFuseResult(0, cap, verts.ctypes.data, src.ctypes.data, used.ctypes.data, 0.0, 0.0)
-    if lib.gpm_fuse(C.byref(d), C.byref(r)) != 0:
+    if lib.gpm_fuse_with_rule(C.byref(d), C.byref(fr), C.byref(r)) != 0:
         raise GipumaError("gpm_fuse: %s" % lib.gpm_last_error().decode())
     k = int(r.count)
     return verts[:k], {"count": k, "source": src[:k], "used": used, "fuse_ms": float(r.fuse_ms), "upload_ms": float(r.upload_ms)}
 
 
 def fuse_batch_dir(out_dir: str, refs, Ps, depth_min: float, depth_max: float, disp_thresh: float = 0.1,
-                   normal_thresh: float = 30.0, num_consistent: int = 3, images=None, cam_scale: float = 1.0, device: int = 0):
+                   normal_thresh: float = 30.0, num_consistent: int = 3, images=None, cam_scale: float = 1.0, device: int = 0,
+                   rule: str = "disparity", reproj_px: float = None, depth_rel: float = None):
     """fuse() over what batch_run(out_dir=...) wrote: <out_dir>/<ref, 8 digits>/{disp,normals}.dmb for each of `refs`.
     Ps and images (None or [n_images, H, W(, 4)]) are the whole sets given to batch_run, indexed by image; the fused views
     are `refs`, in that order."""
+    _fuse_rule(rule, reproj_px, depth_rel)
     maps = []
     for ref in refs:
         base = os.path.join(out_dir, "%08d" % int(ref))
@@ -1232,7 +1268,7 @@ def fuse_batch_dir(out_dir: str, refs, Ps, depth_min: float, depth_max: float, d
         maps.append(np.concatenate([nrm, dep[..., None]], axis=2))
     imgs = None if images is None else np.ascontiguousarray(np.asarray(images)[list(refs)], dtype=np.float32)
     return fuse(np.ascontiguousarray(np.stack(maps), dtype=np.float32), [Ps[r] for r in refs], depth_min, depth_max,
-                disp_thresh, normal_thresh, num_consistent, imgs, cam_scale, device)
+                disp_thresh, normal_thresh, num_consistent, imgs, cam_scale, device, rule, reproj_px, depth_rel)
 
 
 def write_ply(path: str, vertices):

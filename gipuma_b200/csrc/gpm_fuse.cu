@@ -1,10 +1,12 @@
-// gpm_fuse.cu — depth-map fusion (DESIGN.md §12): N per-view world-frame depth + normal maps -> one point cloud.
+// gpm_fuse.cu — depth-map fusion (DESIGN.md §12, §22): N per-view world-frame depth + normal maps -> one point cloud.
 // Compiled on its own, without --use_fast_math (gipuma_b200/build.py): every fp32 operation below is an explicit
-// round-to-nearest intrinsic, denormals are kept, and oracle/fusion_oracle.c restates the same operations in the same order,
-// so the GPU and the restatement agree bit for bit.
+// round-to-nearest intrinsic, denormals are kept, and oracle/fusion_oracle.c (the disparity rule) and
+// oracle/fusion_rule_oracle.c (either rule) restate the same operations in the same order, so the GPU and the restatements
+// agree bit for bit.
 //
 // Per reference view r (ascending), three launches on the fusion's own stream:
-//   k_fuse_pixels   one thread per pixel of view r: consistency test against every other view, running sums in registers,
+//   k_fuse_pixels   one thread per pixel of view r: consistency test against every other view (the disparity or the
+//                   reprojection rule, DESIGN.md §22, a template argument), running sums in registers,
 //                   the candidate vertex staged per pixel, used marks written for fused pixels, a per-block count
 //   k_scan_blocks   one block: exclusive scan of the per-block counts (fixed order, no atomics)
 //   k_compact       order-preserving scatter of the staged vertices into packed 27-byte PLY records + (view, pixel) sources
@@ -34,8 +36,13 @@ struct FuseArgs {
     unsigned char* flag;                           // npix
     int* block_count;                              // blocks
     int n, W, H, channels, num_consistent;
-    float dmin, dmax, disp_thresh, cos_thresh;
+    float dmin, dmax;
+    float thresh;                                  // disparity rule: disp_thresh; reprojection rule: reproj_px
+    float cos_thresh;
+    float depth_rel;                               // reprojection rule only
 };
+// depth_rel fills what was tail padding: the kernel's parameters, and so the disparity rule's code, stay as they were
+static_assert(sizeof(FuseArgs) == 88, "FuseArgs: depth_rel must fit the tail padding");
 
 __device__ __forceinline__ float dot3(const float* a, float x, float y, float z)
 {
@@ -68,17 +75,34 @@ __device__ __forceinline__ int project(const float* cam, const float X[3], int W
     return (int)fv * W + (int)fu;
 }
 
-// Consistency of view j (camera `cam`) with the reference point X of normal n: the target pixel, or -1.
-__device__ __forceinline__ int consistent(const FuseArgs& a, int j, const float* cam, const float X[3], const float4 n,
-                                          float4* tgt, float* u, float* v)
+// Consistency of view j (camera `cam`) with the reference point X of normal n, back-projected from pixel (x, y) of view r
+// (camera `cr`) at depth dr: the target pixel, or -1.  Rule: GPM_FUSE_DISPARITY or GPM_FUSE_REPROJECTION.
+template <int Rule>
+__device__ __forceinline__ int consistent(const FuseArgs& a, int j, const float* cam, const float* cr,
+                                          const float X[3], float x, float y, float dr, const float4 n, float4* tgt, float* u,
+                                          float* v)
 {
     float z;
     const int q = project(cam, X, a.W, a.H, &z, u, v);
     if (q < 0) return -1;
     const float4 t = a.norm4[(size_t)j * a.W * a.H + q];
     if (!(t.w >= a.dmin && t.w <= a.dmax)) return -1;
-    const float fb = __fmul_rn(cam[21], 0.54f);                                    // baseline constant, cameraGeometryUtils.h:305
-    if (!(fabsf(__fsub_rn(__fdiv_rn(fb, z), __fdiv_rn(fb, t.w))) < a.disp_thresh)) return -1;
+    if (Rule == GPM_FUSE_DISPARITY) {
+        const float fb = __fmul_rn(cam[21], 0.54f);                                // baseline constant, cameraGeometryUtils.h:305
+        if (!(fabsf(__fsub_rn(__fdiv_rn(fb, z), __fdiv_rn(fb, t.w))) < a.thresh)) return -1;
+    } else {
+        // the target's own point, projected back into view r: pixel distance to (x, y) and relative depth difference
+        float Xj[3];
+        backproject(cam, *u, *v, t.w, Xj);
+        const float* P = cr + 9;
+        const float hx = __fadd_rn(dot3(P, Xj[0], Xj[1], Xj[2]), P[3]);
+        const float hy = __fadd_rn(dot3(P + 4, Xj[0], Xj[1], Xj[2]), P[7]);
+        const float hz = __fadd_rn(dot3(P + 8, Xj[0], Xj[1], Xj[2]), P[11]);
+        if (!(hz > 0.f)) return -1;
+        const float dx = __fsub_rn(__fdiv_rn(hx, hz), x), dy = __fsub_rn(__fdiv_rn(hy, hz), y);
+        if (!(__fsqrt_rn(__fadd_rn(__fmul_rn(dx, dx), __fmul_rn(dy, dy))) < a.thresh)) return -1;
+        if (!(__fdiv_rn(fabsf(__fsub_rn(hz, dr)), dr) < a.depth_rel)) return -1;
+    }
     const float c = __fadd_rn(__fadd_rn(__fmul_rn(n.x, t.x), __fmul_rn(n.y, t.y)), __fmul_rn(n.z, t.z));
     if (!(c > a.cos_thresh)) return -1;
     *tgt = t;
@@ -106,6 +130,7 @@ __device__ __forceinline__ unsigned to_uchar(float s, float cnt)
     return (unsigned)floorf(__fadd_rn(m, 0.5f));
 }
 
+template <int Rule>
 __global__ void __launch_bounds__(kBlock) k_fuse_pixels(FuseArgs a, const float* __restrict__ cams_g, int r)
 {
     extern __shared__ float cams[];
@@ -118,8 +143,9 @@ __global__ void __launch_bounds__(kBlock) k_fuse_pixels(FuseArgs a, const float*
         const float4 n = a.norm4[(size_t)r * npix + p];
         if (n.w >= a.dmin && n.w <= a.dmax) {
             const float* cr = cams + r * kCamFloats;
+            const float x = (float)(p % a.W), y = (float)(p / a.W);
             float X[3], s[3], sn[3] = {n.x, n.y, n.z}, col[3] = {0.f, 0.f, 0.f};
-            backproject(cr, (float)(p % a.W), (float)(p / a.W), n.w, X);
+            backproject(cr, x, y, n.w, X);
             s[0] = X[0];  s[1] = X[1];  s[2] = X[2];
             add_colour(a, r, p, col);
             int cnt = 0;
@@ -128,7 +154,7 @@ __global__ void __launch_bounds__(kBlock) k_fuse_pixels(FuseArgs a, const float*
                 const float* cj = cams + j * kCamFloats;
                 float4 t;
                 float u, v, Xj[3];
-                const int q = consistent(a, j, cj, X, n, &t, &u, &v);
+                const int q = consistent<Rule>(a, j, cj, cr, X, x, y, n.w, n, &t, &u, &v);
                 if (q < 0) continue;
                 backproject(cj, u, v, t.w, Xj);
                 for (int k = 0; k < 3; k++) s[k] = __fadd_rn(s[k], Xj[k]);
@@ -152,7 +178,7 @@ __global__ void __launch_bounds__(kBlock) k_fuse_pixels(FuseArgs a, const float*
                     if (j == r) continue;
                     float4 t;
                     float u, v;
-                    const int q = consistent(a, j, cams + j * kCamFloats, X, n, &t, &u, &v);
+                    const int q = consistent<Rule>(a, j, cams + j * kCamFloats, cr, X, x, y, n.w, n, &t, &u, &v);
                     if (q >= 0) a.used[(size_t)j * npix + q] = 1;
                 }
             }
@@ -262,17 +288,25 @@ int fail(int code, const std::string& m) { return gpm::set_last_error(code, "gpm
 
 }  // namespace
 
-extern "C" int gpm_fuse(const gpm_fuse_desc* d, gpm_fuse_result* res)
+extern "C" int gpm_fuse(const gpm_fuse_desc* d, gpm_fuse_result* res) { return gpm_fuse_with_rule(d, nullptr, res); }
+
+extern "C" int gpm_fuse_with_rule(const gpm_fuse_desc* d, const gpm_fuse_rule* rule, gpm_fuse_result* res)
 {
     // every argument is checked before the first CUDA call
     if (!d || !res) return fail(GPM_E_ARG, "null descriptor or result");
+    const int kind = rule ? rule->kind : GPM_FUSE_DISPARITY;
+    if (kind != GPM_FUSE_DISPARITY && kind != GPM_FUSE_REPROJECTION) return fail(GPM_E_ARG, "unknown rule kind");
+    if (kind == GPM_FUSE_REPROJECTION) {
+        if (!(std::isfinite(rule->reproj_px) && rule->reproj_px > 0.f)) return fail(GPM_E_ARG, "reproj_px must be finite and > 0");
+        if (!(std::isfinite(rule->depth_rel) && rule->depth_rel > 0.f)) return fail(GPM_E_ARG, "depth_rel must be finite and > 0");
+    }
     if (d->n_views < 2 || d->n_views > GPM_FUSE_MAX_VIEWS) return fail(GPM_E_ARG, "n_views must be in [2, GPM_FUSE_MAX_VIEWS]");
     if (d->width < 1 || d->height < 1 || (long long)d->width * d->height > (1LL << 30))
         return fail(GPM_E_ARG, "bad image size");
     if (!d->norm4 || !d->P) return fail(GPM_E_ARG, "norm4 and P are required");
     if (d->images && d->channels != 1 && d->channels != 4) return fail(GPM_E_ARG, "channels must be 1 or 4");
     if (!(d->depth_min >= 0.f && d->depth_max > d->depth_min)) return fail(GPM_E_ARG, "need 0 <= depth_min < depth_max");
-    if (!(d->disp_thresh > 0.f)) return fail(GPM_E_ARG, "disp_thresh must be > 0");
+    if (kind == GPM_FUSE_DISPARITY && !(d->disp_thresh > 0.f)) return fail(GPM_E_ARG, "disp_thresh must be > 0");
     if (!(d->normal_thresh > 0.f && d->normal_thresh <= 180.f)) return fail(GPM_E_ARG, "normal_thresh must be in (0, 180] degrees");
     if (d->num_consistent < 1) return fail(GPM_E_ARG, "num_consistent must be >= 1");
     if (res->capacity < 0 || (res->capacity > 0 && !res->vertices && !res->source)) return fail(GPM_E_ARG, "bad result buffers");
@@ -324,12 +358,17 @@ extern "C" int gpm_fuse(const gpm_fuse_desc* d, gpm_fuse_result* res)
     a.stage = static_cast<float4*>(b.stage);  a.flag = static_cast<unsigned char*>(b.flag);
     a.block_count = static_cast<int*>(b.counts);
     a.n = n;  a.W = W;  a.H = H;  a.channels = d->images ? d->channels : 0;  a.num_consistent = d->num_consistent;
-    a.dmin = d->depth_min;  a.dmax = d->depth_max;  a.disp_thresh = d->disp_thresh;
+    a.dmin = d->depth_min;  a.dmax = d->depth_max;
+    a.thresh = kind == GPM_FUSE_DISPARITY ? d->disp_thresh : rule->reproj_px;
+    a.depth_rel = kind == GPM_FUSE_DISPARITY ? 0.f : rule->depth_rel;
     a.cos_thresh = (float)std::cos((double)d->normal_thresh * M_PI / 180.0);       // angle < thresh  <=>  dot > cos(thresh)
     const size_t smem = n * sizeof(gpm_fuse_camera);
     long long total = 0;
     for (int r = 0; r < n; r++) {
-        k_fuse_pixels<<<nblocks, kBlock, smem, b.stream>>>(a, static_cast<const float*>(b.cams), r);
+        if (kind == GPM_FUSE_DISPARITY)
+            k_fuse_pixels<GPM_FUSE_DISPARITY><<<nblocks, kBlock, smem, b.stream>>>(a, static_cast<const float*>(b.cams), r);
+        else
+            k_fuse_pixels<GPM_FUSE_REPROJECTION><<<nblocks, kBlock, smem, b.stream>>>(a, static_cast<const float*>(b.cams), r);
         FU(cudaGetLastError());
         k_scan_blocks<<<1, 1024, 0, b.stream>>>(a.block_count, static_cast<int*>(b.offs), nblocks);
         FU(cudaGetLastError());

@@ -390,7 +390,8 @@ int gpm_geo_batch_run_vsel(const gpm_geo_batch_desc* desc, const gpm_job_opts* o
  * processed in ascending order as reference; a valid, unused reference pixel back-projects to X (get3Dpoint in the un-rebased
  * world frame), X is projected into every other view j and rounded to the nearest pixel, and j is consistent when that pixel
  * is inside the image, X is in front of camera j, the pixel's depth is in [depth_min, depth_max], the disparities
- * f_j*0.54/z of X and of the pixel differ by less than disp_thresh and the normals are less than normal_thresh degrees apart.
+ * f_j*0.54/z of X and of the pixel differ by less than disp_thresh and the normals are less than normal_thresh degrees apart
+ * (the disparity rule; gpm_fuse_with_rule below selects the scale-free reprojection rule instead).
  * With at least num_consistent consistent views one vertex is emitted (mean position, normalised normal sum, mean colour)
  * and the pixels involved are marked used; a mark only stops a pixel from being a reference in later passes.
  * Vertices are emitted in (reference view, y, x) order. */
@@ -438,6 +439,25 @@ typedef struct gpm_fuse_result {
     float fuse_ms, upload_ms;
 } gpm_fuse_result;
 int gpm_fuse(const gpm_fuse_desc* desc, gpm_fuse_result* result);
+
+/* The consistency rule of the fusion (DESIGN.md §22).  GPM_FUSE_DISPARITY is the rule above (gpm_fuse).  Under
+ * GPM_FUSE_REPROJECTION, view j is consistent with reference pixel p = (x, y) of view r, depth d_r, when X projects into j
+ * as above (z > 0, in the image, the pixel's depth in [depth_min, depth_max]) and the back-projection X_j of that pixel
+ * (u, v) at its depth, projected back into view r to (x', y') at depth z', satisfies: z' > 0,
+ * sqrt(dx*dx + dy*dy) < reproj_px with dx = x' - x, dy = y' - y, |z' - d_r| / d_r < depth_rel, and the normal test above.
+ * Every operation of this rule is homogeneous in the world's scale, so its decisions do not depend on it; disp_thresh is
+ * not read.  Everything else (cameras, passes, marks, vertex order and averaging) is gpm_fuse's. */
+#define GPM_FUSE_DISPARITY    0
+#define GPM_FUSE_REPROJECTION 1
+typedef struct gpm_fuse_rule {
+    int kind;                          /* GPM_FUSE_DISPARITY or GPM_FUSE_REPROJECTION */
+    float reproj_px;                   /* REPROJECTION: finite, > 0, in pixels of view r */
+    float depth_rel;                   /* REPROJECTION: finite, > 0, relative to d_r */
+} gpm_fuse_rule;
+/* gpm_fuse under `rule`; a NULL rule is gpm_fuse.  Refused with GPM_E_ARG before any CUDA call, besides what gpm_fuse
+ * refuses (except disp_thresh under REPROJECTION): an unknown kind; for REPROJECTION, reproj_px or depth_rel not finite
+ * or <= 0. */
+int gpm_fuse_with_rule(const gpm_fuse_desc* desc, const gpm_fuse_rule* rule, gpm_fuse_result* result);
 
 /* Binary little-endian PLY with the header of storePlyFileBinary (displayUtils.h:84-97) and `count` packed vertices. */
 int gpm_write_ply(const char* path, const unsigned char* vertices, long long count);
