@@ -110,6 +110,10 @@ class GpmMsRestoreOpts(C.Structure):
                 ("restored", C.POINTER(C.c_int))]
 
 
+class GpmRefineOpts(C.Structure):
+    _fields_ = [("kind", C.c_int), ("perturbation", C.c_float)]
+
+
 class GpmFuseCamera(C.Structure):
     _fields_ = [("M_inv", C.c_float * 9), ("P", C.c_float * 12), ("f", C.c_float)]
 
@@ -238,6 +242,14 @@ def load_library():
     L.gpm_ms_batch_run_restore.argtypes = [C.POINTER(GpmMsBatchDesc), C.POINTER(GpmJobOpts), C.POINTER(GpmViewSel),
                                            C.POINTER(GpmMsPriorOpts), C.POINTER(GpmMsRestoreOpts), C.POINTER(GpmMsBatchStats)]
     L.gpm_set_geo_mask.argtypes = [vp, vp, C.c_size_t, C.c_int]
+    L.gpm_set_refinement.argtypes = [vp, C.c_int, C.c_float]
+    L.gpm_batch_run_refine.argtypes = [C.POINTER(GpmBatchDesc), C.POINTER(GpmJobOpts), C.POINTER(GpmViewSel),
+                                       C.POINTER(GpmPriorOpts), C.POINTER(GpmRefineOpts), C.POINTER(GpmBatchStats)]
+    L.gpm_geo_batch_run_refine.argtypes = [C.POINTER(GpmGeoBatchDesc), C.POINTER(GpmJobOpts), C.POINTER(GpmViewSel),
+                                           C.POINTER(GpmPriorOpts), C.POINTER(GpmRefineOpts), C.POINTER(GpmGeoBatchStats)]
+    L.gpm_ms_batch_run_refine.argtypes = [C.POINTER(GpmMsBatchDesc), C.POINTER(GpmJobOpts), C.POINTER(GpmViewSel),
+                                          C.POINTER(GpmMsPriorOpts), C.POINTER(GpmMsRestoreOpts), C.POINTER(GpmRefineOpts),
+                                          C.POINTER(GpmMsBatchStats)]
     L.gpm_fuse_cameras.argtypes = [C.POINTER(C.c_double), C.c_int, C.c_double, C.POINTER(GpmFuseCamera)]
     L.gpm_fuse.argtypes = [C.POINTER(GpmFuseDesc), C.POINTER(GpmFuseResult)]
     L.gpm_fuse_with_rule.argtypes = [C.POINTER(GpmFuseDesc), C.POINTER(GpmFuseRule), C.POINTER(GpmFuseResult)]
@@ -253,7 +265,8 @@ def load_library():
                  "gpm_batch_run_vsel", "gpm_geo_batch_run_vsel", "gpm_set_planar_prior", "gpm_get_planar_prior",
                  "gpm_build_planar_prior", "gpm_set_prior", "gpm_offer_prior", "gpm_batch_run_prior",
                  "gpm_geo_batch_run_prior", "gpm_downsample", "gpm_upsample_planes", "gpm_ms_batch_run", "gpm_ms_batch_run_prior",
-                 "gpm_ms_batch_run_restore", "gpm_set_geo_mask",
+                 "gpm_ms_batch_run_restore", "gpm_set_geo_mask", "gpm_set_refinement", "gpm_batch_run_refine",
+                 "gpm_geo_batch_run_refine", "gpm_ms_batch_run_refine",
                  "gpm_prepare_cameras", "gpm_select_views", "gpm_write_dmb", "gpm_read_dmb", "gpm_write_result_dmb",
                  "gpm_fuse_cameras", "gpm_fuse", "gpm_fuse_with_rule", "gpm_write_ply", "gpm_nearest_dist"):
         getattr(L, name).restype = C.c_int
@@ -510,6 +523,44 @@ def restore_opts(detail_restorer: Optional[dict], params, n_jobs: int, photometr
     return GpmMsRestoreOpts(int(r["photo_iterations"]), float(t32), int(r["iterations"]), restored), restored
 
 
+# Refinement (DESIGN.md §23): "gipuma", the reference's steps of shrinking random offsets (the default), and "acmh", ACMH's
+# five hypotheses from random and perturbed depths and normals.  REFINE_DEFAULTS["perturbation"] is ACMH's published
+# perturbation (0.02), not a value tuned on this project's scenes.
+REFINEMENT = {"gipuma": 0, "acmh": 1}
+REFINE_DEFAULTS = {"perturbation": 0.02}
+
+
+def check_refinement(kind: str, perturbation: float):
+    """The argument rules of gpm_set_refinement, checked before any call into the library: a known kind and a perturbation
+    that is, as the float32 the library receives, finite and in (0, 1).  Returns (the C-ABI's kind, that float32)."""
+    if not isinstance(kind, str) or kind not in REFINEMENT:
+        raise ValueError("refinement must be one of %s (got %r)" % (sorted(REFINEMENT), kind))
+    e = np.float32(np.nan)
+    if not isinstance(perturbation, bool) and isinstance(perturbation, (int, float, np.floating, np.integer)):
+        with np.errstate(over="ignore"):
+            e = np.float32(perturbation)
+    if not (np.isfinite(e) and 0 < e < 1):
+        raise ValueError("perturbation must be a number in (0, 1) in float32 (got %r)" % (perturbation,))
+    return REFINEMENT[kind], e
+
+
+def refine_opts(refinement) -> Optional[GpmRefineOpts]:
+    """gpm_refine_opts of the batch drivers from `refinement`: None (Gipuma's, the library's NULL), a kind ("gipuma" or
+    "acmh") with REFINE_DEFAULTS, or a dict with "kind" and optionally "perturbation"; checked before any call into the
+    library."""
+    if refinement is None:
+        return None
+    if isinstance(refinement, str):
+        refinement = {"kind": refinement}
+    if not isinstance(refinement, dict):
+        raise ValueError("refinement must be None, a kind or a dict (got %r)" % (refinement,))
+    unknown = sorted(set(refinement) - {"kind", "perturbation"})
+    if unknown or "kind" not in refinement:
+        raise ValueError("refinement dict needs 'kind' and may have 'perturbation' (got %r)" % (sorted(refinement),))
+    kind, e = check_refinement(refinement["kind"], refinement.get("perturbation", REFINE_DEFAULTS["perturbation"]))
+    return GpmRefineOpts(kind, float(e))
+
+
 def jbu_params(radius: int = JBU_DEFAULTS["radius"], sigma_space: float = JBU_DEFAULTS["sigma_space"],
                sigma_range: float = JBU_DEFAULTS["sigma_range"]) -> GpmJbuParams:
     """gpm_jbu_params, every argument checked before any call into the library by the rules of gpm_upsample_planes."""
@@ -726,6 +777,13 @@ class Context:
         m = np.empty((self.H, self.W), dtype=np.uint64)
         self._check(self.lib.gpm_get_view_masks(self.h, C.c_void_p(m.ctypes.data)))
         return m
+
+    def set_refinement(self, kind: str = "gipuma", perturbation: float = REFINE_DEFAULTS["perturbation"]):
+        """How each pixel refines its plane (DESIGN.md §23): "gipuma", the reference's steps (the default), or "acmh", ACMH's
+        five hypotheses (d_r, n), (d, n_r), (d_r, n_r), (d, n_t), (d_t, n) of random (r) and perturbed (t) depths and
+        normals, perturbation in (0, 1).  Not with the fused sweep or the source-view shard."""
+        k, e = check_refinement(kind, perturbation)
+        self._check(self.lib.gpm_set_refinement(self.h, k, float(e)))
 
     def set_rng(self, seed: int, mode: int = GPM_RNG_REFERENCE):
         self._check(self.lib.gpm_set_rng(self.h, seed, mode))
@@ -955,15 +1013,18 @@ def _job_stats(n_refs):
 def batch_run(images, Ps, params, refs, devices=(0,), cam_scale: float = 1.0, min_angle: float = 10.0, max_angle: float = 30.0,
               max_views: int = 9, seed: int = 0xC0FFEE, out_dir: Optional[str] = None, want_outputs: bool = True,
               photometric: str = "pm", ncc_min_std: float = NCC_MIN_STD, propagation: str = "fixed",
-              view_selection: str = "off", jvs_params: Optional[dict] = None, planar_prior: Optional[dict] = None):
-    """Reference-view batch in ONE process (gpm_batch_run_prior): `images` [n, H, W] float32 (shared, page-locked once), `Ps`
-    n 3x4 projections, `refs` the reference views to process, `devices` the CUDA ordinals to use (one worker thread each),
+              view_selection: str = "off", jvs_params: Optional[dict] = None, planar_prior: Optional[dict] = None,
+              refinement=None):
+    """Reference-view batch in ONE process (gpm_batch_run_prior; gpm_batch_run_refine with a refinement): `images`
+    [n, H, W] float32 (shared, page-locked once), `Ps` n 3x4 projections, `refs` the reference views to process, `devices` the CUDA ordinals to use (one worker thread each),
     `photometric` the cost, "pm" or "ncc" with min_std `ncc_min_std` (Context.set_photometric), `propagation` "fixed" or
     "adaptive" (Context.set_propagation), `view_selection` "off" or "joint" with `jvs_params` overriding JVS_DEFAULTS
     (Context.set_view_selection; "joint" needs photometric="ncc"), `planar_prior` None or a dict (prior_opts): a prior stage
-    after the params.iterations sweeps of every job (DESIGN.md §18), whose counts come back per job in stats["prior"].
+    after the params.iterations sweeps of every job (DESIGN.md §18), whose counts come back per job in stats["prior"],
+    `refinement` None (Gipuma's), "gipuma", "acmh" or a dict with "kind" and "perturbation" (refine_opts; DESIGN.md §23).
     Returns (norm4 [len(refs), H, W, 4] or None, cost or None, stats dict)."""
     opts = job_opts(photometric, ncc_min_std, propagation)
+    ref_o = refine_opts(refinement)
     vsel = view_sel(view_selection, **(jvs_params or {}))
     check_modes(photometric, view_selection, 1, planar_prior)
     prior, pinfo = prior_opts(planar_prior, params, len(refs), photometric)
@@ -974,7 +1035,8 @@ def batch_run(images, Ps, params, refs, devices=(0,), cam_scale: float = 1.0, mi
     cc = np.empty((len(refs), H, W), np.float32) if want_outputs else None
     d, _keep = _batch_desc(imgs, Ps, params, refs, devices, cam_scale, min_angle, max_angle, max_views, seed, out_dir, n4, cc)
     st = _job_stats(len(refs))
-    rc = lib.gpm_batch_run_prior(C.byref(d), C.byref(opts), C.byref(vsel), C.byref(prior) if prior else None, C.byref(st))
+    args = (C.byref(d), C.byref(opts), C.byref(vsel), C.byref(prior) if prior else None)
+    rc = lib.gpm_batch_run_refine(*args, C.byref(ref_o), C.byref(st)) if ref_o else lib.gpm_batch_run_prior(*args, C.byref(st))
     if rc != 0:
         raise GipumaError("gpm_batch_run failed (%d): %s" % (rc, lib.gpm_batch_last_error().decode()))
     k = len(refs)
@@ -986,7 +1048,7 @@ def geometric_pass(images, Ps, params, refs, geo_iterations: int = 2, weight: fl
                    cam_scale: float = 1.0, min_angle: float = 10.0, max_angle: float = 30.0, max_views: int = 9,
                    seed: int = 0xC0FFEE, devices=(0,), out_dir: Optional[str] = None, photometric: str = "pm",
                    ncc_min_std: float = NCC_MIN_STD, propagation: str = "fixed", view_selection: str = "off",
-                   jvs_params: Optional[dict] = None, planar_prior: Optional[dict] = None):
+                   jvs_params: Optional[dict] = None, planar_prior: Optional[dict] = None, refinement=None):
     """PatchMatch with a geometric-consistency second pass (DESIGN.md §14) for the reference views `refs`, run by the
     native two-pass batch driver (gpm_geo_batch_run) over the worker pool of `devices` (one worker thread and context each;
     a device may be listed more than once).
@@ -1000,13 +1062,14 @@ def geometric_pass(images, Ps, params, refs, geo_iterations: int = 2, weight: fl
     photometric / ncc_min_std: the photometric cost of both passes, as batch_run ("ncc": grey images only); propagation:
     the propagation mode of both passes, as batch_run; view_selection / jvs_params: the view selection of both passes, as
     batch_run (pass 2 starts over at t = 0); planar_prior: a prior stage in pass 1 only, as batch_run (info["prior"]: the
-    counts per pass-1 view, in info["pass1_views"]' order).
+    counts per pass-1 view, in info["pass1_views"]' order); refinement: the refinement of both passes, as batch_run.
     Returns (norm4 [len(refs), H, W, 4], cost [len(refs), H, W], info) with norm4 as batch_run returns it, so fuse and
     evaluate_cloud take it unchanged; info: "pass1_views" (the views pass 1 ran, ascending), "pass1_sweep_s" (in that order)
     and "pass2_sweep_s" (per reference view): CUDA-event seconds of each view's sweep call on its context's stream;
     "views" (image indices of the source views each reference view selected), "device" (the device that ran its pass 2)."""
     check_geometric(weight, max_err)
     opts = job_opts(photometric, ncc_min_std, propagation)
+    ref_o = refine_opts(refinement)
     if int(geo_iterations) != geo_iterations or geo_iterations < 0:
         raise ValueError("geo_iterations must be an integer >= 0")
     imgs = np.ascontiguousarray(images, dtype=np.float32)
@@ -1033,7 +1096,8 @@ def geometric_pass(images, Ps, params, refs, geo_iterations: int = 2, weight: fl
     ref_views = (C.c_int * (k * int(max_views)))()
     jobs = _job_stats(k)                                   # owns the per-job arrays st.batch points into
     st = GpmGeoBatchStats(jobs, 0, p1_views, p1_ms, ref_views)
-    rc = lib.gpm_geo_batch_run_prior(C.byref(g), C.byref(opts), C.byref(vsel), C.byref(prior) if prior else None, C.byref(st))
+    args = (C.byref(g), C.byref(opts), C.byref(vsel), C.byref(prior) if prior else None)
+    rc = lib.gpm_geo_batch_run_refine(*args, C.byref(ref_o), C.byref(st)) if ref_o else lib.gpm_geo_batch_run_prior(*args, C.byref(st))
     if rc != 0:
         raise GipumaError("gpm_geo_batch_run failed (%d): %s" % (rc, lib.gpm_batch_last_error().decode()))
     m = st.n_pass1
@@ -1050,7 +1114,7 @@ def multiscale_pass(images, Ps, params, refs, levels: int = MS_LEVELS, geo_itera
                     seed: int = 0xC0FFEE, devices=(0,), out_dir: Optional[str] = None, photometric: str = "pm",
                     ncc_min_std: float = NCC_MIN_STD, propagation: str = "fixed", view_selection: str = "off",
                     jvs_params: Optional[dict] = None, planar_prior: Optional[dict] = None, geo_prior: Optional[dict] = None,
-                    detail_restorer: Optional[dict] = None):
+                    detail_restorer: Optional[dict] = None, refinement=None):
     """Coarse-to-fine multi-scale PatchMatch (ACMM; DESIGN.md §19) for the reference views `refs`, run by the native
     multi-level batch driver (gpm_ms_batch_run_restore) over the worker pool of `devices`.
 
@@ -1070,6 +1134,7 @@ def multiscale_pass(images, Ps, params, refs, levels: int = MS_LEVELS, geo_itera
     photometric-only estimate (photo_iterations sweeps from init); after the geometric stage, pixels where the geometric
     stage's plane costs photometrically more than `threshold` above the estimate's take the estimate's plane and sweep
     without the geometric term (a per-pixel mask) for `iterations` more sweeps, while the rest keep it.
+    refinement (DESIGN.md §23), as batch_run: the refinement of every sweep, at every level and in every stage.
     Returns (norm4 [len(refs), H, W, 4], cost [len(refs), H, W], info) with norm4 as batch_run returns it, so fuse and
     evaluate_cloud take it unchanged; info: "views" (V, ascending), "level_sweep_s" (CUDA-event sweep seconds summed over
     the views, per level, full size first, prior sweeps included), "level_upsample_s" (host seconds of the upsampling calls,
@@ -1079,6 +1144,7 @@ def multiscale_pass(images, Ps, params, refs, levels: int = MS_LEVELS, geo_itera
     "restored" (detail pixels per reference, None without the restorer)."""
     check_geometric(weight, max_err)
     opts = job_opts(photometric, ncc_min_std, propagation)
+    ref_o = refine_opts(refinement)
     if isinstance(levels, bool) or int(levels) != levels or not 1 <= levels <= MS_MAX_LEVELS:
         raise ValueError("levels must be an integer in 1..%d (got %r)" % (MS_MAX_LEVELS, levels))
     if int(geo_iterations) != geo_iterations or geo_iterations < 0:
@@ -1129,8 +1195,8 @@ def multiscale_pass(images, Ps, params, refs, levels: int = MS_LEVELS, geo_itera
     jobs = _job_stats(k)                                   # owns the per-job arrays st.batch points into
     st = GpmMsBatchStats(jobs, 0, views)
     po = GpmMsPriorOpts(*[C.pointer(stages[s][0]) if s in stages else None for s in ("photometric", "geometric")])
-    rc = lib.gpm_ms_batch_run_restore(C.byref(m), C.byref(opts), C.byref(vsel), C.byref(po), C.byref(ro) if ro else None,
-                                      C.byref(st))
+    args = (C.byref(m), C.byref(opts), C.byref(vsel), C.byref(po), C.byref(ro) if ro else None)
+    rc = lib.gpm_ms_batch_run_refine(*args, C.byref(ref_o), C.byref(st)) if ref_o else lib.gpm_ms_batch_run_restore(*args, C.byref(st))
     if rc != 0:
         raise GipumaError("gpm_ms_batch_run failed (%d): %s" % (rc, lib.gpm_batch_last_error().decode()))
     info = {"views": views[:st.n_views], "level_sweep_s": [t / 1e3 for t in st.level_sweep_ms[:levels]],

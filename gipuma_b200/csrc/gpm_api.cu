@@ -142,6 +142,10 @@ struct gpm_ctx {
     // the geometric term's per-pixel mask (DESIGN.md §21): nonzero bytes switch the term off; read while geo_mask_set
     unsigned char* geo_mask = nullptr;         // [H*W], allocated by the first gpm_set_geo_mask
     bool geo_mask_set = false;
+    // refinement (DESIGN.md §23): GPM_REFINE_GIPUMA, the reference's, or GPM_REFINE_ACMH (gpm_set_refinement)
+    int refine_kind = GPM_REFINE_GIPUMA;
+    float refine_eps = 0.02f;
+    unsigned refine_count = 0;                 // r: k_sweep launches with refinement since gpm_init / gpm_init_planes / gpm_set_rng
 };
 
 namespace {
@@ -211,8 +215,11 @@ bool jvs_on(const gpm_ctx* c) { return c->vsel.kind == GPM_VSEL_JOINT; }
 Mode ctx_mode(const gpm_ctx* c)
 {
     return Mode{c->color == 1, c->opt_neighbours == 20, c->geo_weight > 0.f, ncc_on(c), c->propagation == GPM_PROP_ADAPTIVE, jvs_on(c),
-                c->prior_weight > 0.f, c->geo_weight > 0.f && c->geo_mask_set};
+                c->prior_weight > 0.f, c->geo_weight > 0.f && c->geo_mask_set, c->refine_kind == GPM_REFINE_ACMH};
 }
+
+// the index of the context's mode in the tables of k_cost_eval and k_shard_stage, which do not read refine_acmh
+int eval_bits(const gpm_ctx* c) { return ctx_mode(c).bits() & (GPM_EVAL_MODES - 1); }
 
 const char* conflict_text(ModeConflict k)
 {
@@ -222,6 +229,7 @@ const char* conflict_text(ModeConflict k)
     case ModeConflict::ncc_colour: return "the NCC photometric cost supports grey images only";
     case ModeConflict::prior: return "the planar prior supports grey images without joint view selection";
     case ModeConflict::geomask: return "the geometric term's mask and the planar prior exclude each other";
+    case ModeConflict::refine_fused: return "ACMH's refinement supports the 8-neighbour sweep only (option neighbours = 8)";
     default: return nullptr;
     }
 }
@@ -450,19 +458,20 @@ auto make_table(Entry entry, std::integer_sequence<int, B...>) { return std::arr
 
 const auto kSweep = make_table([](auto b) -> decltype(&k_sweep<false, false>) {
     constexpr Mode m = Mode::of(decltype(b)::value);
-    if constexpr (mode_conflict(m) == ModeConflict::none) return k_sweep<m.color, m.fused, m.geo, m.ncc, m.adaptive, m.jvs, m.prior, m.geomask>;
+    if constexpr (mode_conflict(m) == ModeConflict::none)
+        return k_sweep<m.color, m.fused, m.geo, m.ncc, m.adaptive, m.jvs, m.prior, m.geomask, m.refine_acmh>;
     else return nullptr;
 }, std::make_integer_sequence<int, GPM_MODES>{});
 
 const auto kCostEval = make_table([](auto b) -> decltype(&k_cost_eval<false>) {
     constexpr Mode m = Mode::of(decltype(b)::value);
     if constexpr (mode_conflict(m) == ModeConflict::none) return k_cost_eval<m.color, m.geo, m.ncc, m.prior, m.geomask>; else return nullptr;
-}, std::make_integer_sequence<int, GPM_MODES>{});
+}, std::make_integer_sequence<int, GPM_EVAL_MODES>{});
 
 const auto kShardStage = make_table([](auto b) -> decltype(&k_shard_stage<false>) {
     constexpr Mode m = Mode::of(decltype(b)::value);
     if constexpr (shard_supports(m)) return k_shard_stage<m.color, m.adaptive>; else return nullptr;
-}, std::make_integer_sequence<int, GPM_MODES>{});
+}, std::make_integer_sequence<int, GPM_EVAL_MODES>{});
 
 int launch_colour(gpm_ctx* c, const KParams& P, int colour, int mask)
 {
@@ -470,8 +479,9 @@ int launch_colour(gpm_ctx* c, const KParams& P, int colour, int mask)
     if (!kern) return fail(GPM_E_STATE, "k_sweep has no kernel for this context's mode");
     kern<<<tile_grid(c), P.nwarps * 32, sweep_smem_bytes(c, P), c->stream>>>(P, c->tmap, c->d_cams, c->srcTex, c->planes,
         c->cost, c->rng, c->prov, Memo{c->pid, c->seen, c->refseen, c->memo_mask, c->next_id}, colour, mask, c->d_stats, geo_params(c),
-        jvs_params(c), prior_params(c));
+        jvs_params(c), prior_params(c), AcmhRefine{(unsigned)c->seed ^ (unsigned)(c->seed >> 32), c->refine_count, c->refine_eps});
     c->launches++;
+    if (mask & 4) c->refine_count++;
     CU(cudaGetLastError());
     return GPM_OK;
 }
@@ -479,7 +489,7 @@ int launch_colour(gpm_ctx* c, const KParams& P, int colour, int mask)
 // cost of `planes` at every pixel into `cost` (k_cost_eval: one block per tile, no slices)
 int launch_cost_eval(gpm_ctx* c, const KParams& P, const float4* planes, float* cost)
 {
-    const auto kern = kCostEval[ctx_mode(c).bits()];
+    const auto kern = kCostEval[eval_bits(c)];
     if (!kern) return fail(GPM_E_STATE, "k_cost_eval has no kernel for this context's mode");
     dim3 grid((P.W + GPM_TILE - 1) / GPM_TILE, (P.H + GPM_TILE - 1) / GPM_TILE);
     kern<<<grid, P.nwarps * 32, block_smem_bytes(P, ncc_on(c)), c->stream>>>(P, c->tmap, c->d_cams, c->srcTex, planes, cost, nullptr, geo_params(c),
@@ -489,9 +499,11 @@ int launch_cost_eval(gpm_ctx* c, const KParams& P, const float4* planes, float* 
     return GPM_OK;
 }
 
-// random planes (gipuma.cu:1870-1875) and their identities; the XORWOW states are kept in GPM_RNG_STATEFUL mode
+// random planes (gipuma.cu:1870-1875) and their identities; the XORWOW states are kept in GPM_RNG_STATEFUL mode.  ACMH's
+// refinement counts its launches from here (§23).
 int init_planes(gpm_ctx* c, const KParams& P)
 {
+    c->refine_count = 0;
     dim3 b(16, 16), gr((c->W + 15) / 16, (c->H + 15) / 16);
     k_init_planes<<<gr, b, 0, c->stream>>>(P, c->seed, c->planes, c->rng_mode == GPM_RNG_STATEFUL ? c->rng : nullptr, c->pid);
     c->launches++;
@@ -695,6 +707,7 @@ extern "C" int gpm_set_rng(gpm_ctx* c, unsigned long long seed, int mode)
     DeviceGuard g(c->device);
     c->seed = seed;
     c->rng_mode = mode;
+    c->refine_count = 0;
     c->memo_dirty = true;                            // the refinement memo assumes the random stream it was built under
     if (mode == GPM_RNG_STATEFUL && !c->rng) {
         CU(cudaMalloc(&c->rng, (size_t)c->W * c->H * 6 * sizeof(unsigned)));
@@ -849,6 +862,14 @@ const char* prior_opts_refusal(const gpm_prior_opts* p)
     return p->iterations < 0 ? "prior iterations must be >= 0" : nullptr;
 }
 
+// gpm_set_refinement's argument rules (the fused sweep aside), also those of a batch driver's gpm_refine_opts
+const char* refine_refusal(int kind, float perturbation)
+{
+    if (kind != GPM_REFINE_GIPUMA && kind != GPM_REFINE_ACMH) return "unknown refinement kind";
+    if (!std::isfinite(perturbation) || !(perturbation > 0.f && perturbation < 1.f)) return "perturbation must be finite and in (0, 1)";
+    return nullptr;
+}
+
 // What the batch drivers refuse for a job's options before any CUDA call: the setters' argument checks and the mode rule,
 // for grey (channels 1) or colour (channels 4) images; a prior stage counts as the planar-prior mode.
 const char* job_refusal(const gpm_job_opts* o, const gpm_view_sel* v, const gpm_prior_opts* prior, int channels)
@@ -921,6 +942,17 @@ extern "C" int gpm_set_propagation(gpm_ctx* c, int kind)
     if (const char* bad = propagation_refusal(kind)) return fail(GPM_E_ARG, std::string("gpm_set_propagation: ") + bad);
     if (const int rc = refuse_change(c, "gpm_set_propagation", &Mode::adaptive, kind == GPM_PROP_ADAPTIVE)) return rc;
     c->propagation = kind;
+    return GPM_OK;
+}
+
+// Only the refinement's candidates change; the accept rule and cost(p, plane) do not, so nothing is marked stale.
+extern "C" int gpm_set_refinement(gpm_ctx* c, int kind, float perturbation)
+{
+    if (!c) return fail(GPM_E_ARG, "gpm_set_refinement: null context");
+    if (const char* bad = refine_refusal(kind, perturbation)) return fail(GPM_E_ARG, std::string("gpm_set_refinement: ") + bad);
+    if (const int rc = refuse_change(c, "gpm_set_refinement", &Mode::refine_acmh, kind == GPM_REFINE_ACMH)) return rc;
+    c->refine_kind = kind;
+    c->refine_eps = perturbation;
     return GPM_OK;
 }
 
@@ -1376,6 +1408,7 @@ static int shard_refine_steps(const gpm_params& p)
 // GPM_E_STATE here, but the fused sweep only where it launches (shard_common), with GPM_E_ARG.
 static int shard_refuses_state(gpm_ctx* c)
 {
+    if (c->refine_kind != GPM_REFINE_GIPUMA) return fail(GPM_E_STATE, "view sharding supports Gipuma's refinement only (GPM_REFINE_GIPUMA)");
     Mode m = ctx_mode(c);
     m.fused = false;
     return shard_supports(m) ? GPM_OK : fail(GPM_E_STATE, "view sharding supports neither the geometric-consistency mode, the NCC cost, joint view selection nor the planar prior");
@@ -1424,7 +1457,7 @@ static int shard_common(gpm_ctx* c, int stage, KParams& P)
 // enqueue one stage kernel (stage 0 .. last+1) on the context's stream
 static int shard_launch_stage(gpm_ctx* c, const KParams& P, int colour, int stage, const float* gathered_prev, int world, float* xchg)
 {
-    const auto kern = kShardStage[ctx_mode(c).bits()];
+    const auto kern = kShardStage[eval_bits(c)];
     if (!kern) return fail(GPM_E_STATE, "k_shard_stage has no kernel for this context's mode");
     const int last = 1 + shard_refine_steps(c->prm);
     ShardState S{c->dispbuf, c->candbuf, c->canddepth, c->sflags};

@@ -34,6 +34,7 @@
 namespace gpm {
 const char* job_refusal(const gpm_job_opts* o, const gpm_view_sel* v, const gpm_prior_opts* prior, int channels);     // gpm_api.cu
 bool prior_bound_ok(const gpm_params& p, bool ncc, float geo_weight, float geo_max_err, float prior_weight);        // gpm_api.cu
+const char* refine_refusal(int kind, float perturbation);                                                         // gpm_api.cu
 }
 
 namespace {
@@ -83,17 +84,22 @@ bool plan_view(const gpm_batch_desc* d, int ref, ViewSetup& s)
 gpm_job_opts photo_opts(int kind, float min_std) { return gpm_job_opts{kind, min_std, GPM_PROP_FIXED}; }
 
 const gpm_view_sel kVselOff{GPM_VSEL_OFF, 0.f, 0.f, 0.f, 0, 0, 0.f, 0.f};
+const gpm_refine_opts kRefineGipuma{GPM_REFINE_GIPUMA, 0.02f};      // a NULL gpm_refine_opts
 
-// The per-view setup of a job: photometric cost, propagation, view selection, parameters, reference and source images
-// (images[i]: image i, grey: channels 1, RGBA: 4), view count, RNG.
+// what the _refine drivers refuse of their refinement before any CUDA call, or NULL
+const char* refine_opts_refusal(const gpm_refine_opts* r) { return r ? gpm::refine_refusal(r->kind, r->perturbation) : nullptr; }
+
+// The per-view setup of a job: photometric cost, propagation, view selection, refinement, parameters, reference and source
+// images (images[i]: image i, grey: channels 1, RGBA: 4), view count, RNG.
 int load_view(gpm_ctx* ctx, const gpm_batch_desc* d, const float* const* images, int channels, size_t pitch, const ViewSetup& s,
-              const gpm_job_opts& o, const gpm_view_sel& v)
+              const gpm_job_opts& o, const gpm_view_sel& v, const gpm_refine_opts& r)
 {
     auto set_reference = channels == 4 ? gpm_set_reference_color : gpm_set_reference;
     auto set_view = channels == 4 ? gpm_set_view_color : gpm_set_view;
     int rc = gpm_set_photometric(ctx, o.photometric, o.ncc_min_std);
     if (rc == GPM_OK) rc = gpm_set_propagation(ctx, o.propagation);
     if (rc == GPM_OK) rc = gpm_set_view_selection(ctx, &v);
+    if (rc == GPM_OK) rc = gpm_set_refinement(ctx, r.kind, r.perturbation);
     if (rc == GPM_OK) rc = gpm_set_params(ctx, &s.p);
     if (rc == GPM_OK) rc = set_reference(ctx, images[s.order[0]], pitch, 0, &s.cams[0]);
     for (int v = 0; v < s.nv && rc == GPM_OK; v++) rc = set_view(ctx, v, images[s.source(v)], pitch, 0, &s.cams[s.subset[v]]);
@@ -256,17 +262,19 @@ int prior_off(gpm_ctx* ctx, const gpm_prior_opts* p) { return gpm_set_prior(ctx,
 
 // gpm_batch_run and its _photo / _opts / _vsel / _prior twins; `fn` names the entry point in error messages
 static int batch_run(const char* fn, const gpm_batch_desc* d, const gpm_job_opts* opts, const gpm_view_sel* vsel,
-                     const gpm_prior_opts* prior, gpm_batch_stats* stats)
+                     const gpm_prior_opts* prior, const gpm_refine_opts* refine, gpm_batch_stats* stats)
 {
     clear_err();
     if (!batch_desc_ok(d)) {
         set_err(std::string(fn) + ": bad arguments");
         return GPM_E_ARG;
     }
-    if (const char* bad = gpm::job_refusal(opts, vsel, prior, 1)) {
+    const char* bad_refine = refine_opts_refusal(refine);
+    if (const char* bad = bad_refine ? bad_refine : gpm::job_refusal(opts, vsel, prior, 1)) {
         set_err(std::string(fn) + ": bad arguments: " + bad);
         return GPM_E_ARG;
     }
+    if (!refine) refine = &kRefineGipuma;
     const int n = d->n_images, W = d->width, H = d->height;
     const size_t pitch = d->pitch_bytes ? d->pitch_bytes : (size_t)W * sizeof(float);
     const size_t npix = (size_t)W * H;
@@ -285,7 +293,7 @@ static int batch_run(const char* fn, const gpm_batch_desc* d, const gpm_job_opts
             const int ref = d->ref_indices ? d->ref_indices[job] : job;
             if (ref < 0 || ref >= n) { set_err(std::string(fn) + ": reference index out of range");  return false; }
             if (!plan_view(d, ref, s)) { set_err(std::string(fn) + ": no source view passes the angle filter for reference " + std::to_string(ref));  return false; }
-            int rc = load_view(ctx, d, d->images, 1, pitch, s, *opts, *vsel);
+            int rc = load_view(ctx, d, d->images, 1, pitch, s, *opts, *vsel, *refine);
             float ms = 0.f, ms2 = 0.f;
             if (!prior) {
                 if (rc == GPM_OK) rc = gpm_run(ctx, &ms);
@@ -325,29 +333,35 @@ static int batch_run(const char* fn, const gpm_batch_desc* d, const gpm_job_opts
 extern "C" int gpm_batch_run(const gpm_batch_desc* d, gpm_batch_stats* stats)
 {
     const gpm_job_opts o = photo_opts(GPM_PHOTO_PM, 0.f);
-    return batch_run("gpm_batch_run", d, &o, &kVselOff, nullptr, stats);
+    return batch_run("gpm_batch_run", d, &o, &kVselOff, nullptr, nullptr, stats);
 }
 
 extern "C" int gpm_batch_run_photo(const gpm_batch_desc* d, int kind, float min_std, gpm_batch_stats* stats)
 {
     const gpm_job_opts o = photo_opts(kind, min_std);
-    return batch_run("gpm_batch_run_photo", d, &o, &kVselOff, nullptr, stats);
+    return batch_run("gpm_batch_run_photo", d, &o, &kVselOff, nullptr, nullptr, stats);
 }
 
 extern "C" int gpm_batch_run_opts(const gpm_batch_desc* d, const gpm_job_opts* opts, gpm_batch_stats* stats)
 {
-    return batch_run("gpm_batch_run_opts", d, opts, &kVselOff, nullptr, stats);
+    return batch_run("gpm_batch_run_opts", d, opts, &kVselOff, nullptr, nullptr, stats);
 }
 
 extern "C" int gpm_batch_run_vsel(const gpm_batch_desc* d, const gpm_job_opts* opts, const gpm_view_sel* vsel, gpm_batch_stats* stats)
 {
-    return batch_run("gpm_batch_run_vsel", d, opts, vsel ? vsel : &kVselOff, nullptr, stats);
+    return batch_run("gpm_batch_run_vsel", d, opts, vsel ? vsel : &kVselOff, nullptr, nullptr, stats);
 }
 
 extern "C" int gpm_batch_run_prior(const gpm_batch_desc* d, const gpm_job_opts* opts, const gpm_view_sel* vsel, const gpm_prior_opts* prior,
                                    gpm_batch_stats* stats)
 {
-    return batch_run("gpm_batch_run_prior", d, opts, vsel ? vsel : &kVselOff, prior, stats);
+    return batch_run("gpm_batch_run_prior", d, opts, vsel ? vsel : &kVselOff, prior, nullptr, stats);
+}
+
+extern "C" int gpm_batch_run_refine(const gpm_batch_desc* d, const gpm_job_opts* opts, const gpm_view_sel* vsel, const gpm_prior_opts* prior,
+                                    const gpm_refine_opts* refine, gpm_batch_stats* stats)
+{
+    return batch_run("gpm_batch_run_refine", d, opts, vsel ? vsel : &kVselOff, prior, refine, stats);
 }
 
 
@@ -378,14 +392,16 @@ const char* geo_desc_refusal(const gpm_geo_batch_desc* g, const gpm_job_opts* op
 
 // gpm_geo_batch_run and its _photo / _opts / _vsel twins; `fn` names the entry point in error messages
 static int geo_batch_run(const char* fn, const gpm_geo_batch_desc* g, const gpm_job_opts* opts, const gpm_view_sel* vsel,
-                         const gpm_prior_opts* prior, gpm_geo_batch_stats* stats)
+                         const gpm_prior_opts* prior, const gpm_refine_opts* refine, gpm_geo_batch_stats* stats)
 {
     clear_err();
     std::vector<char> is_ref;
-    if (const char* bad = geo_desc_refusal(g, opts, vsel, prior, is_ref)) {
+    const char* bad_refine = refine_opts_refusal(refine);
+    if (const char* bad = bad_refine ? bad_refine : geo_desc_refusal(g, opts, vsel, prior, is_ref)) {
         set_err(std::string(fn) + ": bad arguments: " + bad);
         return GPM_E_ARG;
     }
+    if (!refine) refine = &kRefineGipuma;
     const gpm_batch_desc* d = &g->batch;
     const int n = d->n_images, W = d->width, H = d->height, n_refs = d->n_refs;
     const size_t pitch = d->pitch_bytes ? d->pitch_bytes : (size_t)W * sizeof(float) * g->channels;
@@ -442,7 +458,7 @@ static int geo_batch_run(const char* fn, const gpm_geo_batch_desc* g, const gpm_
         };
         take_jobs(next1, n_pass1, failed, [&](int job) {          // pass 1: photometric
             const int r = pass1[job];
-            int rc = load_view(ctx, d, d->images, g->channels, pitch, setup[r], *opts, *vsel);
+            int rc = load_view(ctx, d, d->images, g->channels, pitch, setup[r], *opts, *vsel, *refine);
             if (rc == GPM_OK) rc = gpm_init(ctx);
             if (rc == GPM_OK) rc = timer.sweep(ctx, d->params.iterations, &pass1_ms[job]);
             float ms2 = 0.f;
@@ -462,7 +478,7 @@ static int geo_batch_run(const char* fn, const gpm_geo_batch_desc* g, const gpm_
             const int r = ref_of(job);
             const ViewSetup& s = setup[r];
             const float* raw = raw_store + (size_t)raw_slot[r] * npix * 4;
-            int rc = load_view(ctx, d, d->images, g->channels, pitch, s, *opts, *vsel);
+            int rc = load_view(ctx, d, d->images, g->channels, pitch, s, *opts, *vsel, *refine);
             for (int v = 0; v < s.nv && rc == GPM_OK; v++) rc = gpm_set_view_depth(ctx, v, depth_store + (size_t)depth_slot[s.source(v)] * npix, 0, 0);
             if (rc == GPM_OK) rc = gpm_set_geometric(ctx, g->weight, g->max_err);
             if (rc == GPM_OK) rc = gpm_cost_eval(ctx, raw, cost.data(), 0);
@@ -505,30 +521,36 @@ static int geo_batch_run(const char* fn, const gpm_geo_batch_desc* g, const gpm_
 extern "C" int gpm_geo_batch_run(const gpm_geo_batch_desc* g, gpm_geo_batch_stats* stats)
 {
     const gpm_job_opts o = photo_opts(GPM_PHOTO_PM, 0.f);
-    return geo_batch_run("gpm_geo_batch_run", g, &o, &kVselOff, nullptr, stats);
+    return geo_batch_run("gpm_geo_batch_run", g, &o, &kVselOff, nullptr, nullptr, stats);
 }
 
 extern "C" int gpm_geo_batch_run_photo(const gpm_geo_batch_desc* g, int kind, float min_std, gpm_geo_batch_stats* stats)
 {
     const gpm_job_opts o = photo_opts(kind, min_std);
-    return geo_batch_run("gpm_geo_batch_run_photo", g, &o, &kVselOff, nullptr, stats);
+    return geo_batch_run("gpm_geo_batch_run_photo", g, &o, &kVselOff, nullptr, nullptr, stats);
 }
 
 extern "C" int gpm_geo_batch_run_opts(const gpm_geo_batch_desc* g, const gpm_job_opts* opts, gpm_geo_batch_stats* stats)
 {
-    return geo_batch_run("gpm_geo_batch_run_opts", g, opts, &kVselOff, nullptr, stats);
+    return geo_batch_run("gpm_geo_batch_run_opts", g, opts, &kVselOff, nullptr, nullptr, stats);
 }
 
 extern "C" int gpm_geo_batch_run_vsel(const gpm_geo_batch_desc* g, const gpm_job_opts* opts, const gpm_view_sel* vsel,
                                       gpm_geo_batch_stats* stats)
 {
-    return geo_batch_run("gpm_geo_batch_run_vsel", g, opts, vsel ? vsel : &kVselOff, nullptr, stats);
+    return geo_batch_run("gpm_geo_batch_run_vsel", g, opts, vsel ? vsel : &kVselOff, nullptr, nullptr, stats);
 }
 
 extern "C" int gpm_geo_batch_run_prior(const gpm_geo_batch_desc* g, const gpm_job_opts* opts, const gpm_view_sel* vsel,
                                        const gpm_prior_opts* prior, gpm_geo_batch_stats* stats)
 {
-    return geo_batch_run("gpm_geo_batch_run_prior", g, opts, vsel ? vsel : &kVselOff, prior, stats);
+    return geo_batch_run("gpm_geo_batch_run_prior", g, opts, vsel ? vsel : &kVselOff, prior, nullptr, stats);
+}
+
+extern "C" int gpm_geo_batch_run_refine(const gpm_geo_batch_desc* g, const gpm_job_opts* opts, const gpm_view_sel* vsel,
+                                        const gpm_prior_opts* prior, const gpm_refine_opts* refine, gpm_geo_batch_stats* stats)
+{
+    return geo_batch_run("gpm_geo_batch_run_refine", g, opts, vsel ? vsel : &kVselOff, prior, refine, stats);
 }
 
 
@@ -615,7 +637,8 @@ const char* ms_restore_refusal(const gpm_ms_restore_opts* r)
 
 // gpm_ms_batch_run, gpm_ms_batch_run_prior and gpm_ms_batch_run_restore; `fn` names the entry point in error messages
 static int ms_batch_run(const char* fn_name, const gpm_ms_batch_desc* m, const gpm_job_opts* opts, const gpm_view_sel* vsel,
-                        gpm_ms_prior_opts* prior, const gpm_ms_restore_opts* restore, gpm_ms_batch_stats* stats)
+                        gpm_ms_prior_opts* prior, const gpm_ms_restore_opts* restore, const gpm_refine_opts* refine,
+                        gpm_ms_batch_stats* stats)
 {
     const std::string fn = fn_name;
     clear_err();
@@ -634,6 +657,11 @@ static int ms_batch_run(const char* fn_name, const gpm_ms_batch_desc* m, const g
         set_err(fn + ": bad arguments: " + bad);
         return GPM_E_ARG;
     }
+    if (const char* bad = refine_opts_refusal(refine)) {
+        set_err(fn + ": bad arguments: " + bad);
+        return GPM_E_ARG;
+    }
+    if (!refine) refine = &kRefineGipuma;
     const gpm_prior_opts* P_photo = prior ? prior->photometric : nullptr;
     const gpm_prior_opts* P_geo = prior ? prior->geometric : nullptr;
     const gpm_geo_batch_desc* g = &m->geo;
@@ -753,7 +781,7 @@ static int ms_batch_run(const char* fn_name, const gpm_ms_batch_desc* m, const g
         take_jobs(next[1], nV, failed, [&](int k) {                           // 2. coarsest level, photometric
             const int i = views[k];
             gpm_ctx* c = lc[top];
-            int rc = load_view(c, d, imgs[top].data(), ch, pitch[top], setup[top][i], *opts, *vsel);
+            int rc = load_view(c, d, imgs[top].data(), ch, pitch[top], setup[top][i], *opts, *vsel, *refine);
             if (rc == GPM_OK) rc = gpm_init(c);
             if (rc == GPM_OK) rc = timer.sweep(c, d->params.iterations, &sweep_ms[top][k]);
             float ms2 = 0.f, bms = 0.f;                                       // the photometric prior stage (§20)
@@ -792,7 +820,7 @@ static int ms_batch_run(const char* fn_name, const gpm_ms_batch_desc* m, const g
                 gpm_ctx* c = lc[l];
                 const bool restoring = restore && l == 0;
                 float ms = 0.f;
-                int rc = load_view(c, d, imgs[l].data(), ch, pitch[l], s, *opts, *vsel);
+                int rc = load_view(c, d, imgs[l].data(), ch, pitch[l], s, *opts, *vsel, *refine);
                 // restorer step 1 (§21): the photometric-only estimate, with the term off, in the view's context as loaded.
                 // The geometric stage below replaces the whole state (gpm_set_state), so the view is loaded once.  With one
                 // level this repeats the coarsest photometric stage when photo_iterations = params.iterations and there is
@@ -884,17 +912,24 @@ static int ms_batch_run(const char* fn_name, const gpm_ms_batch_desc* m, const g
 extern "C" int gpm_ms_batch_run(const gpm_ms_batch_desc* m, const gpm_job_opts* opts, const gpm_view_sel* vsel,
                                 gpm_ms_batch_stats* stats)
 {
-    return ms_batch_run("gpm_ms_batch_run", m, opts, vsel, nullptr, nullptr, stats);
+    return ms_batch_run("gpm_ms_batch_run", m, opts, vsel, nullptr, nullptr, nullptr, stats);
 }
 
 extern "C" int gpm_ms_batch_run_prior(const gpm_ms_batch_desc* m, const gpm_job_opts* opts, const gpm_view_sel* vsel,
                                       gpm_ms_prior_opts* prior, gpm_ms_batch_stats* stats)
 {
-    return ms_batch_run("gpm_ms_batch_run_prior", m, opts, vsel, prior, nullptr, stats);
+    return ms_batch_run("gpm_ms_batch_run_prior", m, opts, vsel, prior, nullptr, nullptr, stats);
 }
 
 extern "C" int gpm_ms_batch_run_restore(const gpm_ms_batch_desc* m, const gpm_job_opts* opts, const gpm_view_sel* vsel,
                                         gpm_ms_prior_opts* prior, const gpm_ms_restore_opts* restore, gpm_ms_batch_stats* stats)
 {
-    return ms_batch_run("gpm_ms_batch_run_restore", m, opts, vsel, prior, restore, stats);
+    return ms_batch_run("gpm_ms_batch_run_restore", m, opts, vsel, prior, restore, nullptr, stats);
+}
+
+extern "C" int gpm_ms_batch_run_refine(const gpm_ms_batch_desc* m, const gpm_job_opts* opts, const gpm_view_sel* vsel,
+                                       gpm_ms_prior_opts* prior, const gpm_ms_restore_opts* restore, const gpm_refine_opts* refine,
+                                       gpm_ms_batch_stats* stats)
+{
+    return ms_batch_run("gpm_ms_batch_run_refine", m, opts, vsel, prior, restore, refine, stats);
 }

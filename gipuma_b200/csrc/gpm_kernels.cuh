@@ -105,27 +105,31 @@ __host__ __device__ inline int jvs_floats(int V, bool geo) { return (geo ? 18 : 
 // ---- sweep modes: which combinations have kernels --------------------------------------------------------------------
 // A context's mode: colour images, the fused 20-neighbour sweep (option neighbours = 20), the geometric-consistency term
 // (§14), the NCC cost (§15), adaptive checkerboard sampling (§16), joint view selection (§17), the planar prior (§18) and
-// the per-pixel mask of the geometric term (§21).
+// the per-pixel mask of the geometric term (§21) and ACMH's refinement (§23).
 // Kernels are instantiated (gpm_api.cu, kernel tables) and setters accept a change (gpm_set_*) exactly for the modes
 // mode_conflict() passes.
 struct Mode {
-    bool color, fused, geo, ncc, adaptive, jvs, prior, geomask;
+    bool color, fused, geo, ncc, adaptive, jvs, prior, geomask, refine_acmh;
     __host__ __device__ constexpr int bits() const
     {
-        return color | fused << 1 | geo << 2 | ncc << 3 | adaptive << 4 | jvs << 5 | prior << 6 | geomask << 7;
+        return color | fused << 1 | geo << 2 | ncc << 3 | adaptive << 4 | jvs << 5 | prior << 6 | geomask << 7 | refine_acmh << 8;
     }
     __host__ __device__ static constexpr Mode of(int b)
     {
-        return Mode{bool(b & 1), bool(b & 2), bool(b & 4), bool(b & 8), bool(b & 16), bool(b & 32), bool(b & 64), bool(b & 128)};
+        return Mode{bool(b & 1), bool(b & 2), bool(b & 4), bool(b & 8), bool(b & 16), bool(b & 32), bool(b & 64), bool(b & 128),
+                    bool(b & 256)};
     }
 };
-constexpr int GPM_MODES = 256;
+constexpr int GPM_MODES = 512;
+// k_cost_eval and k_shard_stage never read refine_acmh (the highest bit): their tables cover the other eight bits
+constexpr int GPM_EVAL_MODES = 256;
 
-enum class ModeConflict { none, fused, jvs_needs_ncc_grey, ncc_colour, prior, geomask };
+enum class ModeConflict { none, fused, jvs_needs_ncc_grey, ncc_colour, prior, geomask, refine_fused };
 
 // The one rule: the fused sweep has none of the five modes; joint view selection needs the NCC cost (on grey images);
 // the NCC cost needs grey images; the planar prior needs grey images and excludes joint view selection; the geometric
-// term's mask needs the term and excludes the planar prior.  The first conflict found is the reason a refusal gives.
+// term's mask needs the term and excludes the planar prior; ACMH's refinement excludes the fused sweep.  The first
+// conflict found is the reason a refusal gives.
 __host__ __device__ constexpr ModeConflict mode_conflict(Mode m)
 {
     if (m.fused && (m.geo || m.ncc || m.adaptive || m.jvs || m.prior)) return ModeConflict::fused;
@@ -133,14 +137,82 @@ __host__ __device__ constexpr ModeConflict mode_conflict(Mode m)
     if (m.ncc && m.color) return ModeConflict::ncc_colour;
     if (m.prior && (m.color || m.jvs)) return ModeConflict::prior;
     if (m.geomask && (!m.geo || m.prior)) return ModeConflict::geomask;
+    if (m.refine_acmh && m.fused) return ModeConflict::refine_fused;
     return ModeConflict::none;
 }
 
-// The source-view shard (k_shard_stage) exchanges top-n lists of the 8-neighbour sweep's PM costs: no geometric term, NCC
-// cost, joint view selection, planar prior or fused sweep.
+// The source-view shard (k_shard_stage) exchanges top-n lists of the 8-neighbour sweep's PM costs, step by step of
+// Gipuma's refinement: no geometric term, NCC cost, joint view selection, planar prior, fused sweep or ACMH's refinement.
 __host__ __device__ constexpr bool shard_supports(Mode m)
 {
-    return mode_conflict(m) == ModeConflict::none && !m.geo && !m.ncc && !m.jvs && !m.prior && !m.fused;
+    return mode_conflict(m) == ModeConflict::none && !m.geo && !m.ncc && !m.jvs && !m.prior && !m.fused && !m.refine_acmh;
+}
+
+// ---- ACMH's refinement (Xu & Tao 2019; DESIGN.md §23) --------------------------------------------------------------------
+// What the REFINE_ACMH variants of k_sweep read besides KParams: the draws' key and the perturbation.  A kernel parameter of
+// its own, the last one, so that every other kernel parameter keeps its place.
+struct AcmhRefine {
+    unsigned seed;              // (uint32)seed ^ (uint32)(seed >> 32) of gpm_set_rng's 64-bit seed
+    unsigned counter;           // r: k_sweep launches with refinement since gpm_init / gpm_init_planes / gpm_set_rng
+    float eps;                  // perturbation, in (0, 1)
+};
+
+// lowbias32 (C. Wellons, hash-prospector; public domain): a 32-bit integer hash with a strong avalanche
+__host__ __device__ constexpr unsigned acmh_mix(unsigned x)
+{
+    x ^= x >> 16;  x *= 0x7feb352du;  x ^= x >> 15;  x *= 0x846ca68bu;  x ^= x >> 16;
+    return x;
+}
+// key of pixel i in launch r; draw k is acmh_mix(key ^ k), mapped to (0, 1] as xorwow_uniform maps its words
+__host__ __device__ constexpr unsigned acmh_key(unsigned seed, unsigned i, unsigned r) { return acmh_mix(acmh_mix(acmh_mix(seed) ^ i) ^ r); }
+__device__ __forceinline__ float acmh_draw(unsigned key, unsigned k)
+{
+    return ffma(__uint2float_rn(acmh_mix(key ^ k)), 2.3283064365386963e-10f, 1.1641532182693481e-10f);
+}
+
+// Candidate j (0..4) of the refinement of the plane `n` at pixel (px, py): (d_r, n), (d, n_r), (d_r, n_r), (d, n_t), (d_t, n).
+// d is n's depth at p (prior_depth); draws 0 (d_t), 1..3 (n_t), 4 (d_r), 5, 6, ... (n_r, Marsaglia pairs).  Every operation
+// is an IEEE float32 one (no approximate reciprocal or square root), so oracle/pyrefine.py restates it bit for bit.
+__device__ __forceinline__ float4 acmh_candidate(const KParams& P, const AcmhRefine& F, unsigned key, const float4& n, int j, float fpx,
+                                                 float fpy)
+{
+    const RefCam& c = P.ref;
+    const float d = prior_depth(c, n.x, n.y, n.z, n.w, fpx, fpy);
+    // the ray through p, view_vector's formula without the normalisation: a normal faces the camera where n . ray <= 0
+    const float a = fsub(fpx, c.P34[0]), b = fsub(fpy, c.P34[1]), e = fsub(1.0f, c.P34[2]);
+    const float* M = c.M_inv;
+    const float vx = fsub(ffma(e, M[2], ffma(a, M[0], fmul(b, M[1]))), c.C[0]);
+    const float vy = fsub(ffma(e, M[5], ffma(a, M[3], fmul(b, M[4]))), c.C[1]);
+    const float vz = fsub(ffma(e, M[8], ffma(a, M[6], fmul(b, M[7]))), c.C[2]);
+    float nx = n.x, ny = n.y, nz = n.z, depth = d;
+    if (j == 0 || j == 2) {                         // d_r: uniform in disparity, as k_init_planes draws
+        const float disp = ffma(fsub(P.max_disp, P.min_disp), acmh_draw(key, 4u), P.min_disp);
+        depth = __fdiv_rn(fmul(c.f_cam, c.baseline), disp);
+    } else if (j == 4) {                            // d_t
+        const float s = ffma(acmh_draw(key, 0u), 2.0f, -1.0f);
+        depth = fmin_(c.depthMax, fmax_(c.depthMin, fmul(d, ffma(F.eps, s, 1.0f))));
+    }
+    if (j == 1 || j == 2) {                         // n_r: Marsaglia's sphere sampler
+        unsigned k = 5u;
+        float u, v, sum;
+        do {
+            u = ffma(acmh_draw(key, k), 2.0f, -1.0f);
+            v = ffma(acmh_draw(key, k + 1u), 2.0f, -1.0f);
+            k += 2u;
+            sum = ffma(u, u, fmul(v, v));
+        } while (sum >= 1.0f);
+        const float sq = __fsqrt_rn(fsub(1.0f, sum));
+        nx = fmul(fadd(u, u), sq);  ny = fmul(fadd(v, v), sq);  nz = fsub(1.0f, fadd(sum, sum));
+    } else if (j == 3) {                            // n_t: n + U(-eps pi, eps pi) per component, normalised
+        const float dn = fmul(F.eps, 3.14159274f), two = fadd(dn, dn);
+        const float tx = fadd(n.x, ffma(acmh_draw(key, 1u), two, -dn));
+        const float ty = fadd(n.y, ffma(acmh_draw(key, 2u), two, -dn));
+        const float tz = fadd(n.z, ffma(acmh_draw(key, 3u), two, -dn));
+        const float rs = __fdiv_rn(1.0f, __fsqrt_rn(ffma(tz, tz, ffma(tx, tx, fmul(ty, ty)))));
+        nx = fmul(tx, rs);  ny = fmul(ty, rs);  nz = fmul(tz, rs);
+    }
+    if ((j == 1 || j == 2 || j == 3) && dot3(nx, ny, nz, vx, vy, vz) > 0.0f) { nx = -nx;  ny = -ny;  nz = -nz; }
+    return make_float4(nx, ny, nz, plane_d(c, nx, ny, nz, fpx, fpy, depth));
 }
 
 // GEOMASK variants (§21): whether the geometric term is on at the pixel `at` — off where the mask byte is nonzero.  The mask
@@ -349,8 +421,9 @@ __device__ __forceinline__ bool sweep_neighbour(int k, const int& px, const int&
 // each such plane q is offered to q +- (0, 1), q +- (0, 5) (its column group) and q +- (1, 0), q +- (5, 0) (its row group).
 // The four windows of a group lie on one stride-2 lattice, and a sample's dissimilarity against view v is a function of the
 // plane, the view and the sample's absolute texel alone (the propagation sites all use rounding variant 1), so one warp
-// fetches each lattice texel of a group once and runs every target pixel's own chain over it.
-__host__ __device__ constexpr bool shares_samples(Mode m) { return m.bits() == 0; }
+// fetches each lattice texel of a group once and runs every target pixel's own chain over it.  The pass serves either
+// refinement (§23): it only changes how the propagation pass gets its costs, and the refinement follows it unchanged.
+__host__ __device__ constexpr bool shares_samples(Mode m) { return (m.bits() & (GPM_EVAL_MODES - 1)) == 0; }
 
 // Per-warp layout of the plane-major pass, in floats from the warp's scratch (which it overlays: the pass ends before the
 // per-pixel loop starts).  L texels of the union lattice (nside x (nside + 5)); A/left/pos: per fetched texel in fetch order,
@@ -615,13 +688,14 @@ __device__ __forceinline__ void share_costs(const KParams& P, const float* __res
 // sum_j w_j = 0; (5) the fold starts at the current plane's re-scored cost.  Weighted costs are not a pure function of the
 // plane, so neither memo nor the duplicate-of-current skip is used, and the stored cost is tagged GPM_PROV_JVS.  The
 // refinement restates k_sweep's loop body line for line (see shard_refine_candidate).
-template <bool GEO, bool ADAPTIVE>
+// REFINE_ACMH: ACMH's five candidates (§23) instead of Gipuma's steps, scored with the same weights.
+template <bool GEO, bool ADAPTIVE, bool REFINE_ACMH = false>
 __device__ __forceinline__ void jvs_pixel(const KParams& P, const JvsParams& J, const GeoParams* g, const float* __restrict__ sCam,
                                           const float* __restrict__ tile, const WarpScratch& ws, float* __restrict__ jv,
                                           cudaTextureObject_t src, float4* __restrict__ planes, float* __restrict__ cost,
                                           unsigned* __restrict__ rng_state, unsigned char* __restrict__ prov, const Memo& M,
                                           int px, int py, int tile_x0, int tile_y0, int phase_mask, unsigned lane, WarpStats& st,
-                                          bool geo_on = true)
+                                          bool geo_on, const AcmhRefine F)
 {
     const RefCam& cam = P.ref;
     const bool with_geo = GEO && geo_on;            // false at a pixel the geometric term's mask marks (§21)
@@ -728,7 +802,25 @@ __device__ __forceinline__ void jvs_pixel(const KParams& P, const JvsParams& J, 
         const unsigned id = __shfl_sync(GPM_FULL, mine_id, k);
         if (c < cost_now) { norm_now = nb;  cost_now = c;  disp_now = d;  own_id = id; }      // a copy keeps its identity
     }
-    if (phase_mask & 4) {                            // planeRefinement_cu, gipuma.cu:928-994, scored with the same weights
+    if constexpr (REFINE_ACMH) {
+        if (phase_mask & 4) {
+            bool any_accept = false;
+            const float4 start = norm_now;
+            const unsigned key = acmh_key(F.seed, (unsigned)center, F.counter);
+            for (int j = 0; j < 5; j++) {
+                const float4 cand = acmh_candidate(P, F, key, start, j, fpx, fpy);
+                eval_row(cand.x, cand.y, cand.z, cand.w, 8);
+                __syncwarp();
+                const float c = score(8);
+                if (c < cost_now) { any_accept = true;  cost_now = c;  norm_now = cand; }
+            }
+            if (any_accept) {                                 // a new plane: one fresh identity
+                unsigned fresh = 0u;
+                if (lane == 0) fresh = atomicAdd(M.next_id, 1u);
+                own_id = __shfl_sync(GPM_FULL, fresh, 0);
+            }
+        }
+    } else if (phase_mask & 4) {                     // planeRefinement_cu, gipuma.cu:928-994, scored with the same weights
         bool any_accept = false;
         Xorwow r = {0u, 0u, 0u, 0u, 0u, 0u};
         if (P.rng_mode == 1) {
@@ -792,16 +884,18 @@ __device__ __forceinline__ void jvs_pixel(const KParams& P, const JvsParams& J, 
 // selection (§17; NCC only), every pixel goes through jvs_pixel; J is only read in those variants.  PRIOR: every
 // hypothesis' cost carries the planar prior's term (§18; grey, no joint view selection); R is only read there.  GEOMASK
 // (with GEO, without PRIOR): every hypothesis of a pixel R.geo_mask marks costs what it costs without the term (§21).
+// REFINE_ACMH (not FUSED): the refinement tries ACMH's five candidates (§23) instead of Gipuma's steps; F is only read there.
 template <bool COLOR, bool FUSED, bool GEO = false, bool NCC = false, bool ADAPTIVE = false, bool JVS = false, bool PRIOR = false,
-          bool GEOMASK = false>
+          bool GEOMASK = false, bool REFINE_ACMH = false>
 __global__ void __launch_bounds__(GPM_LB_THREADS, GPM_LB_BLOCKS)
 k_sweep(const __grid_constant__ KParams P, const __grid_constant__ CUtensorMap tmap, const ViewCam* __restrict__ cams,
         cudaTextureObject_t src, float4* __restrict__ planes, float* __restrict__ cost,
         unsigned* __restrict__ rng_state, unsigned char* __restrict__ prov, Memo M, int colour, int phase_mask,
-        unsigned long long* __restrict__ stats, const __grid_constant__ GeoParams G, const JvsParams J, const PriorParams R)
+        unsigned long long* __restrict__ stats, const __grid_constant__ GeoParams G, const JvsParams J, const PriorParams R,
+        const AcmhRefine F)
 {
-    static_assert(mode_conflict(Mode{COLOR, FUSED, GEO, NCC, ADAPTIVE, JVS, PRIOR, GEOMASK}) == ModeConflict::none, "no such sweep mode (mode_conflict)");
-    constexpr bool SHARE = shares_samples(Mode{COLOR, FUSED, GEO, NCC, ADAPTIVE, JVS, PRIOR, GEOMASK});
+    static_assert(mode_conflict(Mode{COLOR, FUSED, GEO, NCC, ADAPTIVE, JVS, PRIOR, GEOMASK, REFINE_ACMH}) == ModeConflict::none, "no such sweep mode (mode_conflict)");
+    constexpr bool SHARE = shares_samples(Mode{COLOR, FUSED, GEO, NCC, ADAPTIVE, JVS, PRIOR, GEOMASK, REFINE_ACMH});
     const GeoParams* g = (GEO || NCC) ? &G : nullptr;
     extern __shared__ __align__(128) float smem[];
     float* tile = smem;
@@ -842,9 +936,9 @@ k_sweep(const __grid_constant__ KParams P, const __grid_constant__ CUtensorMap t
         colour_pixel(idx, colour, px, py);
         if constexpr (JVS) {
             if (px < W && py < H)
-                jvs_pixel<GEO, ADAPTIVE>(P, J, g, sCam, tile, ws, warp_base + warp_scratch_floats(P.ns_pad, P.V, P.color, NCC), src, planes,
-                                         cost, rng_state, prov, M, px, py, tile_x0, tile_y0, phase_mask, lane, st,
-                                         geo_at<GEOMASK>(R, (size_t)py * W + px));
+                jvs_pixel<GEO, ADAPTIVE, REFINE_ACMH>(P, J, g, sCam, tile, ws, warp_base + warp_scratch_floats(P.ns_pad, P.V, P.color, NCC), src,
+                                                      planes, cost, rng_state, prov, M, px, py, tile_x0, tile_y0, phase_mask, lane, st,
+                                                      geo_at<GEOMASK>(R, (size_t)py * W + px), F);
         } else if (px < W && py < H) {
             const size_t center = (size_t)py * W + px;
             bool window_ready = false;          // the per-pixel window data is only built if something gets evaluated
@@ -956,15 +1050,40 @@ k_sweep(const __grid_constant__ KParams P, const __grid_constant__ CUtensorMap t
             unsigned new_mask = mmask | (cand_mask & NCMASK);
             // The refinement candidates are a pure function of (pixel, plane at refinement start) in GPM_RNG_REFERENCE
             // mode (zero-state stream; disp_now == plane_depth(norm_now) here), so a refinement that rejected all its steps
-            // from exactly this plane before would reject them again.
+            // from exactly this plane before would reject them again.  ACMH's candidates also depend on the launch counter:
+            // that refinement neither reads nor writes this memo (§23).
             bool refine = (phase_mask & 4) != 0;
-            if (refine && P.memo && P.rng_mode == 0 && (mmask & GPM_MEMO_REFINE)) {
+            if (!REFINE_ACMH && refine && P.memo && P.rng_mode == 0 && (mmask & GPM_MEMO_REFINE)) {
                 if (M.refseen[center] == own_id) {
                     refine = false;
                     st.skip += 3;
                 }
             }
-            if (refine) {
+            if (REFINE_ACMH && refine) {
+                if (!window_ready) { setup_window<COLOR, NCC>(P, tile + P.tile_xo, ws, px, py, tile_x0, tile_y0, lane);  window_ready = true; }
+                bool any_accept = false;
+                const unsigned rsite = NCC ? GPM_PROV_NCC : 0u;
+                const float4 start = norm_now;
+                const unsigned key = acmh_key(F.seed, (unsigned)center, F.counter);
+                for (int j = 0; j < 5; j++) {               // in order, strict <, as the propagation (gipuma.cu:986-990)
+                    const float4 cand = acmh_candidate(P, F, key, start, j, fpx, fpy);
+                    float pr = 0.0f;
+                    if constexpr (PRIOR) pr = pp.of(P, R, cand, fpx, fpy);
+                    const float c = eval_plane<0, COLOR, GEO, NCC, false, PRIOR>(P, sCam, ws, src, cand.x, cand.y, cand.z, cand.w, cost_now, lane,
+                                                                                 st, nullptr, nullptr, 0u, g, fpx, fpy, pr, gon);
+                    if (c < cost_now) {
+                        prov_now = (int)rsite;
+                        any_accept = true;
+                        cost_now = c;
+                        norm_now = cand;
+                    }
+                }
+                if (any_accept) {                                 // a new plane: one fresh identity for the pixel's final plane
+                    unsigned fresh = 0u;
+                    if (lane == 0) fresh = atomicAdd(M.next_id, 1u);
+                    own_id = __shfl_sync(GPM_FULL, fresh, 0);
+                }
+            } else if (refine) {
                 if (!window_ready) { setup_window<COLOR, NCC>(P, tile + P.tile_xo, ws, px, py, tile_x0, tile_y0, lane);  window_ready = true; }
                 const unsigned id_start = own_id;
                 bool any_accept = false;

@@ -89,17 +89,20 @@ int gpm_set_view_color(gpm_ctx* ctx, int v, const float* rgba, size_t pitch_byte
 int gpm_set_num_views(gpm_ctx* ctx, int n_views);
 
 /* ---- mode compatibility -------------------------------------------------------------------------------------------------
- * A context sweeps in one mode of eight fields: colour images (fixed by the first image upload), the fused 20-neighbour
+ * A context sweeps in one mode of nine fields: colour images (fixed by the first image upload), the fused 20-neighbour
  * sweep (option "neighbours" = 20), the geometric-consistency term, the NCC cost, adaptive sampling, joint view selection,
- * the planar prior (DESIGN.md §14–§18) and the geometric term's per-pixel mask (§21; it counts while the term is on).
+ * the planar prior (DESIGN.md §14–§18), the geometric term's per-pixel mask (§21; it counts while the term is on) and
+ * ACMH's refinement (§23).
  * Every combination exists except:
  *   - the fused sweep with the geometric term, the NCC cost, adaptive sampling, joint view selection or the planar prior;
  *   - joint view selection without the NCC cost, and so with colour images;
  *   - the NCC cost with colour images;
  *   - the planar prior with colour images or with joint view selection;
- *   - a geometric term's mask with the planar prior (whether the term is on or not).
+ *   - a geometric term's mask with the planar prior (whether the term is on or not);
+ *   - ACMH's refinement with the fused sweep.
  * A call that would make one of these is refused and changes nothing.  gpm_set_geometric, gpm_set_photometric,
- * gpm_set_propagation, gpm_set_view_selection, gpm_set_prior, gpm_set_geo_mask and gpm_set_option("neighbours") return
+ * gpm_set_propagation, gpm_set_view_selection, gpm_set_prior, gpm_set_geo_mask, gpm_set_refinement and
+ * gpm_set_option("neighbours") return
  * GPM_E_ARG, whichever of the two fields is set last.  A colour image upload (gpm_set_reference_color, gpm_set_view_color) returns GPM_E_ARG
  * while joint view selection or the planar prior is on and GPM_E_STATE while only the NCC cost is.  The batch drivers
  * refuse the same combinations of their job options and image type with GPM_E_ARG before any CUDA call.
@@ -107,7 +110,8 @@ int gpm_set_num_views(gpm_ctx* ctx, int n_views);
  * is on, every
  * gpm_shard_* call taking a context returns GPM_E_STATE (gpm_shard_num_stages and gpm_shard_stage_floats return -1), and
  * gpm_set_geometric refuses to turn the term on with GPM_E_STATE once a shard communicator is set.  gpm_shard_stage,
- * gpm_shard_finish_init and gpm_shard_run refuse the fused sweep with GPM_E_ARG. */
+ * gpm_shard_finish_init and gpm_shard_run refuse the fused sweep with GPM_E_ARG.  The shard exchanges Gipuma's refinement
+ * steps one by one: while ACMH's refinement is on, every gpm_shard_* call taking a context returns GPM_E_STATE as well. */
 
 /* ---- geometric consistency (DESIGN.md §14) ----------------------------------------------------------------------------
  * A second PatchMatch pass may score each hypothesis against the source views' own depth maps as well: with weight > 0 the
@@ -186,6 +190,22 @@ int gpm_set_view_selection(gpm_ctx* ctx, const gpm_view_sel* vsel);
 /* The selected-views mask of every pixel ([height*width], bit j = view j), host memory; all zero before the first JOINT
  * launch. */
 int gpm_get_view_masks(gpm_ctx* ctx, unsigned long long* masks);
+
+/* ---- refinement (DESIGN.md §23) ----------------------------------------------------------------------------------------
+ * GPM_REFINE_GIPUMA (the default) refines each pixel with Gipuma's steps of shrinking random offsets (gipuma.cu:928-994),
+ * drawn as gpm_set_rng's mode says.  GPM_REFINE_ACMH is the multi-hypothesis refinement of ACMH (Xu & Tao, CVPR 2019): from
+ * the pixel's plane (n, depth d at the pixel) at the start of its refinement it tries, in this order, (d_r, n), (d, n_r),
+ * (d_r, n_r), (d, n_t), (d_t, n), each accepted when its cost is strictly below the running cost: d_r uniform in disparity
+ * on [min_disparity, max_disparity], n_r a uniform camera-facing unit normal, d_t = clamp(d (1 + perturbation U(-1, 1)),
+ * depthMin, depthMax), n_t = n + perturbation * pi * U(-1, 1) per component, normalised and facing the camera.  Its draws
+ * are a stateless hash of (gpm_set_rng's seed, pixel, launch counter, draw index), the same in both RNG modes; the launch
+ * counter counts the gpm_sweep / gpm_phase launches with refinement since gpm_init, gpm_init_planes or gpm_set_rng.  Every
+ * cost mode, grey or colour, and both propagation modes; not the fused sweep or the source-view shard.  A switch marks
+ * nothing stale: only the candidates change.
+ * Refused with GPM_E_ARG: an unknown kind, a perturbation not finite or outside (0, 1).  Other modes: "mode
+ * compatibility".  A refused call changes nothing. */
+enum { GPM_REFINE_GIPUMA = 0, GPM_REFINE_ACMH = 1 };
+int gpm_set_refinement(gpm_ctx* ctx, int kind, float perturbation);
 
 /* Seed of the per-pixel curand_init(seed, y, x) at initialisation (gipuma.cu:1019; the reference uses
  * clock64()) and the refinement RNG mode. */
@@ -668,6 +688,24 @@ typedef struct gpm_ms_restore_opts {
 } gpm_ms_restore_opts;
 int gpm_ms_batch_run_restore(const gpm_ms_batch_desc* desc, const gpm_job_opts* opts, const gpm_view_sel* vsel,
                              gpm_ms_prior_opts* prior, const gpm_ms_restore_opts* restore, gpm_ms_batch_stats* stats);
+
+/* ---- the batch drivers' refinement (DESIGN.md §23) ----------------------------------------------------------------------
+ * Each _refine entry is the newest entry of its family with gpm_set_refinement(kind, perturbation) in every job's setup,
+ * so that every sweep of the job uses it: both passes of the geometric driver, and every level and every stage
+ * (photometric, geometric, prior and restorer sweeps) of the multi-level one.  refine NULL is Gipuma's refinement:
+ * gpm_batch_run_prior, gpm_geo_batch_run_prior and gpm_ms_batch_run_restore are these with NULL.  Refused with GPM_E_ARG
+ * before any CUDA call, besides what those refuse: what gpm_set_refinement refuses of its arguments. */
+typedef struct gpm_refine_opts {
+    int   kind;                        /* GPM_REFINE_GIPUMA or GPM_REFINE_ACMH */
+    float perturbation;                /* in (0, 1); ACMH: 0.02 */
+} gpm_refine_opts;
+int gpm_batch_run_refine(const gpm_batch_desc* desc, const gpm_job_opts* opts, const gpm_view_sel* vsel, const gpm_prior_opts* prior,
+                         const gpm_refine_opts* refine, gpm_batch_stats* stats);
+int gpm_geo_batch_run_refine(const gpm_geo_batch_desc* desc, const gpm_job_opts* opts, const gpm_view_sel* vsel,
+                             const gpm_prior_opts* prior, const gpm_refine_opts* refine, gpm_geo_batch_stats* stats);
+int gpm_ms_batch_run_refine(const gpm_ms_batch_desc* desc, const gpm_job_opts* opts, const gpm_view_sel* vsel,
+                            gpm_ms_prior_opts* prior, const gpm_ms_restore_opts* restore, const gpm_refine_opts* refine,
+                            gpm_ms_batch_stats* stats);
 
 #ifdef __cplusplus
 }
