@@ -237,3 +237,42 @@ def accept(planes, cost, cand, cand_cost, where):
         cost = np.where(take, cand_cost[j], cost).astype(np.float32)
         changed |= take
     return planes, cost, changed
+
+
+# ---- under joint view selection (jvs_pixel<..., REFINE_ACMH> in gpm_kernels.cuh) -----------------------------------------
+# The refinement follows the launch's propagation fold in the same pixel and reuses its view weights w, which the launch's
+# candidates in E decided (oracle/pyjvs.py; E is empty in a launch without propagation bits, so w then holds w_keep for
+# the remembered views and 0 for the others).  Each of the five candidates of the plane the fold ended with is scored
+# sum_j w_j c_j / sum_j w_j over its own per-view row (the kernel's row 8), or by the combination rule where sum_j w_j = 0,
+# and accepted in candidate order with strict <.  The new selected-views mask is the propagation's, {j : w_j > 0}.
+
+def jvs_accept(w, planes, cost, cand, cand_rows, cand_fallback, where):
+    """The refinement's accept under joint view selection.  w [H, W, V]: the launch's weights; planes, cost: the state
+    after the launch's fold; cand [5, H, W, 4]; cand_rows [5, H, W, V] float32: each candidate's per-view costs (NCC, plus
+    the geometric term where it is on); cand_fallback [5, H, W]: the combination rule's cost of each candidate.  Returns
+    (planes, cost, changed) as accept()."""
+    from oracle import pyjvs
+    costs = [pyjvs.weighted(w, cand_rows[j], cand_fallback[j]) for j in range(len(cand))]
+    return accept(planes, cost, cand, costs, where)
+
+
+def jvs_expected(planes, cost, masks, colour, mask, rows_of, fallback_of, ref_cam, cam, min_disp, max_disp, depth_min,
+                 depth_max, eps, seed, r, params, t, adaptive=False):
+    """State after one joint-view-selection launch with ACMH's refinement (mask bits 0 / 1 / 2: close / far / refine, as
+    gpm_phase takes them) of checkerboard colour `colour`: oracle.pyjvs.expected's propagation, then, with bit 2, the
+    refinement of launch r (the context's refinement counter).  rows_of, fallback_of, ref_cam, params and t as
+    pyjvs.expected takes them; cam the reference camera as a gpm_camera (api.pack_camera).  Returns (planes, cost, masks,
+    ambiguous, refined), refined marking the pixels that took a refinement candidate."""
+    from oracle import pyjvs
+    det = {}
+    p, c, m, amb = pyjvs.expected(planes, cost, masks, colour, mask & 3, rows_of, fallback_of, ref_cam, depth_min, depth_max,
+                                  params, t, adaptive=adaptive, details=det)
+    refined = np.zeros(c.shape, bool)
+    if mask & 4:
+        H, W = c.shape
+        ys, xs = np.mgrid[0:H, 0:W]
+        cand = candidates(p, cam, min_disp, max_disp, depth_min, depth_max, eps, seed, r)
+        rows = np.stack([rows_of(np.ascontiguousarray(cand[j]))[1] for j in range(len(cand))])
+        fb = np.stack([fallback_of(np.ascontiguousarray(cand[j])) for j in range(len(cand))])
+        p, c, refined = jvs_accept(det["w"], p, c, cand, rows, fb, ((xs + ys) & 1) == colour)
+    return p, c, m, amb, refined

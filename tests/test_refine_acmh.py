@@ -195,6 +195,84 @@ def test_accept_is_in_order_and_strict():
     assert changed.tolist() == [[True, True, False, False]]
 
 
+def test_jvs_accept_scores_with_the_launch_weights():
+    """Under joint view selection each candidate costs sum w c / sum w over its own row (the combination rule's cost
+    where sum w = 0), accepted in order with strict <: a tie keeps the running plane, a NaN anywhere in a row (0 * NaN is
+    NaN) rejects the candidate, a NaN running cost accepts nothing, and pixels outside `where` keep their state."""
+    from oracle import pyrefine as R
+    V = 3
+    w = np.array([[[0.5, 0.0, 0.5], [0.5, 0.0, 0.5], [0.0, 0.0, 0.0], [0.5, 0.0, 0.5], [0.5, 0.5, 0.5], [0.5, 0.0, 0.5]]], f32)
+    cost = np.array([[1.0, 1.0, 1.0, np.nan, 1.0, 1.0]], f32)
+    planes = np.zeros((1, 6, 4), f32)
+    cand = np.stack([np.full((1, 6, 4), j + 1, f32) for j in range(5)])
+    rows = np.full((5, 1, 6, V), 3.0, f32)
+    fb = np.full((5, 1, 6), 3.0, f32)
+    # pixel 0: candidate 1 ties the running cost (0.5 * 1 + 0.5 * 1) / 1 = 1, candidate 3 is strictly below, 4 ties it
+    rows[1, 0, 0] = [1.0, 9.0, 1.0]
+    rows[3, 0, 0] = [0.5, 9.0, 0.25]
+    rows[4, 0, 0] = [0.25, 9.0, 0.5]
+    # pixel 1: NaN in the unweighted view of candidate 0 rejects it; candidate 2 wins
+    rows[0, 0, 1] = [0.0, np.nan, 0.0]
+    rows[2, 0, 1] = [0.5, 0.0, 0.5]
+    # pixel 2: no weight, so the fallback decides: candidate 4's 0.25
+    fb[4, 0, 2] = 0.25
+    rows[0, 0, 2] = 0.0                                        # a row the weights ignore
+    # pixel 3: NaN running cost; pixel 4: outside `where`; pixel 5: nothing below 1
+    rows[:, 0, 3] = 0.0
+    rows[:, 0, 4] = 0.0
+    where = np.array([[True, True, True, True, False, True]])
+    p, c, changed = R.jvs_accept(w, planes, cost, cand, rows, fb, where)
+    assert c[0, 0] == f32(0.375) and p[0, 0, 0] == 4.0          # 0.5 * 0.5 + 0.5 * 0.25 = 0.375, the tie of 4 rejected
+    assert c[0, 1] == f32(0.5) and p[0, 1, 0] == 3.0
+    assert c[0, 2] == f32(0.25) and p[0, 2, 0] == 5.0
+    assert np.isnan(c[0, 3]) and c[0, 4] == 1.0 and c[0, 5] == 1.0
+    assert changed.tolist() == [[True, True, True, False, False, False]]
+    assert not p[0, 3:].any()
+
+
+def test_jvs_expected_refinement_alone_keeps_remembered_views():
+    """A launch of the refinement alone (mask 4) offers no candidate, so E is empty: every remembered view weighs w_keep,
+    the others 0, the new masks equal the remembered ones at the launch's colour, and the five candidates are scored with
+    those weights from the start plane; a pixel with no remembered view falls back to the combination rule."""
+    from oracle import pyjvs, pyrefine as R
+    sc, cam = _scene()
+    H, W, V = sc.rows, sc.cols, 3
+    rng = np.random.default_rng(17)
+    planes = _start_planes(sc, cam, rng)
+    masks = rng.integers(0, 8, (H, W)).astype(np.uint64)
+    ys, xs = np.mgrid[0:H, 0:W]
+
+    def rows_of(pl):                                           # a deterministic per-view cost of each plane
+        b = pl.view(np.uint32).astype(np.uint64).sum(axis=-1)
+        m = np.stack([((b * (2 * j + 3)) % 1009).astype(f32) / f32(500.0) for j in range(V)], axis=-1).astype(f32)
+        return m, m
+
+    def fallback_of(pl):
+        return rows_of(pl)[0].mean(axis=-1).astype(f32)
+    cost = pyjvs.weighted(pyjvs.weights(np.zeros((0, H, W, V), f32), np.zeros((0, H, W), bool), pyjvs.mask_bits(masks, V),
+                                        {}, 1), rows_of(planes)[1], fallback_of(planes))
+    prm = sc.params
+    for colour in (0, 1):
+        mine = ((xs + ys) & 1) == colour
+        args = (rows_of, fallback_of, sc.cameras[0], cam, prm.min_disparity, prm.max_disparity, prm.depthMin, prm.depthMax,
+                0.02, 99, 5, {}, 1)
+        p, c, m, amb, refined = R.jvs_expected(planes, cost, masks, colour, 4, *args)
+        assert not amb.any() and np.array_equal(m, masks)
+        w = np.where(pyjvs.mask_bits(masks, V), f32(pyjvs.DEFAULTS["w_keep"]), f32(0.0)).astype(f32)
+        cand = R.candidates(planes, cam, prm.min_disparity, prm.max_disparity, prm.depthMin, prm.depthMax, 0.02, 99, 5)
+        want_c = cost.copy()
+        want_p = planes.copy()
+        for j in range(5):
+            cj = pyjvs.weighted(w, rows_of(cand[j])[1], fallback_of(cand[j]))
+            take = mine & (cj < want_c)
+            want_c = np.where(take, cj, want_c)
+            want_p = np.where(take[..., None], cand[j], want_p)
+        assert np.array_equal(p.view(np.uint32), want_p.view(np.uint32)) and np.array_equal(c.view(np.uint32), want_c.view(np.uint32))
+        assert refined.any() and not refined[~mine].any() and (masks == 0).any()
+        # the other colour is untouched
+        assert np.array_equal(p[~mine].view(np.uint32), planes[~mine].view(np.uint32))
+
+
 def test_struct_layout_matches_ctypes(tmp_path):
     from gipuma_b200 import api
     fields = ["kind", "perturbation"]
