@@ -144,6 +144,28 @@ class GpmNnResult(C.Structure):
                 ("cell_size", C.c_float), ("n_cells", C.c_longlong)]
 
 
+class GpmTsdfDesc(C.Structure):
+    _fields_ = [("n_views", C.c_int), ("width", C.c_int), ("height", C.c_int), ("depth", C.c_void_p), ("on_device", C.c_int),
+                ("P", C.POINTER(C.c_double)), ("cam_scale", C.c_double), ("depth_min", C.c_float), ("depth_max", C.c_float),
+                ("origin", C.c_float * 3), ("voxel", C.c_float), ("dims", C.c_int * 3), ("trunc", C.c_float),
+                ("device", C.c_int)]
+
+
+class GpmTsdfResult(C.Structure):
+    _fields_ = [("D", C.c_void_p), ("weight", C.c_void_p), ("upload_ms", C.c_float), ("integrate_ms", C.c_float)]
+
+
+class GpmMeshDesc(C.Structure):
+    _fields_ = [("D", C.c_void_p), ("weight", C.c_void_p), ("on_device", C.c_int), ("origin", C.c_float * 3),
+                ("voxel", C.c_float), ("dims", C.c_int * 3), ("min_weight", C.c_int), ("device", C.c_int)]
+
+
+class GpmMeshResult(C.Structure):
+    _fields_ = [("n_vertices", C.c_longlong), ("n_faces", C.c_longlong), ("vertex_capacity", C.c_longlong),
+                ("face_capacity", C.c_longlong), ("vertices", C.c_void_p), ("faces", C.c_void_p),
+                ("upload_ms", C.c_float), ("extract_ms", C.c_float)]
+
+
 # one vertex of the fused point cloud: the packed 27-byte record of storePlyFileBinary (displayUtils.h:84-142)
 PLY_VERTEX = np.dtype([("x", "<f4"), ("y", "<f4"), ("z", "<f4"), ("nx", "<f4"), ("ny", "<f4"), ("nz", "<f4"),
                        ("red", "u1"), ("green", "u1"), ("blue", "u1")])
@@ -255,6 +277,9 @@ def load_library():
     L.gpm_fuse_with_rule.argtypes = [C.POINTER(GpmFuseDesc), C.POINTER(GpmFuseRule), C.POINTER(GpmFuseResult)]
     L.gpm_write_ply.argtypes = [C.c_char_p, vp, C.c_longlong]
     L.gpm_nearest_dist.argtypes = [C.POINTER(GpmNnDesc), C.POINTER(GpmNnResult)]
+    L.gpm_tsdf_integrate.argtypes = [C.POINTER(GpmTsdfDesc), C.POINTER(GpmTsdfResult)]
+    L.gpm_mesh_extract.argtypes = [C.POINTER(GpmMeshDesc), C.POINTER(GpmMeshResult)]
+    L.gpm_write_ply_mesh.argtypes = [C.c_char_p, vp, C.c_longlong, vp, C.c_longlong]
     for name in ("gpm_create", "gpm_set_params", "gpm_set_reference", "gpm_set_view", "gpm_set_reference_color",
                  "gpm_set_view_color", "gpm_set_num_views", "gpm_set_view_depth", "gpm_set_geometric", "gpm_set_photometric",
                  "gpm_set_propagation", "gpm_set_view_selection", "gpm_get_view_masks", "gpm_set_rng", "gpm_set_state", "gpm_get_state", "gpm_init", "gpm_sweep", "gpm_phase",
@@ -268,7 +293,8 @@ def load_library():
                  "gpm_ms_batch_run_restore", "gpm_set_geo_mask", "gpm_set_refinement", "gpm_batch_run_refine",
                  "gpm_geo_batch_run_refine", "gpm_ms_batch_run_refine",
                  "gpm_prepare_cameras", "gpm_select_views", "gpm_write_dmb", "gpm_read_dmb", "gpm_write_result_dmb",
-                 "gpm_fuse_cameras", "gpm_fuse", "gpm_fuse_with_rule", "gpm_write_ply", "gpm_nearest_dist"):
+                 "gpm_fuse_cameras", "gpm_fuse", "gpm_fuse_with_rule", "gpm_write_ply", "gpm_nearest_dist",
+                 "gpm_tsdf_integrate", "gpm_mesh_extract", "gpm_write_ply_mesh"):
         getattr(L, name).restype = C.c_int
     _lib = L
     return L
@@ -1466,3 +1492,215 @@ def evaluate_cloud(rec, gt, max_dist: float = 20.0, taus=(0.5, 1.0, 2.0)) -> dic
     out = cloud_scores(host[0], host[1], max_dist, taus)
     out["accuracy_timing"], out["completeness_timing"] = t_rec, t_gt
     return out
+
+
+# ---- meshing (gpm_tsdf_integrate, gpm_mesh_extract; DESIGN.md §24) ------------------------------------------------------
+
+# Truncation in voxels and minimum number of views per lattice point: measured with tools/mesh_bench.py on an H100 (DESIGN.md
+# §24), the best mean F-score at 0.5 unit over the smooth scene's three PM runs at a voxel of 1 unit (the only part of the
+# sweep measured so far).
+MESH_DEFAULTS = {"trunc_voxels": 3.0, "min_weight": 3}
+MESH_MAX_DIM = 2048                                               # GPM_MESH_MAX_DIM
+GPM_FUSE_MAX_VIEWS = 256
+_INT_MAX = 2 ** 31 - 1
+
+
+def _f32(x) -> float:
+    return C.c_float(float(x)).value                              # the float the C-ABI receives
+
+
+def _check_box(origin, voxel, dims):
+    """The box rules of gpm_tsdf_integrate and gpm_mesh_extract; returns (origin floats, voxel, (nx, ny, nz))."""
+    o = [float(x) for x in origin]
+    if len(o) != 3 or not all(np.isfinite(_f32(x)) for x in o):
+        raise ValueError("origin must be 3 finite numbers")
+    d = [int(x) for x in dims]
+    if len(d) != 3 or not all(2 <= x <= MESH_MAX_DIM for x in d):
+        raise ValueError("dims must be 3 integers in [2, %d], not %r" % (MESH_MAX_DIM, tuple(dims)))
+    if d[0] * d[1] * d[2] > _INT_MAX:
+        raise ValueError("dims %r: more than 2^31 - 1 voxels" % (tuple(d),))
+    s = _f32(voxel)
+    if not (np.isfinite(s) and s > 0):
+        raise ValueError("voxel must be finite and > 0, not %r" % (voxel,))
+    return o, float(voxel), tuple(d)
+
+
+def _check_min_weight(min_weight) -> int:
+    if int(min_weight) != min_weight or int(min_weight) < 1:
+        raise ValueError("min_weight must be an integer >= 1, not %r" % (min_weight,))
+    return int(min_weight)
+
+
+def _tensor_device(a, device):
+    """(is_device, device ordinal) of a buffer: a CUDA tensor's own device, which a given `device` must match."""
+    if hasattr(a, "is_cuda") and a.is_cuda:
+        if device is not None and int(device) != a.device.index:
+            raise ValueError("device %d differs from the tensor's %s" % (device, a.device))
+        return True, a.device.index
+    return False, 0 if device is None else int(device)
+
+
+def tsdf_integrate(depth, Ps, origin, voxel: float, dims, trunc: float, depth_min: float, depth_max: float,
+                   cam_scale: float = 1.0, device: Optional[int] = None):
+    """Integrate N depth maps into a truncated signed distance volume on the GPU (gpm_tsdf_integrate, DESIGN.md §24).
+
+    depth: [N, H, W] float32 (the w of batch_run's norm4, or the disp.dmb files; 0 and depths outside [depth_min,
+    depth_max] are invalid), numpy or torch (host or CUDA); Ps: the N 3x4 projection matrices of those views; origin: the
+    box's corner; voxel: its edge; dims: (nx, ny, nz); trunc: the truncation in world units.  Returns (D, Wt, info): D
+    float32 and Wt uint16 volumes [nz, ny, nx] (NaN where Wt = 0) in the inputs' kind of memory (numpy, or CUDA tensors
+    on the input's device), info with upload_ms and integrate_ms (CUDA events)."""
+    o, s, d = _check_box(origin, voxel, dims)
+    t = _f32(trunc)
+    if not (np.isfinite(t) and t > 0):
+        raise ValueError("trunc must be finite and > 0, not %r" % (trunc,))
+    lo, hi = _f32(depth_min), _f32(depth_max)
+    if not (np.isfinite(lo) and np.isfinite(hi) and 0 <= lo < hi):
+        raise ValueError("need finite 0 <= depth_min < depth_max")
+    if not (cam_scale > 0):
+        raise ValueError("cam_scale must be > 0")
+    shape = tuple(depth.shape)
+    if len(shape) != 3 or not 1 <= shape[0] <= GPM_FUSE_MAX_VIEWS or len(Ps) != shape[0]:
+        raise ValueError("depth must be [N, H, W], 1 <= N <= %d, with one projection matrix per view" % GPM_FUSE_MAX_VIEWS)
+    if isinstance(depth, np.ndarray) and (depth.dtype != np.float32 or not depth.flags["C_CONTIGUOUS"]):
+        depth = np.ascontiguousarray(depth, dtype=np.float32)
+    on_dev, dev = _tensor_device(depth, device)
+    lib = load_library()
+    n, H, W = shape
+    pd, _ = _ptr(depth)
+    if on_dev:
+        import torch
+        D = torch.empty((d[2], d[1], d[0]), dtype=torch.float32, device=depth.device)
+        Wt = torch.empty((d[2], d[1], d[0]), dtype=torch.uint16, device=depth.device)
+        pD, pW = D.data_ptr(), Wt.data_ptr()
+    else:
+        D = np.empty((d[2], d[1], d[0]), np.float32)
+        Wt = np.empty((d[2], d[1], d[0]), np.uint16)
+        pD, pW = D.ctypes.data, Wt.ctypes.data
+    P = np.ascontiguousarray(np.stack([np.asarray(p, dtype=np.float64) for p in Ps]).reshape(-1))
+    desc = GpmTsdfDesc(n, W, H, pd, int(on_dev), P.ctypes.data_as(C.POINTER(C.c_double)), float(cam_scale), float(depth_min),
+                       float(depth_max), (C.c_float * 3)(*o), s, (C.c_int * 3)(*d), float(trunc), dev)
+    r = GpmTsdfResult(pD, pW, 0.0, 0.0)
+    if lib.gpm_tsdf_integrate(C.byref(desc), C.byref(r)) != 0:
+        raise GipumaError(lib.gpm_last_error().decode())
+    return D, Wt, {"upload_ms": float(r.upload_ms), "integrate_ms": float(r.integrate_ms)}
+
+
+def extract_mesh(D, Wt, origin, voxel: float, min_weight: int, device: Optional[int] = None):
+    """Marching tetrahedra on the lattice of voxel centres on the GPU (gpm_mesh_extract, DESIGN.md §24).
+
+    D: float32 and Wt: uint16 volumes [nz, ny, nx], both numpy or both CUDA tensors (what tsdf_integrate returns); a
+    point is valid when Wt >= min_weight and inside when D < 0.  Calls once to count and once to fill.  Returns
+    (vertices [V, 3] float32, faces [F, 3] int32, counter-clockwise seen from outside, info with upload_ms and extract_ms
+    of the filling call)."""
+    shape = tuple(D.shape)
+    if len(shape) != 3 or tuple(Wt.shape) != shape:
+        raise ValueError("D and Wt must be [nz, ny, nx] volumes of one shape")
+    o, s, d = _check_box(origin, voxel, shape[::-1])
+    mw = _check_min_weight(min_weight)
+    on_dev, dev = _tensor_device(D, device)
+    if _tensor_device(Wt, None)[0] != on_dev:
+        raise ValueError("D and Wt must both be host or both be CUDA buffers")
+    if on_dev:
+        import torch
+        if D.dtype != torch.float32 or Wt.dtype != torch.uint16 or Wt.device != D.device:
+            raise TypeError("D must be float32 and Wt uint16, on one device")
+        torch.cuda.current_stream(D.device).synchronize()
+        D, Wt = D.contiguous(), Wt.contiguous()
+        pD, pW = D.data_ptr(), Wt.data_ptr()
+    else:
+        if not isinstance(D, np.ndarray) or D.dtype != np.float32 or not isinstance(Wt, np.ndarray) or Wt.dtype != np.uint16:
+            raise TypeError("D must be float32 and Wt uint16 numpy arrays (or CUDA tensors)")
+        D, Wt = np.ascontiguousarray(D), np.ascontiguousarray(Wt)
+        pD, pW = D.ctypes.data, Wt.ctypes.data
+    lib = load_library()
+    desc = GpmMeshDesc(pD, pW, int(on_dev), (C.c_float * 3)(*o), s, (C.c_int * 3)(*d), mw, dev)
+    r = GpmMeshResult(0, 0, 0, 0, None, None, 0.0, 0.0)
+    rc = lib.gpm_mesh_extract(C.byref(desc), C.byref(r))              # count
+    if rc != 0 and not (rc == -1 and (r.n_vertices > 0 or r.n_faces > 0) and r.n_vertices <= _INT_MAX):
+        raise GipumaError(lib.gpm_last_error().decode())
+    verts = np.zeros((max(int(r.n_vertices), 1), 3), np.float32)
+    faces = np.zeros((max(int(r.n_faces), 1), 3), np.int32)
+    r = GpmMeshResult(0, 0, int(r.n_vertices), int(r.n_faces), verts.ctypes.data, faces.ctypes.data, 0.0, 0.0)
+    if lib.gpm_mesh_extract(C.byref(desc), C.byref(r)) != 0:         # fill
+        raise GipumaError(lib.gpm_last_error().decode())
+    return verts[:r.n_vertices], faces[:r.n_faces], {"upload_ms": float(r.upload_ms), "extract_ms": float(r.extract_ms)}
+
+
+def mesh(depth, Ps, origin, voxel: float, dims, depth_min: float, depth_max: float, trunc: Optional[float] = None,
+         min_weight: Optional[int] = None, cam_scale: float = 1.0, device: Optional[int] = None):
+    """tsdf_integrate then extract_mesh.  trunc (world units) defaults to MESH_DEFAULTS["trunc_voxels"] voxels and
+    min_weight to MESH_DEFAULTS["min_weight"].  Returns (vertices, faces, info with both stages' times)."""
+    trunc = MESH_DEFAULTS["trunc_voxels"] * float(voxel) if trunc is None else trunc
+    min_weight = MESH_DEFAULTS["min_weight"] if min_weight is None else min_weight
+    _check_min_weight(min_weight)
+    D, Wt, i1 = tsdf_integrate(depth, Ps, origin, voxel, dims, trunc, depth_min, depth_max, cam_scale, device)
+    v, f, i2 = extract_mesh(D, Wt, origin, voxel, min_weight)
+    return v, f, {"upload_ms": i1["upload_ms"], "integrate_ms": i1["integrate_ms"], "extract_ms": i2["extract_ms"]}
+
+
+def _mesh_arrays(vertices, faces):
+    v = np.ascontiguousarray(vertices, dtype=np.float32)
+    f = np.ascontiguousarray(faces, dtype=np.int32)
+    if v.ndim != 2 or v.shape[1] != 3 or f.ndim != 2 or f.shape[1] != 3:
+        raise ValueError("vertices must be [V, 3] and faces [F, 3]")
+    if len(f) and (f.min() < 0 or f.max() >= len(v)):
+        raise ValueError("a face index is outside [0, %d)" % len(v))
+    return v, f
+
+
+def write_ply_mesh(path: str, vertices, faces):
+    """Binary little-endian PLY: float x, y, z per vertex, `property list uchar int vertex_indices` per face."""
+    v, f = _mesh_arrays(vertices, faces)
+    if load_library().gpm_write_ply_mesh(path.encode(), v.ctypes.data if len(v) else None, len(v),
+                                         f.ctypes.data if len(f) else None, len(f)) != 0:
+        raise GipumaError("gpm_write_ply_mesh: cannot write %s" % path)
+
+
+def read_ply_mesh(path: str):
+    """(vertices [V, 3] float32, faces [F, 3] int32) of a PLY mesh in the layout write_ply_mesh writes."""
+    with open(path, "rb") as fh:
+        data = fh.read()
+    end = data.find(b"end_header\n")
+    if not data.startswith(b"ply\n") or end < 0:
+        raise GipumaError("%s: not a PLY file" % path)
+    header = data[:end].decode("ascii").splitlines()
+    want = ["ply", "format binary_little_endian 1.0", None, "property float x", "property float y", "property float z",
+            None, "property list uchar int vertex_indices"]
+    if len(header) != len(want) or any(w is not None and h != w for h, w in zip(header, want)) or \
+            not header[2].startswith("element vertex ") or not header[6].startswith("element face "):
+        raise GipumaError("%s: not the x, y, z + vertex_indices binary layout" % path)
+    nv, nf = int(header[2].split()[2]), int(header[6].split()[2])
+    body = data[end + len(b"end_header\n"):]
+    if len(body) != 12 * nv + 13 * nf:
+        raise GipumaError("%s: %d bytes of data for %d vertices and %d faces" % (path, len(body), nv, nf))
+    v = np.frombuffer(body, dtype="<f4", count=3 * nv).reshape(nv, 3).copy()
+    rec = np.frombuffer(body, dtype=np.dtype([("n", "u1"), ("i", "<i4", 3)]), offset=12 * nv, count=nf)
+    if (rec["n"] != 3).any():
+        raise GipumaError("%s: a face is not a triangle" % path)
+    return v, rec["i"].astype(np.int32)
+
+
+def sample_mesh(vertices, faces, spacing: float) -> np.ndarray:
+    """Points on a triangle mesh, deterministic, for scoring it with evaluate_cloud as DTU's surface track does: each face
+    a, b, c with n = ceil(longest edge / spacing) (at least 1) gives the barycentric lattice points
+    a + (i / n)(b - a) + (j / n)(c - a), i, j >= 0, i + j <= n, computed in float64.  Faces in order; within a face
+    i-major.  Returns (M, 3) float32."""
+    if not (np.isfinite(spacing) and spacing > 0):
+        raise ValueError("spacing must be finite and > 0")
+    v, f = _mesh_arrays(vertices, faces)
+    if not len(f):
+        return np.zeros((0, 3), np.float32)
+    V = v.astype(np.float64)
+    a, b, c = V[f[:, 0]], V[f[:, 1]], V[f[:, 2]]
+    L = np.max(np.stack([np.linalg.norm(b - a, axis=1), np.linalg.norm(c - b, axis=1), np.linalg.norm(a - c, axis=1)]), axis=0)
+    n = np.maximum(1, np.ceil(L / spacing)).astype(np.int64)
+    per = (n + 1) * (n + 2) // 2
+    start = np.concatenate([[0], np.cumsum(per)])
+    out = np.empty((int(start[-1]), 3), np.float64)
+    for m in np.unique(n):
+        sel = np.nonzero(n == m)[0]
+        i, j = np.array([(i, j) for i in range(m + 1) for j in range(m + 1 - i)], dtype=np.float64).T / m
+        pts = a[sel, None, :] + i[None, :, None] * (b - a)[sel, None, :] + j[None, :, None] * (c - a)[sel, None, :]
+        idx = start[sel][:, None] + np.arange(len(i))[None, :]
+        out[idx.reshape(-1)] = pts.reshape(-1, 3)
+    return out.astype(np.float32)

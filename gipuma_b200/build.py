@@ -20,10 +20,11 @@ ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 # --use_fast_math: same arithmetic mode as the reference's build (CMakeLists.txt:23); the kernels pin every
 # operation with explicit .rn.ftz intrinsics on top of it (gpm_device.cuh).
 COMMON = ["-O3", "--use_fast_math", "-std=c++17", "-lineinfo", "-Xcompiler", "-fPIC", "-shared"] + ARCH
-# The fusion (gpm_fuse.cu), the cloud distances (gpm_cloud.cu) and the pyramid / plane upsampling (gpm_scale.cu) are compiled
-# on their own in IEEE mode: denormals kept, no contraction, so that the fusion's decisions are exactly those of the scalar
-# restatement oracle/fusion_oracle.c (DESIGN.md §12), every distance is exactly that of the brute-force restatement
-# oracle/pycloud.py (§13) and every pyramid and upsampled value that of oracle/pyscale.py (§19).
+# The fusion (gpm_fuse.cu), the cloud distances (gpm_cloud.cu), the pyramid / plane upsampling (gpm_scale.cu) and the
+# meshing (gpm_mesh.cu) are compiled on their own in IEEE mode: denormals kept, no contraction, so that the fusion's
+# decisions are exactly those of the scalar restatement oracle/fusion_oracle.c (DESIGN.md §12), every distance is exactly
+# that of the brute-force restatement oracle/pycloud.py (§13), every pyramid and upsampled value that of oracle/pyscale.py
+# (§19) and every volume, vertex and face that of oracle/mesh_oracle.c (§24).
 FUSE = ["-O3", "-std=c++17", "-lineinfo", "-Xcompiler", "-fPIC", "-ftz=false", "-prec-div=true", "-prec-sqrt=true",
         "-fmad=false", "-c"] + ARCH
 
@@ -44,7 +45,7 @@ def _run(cmd):
 def build_library(force: bool = False) -> str:
     csrc = lambda *names: [os.path.join(HERE, "csrc", f) for f in names]
     fast = csrc("gpm_api.cu", "gpm_host.cpp", "gpm_batch.cpp", "gpm_prior.cpp")
-    ieee = csrc("gpm_fuse.cu", "gpm_cloud.cu", "gpm_scale.cu")
+    ieee = csrc("gpm_fuse.cu", "gpm_cloud.cu", "gpm_scale.cu", "gpm_mesh.cu")
     headers = csrc("gpm_kernels.cuh", "gpm_device.cuh", "gpm_scale.cuh") + [os.path.join(ROOT, "include", "gipuma_b200.h")]
     out = os.path.join(HERE, "libgipuma_b200.so")
     stamp = out + ".sig"

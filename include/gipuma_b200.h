@@ -510,6 +510,85 @@ typedef struct gpm_nn_result {
 } gpm_nn_result;
 int gpm_nearest_dist(const gpm_nn_desc* desc, gpm_nn_result* result);
 
+/* ---- meshing (DESIGN.md §24): depth maps -> truncated signed distance volume -> triangle mesh.  Both stages are fp32, one
+ * IEEE round-to-nearest step per operation in the order DESIGN.md §24 states, so they are deterministic and independent of
+ * where the inputs live.  The volume is an axis-aligned box of nx * ny * nz voxels (each in 2..2048, at most 2^31 - 1 in
+ * all) of edge `voxel`; voxel (i, j, k) has its centre at origin + ((i, j, k) + 0.5) * voxel and is element
+ * (k * ny + j) * nx + i of every volume (x fastest). */
+#define GPM_MESH_MAX_DIM 2048
+
+/* TSDF integration.  Per voxel centre X and view n in ascending order: h = P_n [X, 1] (the fusion's camera, gpm_fuse_cameras)
+ * and z = h_2; the view is skipped unless z > 0, the pixel u = floor(h0/z + 0.5), v = floor(h1/z + 0.5) is in the image, its
+ * depth d is > 0 and in [depth_min, depth_max], and sdf = d - z >= -trunc.  Otherwise S += min(sdf, trunc) / trunc and
+ * Wt += 1.  D = S / Wt, a NaN (bits 0x7fffffff) where Wt = 0. */
+typedef struct gpm_tsdf_desc {
+    int n_views, width, height;        /* 1 <= n_views <= GPM_FUSE_MAX_VIEWS */
+    const float* depth;                /* n_views * height*width floats: depth along each camera's z axis (norm4.w) */
+    int on_device;                     /* depth, result->D and result->weight are device pointers on `device` (1) or host (0) */
+    const double* P;                   /* n_views row-major 3x4 projection matrices, as passed to gpm_batch_run */
+    double cam_scale;                  /* > 0, as gpm_fuse_cameras */
+    float depth_min, depth_max;        /* finite, 0 <= depth_min < depth_max */
+    float origin[3];                   /* finite: the corner of the box, world units */
+    float voxel;                       /* finite, > 0 */
+    int dims[3];                       /* nx, ny, nz */
+    float trunc;                       /* finite, > 0, world units */
+    int device;                        /* CUDA device ordinal */
+} gpm_tsdf_desc;
+
+/* D (nz*ny*nx floats) and weight (nz*ny*nx uint16) are caller memory of the inputs' kind.  upload_ms: the depth maps'
+ * host-to-device copy (0 for device inputs); integrate_ms: the integration kernel.  CUDA events. */
+typedef struct gpm_tsdf_result {
+    float* D;
+    unsigned short* weight;
+    float upload_ms, integrate_ms;
+} gpm_tsdf_result;
+/* Refused with GPM_E_ARG before any CUDA call: null pointers, n_views outside 1..GPM_FUSE_MAX_VIEWS, an image size < 1 or
+ * over 2^30 pixels, dims outside 2..GPM_MESH_MAX_DIM or over 2^31 - 1 voxels, voxel or trunc not finite or <= 0, a
+ * non-finite origin, a bad depth range, a projection matrix gpm_fuse_cameras refuses.  The call allocates its own stream
+ * and buffers and frees them before returning; an allocation failure is GPM_E_CUDA. */
+int gpm_tsdf_integrate(const gpm_tsdf_desc* desc, gpm_tsdf_result* result);
+
+/* Surface extraction by marching tetrahedra on the lattice of voxel centres.  A point is valid when weight >= min_weight
+ * and inside when D < 0 (so -0.0 is outside).  Each cube of 8 neighbouring points splits into the 6 Kuhn tetrahedra
+ * 0, e_a, e_a + e_b, 1 for the axis permutations (a, b, c) = xyz, xzy, yxz, yzx, zxy, zyx in that order; a tetrahedron is
+ * meshed when its 4 corners are valid.  Each crossing edge (one corner inside, one outside) of a meshed tetrahedron gives
+ * one vertex, identified by its lower end p and its direction (x, y, z, x+y, x+z, y+z, x+y+z), at x_p + t (x_q - x_p)
+ * per axis with t = D_p / (D_p - D_q); vertex ids run in (lattice index of p, direction) order.  A meshed tetrahedron with
+ * 1 or 3 inside corners gives 1 triangle, with 2 gives 2 (the split of DESIGN.md §24); faces wind counter-clockwise seen
+ * from outside and come in (cube, tetrahedron) order. */
+typedef struct gpm_mesh_desc {
+    const float* D;                    /* nz*ny*nx floats */
+    const unsigned short* weight;      /* nz*ny*nx */
+    int on_device;                     /* D and weight are device pointers on `device` (1) or host memory (0) */
+    float origin[3];                   /* finite */
+    float voxel;                       /* finite, > 0 */
+    int dims[3];                       /* nx, ny, nz */
+    int min_weight;                    /* >= 1 */
+    int device;                        /* CUDA device ordinal */
+} gpm_mesh_desc;
+
+/* Caller-sized host result.  n_vertices and n_faces always receive the counts.  Up to vertex_capacity vertices (3 floats
+ * x, y, z each) and face_capacity faces (3 vertex ids each) are written; when a count exceeds its capacity the call
+ * returns GPM_E_ARG after the whole extraction, so a caller may retry with the counts.  A mesh of 2^31 or more vertices is
+ * refused with GPM_E_ARG (ids are int).  upload_ms: the volumes' host-to-device copies (0 for device inputs); extract_ms:
+ * the extraction kernels, up to the downloads.  CUDA events. */
+typedef struct gpm_mesh_result {
+    long long n_vertices, n_faces;
+    long long vertex_capacity, face_capacity;
+    float* vertices;                   /* NULL or vertex_capacity * 3 floats */
+    int* faces;                        /* NULL or face_capacity * 3 ints */
+    float upload_ms, extract_ms;
+} gpm_mesh_result;
+/* Refused with GPM_E_ARG before any CUDA call: null pointers, dims outside 2..GPM_MESH_MAX_DIM or over 2^31 - 1 points,
+ * voxel not finite or <= 0, a non-finite origin, min_weight < 1, a negative capacity or a missing buffer for a positive
+ * one.  The call allocates its own stream and buffers and frees them before returning; an allocation failure is
+ * GPM_E_CUDA. */
+int gpm_mesh_extract(const gpm_mesh_desc* desc, gpm_mesh_result* result);
+
+/* Binary little-endian PLY: `float x, y, z` per vertex, `property list uchar int vertex_indices` per face.  Refused with
+ * GPM_E_ARG: negative counts, missing buffers, a face index outside [0, n_vertices). */
+int gpm_write_ply_mesh(const char* path, const float* vertices, long long n_vertices, const int* faces, long long n_faces);
+
 const char* gpm_last_error(void);
 const char* gpm_version(void);
 
