@@ -1604,8 +1604,10 @@ def extract_mesh(D, Wt, origin, voxel: float, min_weight: int, device: Optional[
         import torch
         if D.dtype != torch.float32 or Wt.dtype != torch.uint16 or Wt.device != D.device:
             raise TypeError("D must be float32 and Wt uint16, on one device")
-        torch.cuda.current_stream(D.device).synchronize()
+        # a non-contiguous view is copied on torch's stream; gpm_mesh_extract reads on its own stream, so the copy must be
+        # finished before the call: copy first, then synchronise
         D, Wt = D.contiguous(), Wt.contiguous()
+        torch.cuda.current_stream(D.device).synchronize()
         pD, pW = D.data_ptr(), Wt.data_ptr()
     else:
         if not isinstance(D, np.ndarray) or D.dtype != np.float32 or not isinstance(Wt, np.ndarray) or Wt.dtype != np.uint16:

@@ -5,6 +5,8 @@ the surface."""
 import numpy as np
 import pytest
 
+from conftest import bits_equal
+
 pytestmark = pytest.mark.gpu
 
 DMIN, DMAX = 300.0, 800.0
@@ -122,6 +124,20 @@ def _adversarial():
     out.append(("NaN where Wt = 0", D, Wt, 1))
     D = rng.choice(np.array([-0.0, 0.0, -1.0, 1.0, 1e-30, -1e-45], np.float32), (6, 7, 8))
     out.append(("zeros, signed zeros and denormals", D, np.ones(D.shape, np.uint16), 1))
+    # long thin boxes, (nx, ny, nz) = (2048, 2, 3), (3, 2048, 2), (2, 3, 2048), and a 2048 x 2048 x 2 sheet: per-axis
+    # neighbour offsets and many blocks per scan
+    for shape in ((3, 2, 2048), (2, 2048, 3), (2048, 3, 2), (2, 2048, 2048)):
+        D = rng.standard_normal(shape).astype(np.float32)
+        out.append(("dims %s" % (shape[::-1],), D, rng.integers(0, 3, shape).astype(np.uint16), 1))
+    # infinite, NaN and +-FLT_MAX values at valid points: dp - dq overflows, t is NaN or 0
+    big = np.finfo(np.float32).max
+    D = rng.choice(np.array([np.inf, -np.inf, np.nan, big, -big, 1.0, -1.0, -0.0], np.float32), (7, 8, 9))
+    out.append(("inf, NaN and FLT_MAX at valid points", D, np.ones(D.shape, np.uint16), 1))
+    # the largest weight: min_weight 65535 keeps the points at 65535, 65536 keeps none
+    D = rng.standard_normal((6, 7, 8)).astype(np.float32)
+    Wt = rng.choice(np.array([65535, 65534, 1], np.uint16), D.shape)
+    out.append(("Wt 65535, min_weight 65535", D, Wt, 65535))
+    out.append(("Wt 65535, min_weight 65536", D, Wt, 65536))
     return out
 
 
@@ -134,7 +150,9 @@ def test_gpu_mesh_on_adversarial_volumes(case):
     origin, voxel = (0.25, -3.0, 1.5), 0.75
     v, f, _ = api.extract_mesh(D, Wt, origin, voxel, mw)
     ov, of = pymesh.extract(D, Wt, origin, voxel, mw)
-    assert _bits_equal(v, ov) and np.array_equal(f, of), name
+    # bit for bit, NaN equal to NaN: where dp - dq is inf - inf or overflows, the GPU's NaN is 0x7fffffff and the host's
+    # keeps the sign and payload of the NaN it came from
+    assert v.shape == ov.shape and bits_equal(v, ov) == 0 and np.array_equal(f, of), name
     dv, df, _ = api.extract_mesh(torch.from_numpy(D).cuda(), torch.from_numpy(Wt.astype(np.int32)).to(torch.uint16).cuda(),
                                  origin, voxel, mw)
     assert _bits_equal(dv, v) and np.array_equal(df, f), name
@@ -142,6 +160,8 @@ def test_gpu_mesh_on_adversarial_volumes(case):
         assert len(v) == 0 and len(f) == 0
     if name == "one valid tetrahedron":
         assert len(v) == 3 and len(f) == 1
+    if name.startswith("Wt 65535"):
+        assert (len(f) > 0) == (mw == 65535)
 
 
 def test_gpu_tsdf_with_a_box_partly_behind_a_camera(rig):
